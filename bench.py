@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — loop-closure queries/sec on B200 (BASELINE.json metric) + roofline + CPU baseline.
+"""bench.py — loop-closure queries/sec on H100 (BASELINE.json metric) + roofline + CPU baseline.
 
     python bench.py --gpus 1 --steps 30 --warmup 3
+    python bench.py --gpus 1 --steps 30 --warmup 3 --dump-outputs DIR   # + the last timed step's outputs as DIR/<name>.npy
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --impl reference          # the reference's CPU algorithm on the host cores
 
@@ -21,6 +22,8 @@ likelihood arg-max is a true loop closure and its verification succeeds.
           word ids + likelihood + verified poses out; H2D/D2H inside the timed region).
 `roofline` the dictionary-NN kernel (knn2_tensor_kernel; knn2_hamming_kernel with LCD_NN_TENSOR=0), timed live with CUDA events on its stream.
 `cpu_baseline` / --impl reference: cv2.ORB + the oracle port of the reference algorithm on the host cores.
+--dump-outputs DIR  writes what the timed device path returned in its last timed step (word ids, likelihood rows, hypotheses,
+          verification results) as float32 / float64 .npy files; the inputs are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -63,22 +66,22 @@ def peaks():
     if p.exists():
         d = json.loads(p.read_text())
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)", float(d.get("sm_max_mhz", 1965.0))
-    return 6650.0, "fallback (B200_PROFILING.md)", 1965.0
+    return 3350.0, "H100 SXM data sheet (HBM3 3.35 TB/s)", 1980.0
 
 
 def tensor_peak_tops():
     """Dense s8 tensor peak in Tera-op/s: MEASURED_PEAKS.json holds the measured bf16 figure (burst: the kernel is timed
-    alone); tcgen05 kind::i8 runs at twice the bf16 rate (K=32 per instruction against K=16), so the s8 roof is 2x it."""
+    alone); wgmma .s8 runs at twice the bf16 rate (K=32 per instruction against K=16), so the s8 roof is 2x it."""
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         d = json.loads(p.read_text())
         if "bf16_tflops" in d:
             return 2.0 * float(d["bf16_tflops"]), "2 x measured bf16 dense (MEASURED_PEAKS.json bf16_tflops, burst)"
-    return 2.0 * 2250.0, "2 x nominal bf16 dense (B200_PROFILING.md fallback)"
+    return 2.0 * 989.4, "2 x H100 SXM data-sheet bf16 dense (989.4 TFLOP/s at 700 W)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index: int):
         self.f = tempfile.NamedTemporaryFile("w+", suffix=".csv", delete=False)
@@ -122,6 +125,26 @@ class ClockSampler:
         except OSError:
             pass
         return out
+
+
+def dump_outputs(out_dir: str, words, likelihood, hypothesis, verify) -> None:
+    """The outputs of one step as out_dir/<name>.npy: ids as float64 (exact), likelihood as float32, and the verification results of
+    every frame (ok, match and inlier counts, rvec, tvec, 6x6 covariance) as float64.  At most 64 MB: a larger likelihood block keeps a
+    fixed, seeded sample of its rows."""
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    likelihood = np.asarray(likelihood, np.float32)
+    budget = 48 << 20
+    if likelihood.nbytes > budget:
+        rows = np.sort(np.random.default_rng(0).choice(len(likelihood), budget // likelihood[0].nbytes, replace=False))
+        np.save(d / "likelihood_rows.npy", rows.astype(np.float64))
+        likelihood = likelihood[rows]
+    np.save(d / "likelihood.npy", likelihood)
+    np.save(d / "words.npy", np.asarray(words, np.float64))
+    np.save(d / "hypothesis.npy", np.asarray(hypothesis, np.float64))
+    np.save(d / "verify_counts.npy", np.array([[r["ok"], r["n_matches"], r["n_inliers"]] for r in verify], np.float64))
+    np.save(d / "verify_pose.npy", np.array([np.concatenate([np.ravel(r["rvec"]), np.ravel(r["tvec"])]) for r in verify], np.float64))
+    np.save(d / "verify_covariance.npy", np.array([np.ravel(r["covariance"]) for r in verify], np.float64))
 
 
 def parallelism_text(world_size: int, batch: int) -> str:
@@ -417,6 +440,10 @@ def run_b200(args):
     last_pool = (args.steps - 1) % n_pool
     true_places = places[last_pool * BL:(last_pool + 1) * BL]
     hyp_d, res_d = eng.process_fetch(nf)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, words=d_words.view(-1, F_FEATS).cpu().numpy(), likelihood=d_like.view(-1, S_SIGS).cpu().numpy(),
+                     hypothesis=hyp_d, verify=res_d)
+
     def hit_rate(hyp):
         known = true_places >= 0
         return float(np.mean((world.sig_place[np.maximum(hyp, 1) - 1] == true_places)[known] & (hyp[known] > 0))) if known.any() else None
@@ -570,30 +597,17 @@ def run_b200(args):
     pairs = float(rows_local) * nq
     popc_per_pair = 5  # LCD_NN_VARIANT=2: partial carry-save tree, 8 XOR words -> 5 POPC
     sm_clk = (clocks or {}).get("sm_mhz") or sm_max
-    popc_peak = 16.0 * 148 * sm_clk * 1e6  # 16 POPC lanes / clk / SM, measured (profiles/r01_nn_sweep.json)
-    traffic = None
-    tp = ROOT / "profiles" / "roofline_traffic.json"
-    if tp.exists():
-        try:
-            traffic = json.loads(tp.read_text()).get("knn2_hamming_kernel_dram_bytes_per_launch")
-        except Exception:
-            traffic = None
+    popc_peak = 16.0 * torch.cuda.get_device_properties(local).multi_processor_count * sm_clk * 1e6  # 16 POPC lanes / clk / SM
     share = dict({k + "_ms": v[0] / args.steps for k, v in prof.items()}, step_ms=dev_ms / args.steps)
     if os.environ.get("LCD_NN_TENSOR", "1") != "0":
-        # dominant kernel: knn2_tensor_kernel (tcgen05 kind::i8).  Algorithmic work per launch = one s8 multiply-add per
+        # dominant kernel: knn2_tensor_kernel (wgmma .s32.s8.s8).  Algorithmic work per launch = one s8 multiply-add per
         # (query, word, descriptor bit): 2 * Q * W * 256 operations (DESIGN.md §4).
         ops = 2.0 * pairs * DESC_BYTES * 8
         tpeak, tsrc = tensor_peak_tops()
         ach = ops / nn_avg_s / 1e12 if nn_avg_s > 0 else 0.0
-        traffic_t = None
-        if tp.exists():
-            try:
-                traffic_t = json.loads(tp.read_text()).get("knn2_tensor_kernel_dram_bytes_per_launch")
-            except Exception:
-                traffic_t = None
         roofline = {
-            "kernel": "knn2_tensor_kernel (tcgen05.mma kind::i8, M128 N256 K32)", "bound": "tensor", "achieved": ach, "peak": tpeak,
-            "unit": "TFLOP/s", "frac": ach / tpeak, "peak_source": tsrc, "traffic": traffic_t,
+            "kernel": "knn2_tensor_kernel (wgmma .s32.s8.s8, M64 N256 K32 per warpgroup, 128 queries per CTA)", "bound": "tensor", "achieved": ach,
+            "peak": tpeak, "unit": "TFLOP/s", "frac": ach / tpeak, "peak_source": tsrc,
             "algorithmic_ops_per_launch": ops, "algorithmic_bytes_per_launch": alg_bytes,
             "avg_launch_ms": nn_avg_s * 1e3, "launches_timed": int(nn_launches),
             "note": "s8 operations counted as FLOPs of the +-1 encoded Hamming GEMM; results are exact integers (parity tests)",
@@ -602,7 +616,7 @@ def run_b200(args):
     else:
         roofline = {
             "kernel": "knn2_hamming_kernel<8,8,2>", "bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak,
-            "peak_source": peak_src, "traffic": traffic, "algorithmic_bytes_per_launch": alg_bytes,
+            "peak_source": peak_src, "algorithmic_bytes_per_launch": alg_bytes,
             "avg_launch_ms": nn_avg_s * 1e3, "launches_timed": int(nn_launches),
             "binding_resource": "integer pipes (POPC 16 lanes/clk/SM on XU + LOP3 on ALU): the vocabulary is SMEM/L2 resident, see DESIGN.md §4",
             "pairs_per_s": pairs / nn_avg_s if nn_avg_s > 0 else 0.0,
@@ -628,7 +642,6 @@ def run_b200(args):
             "bound": "integer pipes (POPC 16 lanes/clk/SM)", "popc_per_s": pairs * popc_per_pair / p_s if p_s > 0 else 0.0,
             "popc_peak_per_s": popc_peak, "popc_frac": (pairs * popc_per_pair / p_s) / popc_peak if p_s > 0 else 0.0,
             "hbm_GBps": alg_bytes / p_s / 1e9 if p_s > 0 else 0.0, "hbm_frac": (alg_bytes / p_s / 1e9) / hbm_peak if p_s > 0 else 0.0,
-            "traffic": traffic,
         }
 
     # ---- CPU baseline (rank 0 at N=1) and the oracle cross-check of this very run (every N) -------------------------------
@@ -685,7 +698,6 @@ def run_b200(args):
     roofline["stage_orb"] = {"stage": "detect (all orb_* kernels of one step)", "bound": "hbm (nominal; measured: instruction issue, DESIGN.md 4.3)",
                              "algorithmic_bytes_per_step": orb_bytes, "avg_ms": orb_s * 1e3, "achieved": orb_bytes / orb_s / 1e9 if orb_s > 0 else 0.0,
                              "peak": hbm_peak, "unit": "GB/s", "frac": (orb_bytes / orb_s / 1e9) / hbm_peak if orb_s > 0 else 0.0}
-    roofline["traffic_source"] = "profiles/roofline_traffic.json: dram__bytes_read.sum + dram__bytes_write.sum of one `ncu --set full` capture of this command, per launch"
     roofline["timing_note"] = "per-kernel times come from CUDA events recorded around every launch inside the timed region (lcd_profile_enable(1)): the step time includes those events"
 
     line = {
@@ -888,7 +900,7 @@ def run_reference_c4(args):
 
 
 def run_c4(args):
-    """configs[3] on one B200: quantise + score of `batch` frames of 1000 float descriptors against 1M words / 100k signatures."""
+    """configs[3] on one H100: quantise + score of `batch` frames of 1000 float descriptors against 1M words / 100k signatures."""
     import torch
 
     from oracle import oracle_py as orc
@@ -976,21 +988,17 @@ def run_c4(args):
     flops = 2.0 * nq * W * C4_DIM
     alg_bytes = W * C4_DIM * 4 + nq * C4_DIM * 4 + nq * 16  # SURVEY 8(d): W*D + Q*D + Q*16
     tp = ROOT / "MEASURED_PEAKS.json"
-    f16_peak = float(json.loads(tp.read_text()).get("bf16_tflops", 2250.0)) if tp.exists() else 2250.0
-    traffic = None
-    rt = ROOT / "profiles" / "roofline_traffic.json"
-    if rt.exists():
-        traffic = json.loads(rt.read_text()).get("knn2_tensor_f32_kernel_dram_bytes_per_launch")
+    f16_peak = float(json.loads(tp.read_text()).get("bf16_tflops", 989.4)) if tp.exists() else 989.4
     roofline = {
-        "kernel": "float dictionary NN = knn2_tensor_f32_kernel (tcgen05.mma kind::f16, M128 N256 K16, pre-pass + main pass) + rerank_l2_kernel + "
+        "kernel": "float dictionary NN = knn2_tensor_f32_kernel (wgmma .f32.f16.f16, M64 N256 K16 per warpgroup, pre-pass + main pass) + rerank_l2_kernel + "
                   "knn2_l2_fallback_kernel, timed together",
         "bound": "tensor", "achieved": flops / nn_s / 1e12 if nn_s > 0 else 0.0, "peak": f16_peak, "unit": "TFLOP/s",
         "frac": (flops / nn_s / 1e12) / f16_peak if nn_s > 0 else 0.0,
-        "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst; fp16 and bf16 run at the same tcgen05 rate)" if tp.exists() else "nominal 2250 (B200_PROFILING.md)",
-        "traffic": traffic, "algorithmic_flops_per_step": flops, "algorithmic_bytes_per_step": alg_bytes, "avg_ms": nn_s * 1e3, "steps_timed": int(nn_n),
+        "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst; fp16 and bf16 run at the same wgmma rate)" if tp.exists() else "H100 SXM data-sheet fp16 dense (989.4 TFLOP/s at 700 W)",
+        "algorithmic_flops_per_step": flops, "algorithmic_bytes_per_step": alg_bytes, "avg_ms": nn_s * 1e3, "steps_timed": int(nn_n),
         "hbm": {"achieved": alg_bytes / nn_s / 1e9 if nn_s > 0 else 0.0, "peak": hbm_peak, "unit": "GB/s", "frac": (alg_bytes / nn_s / 1e9) / hbm_peak if nn_s > 0 else 0.0,
                 "peak_source": peak_src, "note": "algorithmic bytes of ONE step (vocabulary read once per batch of frames); the kernel is epilogue / tensor bound, "
-                                                 "not HBM bound: the fp16 word image streams once per step (DESIGN.md 4.4)"},
+                                                 "not HBM bound: the fp16 word image streams once per step"},
         "step_share_ms": {k + "_ms": v[0] / args.steps for k, v in prof.items()},
         "filter": {"candidates_per_query": n_cand / nq, "queries_redone_by_exact_scan": n_fallback, "queries": nq,
                    "dictionary_rows_converted_to_fp16_since_start": rows_conv},
@@ -1037,7 +1045,11 @@ def main():
     ap.add_argument("--config", default="c2", choices=["c2", "c4"], help="c2 = BASELINE configs[1] (headline); c4 = configs[3]: float descriptors, 1M words")
     ap.add_argument("--words", type=int, default=0, help="c4: dictionary rows (default 1 000 000)")
     ap.add_argument("--signatures", type=int, default=0, help="c4: signatures in the map (default 100 000)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step (c2 headline) as DIR/<name>.npy, float32 / float64, at most 64 MB")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "b200" or args.config != "c2"):
+        ap.error("--dump-outputs applies to the GPU headline (--impl b200 --config c2)")
     if args.warmup < 3 and args.impl == "b200":
         args.warmup = 3
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 /*
- * lcd_b200.h — C ABI of the B200-native loop-closure hot path
+ * lcd_b200.h — C ABI of the H100-native loop-closure hot path
  * (detect -> quantise -> score -> verify) that drops in behind
  * rtabmap::Memory / VWDictionary / Signature / Feature2D.
  *

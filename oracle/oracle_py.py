@@ -6,6 +6,7 @@ TEST INFRASTRUCTURE ONLY: checker for tests/, smoke() and bench.py's CPU baselin
 from __future__ import annotations
 
 import ctypes as C
+import os
 import subprocess
 from pathlib import Path
 
@@ -23,12 +24,20 @@ _I = C.c_int
 _F = C.c_float
 
 
+def _reference_present() -> bool:
+    """True when the reference's sources can be read (a user without access to them sees no reference, not an error)."""
+    try:
+        return REFERENCE_ROOT.is_dir() and os.access(REFERENCE_ROOT, os.R_OK | os.X_OK)
+    except OSError:
+        return False
+
+
 def build(with_ref: bool = True) -> None:
     """Compile liboracle.so (always) and _ref/libref_flann.so (when /root/reference is present)."""
     srcs = [HERE / "oracle.cpp", HERE / "oracle_verify.cpp", HERE / "pnp_math.h"]
     if not LIB.exists() or LIB.stat().st_mtime < max(s.stat().st_mtime for s in srcs):
         subprocess.run(["make", "-C", str(HERE), "liboracle.so"], check=True, capture_output=True)
-    if with_ref and REFERENCE_ROOT.exists() and not REF_LIB.exists():
+    if with_ref and not REF_LIB.exists() and _reference_present():
         subprocess.run(["make", "-C", str(HERE), "ref"], check=True, capture_output=True)
 
 
@@ -80,7 +89,7 @@ def ref_lib():
     global _ref
     if _ref is None:
         if not REF_LIB.exists():
-            if REFERENCE_ROOT.exists():
+            if _reference_present():
                 build(with_ref=True)
             else:
                 return None

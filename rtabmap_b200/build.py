@@ -1,8 +1,8 @@
-"""Build the CUDA extension (sm_100a) in-tree with nvcc.
+"""Build the CUDA extension (sm_90a) in-tree with nvcc.
 
 The product is ONE shared library, rtabmap_b200/lib/liblcd_b200.so, exporting the C ABI of
 include/lcd_b200.h.  It is compiled with
-``-gencode arch=compute_100a,code=sm_100a -lineinfo`` (cross-compiles without a GPU) and is
+``-gencode arch=compute_90a,code=sm_90a -lineinfo`` (cross-compiles without a GPU) and is
 git-ignored but travels to the GPU box with the gpurun snapshot.
 """
 from __future__ import annotations
@@ -19,7 +19,7 @@ SOURCES = ["engine.cu"]
 HEADERS = ["common.cuh", "nn_hamming.cuh", "nn_tensor.cuh", "l2_path.cuh", "nn_tensor_f32.cuh", "resolve.cuh", "score.cuh", "bayes.cuh", "verify.cuh", "match_bf.cuh", "pnp_device.cuh", "orb.cuh", "orb_pattern.h", "../../include/lcd_b200.h"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "--fmad=false",  # fp64 PnP code must round like the host oracle; the integer kernels do not care
     "-shared", "-Xcompiler", "-fPIC",

@@ -1,4 +1,4 @@
-// common.cuh — shared device helpers for the loop-closure hot-path kernels (sm_100a).
+// common.cuh — shared device helpers for the loop-closure hot-path kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

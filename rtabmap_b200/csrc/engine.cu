@@ -252,7 +252,7 @@ struct lcd_engine
 	PinBuf<PackedVerifyResult> h_packed;
 	PinBuf<int> h_overflow;
 	std::atomic<long long> launches{0};
-	int sm_count = 148;
+	int sm_count = 132;
 	int smem_optin = 0;
 
 	// --- vocabulary: rows [0,n_indexed) searchable, [n_indexed, n_indexed+n_pending) not indexed
@@ -351,7 +351,7 @@ struct lcd_engine
 	int nn_f32_tensor = 1;      // LCD_NN_F32_TENSOR=0 forces the exact CUDA-core kernel
 	int nn_last_f32_tensor = 0;
 	long long tf_img_builds = 0; // rows expanded so far (diagnostics: the image is built once per dictionary change)
-	int nn_tensor = 1;   // 256-bit descriptors: tcgen05 int8 path (nn_tensor.cuh); 0 = POPC kernel (nn_hamming.cuh)
+	int nn_tensor = 1;   // 256-bit descriptors: wgmma int8 path (nn_tensor.cuh); 0 = POPC kernel (nn_hamming.cuh)
 	int nn_last_tensor = 0; // which kernel the last run_knn used (bench / diagnostics)
 	// mapping mode (lcd_map_*): detection of frame t+1 on the ORB stream while frame t is quantised and scored
 	struct MapSlot
@@ -717,7 +717,7 @@ int run_knn(lcd_engine * e, const uint32_t * d_q, int nq_total, int n_rows, int 
 			const int real_sp = (n_wtiles + tps - 1) / tps;
 			if (real_sp != sp) continue;
 			const long waves = (static_cast<long>(n_qtiles) * sp + e->sm_count - 1) / e->sm_count;
-			const long cost = waves * (tps + 3); // +3: prologue (TMEM alloc, first loads) and drain, in tile times
+			const long cost = waves * (tps + 3); // +3: prologue (barrier init, first loads) and drain, in tile times
 			if (best_cost < 0 || cost < best_cost)
 			{
 				best_cost = cost;
@@ -743,7 +743,7 @@ int run_knn(lcd_engine * e, const uint32_t * d_q, int nq_total, int n_rows, int 
 		}
 		LCD_CUDA(e, cudaFuncSetAttribute(knn2_tensor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kTcSmemBytes)));
 		prof_mark(e, LCD_PROF_NN, s);
-		// A CTA walks several (query tile, word split) items with one TMEM allocation and a running pipeline (LCD_NN_PERSIST=0: one CTA
+		// A CTA walks several (query tile, word split) items with one set of barriers and a running pipeline (LCD_NN_PERSIST=0: one CTA
 		// per item, as r01).  Unsharded: one CTA per SM takes them all.  Inside the sharded step the search runs beside NCCL kernels that
 		// need a few SMs now and then: a grid that holds every SM until the end starves them and then waits for them (measured at 4 ranks:
 		// 1.35 -> 1.48 ms), so there a CTA takes only enough items for ~96 word tiles and the grid stays several waves deep.
@@ -1065,7 +1065,7 @@ int localize_dev(lcd_engine * e, const uint32_t * d_q, int n_frames, int nq, int
 extern "C" {
 
 int lcd_abi_version(void) { return 2; }
-const char * lcd_build_arch(void) { return "sm_100a"; }
+const char * lcd_build_arch(void) { return "sm_90a"; }
 
 const char * lcd_last_error(const lcd_engine * e) { return e ? e->err.c_str() : g_create_error.c_str(); }
 long long lcd_launch_count(const lcd_engine * e) { return e ? e->launches.load() : 0; }

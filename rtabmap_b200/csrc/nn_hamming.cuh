@@ -6,7 +6,7 @@
 // (dist.h:533-580) and KNNSimpleResultSet::addPoint (util/result_set.h:151-172), as
 // called from VWDictionary::addNewWords (corelib/src/VWDictionary.cpp:1015-1024).
 //
-// Design (B200): the vocabulary is split into contiguous row chunks, one per CTA.  A CTA
+// Design (H100): the vocabulary is split into contiguous row chunks, one per CTA.  A CTA
 // pulls its chunk from L2/HBM into shared memory ONCE with 1-D bulk async copies (TMA
 // engine, mbarrier completion), so the vocabulary is read exactly once per launch
 // (algorithmic bytes W*D).  Each thread keeps TQ query descriptors in registers and walks

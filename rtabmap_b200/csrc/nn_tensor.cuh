@@ -1,26 +1,23 @@
-// nn_tensor.cuh — exact Hamming 2-NN of 256-bit descriptors on the 5th-generation tensor cores (sm_100a).
+// nn_tensor.cuh — exact Hamming 2-NN of 256-bit descriptors on the Hopper tensor cores (sm_90a, wgmma).
 //
 // The all-pairs distance matrix of VWDictionary::addNewWords / findNN (reference: corelib/src/VWDictionary.cpp:1004-1118,
 // the brute-force branch, and rtflann's LinearIndex::findNeighbors, rtflann/algorithms/linear_index.h:113-123) is
 // GEMM-shaped: with every descriptor bit b encoded as the signed byte 2b-1 the dot product of two descriptors is
 //     a . w = 256 - 2 * hamming(a, w),
-// an integer the tensor cores accumulate exactly in s32 (tcgen05.mma kind::i8).  The packed key order of
+// an integer the tensor cores accumulate exactly in s32 (wgmma .s32.s8.s8).  The packed key order of
 // common.cuh, (distance << 22) | row, is recovered in the epilogue as ((256 - acc) << 21) + row, so the result is
 // bit-identical to the POPC kernel of nn_hamming.cuh (and to the oracle).
 //
-// One CTA owns a tile of 128 queries (the M dimension; the tile's accumulator rows are the 128 TMEM lanes, so
-// each epilogue thread owns one query and keeps its running top-2 in registers) and a contiguous range of
-// 256-word tiles (N).  Roles:
-//   warp 0  producer  : cp.async.bulk (TMA engine) of the pre-tiled, pre-swizzled word image into smem (the image is cached with the
-//                       dictionary); the query tile is expanded in place by the epilogue warps from its packed form
-//   warp 1  MMA       : one thread issues 8 x tcgen05.mma (M128 N256 K32) per word tile into one of two TMEM
-//                       accumulator stages, then tcgen05.commit to the smem-empty and accumulator-full barriers
-//   warp 2  TMEM alloc/dealloc (512 columns)
-//   warps 4-19 epilogue: warp w reads TMEM lanes 32*(w%4).. (its queries) and the 64 columns of column group
-//                       (w-4)/4: two tcgen05.ld.x32 in flight, a max over the 64 values against the running
-//                       second-best filters almost every group, only improving candidates reach the key insert
+// One CTA owns a tile of 128 queries and a contiguous range of 256-word tiles.  Roles (three warpgroups):
+//   warpgroup 0  producer : one thread issues cp.async.bulk (TMA engine) of the pre-tiled, pre-swizzled word image into a ring of
+//                           shared-memory stages (the image is cached with the dictionary)
+//   warpgroups 1-2 consumers: warpgroup c owns queries [64 (c-1), 64 c) of the tile.  It expands its half of the query tile in place
+//                           from the packed form, issues 8 x wgmma.mma_async (M64 N256 K32) per word tile with the accumulators in
+//                           registers, releases the stage and runs the top-2 epilogue while the other consumer's MMAs use the
+//                           tensor cores.  Each query row is spread over the 4 threads of a lane quad (64 columns each), and each
+//                           thread keeps its own running top-2, written out as one of kTcEpiGroups partial results.
 //
-// Operand images (written by the expand kernels below): K-major, 128-byte swizzle (the canonical UMMA/TMA layout:
+// Operand images (written by the expand kernels below): K-major, 128-byte swizzle (the canonical GMMA/TMA layout:
 // 16-byte chunk c of row r of every 8-row x 128-byte block sits at chunk c ^ (r & 7)), split in K/128 "atoms":
 //   query tile : [atom][128 rows][128 B]            (32 KB for 256-bit descriptors)
 //   word tile  : [atom][256 rows][128 B]            (64 KB)
@@ -30,14 +27,13 @@
 
 namespace lcd {
 
-constexpr int kTcBM = 128;       // queries per CTA tile (UMMA M)
-constexpr int kTcBN = 256;       // words per tile (UMMA N)
+constexpr int kTcBM = 128;       // queries per CTA tile (two consumer warpgroups of M64)
+constexpr int kTcBN = 256;       // words per tile (wgmma N)
 constexpr int kTcK = 256;        // descriptor bits = int8 K extent
 constexpr int kTcAtoms = kTcK / 128;
-constexpr int kTcStages = 3;     // word-tile smem stages
-constexpr int kTcEpiGroups = 4;  // column groups of a tile, one set of 4 epilogue warps each
-constexpr int kTcEpiCols = kTcBN / kTcEpiGroups;
-constexpr int kTcThreads = 128 + 128 * kTcEpiGroups;
+constexpr int kTcStages = 3;     // word-tile smem stages (3 x 64 KB + the 32 KB query tile fit the 227 KB a block may use)
+constexpr int kTcEpiGroups = 4;  // partial results per query and split: the 4 threads of a lane quad that share a query row
+constexpr int kTcThreads = 384;  // producer warpgroup + two consumer warpgroups
 constexpr uint32_t kTcABytes = kTcBM * kTcK;
 constexpr uint32_t kTcBBytes = kTcBN * kTcK;
 constexpr size_t kTcSmemBytes = 1024 /* alignment slack */ + kTcABytes + kTcStages * kTcBBytes + 256 /* barriers */;
@@ -77,81 +73,75 @@ __global__ void tc_expand_kernel(const uint32_t * __restrict__ src /* [n_rows][8
 	dst[off16] = v;
 }
 
-// ---- tcgen05 / TMEM PTX wrappers ---------------------------------------------------------------
+// ---- Hopper mbarrier / wgmma helpers ---------------------------------------------------------------
 __device__ __forceinline__ void mbar_arrive(uint64_t * bar)
 {
 	asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_alloc(uint32_t * smem_dst, uint32_t cols)
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// named barrier over the 128 threads of one warpgroup (id 0 is __syncthreads)
+__device__ __forceinline__ void wg_bar_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+// shared-memory matrix descriptor (GMMA): K-major, SWIZZLE_128B, 8-row groups 1024 B apart
+__device__ __forceinline__ uint64_t wg_smem_desc(uint32_t saddr)
 {
-	asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(cols) : "memory");
-	asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+	uint64_t d = 0;
+	d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);        // start address  [0,14)
+	d |= static_cast<uint64_t>(1) << 16;                         // leading byte offset (unused for swizzled K-major)
+	d |= static_cast<uint64_t>(1024 >> 4) << 32;                 // stride byte offset [32,46)
+	d |= static_cast<uint64_t>(1) << 62;                         // layout type [62,64): SWIZZLE_128B
+	return d;
 }
-__device__ __forceinline__ void tc_dealloc(uint32_t taddr, uint32_t cols)
-{
-	asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tc_commit(uint64_t * bar)
-{
-	asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, s8 x s8 -> s32, M128 x N256 x K32
-__device__ __forceinline__ void tc_mma_i8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
+// D[regs] (+)= A[smem] * B[smem]^T, s8 x s8 -> s32, M64 x N256 x K32 over one warpgroup.  Accumulator fragment: thread (warp w,
+// lane l) holds rows 16 w + l / 4 (d[4 i], d[4 i + 1]) and 16 w + l / 4 + 8 (d[4 i + 2], d[4 i + 3]) at columns 8 i + 2 (l % 4) + {0, 1}.
+__device__ __forceinline__ void wg_mma_i8(int (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
 {
 	asm volatile(
 		"{\n"
 		".reg .pred p;\n"
-		"setp.ne.b32 p, %4, 0;\n"
-		"tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n"
-		"}\n" ::"r"(tmem_d),
-		"l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-		: "memory");
-}
-// shared-memory matrix descriptor: K-major, SWIZZLE_128B, 8-row groups 1024 B apart (cute::UMMA::SmemDescriptor)
-__device__ __forceinline__ uint64_t tc_smem_desc(uint32_t saddr)
-{
-	uint64_t d = 0;
-	d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);        // start address  [0,14)
-	d |= static_cast<uint64_t>(0) << 16;                         // leading byte offset (unused for swizzled K-major)
-	d |= static_cast<uint64_t>(1024 >> 4) << 32;                 // stride byte offset [32,46)
-	d |= static_cast<uint64_t>(1) << 46;                         // descriptor version (sm_100)
-	d |= static_cast<uint64_t>(2) << 61;                         // SWIZZLE_128B
-	return d;
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): s32 accumulator, s8 x s8, both K-major
-__device__ __forceinline__ constexpr uint32_t tc_idesc_i8(int m, int n)
-{
-	return (2u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
-}
-// 32 consecutive accumulator columns of this thread's TMEM lane
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, int (&v)[32])
-{
-	asm volatile(
-		"tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+		"setp.ne.b32 p, %130, 0;\n"
+		"wgmma.mma_async.sync.aligned.m64n256k32.s32.s8.s8 "
 		"{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-		"%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-		: "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-		  "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-		  "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-		  "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-		: "r"(taddr)
+		"%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+		"%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+		"%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+		"%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+		"%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+		"%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+		"%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+		"%128, %129, p;\n"
+		"}\n"
+		: "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+		  "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+		  "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+		  "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+		  "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+		  "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+		  "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+		  "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]),
+		  "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]),
+		  "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]),
+		  "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]),
+		  "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]),
+		  "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]),
+		  "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]), "+r"(d[111]),
+		  "+r"(d[112]), "+r"(d[113]), "+r"(d[114]), "+r"(d[115]), "+r"(d[116]), "+r"(d[117]), "+r"(d[118]), "+r"(d[119]),
+		  "+r"(d[120]), "+r"(d[121]), "+r"(d[122]), "+r"(d[123]), "+r"(d[124]), "+r"(d[125]), "+r"(d[126]), "+r"(d[127])
+		: "l"(adesc), "l"(bdesc), "r"(accumulate)
 		: "memory");
 }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ---- the kernel ------------------------------------------------------------------------------------
 // neg32 = (uint32_t)-32, passed as an argument so that the key arithmetic stays an IMAD on the FMA pipe instead of being
 // strength-reduced to a shift-add on the ALU pipe, which the min/max network needs.
 // Work items = (query tile, word split) pairs, item = split * n_qtiles + qtile.  The grid is PERSISTENT: CTA b runs items b, b + gridDim.x,
-// ... with one TMEM allocation and one set of barriers; the word-tile stream, the MMA issue and the two accumulator stages run on across
-// item boundaries (all barrier phases are functions of a CTA-wide running tile count), and the epilogue warps write the next item's query
-// tile into shared memory as soon as the last MMA of the current item has completed, before they read that last accumulator out.  What
-// an item boundary costs is that expansion (a few hundred cycles) instead of a CTA launch, a TMEM allocation and a pipeline fill — which
-// is what a word-range shard with few tiles per item was paying (24 tiles per item at 8 ranks).
-// partial[(split * kTcEpiGroups + column group) * nq + query] = (best key, second key) over the rows of that split that fall in that
-// column group of their tile.
+// ... with one set of barriers; the word-tile stream runs on across item boundaries (all barrier phases are functions of a CTA-wide
+// running tile count), and the packed queries of the next item are loaded into registers while the current item runs.  What an item
+// boundary costs is the in-place expansion of the query tile instead of a CTA launch and a pipeline fill — which is what a word-range
+// shard with few tiles per item was paying.
+// partial[(split * kTcEpiGroups + quad) * nq + query] = (best key, second key) over the rows of that split that fall in the 64 columns of
+// each tile owned by lane quad position `quad` (columns 8 i + 2 quad + {0, 1}).
 __global__ void __launch_bounds__(kTcThreads, 1)
 knn2_tensor_kernel(const uint4 * __restrict__ word_img, int n_rows, int row_offset, const uint32_t * __restrict__ queries /* [nq][8] packed */, int nq,
                    uint2 * __restrict__ partial, int tiles_per_split, uint32_t neg32, int n_qtiles, int n_splits)
@@ -162,13 +152,9 @@ knn2_tensor_kernel(const uint4 * __restrict__ word_img, int n_rows, int row_offs
 	unsigned char * sB = smem + kTcABytes;
 	uint64_t * bars = reinterpret_cast<uint64_t *>(sB + kTcStages * kTcBBytes);
 	uint64_t * full = bars;                    // [kTcStages] word tile landed
-	uint64_t * empty = bars + kTcStages;       // [kTcStages] word tile consumed by the MMAs
-	uint64_t * tfull = bars + 2 * kTcStages;   // [2] accumulator stage complete
-	uint64_t * tempty = tfull + 2;             // [2] accumulator stage drained by the epilogue
-	uint64_t * afull = tempty + 2;             // [1] query tile of the item written (phase = item count of this CTA)
-	uint32_t * tmem_slot = reinterpret_cast<uint32_t *>(afull + 1);
+	uint64_t * empty = bars + kTcStages;       // [kTcStages] word tile consumed by both consumer warpgroups
 
-	const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+	const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
 	const int n_tiles_total = (n_rows + kTcBN - 1) / kTcBN;
 	const int n_items = n_qtiles * n_splits;
 	// tiles of an item (every role walks the same item sequence and keeps the same running tile count)
@@ -182,25 +168,15 @@ knn2_tensor_kernel(const uint4 * __restrict__ word_img, int n_rows, int row_offs
 		for (int s = 0; s < kTcStages; ++s)
 		{
 			mbar_init(&full[s], 1);
-			mbar_init(&empty[s], 1);
+			mbar_init(&empty[s], 2); // one arrival per consumer warpgroup
 		}
-		for (int s = 0; s < 2; ++s)
-		{
-			mbar_init(&tfull[s], 1);
-			mbar_init(&tempty[s], 4 * kTcEpiGroups); // one arrival per epilogue warp
-		}
-		mbar_init(afull, 4 * kTcEpiGroups); // the epilogue warps expand the query tile in place (one arrival per warp)
 		mbar_fence_init();
 	}
-	if (warp == 2) tc_alloc(tmem_slot, 512);
-	tc_fence_before();
 	__syncthreads();
-	tc_fence_after();
-	const uint32_t tmem_base = *tmem_slot;
 
-	if (warp == 0)
+	if (wg == 0)
 	{
-		if (lane == 0)
+		if (tid == 0)
 		{
 			int g = 0; // running tile count of this CTA
 			for (int item = blockIdx.x; item < n_items; item += gridDim.x)
@@ -218,131 +194,100 @@ knn2_tensor_kernel(const uint4 * __restrict__ word_img, int n_rows, int row_offs
 				}
 			}
 		}
+		return;
 	}
-	else if (warp == 1)
-	{
-		if (lane == 0)
-		{
-			constexpr uint32_t idesc = tc_idesc_i8(kTcBM, kTcBN);
-			const uint32_t a_base = smem_u32(sA);
-			int g = 0, k = 0;
-			for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++k)
-			{
-				int tile_begin;
-				const int n_tiles = item_tiles(item, tile_begin);
-				mbar_wait(afull, k & 1);
-				tc_fence_after();
-				for (int t = 0; t < n_tiles; ++t, ++g)
-				{
-					const int s = g % kTcStages, acc = g & 1;
-					if (g >= 2) mbar_wait(&tempty[acc], ((g >> 1) - 1) & 1);
-					mbar_wait(&full[s], (g / kTcStages) & 1);
-					tc_fence_after();
-					const uint32_t b_base = smem_u32(sB + s * kTcBBytes);
-					const uint32_t d_addr = tmem_base + static_cast<uint32_t>(acc * kTcBN);
+
+	// consumer warpgroup c: query rows [64 c, 64 c + 64) of the tile
+	const int c = wg - 1;
+	const int et = tid - 128 * wg;
+	const int quad = lane & 3;
+	const int r_lo = c * 64 + (et >> 5) * 16 + (lane >> 2); // tile rows of this thread's accumulators: r_lo and r_lo + 8
+	// The query half goes from its packed form (32 B per descriptor) straight into the swizzled +-1 byte image in shared memory:
+	// no expanded copy of the queries ever touches HBM.  One 16-byte chunk (16 descriptor bits) per thread and step.
+	uint4 * sA4 = reinterpret_cast<uint4 *>(sA);
+	constexpr int kItems = 64 * 16 / 128; // chunks per thread: same chunk column, rows 8 apart
+	const int chunk = et & 15, er0 = c * 64 + (et >> 4);
+	uint32_t w[kItems];
+	auto load_packed = [&](int qtile) { // all loads in flight before the first use: one memory round trip
 #pragma unroll
-					for (int ks = 0; ks < kTcK / 32; ++ks)
-					{
-						const uint32_t atom = ks >> 2, koff = (ks & 3) * 32;
-						const uint64_t ad = tc_smem_desc(a_base + atom * (kTcBM * 128) + koff);
-						const uint64_t bd = tc_smem_desc(b_base + atom * (kTcBN * 128) + koff);
-						tc_mma_i8(d_addr, ad, bd, idesc, ks > 0 ? 1u : 0u);
-					}
-					tc_commit(&empty[s]);  // smem stage reusable once these MMAs have read it
-					tc_commit(&tfull[acc]); // accumulator stage complete
-				}
-			}
+		for (int j = 0; j < kItems; ++j)
+		{
+			const int q = qtile * kTcBM + er0 + 8 * j;
+			w[j] = q < nq ? __ldg(queries + static_cast<size_t>(q) * 8 + (chunk >> 1)) : 0u;
 		}
-	}
-	else if (warp >= 4)
-	{
-		// The query tile goes from its packed form (32 B per descriptor) straight into the swizzled +-1 byte image in shared memory:
-		// no expanded copy of the queries ever touches HBM.  One 16-byte chunk (16 descriptor bits) per thread and step.
-		const int et = tid - 128;
-		uint4 * sA4 = reinterpret_cast<uint4 *>(sA);
-		constexpr int kItems = kTcBM * 16 / (128 * kTcEpiGroups); // chunks per thread: same chunk column, rows 32 apart
-		constexpr int kRowStep = 128 * kTcEpiGroups / 16;
-		const int chunk = et & 15, r0 = et >> 4;
-		uint32_t w[kItems];
-		auto load_packed = [&](int qtile) { // all loads in flight before the first use: one memory round trip
+	};
+	auto expand_tile = [&](int qtile) {
 #pragma unroll
-			for (int j = 0; j < kItems; ++j)
-			{
-				const int q = qtile * kTcBM + r0 + j * kRowStep;
-				w[j] = q < nq ? __ldg(queries + static_cast<size_t>(q) * 8 + (chunk >> 1)) : 0u;
-			}
-		};
-		auto expand_tile = [&](int qtile) {
-#pragma unroll
-			for (int j = 0; j < kItems; ++j)
-			{
-				const int r = r0 + j * kRowStep;
-				uint4 v = make_uint4(0, 0, 0, 0);
-				if (qtile * kTcBM + r < nq)
-				{
-					const uint32_t bits = (w[j] >> ((chunk & 1) * 16)) & 0xFFFFu;
-					v.x = expand4(bits & 15u);
-					v.y = expand4((bits >> 4) & 15u);
-					v.z = expand4((bits >> 8) & 15u);
-					v.w = expand4((bits >> 12) & 15u);
-				}
-				const int atom = chunk >> 3, c = chunk & 7;
-				sA4[atom * (kTcBM * 8) + r * 8 + (c ^ (r & 7))] = v;
-			}
-			asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); // generic-proxy writes -> visible to the tensor core's async proxy
-			__syncwarp();
-			if (lane == 0) mbar_arrive(afull);
-		};
-		const int quarter = warp & 3;                 // TMEM lanes [32*quarter, 32*quarter+32) (hardware: warp id % 4)
-		const int cg = (warp - 4) >> 2;               // column group
-		int g = 0;
-		if (static_cast<int>(blockIdx.x) < n_items)
+		for (int j = 0; j < kItems; ++j)
 		{
-			load_packed(static_cast<int>(blockIdx.x) % n_qtiles);
-			expand_tile(static_cast<int>(blockIdx.x) % n_qtiles);
+			const int r = er0 + 8 * j;
+			uint4 v = make_uint4(0, 0, 0, 0);
+			if (qtile * kTcBM + r < nq)
+			{
+				const uint32_t bits = (w[j] >> ((chunk & 1) * 16)) & 0xFFFFu;
+				v.x = expand4(bits & 15u);
+				v.y = expand4((bits >> 4) & 15u);
+				v.z = expand4((bits >> 8) & 15u);
+				v.w = expand4((bits >> 12) & 15u);
+			}
+			const int atom = chunk >> 3, cc = chunk & 7;
+			sA4[atom * (kTcBM * 8) + r * 8 + (cc ^ (r & 7))] = v;
 		}
-		for (int item = blockIdx.x; item < n_items; item += gridDim.x)
-		{
-			int tile_begin;
-			const int n_tiles = item_tiles(item, tile_begin);
-			const int qtile = item % n_qtiles, split = item / n_qtiles;
-			const int next = item + static_cast<int>(gridDim.x);
-			const bool has_next = next < n_items;
-			if (has_next) load_packed(next % n_qtiles); // in registers long before the boundary
-			const int qi = qtile * kTcBM + quarter * 32 + lane;
-			uint32_t k1 = kKeyNone, k2 = kKeyNone;
-			int thr = -100000;                            // accumulator value a candidate has to exceed to enter the top-2
-			for (int t = 0; t < n_tiles; ++t, ++g)
-			{
-				const int acc = g & 1;
-				mbar_wait(&tfull[acc], (g >> 1) & 1);
-				tc_fence_after();
-				// last tile of the item: every MMA that reads the query tile has completed -> write the next item's tile now, so that its
-				// first MMAs run while this accumulator is read out
-				if (t == n_tiles - 1 && has_next) expand_tile(next % n_qtiles);
-				const int row0 = (tile_begin + t) * kTcBN + cg * kTcEpiCols;
-				const int valid = n_rows - row0;              // columns of this group that are real words (may be <= 0)
-				const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + static_cast<uint32_t>(acc * kTcBN + cg * kTcEpiCols);
-				int v[kTcEpiCols];
+		asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); // generic-proxy writes -> visible to the tensor core's async proxy
+		wg_bar_sync(1 + c);
+	};
+	const uint32_t a_base = smem_u32(sA) + static_cast<uint32_t>(c * 64 * 128);
+	int acc[128];
 #pragma unroll
-				for (int c0 = 0; c0 < kTcEpiCols; c0 += 32) tc_ld32(taddr + c0, *reinterpret_cast<int(*)[32]>(&v[c0]));
-				tc_wait_ld();
-				// the accumulator stage is free as soon as the values are in registers
-				tc_fence_before();
-				__syncwarp();
-				if (lane == 0) mbar_arrive(&tempty[acc]);
-				if (valid >= kTcEpiCols)
+	for (int i = 0; i < 128; ++i) acc[i] = 0;
+	int g = 0;
+	if (static_cast<int>(blockIdx.x) < n_items) load_packed(static_cast<int>(blockIdx.x) % n_qtiles);
+	for (int item = blockIdx.x; item < n_items; item += gridDim.x)
+	{
+		int tile_begin;
+		const int n_tiles = item_tiles(item, tile_begin);
+		const int qtile = item % n_qtiles, split = item / n_qtiles;
+		wg_bar_sync(1 + c); // every warp of this warpgroup is past the MMAs that read the previous query tile
+		expand_tile(qtile);
+		const int next = item + static_cast<int>(gridDim.x);
+		if (next < n_items) load_packed(next % n_qtiles); // in registers long before the boundary
+		uint32_t k1[2] = {kKeyNone, kKeyNone}, k2[2] = {kKeyNone, kKeyNone};
+		int thr[2] = {-100000, -100000}; // accumulator value a candidate has to exceed to enter the top-2
+		for (int t = 0; t < n_tiles; ++t, ++g)
+		{
+			const int s = g % kTcStages;
+			mbar_wait(&full[s], (g / kTcStages) & 1);
+			__syncwarp(); // wgmma is .aligned: the warp issues it converged
+			const uint32_t b_base = smem_u32(sB + s * kTcBBytes);
+			wg_fence();
+#pragma unroll
+			for (int ks = 0; ks < kTcK / 32; ++ks)
+			{
+				const uint32_t atom = ks >> 2, koff = (ks & 3) * 32;
+				wg_mma_i8(acc, wg_smem_desc(a_base + atom * (kTcBM * 128) + koff), wg_smem_desc(b_base + atom * (kTcBN * 128) + koff), ks > 0 ? 1u : 0u);
+			}
+			wg_commit();
+			wg_wait_all();
+			// the stage is free as soon as the MMAs have completed: the accumulators are in registers
+			if (et == 0) mbar_arrive(&empty[s]);
+			const int row0 = (tile_begin + t) * kTcBN;
+			const int valid = n_rows - row0; // columns of this tile that are real words
+#pragma unroll
+			for (int h = 0; h < 2; ++h)
+			{
+				if (valid >= kTcBN)
 				{
-					// Branch-free top-2 over the 64 columns with 16-bit keys, two columns per register:
+					// Branch-free top-2 over this thread's 64 columns of the row with 16-bit keys, two columns per register:
 					//   key16 = distance * 64 + j = acc * (-32) + (8192 + j)   (distance = (256 - acc) / 2 <= 256, j < 32)
-					// The low half-word carries column j, the high half-word column j + 32; S = acc_hi * 65536 + acc_lo and
+					// The low half-word carries local column j, the high half-word local column j + 32; S = acc_hi * 65536 + acc_lo and
 					// K = S * (-32) + (8192 + j) * 65537 is that pair of keys exactly (every field stays in [0, 65536), so no
 					// carry crosses the halves).  Two IMADs (FMA pipe) and three VIMNMX.U16x2 (ALU pipe) per column pair.
 					uint32_t p1 = 0xFFFFFFFFu, p2 = 0xFFFFFFFFu;
 #pragma unroll
 					for (int j = 0; j < 32; ++j)
 					{
-						const uint32_t sp = static_cast<uint32_t>(v[j + 32]) * 65536u + static_cast<uint32_t>(v[j]);
+						const int lo = 4 * (j >> 1) + 2 * h + (j & 1); // local column j; local column j + 32 is lo + 64
+						const uint32_t sp = static_cast<uint32_t>(acc[lo + 64]) * 65536u + static_cast<uint32_t>(acc[lo]);
 						const uint32_t kp = sp * neg32 + static_cast<uint32_t>(8192 + j) * 65537u;
 						const uint32_t mx = __vmaxu2(p1, kp);
 						p1 = __vminu2(p1, kp);
@@ -350,43 +295,45 @@ knn2_tensor_kernel(const uint4 * __restrict__ word_img, int n_rows, int row_offs
 					}
 					// the four survivors (two per half) go into the running packed keys only if they can improve them
 					const uint32_t best16 = min(p1 & 0xFFFFu, p1 >> 16);
-					if (static_cast<int>(best16 >> 6) * 2 < kTcK - thr)
+					if (static_cast<int>(best16 >> 6) * 2 < kTcK - thr[h])
 					{
-						const uint32_t base = static_cast<uint32_t>(row_offset + row0);
-						const uint32_t c[4] = {p1 & 0xFFFFu, p2 & 0xFFFFu, p1 >> 16, p2 >> 16};
+						const uint32_t base = static_cast<uint32_t>(row_offset + row0 + 2 * quad);
+						const uint32_t cand[4] = {p1 & 0xFFFFu, p2 & 0xFFFFu, p1 >> 16, p2 >> 16};
 #pragma unroll
 						for (int u = 0; u < 4; ++u)
 						{
-							const uint32_t key = ((c[u] >> 6) << kKeyShift) + base + (c[u] & 63u) + (u >= 2 ? 32u : 0u);
-							top2_insert(k1, k2, key);
+							const uint32_t lc = (cand[u] & 63u) + (u >= 2 ? 32u : 0u); // local column -> tile column 8 (lc / 2) + 2 quad + lc % 2
+							const uint32_t key = ((cand[u] >> 6) << kKeyShift) + base + 8u * (lc >> 1) + (lc & 1u);
+							top2_insert(k1[h], k2[h], key);
 						}
-						thr = k2 == kKeyNone ? -100000 : kTcK - 2 * static_cast<int>(k2 >> kKeyShift);
+						thr[h] = k2[h] == kKeyNone ? -100000 : kTcK - 2 * static_cast<int>(k2[h] >> kKeyShift);
 					}
 				}
 				else if (valid > 0)
 				{
 					// last, partly filled tile: plain insertion of the real columns
 #pragma unroll
-					for (int j = 0; j < kTcEpiCols; ++j)
+					for (int lc = 0; lc < 64; ++lc)
 					{
-						if (j < valid)
+						const int col = 8 * (lc >> 1) + 2 * quad + (lc & 1);
+						if (col < valid)
 						{
-							const uint32_t key = (static_cast<uint32_t>(kTcK - v[j]) << (kKeyShift - 1)) + static_cast<uint32_t>(row_offset + row0 + j);
-							top2_insert(k1, k2, key);
+							const int a = acc[4 * (lc >> 1) + 2 * h + (lc & 1)];
+							const uint32_t key = (static_cast<uint32_t>(kTcK - a) << (kKeyShift - 1)) + static_cast<uint32_t>(row_offset + row0 + col);
+							top2_insert(k1[h], k2[h], key);
 						}
 					}
-					thr = k2 == kKeyNone ? -100000 : kTcK - 2 * static_cast<int>(k2 >> kKeyShift);
+					thr[h] = k2[h] == kKeyNone ? -100000 : kTcK - 2 * static_cast<int>(k2[h] >> kKeyShift);
 				}
-				__syncwarp();
 			}
-			if (n_tiles == 0 && has_next) expand_tile(next % n_qtiles); // (an item without tiles: nothing reads the query tile)
-			if (qi < nq) partial[(static_cast<size_t>(split) * kTcEpiGroups + cg) * nq + qi] = make_uint2(k1, k2);
+		}
+#pragma unroll
+		for (int h = 0; h < 2; ++h)
+		{
+			const int qi = qtile * kTcBM + r_lo + 8 * h;
+			if (qi < nq) partial[(static_cast<size_t>(split) * kTcEpiGroups + quad) * nq + qi] = make_uint2(k1[h], k2[h]);
 		}
 	}
-
-	tc_fence_before();
-	__syncthreads();
-	if (warp == 2) tc_dealloc(tmem_base, 512);
 }
 
 } // namespace lcd

@@ -1,5 +1,5 @@
 // nn_tensor_f32.cuh — exact squared-L2 2-NN of FLOAT descriptors (SURF-64 / SIFT-128 sized rows) with the distance matrix on the
-// 5th-generation tensor cores (sm_100a): BASELINE configs[3], "tensor cores ... if SURF/float descriptors make it a true dense GEMM".
+// Hopper tensor cores (sm_90a, wgmma): BASELINE configs[3], "tensor cores ... if SURF/float descriptors make it a true dense GEMM".
 //
 // Replaces, for CV_32F descriptors: FlannIndex::knnSearch(k = 2) on a LinearIndex (corelib/src/FlannIndex.cpp:701-745 ->
 // rtflann::L2<float>::operator(), rtflann/algorithms/dist.h:133-180, KNNSimpleResultSet, rtflann/util/result_set.h:151-172), whose
@@ -9,10 +9,10 @@
 //   1. operands rounded to fp16 (round to nearest, no scaling; |x| < 65504 is checked) in pre-tiled, 128-byte-swizzled K-major
 //      images: the word image is built once per dictionary change and CACHED (half the bytes of the fp32 rows: the 1M x 64
 //      vocabulary streams as 128 MB), the query image per call;
-//   2. knn2_tensor_f32_kernel: tcgen05.mma kind::f16 (M128 N256 K16, fp32 accumulators in TMEM).  The word image holds -2 w and one
+//   2. knn2_tensor_f32_kernel: wgmma .f32.f16.f16 (M64 N256 K16 per warpgroup, fp32 accumulators in registers).  The word image holds -2 w and one
 //      extra K-step holds |w|^2 (as an fp16 hi + lo pair against a constant column of the query image), so the accumulator IS
-//      v = |w|^2 - 2 q.w (= approximate squared distance minus |q|^2): the epilogue is a running minimum over the columns (one
-//      three-input FMNMX per two columns) and appends to the query's CANDIDATE LIST every row with v <= t2 + 2 eps, where t2 is the
+//      v = |w|^2 - 2 q.w (= approximate squared distance minus |q|^2): the epilogue is a running minimum over the columns
+//      and appends to the query's CANDIDATE LIST every row with v <= t2 + 2 eps, where t2 is the
 //      second-smallest v this thread has seen so far (initialised from a shared per-query bound);
 //   3. rerank_l2_kernel computes the exact rtflann-order distance of every candidate from the fp32 rows and keeps the best two by
 //      (distance, row) — the same packed 64-bit keys as the exact kernel of l2_path.cuh, consumed by the same resolve kernel;
@@ -36,11 +36,9 @@
 
 namespace lcd {
 
-constexpr int kTfBM = 128;          // queries per CTA tile (UMMA M)
-constexpr int kTfBN = 256;          // words per tile (UMMA N)
-constexpr int kTfEpiGroups = 4;     // column groups of a tile, one set of 4 epilogue warps each
-constexpr int kTfEpiCols = kTfBN / kTfEpiGroups;
-constexpr int kTfThreads = 128 + 128 * kTfEpiGroups;
+constexpr int kTfBM = 128;          // queries per CTA tile (two consumer warpgroups of M64)
+constexpr int kTfBN = 256;          // words per tile (wgmma N)
+constexpr int kTfThreads = 384;     // producer warpgroup + two consumer warpgroups
 constexpr int kTfCandCap = 96;      // candidate rows kept per query; more -> exact fallback for that query
 constexpr int kTfMinRows = 4096;    // below this the exact CUDA-core kernel is used
 constexpr int kTfPrepassTiles = 16; // rows [0, 4096): the bound-only pre-pass that initialises the per-query bound
@@ -173,33 +171,52 @@ __global__ void tf_query_init_kernel(const float * __restrict__ q, int nq, float
 	tau[i] = 0xFF800000u; // f2ord(+inf): no bound yet
 }
 
-// D[tmem] (+)= A[smem] * B[smem]^T, f16 x f16 -> f32, M128 x N256 x K16
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
+// D[regs] (+)= A[smem] * B[smem]^T, f16 x f16 -> f32, M64 x N256 x K16 over one warpgroup (same fragment layout as wg_mma_i8)
+__device__ __forceinline__ void wg_mma_f16(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
 {
 	asm volatile(
 		"{\n"
 		".reg .pred p;\n"
-		"setp.ne.b32 p, %4, 0;\n"
-		"tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-		"}\n" ::"r"(tmem_d),
-		"l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+		"setp.ne.b32 p, %130, 0;\n"
+		"wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+		"{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+		"%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+		"%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+		"%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+		"%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+		"%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+		"%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+		"%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+		"%128, %129, p, 1, 1, 0, 0;\n"
+		"}\n"
+		: "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+		  "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+		  "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+		  "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+		  "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+		  "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+		  "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+		  "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+		  "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+		  "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+		  "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+		  "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+		  "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+		  "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+		  "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+		  "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+		: "l"(adesc), "l"(bdesc), "r"(accumulate)
 		: "memory");
 }
-// instruction descriptor: f32 accumulator, f16 x f16, both K-major
-__device__ __forceinline__ constexpr uint32_t tc_idesc_f16(int m, int n)
-{
-	return (1u << 4) | (0u << 7) | (0u << 10) | (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
-}
 
-// shared-memory matrix descriptor of an UN-swizzled K-major operand slab of one K-step (16 halves): 8 x 16-byte core matrices, the two
-// k-chunks of a row group 128 B apart (leading byte offset), row groups 256 B apart (stride byte offset)
-__device__ __forceinline__ uint64_t tc_smem_desc_noswz(uint32_t saddr)
+// shared-memory matrix descriptor (GMMA) of an UN-swizzled K-major operand slab of one K-step (16 halves): 8 x 16-byte core matrices,
+// the two k-chunks of a row group 128 B apart (leading byte offset), row groups 256 B apart (stride byte offset)
+__device__ __forceinline__ uint64_t wg_smem_desc_noswz(uint32_t saddr)
 {
 	uint64_t d = 0;
 	d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);        // start address  [0,14)
 	d |= static_cast<uint64_t>(128 >> 4) << 16;                  // leading byte offset [16,30): next core matrix along K
 	d |= static_cast<uint64_t>(256 >> 4) << 32;                  // stride byte offset [32,46): next 8-row group
-	d |= static_cast<uint64_t>(1) << 46;                         // descriptor version (sm_100)
 	return d;                                                    // layout type 0: no swizzle
 }
 
@@ -221,9 +238,9 @@ struct TfArgs
 	int emit;                    // 0: bound-only pre-pass
 };
 
-// grid = (query tiles, splits).  Roles as in knn2_tensor_kernel (nn_tensor.cuh): warp 0 producer (bulk copies of the word tiles and
-// their augmentation slabs), warp 1 MMA issuer, warp 2 TMEM allocator, warps 4-19 epilogue (thread = one query = one TMEM lane,
-// column group (warp - 4) / 4).
+// grid = (query tiles, splits).  Roles as in knn2_tensor_kernel (nn_tensor.cuh): warpgroup 0 producer (bulk copies of the query tile and
+// of the word tiles with their augmentation slabs), warpgroups 1-2 consumers (wgmma M64 per warpgroup, accumulators in registers; a
+// thread holds two query rows of 64 columns each).
 template <int DIM>
 __global__ void __launch_bounds__(kTfThreads, 1)
 knn2_tensor_f32_kernel(const TfArgs a)
@@ -237,13 +254,10 @@ knn2_tensor_f32_kernel(const TfArgs a)
 	unsigned char * sB = smem + Cfg::a_bytes + Cfg::a_aug_bytes; // stages of (word tile, augmentation slab)
 	uint64_t * bars = reinterpret_cast<uint64_t *>(sB + kStages * kStageBytes);
 	uint64_t * full = bars;                     // [kStages] word tile landed
-	uint64_t * empty = full + kStages;          // [kStages] word tile consumed by the MMAs
-	uint64_t * tfull = empty + kStages;         // [2] accumulator stage complete
-	uint64_t * tempty = tfull + 2;              // [2] accumulator stage drained
-	uint64_t * afull = tempty + 2;              // [1] query tile landed
-	uint32_t * tmem_slot = reinterpret_cast<uint32_t *>(afull + 1);
+	uint64_t * empty = full + kStages;          // [kStages] word tile consumed by both consumer warpgroups
+	uint64_t * afull = empty + kStages;         // [1] query tile landed
 
-	const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+	const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
 	const int tile_begin = a.tile_begin + blockIdx.y * a.tiles_per_split;
 	const int tile_end = min(a.tile_end, tile_begin + a.tiles_per_split);
 	const int n_tiles = max(0, tile_end - tile_begin);
@@ -254,25 +268,16 @@ knn2_tensor_f32_kernel(const TfArgs a)
 		for (int s = 0; s < kStages; ++s)
 		{
 			mbar_init(&full[s], 1);
-			mbar_init(&empty[s], 1);
-		}
-		for (int s = 0; s < 2; ++s)
-		{
-			mbar_init(&tfull[s], 1);
-			mbar_init(&tempty[s], 4 * kTfEpiGroups);
+			mbar_init(&empty[s], 2);
 		}
 		mbar_init(afull, 1);
 		mbar_fence_init();
 	}
-	if (warp == 2) tc_alloc(tmem_slot, 512);
-	tc_fence_before();
 	__syncthreads();
-	tc_fence_after();
-	const uint32_t tmem_base = *tmem_slot;
 
-	if (warp == 0)
+	if (wg == 0)
 	{
-		if (lane == 0 && n_tiles > 0)
+		if (tid == 0 && n_tiles > 0)
 		{
 			mbar_arrive_expect_tx(afull, Cfg::a_bytes + Cfg::a_aug_bytes);
 			bulk_g2s(sA, reinterpret_cast<const unsigned char *>(a.query_img) + static_cast<size_t>(qtile) * Cfg::a_bytes, Cfg::a_bytes, afull);
@@ -291,104 +296,98 @@ knn2_tensor_f32_kernel(const TfArgs a)
 				         Cfg::b_aug_bytes, &full[s]);
 			}
 		}
+		return;
 	}
-	else if (warp == 1)
-	{
-		if (lane == 0 && n_tiles > 0)
-		{
-			constexpr uint32_t idesc = tc_idesc_f16(kTfBM, kTfBN);
-			const uint32_t a_base = smem_u32(sA);
-			const uint64_t a_aug = tc_smem_desc_noswz(a_base + Cfg::a_bytes);
-			mbar_wait(afull, 0);
-			for (int t = 0; t < n_tiles; ++t)
-			{
-				const int s = t % kStages, acc = t & 1;
-				if (t >= 2) mbar_wait(&tempty[acc], ((t >> 1) - 1) & 1);
-				mbar_wait(&full[s], (t / kStages) & 1);
-				tc_fence_after();
-				const uint32_t b_base = smem_u32(sB + s * kStageBytes);
-				const uint32_t d_addr = tmem_base + static_cast<uint32_t>(acc * kTfBN);
+
+	// consumer warpgroup c: query rows [64 c, 64 c + 64) of the tile
+	const int c = wg - 1;
+	const int et = tid - 128 * wg;
+	const int quad = lane & 3;
+	const int r_lo = c * 64 + (et >> 5) * 16 + (lane >> 2); // tile rows of this thread: r_lo and r_lo + 8
+	int qi[2];
+	bool live[2];
+	float margin[2], t1[2], t2[2];
 #pragma unroll
-				for (int ks = 0; ks < DIM / 16; ++ks)
-				{
-					const uint32_t atom = ks >> 2, koff = (ks & 3) * 32; // 16 halves = 32 bytes per K step, 4 steps per 128-byte atom
-					const uint64_t ad = tc_smem_desc(a_base + atom * (kTfBM * 128) + koff);
-					const uint64_t bd = tc_smem_desc(b_base + atom * (kTfBN * 128) + koff);
-					tc_mma_f16(d_addr, ad, bd, idesc, ks > 0 ? 1u : 0u);
-				}
-				// the augmentation K-step: + kTfAugScale * (hi + lo) = + |w|^2
-				tc_mma_f16(d_addr, a_aug, tc_smem_desc_noswz(b_base + Cfg::b_bytes), idesc, 1u);
-				tc_commit(&empty[s]);
-				tc_commit(&tfull[acc]);
-			}
-		}
-	}
-	else if (warp >= 4)
+	for (int h = 0; h < 2; ++h)
 	{
-		const int quarter = warp & 3;
-		const int cg = (warp - 4) >> 2;
-		const int qi = qtile * kTfBM + quarter * 32 + lane;
-		const bool live = qi < a.nq;
-		float margin = 0.0f, t1 = INFINITY, t2 = INFINITY;
-		if (live)
+		qi[h] = qtile * kTfBM + r_lo + 8 * h;
+		live[h] = qi[h] < a.nq;
+		margin[h] = 0.0f;
+		t1[h] = INFINITY;
+		t2[h] = INFINITY;
+		if (live[h])
 		{
-			const float q2 = a.qn[qi], w2 = __uint_as_float(*a.wmax2_bits);
+			const float q2 = a.qn[qi[h]], w2 = __uint_as_float(*a.wmax2_bits);
 			const float eps = 1.02f * 0.001953125f * sqrtf(q2) * sqrtf(w2) + 3.0517578125e-05f * (q2 + w2) + 4.0e-6f;
-			margin = 2.0f * eps;
-			t2 = ord2f(a.tau[qi]);
+			margin[h] = 2.0f * eps;
+			t2[h] = ord2f(a.tau[qi[h]]);
 		}
-		const int emit = a.emit;
-		for (int t = 0; t < n_tiles; ++t)
-		{
-			const int acc = t & 1;
-			mbar_wait(&tfull[acc], (t >> 1) & 1);
-			tc_fence_after();
-			const int row0 = (tile_begin + t) * kTfBN + cg * kTfEpiCols;
-			const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + static_cast<uint32_t>(acc * kTfBN + cg * kTfEpiCols);
-			int v[kTfEpiCols];
+	}
+	if (n_tiles == 0) return;
+	const int emit = a.emit;
+	const uint32_t a_base = smem_u32(sA) + static_cast<uint32_t>(c * 64 * 128);
+	const uint64_t a_aug = wg_smem_desc_noswz(smem_u32(sA + Cfg::a_bytes) + static_cast<uint32_t>(c * 8 * 256));
+	float acc[128];
 #pragma unroll
-			for (int c0 = 0; c0 < kTfEpiCols; c0 += 32) tc_ld32(taddr + c0, *reinterpret_cast<int(*)[32]>(&v[c0]));
-			tc_wait_ld();
-			// the accumulator stage is free as soon as the values are in registers
-			tc_fence_before();
-			__syncwarp();
-			if (lane == 0) mbar_arrive(&tempty[acc]);
+	for (int i = 0; i < 128; ++i) acc[i] = 0.0f;
+	mbar_wait(afull, 0);
+	for (int t = 0; t < n_tiles; ++t)
+	{
+		const int s = t % kStages;
+		mbar_wait(&full[s], (t / kStages) & 1);
+		__syncwarp(); // wgmma is .aligned: the warp issues it converged
+		const uint32_t b_base = smem_u32(sB + s * kStageBytes);
+		wg_fence();
+#pragma unroll
+		for (int ks = 0; ks < DIM / 16; ++ks)
+		{
+			const uint32_t atom = ks >> 2, koff = (ks & 3) * 32; // 16 halves = 32 bytes per K step, 4 steps per 128-byte atom
+			wg_mma_f16(acc, wg_smem_desc(a_base + atom * (kTfBM * 128) + koff), wg_smem_desc(b_base + atom * (kTfBN * 128) + koff), ks > 0 ? 1u : 0u);
+		}
+		// the augmentation K-step: + kTfAugScale * (hi + lo) = + |w|^2
+		wg_mma_f16(acc, a_aug, wg_smem_desc_noswz(b_base + Cfg::b_bytes), 1u);
+		wg_commit();
+		wg_wait_all();
+		// the stage is free as soon as the MMAs have completed: the accumulators are in registers
+		if (et == 0) mbar_arrive(&empty[s]);
+		const int row0 = (tile_begin + t) * kTfBN;
+#pragma unroll
+		for (int h = 0; h < 2; ++h)
+		{
 			float m = INFINITY;
 #pragma unroll
-			for (int j = 0; j < kTfEpiCols; j += 2) m = fminf(m, fminf(__int_as_float(v[j]), __int_as_float(v[j + 1])));
-			if (live && m <= t2 + margin)
+			for (int i = 0; i < 32; ++i) m = fminf(m, fminf(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]));
+			if (live[h] && m <= t2[h] + margin[h])
 			{
 				// rare: some column of this tile may belong to the two nearest rows
 #pragma unroll
-				for (int j = 0; j < kTfEpiCols; ++j)
+				for (int lc = 0; lc < 64; ++lc)
 				{
-					const float x = __int_as_float(v[j]);
+					const float x = acc[4 * (lc >> 1) + 2 * h + (lc & 1)];
+					const int row = row0 + 8 * (lc >> 1) + 2 * quad + (lc & 1);
 					// rows past n_rows of the cached image are words that are not searchable in this call (not indexed yet)
-					if (x <= t2 + margin && x < INFINITY && row0 + j < a.n_rows)
+					if (x <= t2[h] + margin[h] && x < INFINITY && row < a.n_rows)
 					{
 						if (emit)
 						{
-							const int pos = atomicAdd(&a.cand_count[qi], 1);
-							if (pos < kTfCandCap) a.cand[static_cast<size_t>(qi) * kTfCandCap + pos] = static_cast<uint32_t>(row0 + j);
+							const int pos = atomicAdd(&a.cand_count[qi[h]], 1);
+							if (pos < kTfCandCap) a.cand[static_cast<size_t>(qi[h]) * kTfCandCap + pos] = static_cast<uint32_t>(row);
 						}
 						// t2 only ever tightens: it starts as the shared bound while t1 is still unknown (+inf)
-						if (x < t1)
+						if (x < t1[h])
 						{
-							t2 = fminf(t2, t1);
-							t1 = x;
+							t2[h] = fminf(t2[h], t1[h]);
+							t1[h] = x;
 						}
-						else if (x < t2) t2 = x;
+						else if (x < t2[h]) t2[h] = x;
 					}
 				}
 			}
-			__syncwarp();
 		}
-		if (live && t2 < INFINITY) atomicMin(&a.tau[qi], f2ord(t2));
 	}
-
-	tc_fence_before();
-	__syncthreads();
-	if (warp == 2) tc_dealloc(tmem_base, 512);
+#pragma unroll
+	for (int h = 0; h < 2; ++h)
+		if (live[h] && t2[h] < INFINITY) atomicMin(&a.tau[qi[h]], f2ord(t2[h]));
 }
 
 // ---- exact re-rank of the candidate lists: one warp per query -----------------------------------------------------------------

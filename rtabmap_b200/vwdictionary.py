@@ -32,7 +32,7 @@ def _to_bool(v: str) -> bool:
 
 class VWDictionaryB200:
     """Drop-in for VWDictionary: incremental / fixed visual vocabulary with exact k=2 NN + NNDR
-    quantisation and the word -> signature inverted index, resident on one B200."""
+    quantisation and the word -> signature inverted index, resident on one H100."""
 
     def __init__(self, parameters: Optional[Dict[str, str]] = None, device: int = 0, desc_type: int = LCD_DESC_U8,
                  desc_dim: int = 32, **engine_kwargs):

@@ -37,7 +37,7 @@ def test_header_is_c99_and_every_symbol_links(tmp_path):
     out = subprocess.run([str(exe)], capture_output=True, text=True, timeout=120)
     assert out.returncode == 0, out.stderr
     n, abi, arch, created, *msg = out.stdout.split(" ", 4)
-    assert int(n) == len(names) and int(abi) >= 1 and arch == "sm_100a"
+    assert int(n) == len(names) and int(abi) >= 1 and arch == "sm_90a"
     import torch
     if not torch.cuda.is_available():
         # no device here: creation must fail with an explanation, never hand back a CPU engine

@@ -27,7 +27,7 @@ def test_library_exports_every_declared_symbol():
     for s in declared_symbols():
         assert hasattr(lib, s), f"liblcd_b200.so does not export {s}"
     assert lib.lcd_abi_version() == 2
-    assert lib.lcd_build_arch() == b"sm_100a"
+    assert lib.lcd_build_arch() == b"sm_90a"
 
 
 def test_ctypes_table_matches_header():

@@ -14,6 +14,7 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+from golden_util import ref_knn2
 from oracle import feature2d_py as f2d
 from oracle import oracle_py as orc
 from rtabmap_b200 import Engine, synth
@@ -204,10 +205,10 @@ def test_c3_mapping_stream_720p_grows_past_262144_words():
     assert eng.indexed_size() > 262144
     # the re-observed frames found words created by this stream (ids above the initial vocabulary)
     assert (g > W0).sum() > 100
-    # exact 2-NN over the grown dictionary against the reference's own compiled rtflann
+    # exact 2-NN over the grown dictionary against the reference's own rtflann (stored answers)
     q = synth.flip_bits(np.concatenate([vocab[rng.integers(0, W0, 100)], feats[2][1][:100]]), 0.05, rng)
     gi, gv = eng.get_indexed()
-    r_idx, r_dist = orc.ref_knn2(gv, q)
+    r_idx, r_dist = ref_knn2(gv, q)
     i1, d1, i2, d2 = eng.knn2(q)
     assert np.array_equal(i1, gi[r_idx[:, 0]]) and np.array_equal(i2, gi[r_idx[:, 1]])
     assert np.array_equal(d1, r_dist[:, 0].astype(np.float32)) and np.array_equal(d2, r_dist[:, 1].astype(np.float32))
@@ -216,7 +217,7 @@ def test_c3_mapping_stream_720p_grows_past_262144_words():
 # --------------------------------------------------------------------------------------- C4 ---
 def test_c4_float_quantiser_over_a_million_rows():
     """configs[3] size: SURF-like 64-D float descriptors against 1 100 000 dictionary rows (beyond 2^20): exact squared-L2 2-NN ids and
-    distances bit for bit against the reference's compiled rtflann (oracle/_ref), then the NNDR / new-word pass against the oracle."""
+    distances bit for bit against the reference's rtflann (tests/golden/ref_knn2.npz), then the NNDR / new-word pass against the oracle."""
     W = 1_100_000
     vocab = synth.make_float_vocabulary(W, 64, 21)
     ids = np.arange(1, W + 1, dtype=np.int32)
@@ -233,7 +234,7 @@ def test_c4_float_quantiser_over_a_million_rows():
     q[-8:-4] = q[-16:-12] + np.float32(1e-3)            # near copies of new descriptors inside the frame
     q = np.ascontiguousarray(q, np.float32)
     i1, d1, i2, d2 = eng.knn2(q)
-    r_idx, r_dist = orc.ref_knn2(vocab, q)
+    r_idx, r_dist = ref_knn2(vocab, q)
     assert np.array_equal(i1, ids[r_idx[:, 0]]) and np.array_equal(i2, ids[r_idx[:, 1]])
     assert np.array_equal(d1, r_dist[:, 0]) and np.array_equal(d2, r_dist[:, 1])
     assert (i1[:8] == ids[src[:8]]).all()

@@ -113,7 +113,7 @@ def test_float_engine_rejects_binary_only_calls():
 # ---------------------------------------------------------------- tensor-core filter + exact re-rank (nn_tensor_f32.cuh) ----------
 @pytest.mark.parametrize("dim,n_words", [(64, 4096), (64, 20000), (64, 70001), (128, 9000)])
 def test_tensor_filter_is_bit_identical_to_the_exact_kernel(dim, n_words):
-    """Dictionaries of >= 4096 float rows go through the tcgen05 fp16 GEMM filter + exact re-rank; ids and fp32 distances must equal
+    """Dictionaries of >= 4096 float rows go through the wgmma fp16 GEMM filter + exact re-rank; ids and fp32 distances must equal
     the exact CUDA-core scan (and the rtflann-pinned oracle) bit for bit."""
     eng, o, vocab, ids = pair(n_words, dim, seed=3 * dim + n_words)
     rng = np.random.default_rng(17)

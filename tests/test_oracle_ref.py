@@ -1,12 +1,11 @@
-"""Pin the restated linear 2-NN scan (oracle/oracle.cpp) against the REFERENCE'S OWN rtflann,
-compiled from /root/reference by oracle/Makefile into oracle/_ref/libref_flann.so.
+"""Pin the restated linear 2-NN scan (oracle/oracle.cpp) against the REFERENCE'S OWN rtflann (its answers stored in
+tests/golden/ref_knn2.npz, checked live where oracle/Makefile has compiled it into oracle/_ref/libref_flann.so).
 Covers Hamming (ORB) and squared-L2 (SURF) incl. exact ties and fewer than two rows."""
 import numpy as np
 import pytest
 
+from golden_util import ref_knn2
 from oracle import oracle_py as orc
-
-pytestmark = pytest.mark.skipif(orc.ref_lib() is None, reason="oracle/_ref not built (no /root/reference)")
 
 
 @pytest.mark.parametrize("rows,dim", [(1, 32), (2, 32), (3, 32), (777, 32), (4096, 32), (1000, 16), (500, 64)])
@@ -20,7 +19,7 @@ def test_hamming_matches_rtflann(rows, dim):
         q[0] = data[1]
         q[1] = data[rows - 1]
         q[2] = np.bitwise_xor(data[3], 1)
-    i_ref, d_ref = orc.ref_knn2(data, q)
+    i_ref, d_ref = ref_knn2(data, q)
     i_orc, d_orc = orc.knn2_raw(data, q)
     assert np.array_equal(i_ref, i_orc)
     valid = i_ref >= 0
@@ -36,7 +35,7 @@ def test_l2_matches_rtflann_bit_exact(rows, dim):
     if rows > 10:
         data[7] = data[2]
         q[0] = data[2]
-    i_ref, d_ref = orc.ref_knn2(data, q)
+    i_ref, d_ref = ref_knn2(data, q)
     i_orc, d_orc = orc.knn2_raw(data, q)
     assert np.array_equal(i_ref, i_orc)
     # same float summation order as rtflann::L2 (dist.h:158-166): identical bits
@@ -46,14 +45,14 @@ def test_l2_matches_rtflann_bit_exact(rows, dim):
 # ---- the quantiser loop, replayed on the reference's own primitives ---------------------------------------------------
 def _replay_add_new_words(index_ids, index_desc, frame, nndr, last_id, incremental=True, cmp_new=True):
     """VWDictionary::addNewWords "Process results" loop (VWDictionary.cpp:1088-1219) written a second time, independently of
-    oracle/oracle.cpp, on the primitives the reference itself calls: its own rtflann LinearIndex (compiled into oracle/_ref)
+    oracle/oracle.cpp, on the primitives the reference itself calls: its own rtflann LinearIndex (stored answers)
     for the index search and cv::BFMatcher::knnMatch (OpenCV, the installed cv2) for the words created by the same frame.
     fullResults is a std::multimap<float,int>: a stable sort by distance of the insertion sequence."""
     import cv2
 
     binary = frame.dtype == np.uint8
     bf = cv2.BFMatcher(cv2.NORM_HAMMING if binary else cv2.NORM_L2SQR)
-    idx_all, dist_all = (orc.ref_knn2(index_desc, frame) if len(index_desc) else (None, None))
+    idx_all, dist_all = (ref_knn2(index_desc, frame) if len(index_desc) else (None, None))
     new_desc, new_ids, out = [], [], []
     for i in range(len(frame)):
         full = []
@@ -149,7 +148,7 @@ def test_find_nn_against_reference_primitives(kind):
     o.update()
     o.add_words(pend_ids, pend)            # not indexed: no update()
     o.last_word_id = 2060
-    idx, dist = orc.ref_knn2(vocab, q)
+    idx, dist = ref_knn2(vocab, q)
     mni = bf.knnMatch(q, pend, k=2)
     want = np.zeros(len(q), np.int32)
     for i in range(len(q)):

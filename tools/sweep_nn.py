@@ -1,4 +1,4 @@
-"""NN-kernel tuning sweep on a real B200 (run under gpurun): times the dictionary-NN kernel and
+"""NN-kernel tuning sweep on a real H100 : times the dictionary-NN kernel and
 the fused quantise->score batch for the knob combinations given by env LCD_NN_* values."""
 import itertools
 import json

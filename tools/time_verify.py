@@ -1,4 +1,4 @@
-"""Time the verification kernels on a B200 (run under gpurun)."""
+"""Time the verification kernels on a H100 ."""
 import json
 import sys
 import time

@@ -1,5 +1,5 @@
 // tma_probe.cu — diagnostic: which way of handing a CUtensorMap to cp.async.bulk.tensor works on this driver / GPU.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -o gpurun_out/tma_probe tools/tma_probe.cu && gpurun_out/tma_probe
+//   nvcc -gencode arch=compute_90a,code=sm_90a -o /tmp/tma_probe tools/tma_probe.cu && /tmp/tma_probe
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cstdio>
