@@ -433,15 +433,19 @@ int lcd_verify_top_dev(lcd_engine * e, const void * d_queries, const float * d_u
 /* ---- word-range sharding across GPUs (SURVEY.md §8(e)) ---------------------------
  * Each rank owns the words whose row (in ascending id order) falls in its range; rows
  * are numbered globally: set the global row offset of this shard so that packed top-2
- * keys (dist<<22 | global_row) from different ranks merge with the reference's
- * tie-break (lowest row = lowest id). */
+ * keys from different ranks merge with the reference's tie-break (lowest row = lowest id).
+ * The key width is a property of the engine:
+ *   binary (LCD_DESC_U8):  2 x u32 per query, (dist << 22) | global_row, 0xFFFFFFFF = none;
+ *   float (LCD_DESC_F32):  2 x u64 per query, (float bits of the squared distance << 32) | global_row,
+ *                          0xFFFFFFFFFFFFFFFF = none (4 u32 words per query behind the uint32_t pointers).
+ * Unsigned order of a key is (distance, lowest global row) order in both layouts. */
 int lcd_shard_set_row_offset(lcd_engine * e, int global_row_offset);
-/* stage 1: local top-2 keys of every query over this rank's rows -> d_keys_out[2*nq] u32
- * (0xFFFFFFFF = none).  All-gather these across ranks, then call stage 2 on every rank. */
+/* stage 1: local top-2 keys of every query over this rank's rows -> d_keys_out (2*nq u32 for
+ * binary engines, 2*nq u64 for float engines).  All-gather these across ranks, then call stage 2 on every rank. */
 int lcd_shard_knn2_keys_dev(lcd_engine * e, const void * d_queries, int nq, uint32_t * d_keys_out,
                             void * stream);
 /* stage 2, sharded by FRAME (what scales): every rank resolves only its own frames [frame0, frame0+n_frames) of the job's
- * n_frames_total — merge of the G gathered key sets [G][2 * n_frames_total * nq] + NNDR / new-word pass — and writes their
+ * n_frames_total — merge of the G gathered key sets [G][n_frames_total * nq] key pairs + NNDR / new-word pass — and writes their
  * word ids (d_word_ids_out[n_frames*nq], 0 in padding rows; d_n_per_frame[n_frames_total] valid descriptors per frame or NULL).
  * All-gather the word ids, then lcd_shard_score_ids_dev on every rank accumulates this rank's share (its word range) of the
  * TF-IDF scores of ALL frames from the ids (uUniqueKeys + "id > 0" filter of Memory::computeLikelihood, Memory.cpp:2238-2256)
@@ -452,7 +456,7 @@ int lcd_shard_resolve_frames_dev(lcd_engine * e, const void * d_queries_all, int
                                  const int * d_n_per_frame, int * d_word_ids_out, void * stream);
 int lcd_shard_score_ids_dev(lcd_engine * e, const int * d_word_ids_all, int n_frames, int nq_per_frame,
                             const int * d_sig_ids, int ns, int n_total, long long * d_scores_out, void * stream);
-/* stage 2: merge G gathered key sets [G][2*nq], run the replicated NNDR / new-word pass,
+/* stage 2: merge G gathered key sets [G][nq] key pairs, run the replicated NNDR / new-word pass,
  * and accumulate this rank's share of the TF-IDF scores into d_scores_out[n_frames*ns]
  * (fixed-point int64, exact and order-independent; all-reduce(sum) them, then call
  * lcd_shard_finalize_dev).  d_row_ids: global row -> word id table [total_rows]. */
@@ -487,6 +491,18 @@ int lcd_shard_process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d
                                  int depth_type, const lcd_orb_params * params, int incremental, float nndr, int new_words_compared_together,
                                  const int * d_sig_ids, int ns, int n_total, const int * d_row_ids_global, int last_word_id,
                                  const lcd_verify_params * vp, int * d_word_ids_out, float * d_likelihood_out, void * stream);
+/* The same step on descriptors the caller already has on the device, for binary and float engines alike: lcd_localize_batch_dev
+ * semantics (quantise + score of n_frames independent LOCAL frames of nq_per_frame descriptors each, no mutation) with the dictionary and
+ * the inverted index sharded by word range over the engine's communicator.  All-gather of the descriptors, top-2 keys over the local
+ * word range, all-to-all of the keys (2 x u32 or 2 x u64 per query, see above), merge + NNDR / new-word pass of the local frames,
+ * all-gather of their word ids, TF-IDF of all frames over the local word range, reduce-scatter of the exact fixed-point sums, likelihood
+ * of the local frames.  No verification.  Every rank must call it with the same n_frames and nq_per_frame.  d_word_ids_out[n_frames *
+ * nq_per_frame] (may be NULL), d_likelihood_out[n_frames * ns]: equal to lcd_localize_batch_dev on one unsharded engine (word ids bit
+ * for bit, likelihood from the same exact sums). */
+int lcd_shard_localize_batch_dev(lcd_engine * e, const void * d_queries, int n_frames, int nq_per_frame,
+                                 int incremental, float nndr, int new_words_compared_together,
+                                 const int * d_sig_ids, int ns, int n_total, const int * d_row_ids_global, int last_word_id,
+                                 int * d_word_ids_out, float * d_likelihood_out, void * stream);
 
 /* ---- measurement hooks ---------------------------------------------------------------
  * Optional per-kernel timing with CUDA events recorded on the launching stream around

@@ -174,6 +174,7 @@ SIGNATURES = {
     "lcd_shard_comm_adopt": (_I, [_P, _P, _I, _I]),
     "lcd_shard_comm_destroy": (_I, [_P]),
     "lcd_shard_process_frames_dev": (_I, [_P, _I, _P, _I, _I, _I, _P, _I, _P, _I, _F, _I, _P, _I, _I, _P, _I, _P, _P, _P, _P]),
+    "lcd_shard_localize_batch_dev": (_I, [_P, _P, _I, _I, _I, _F, _I, _P, _I, _I, _P, _I, _P, _P, _P]),
     "lcd_profile_enable": (_I, [_P, _I]),
     "lcd_profile_read": (_I, [_P, _I, _P, _P]),
     "lcd_profile_reset": (_I, [_P]),
@@ -796,15 +797,27 @@ class Engine:
                                                             C.c_void_p(d_row_ids_global), int(last_word_id), C.byref(vp) if vp is not None else None,
                                                             C.c_void_p(d_words_out or None), C.c_void_p(d_like_out), C.c_void_p(stream or None)))
 
+    def shard_localize_batch_dev(self, d_queries: int, n_frames: int, nq: int, d_sig_ids: int, ns: int, n_total: int, d_row_ids_global: int,
+                                 last_word_id: int, d_words_out: int, d_like_out: int, incremental: bool = True, nndr: float = 0.8,
+                                 cmp_new: bool = True, stream: int = 0):
+        """localize_batch_dev of this rank's n_frames frames with the dictionary sharded by word range over the engine's communicator
+        (binary or float engines); every rank passes the same n_frames and nq."""
+        self._check(self._lib.lcd_shard_localize_batch_dev(self._h, C.c_void_p(d_queries), n_frames, nq, int(incremental), float(nndr), int(cmp_new),
+                                                            C.c_void_p(d_sig_ids), ns, int(n_total), C.c_void_p(d_row_ids_global), int(last_word_id),
+                                                            C.c_void_p(d_words_out or None), C.c_void_p(d_like_out), C.c_void_p(stream or None)))
+
     def shard_set_row_offset(self, off: int):
         self._check(self._lib.lcd_shard_set_row_offset(self._h, int(off)))
 
     def shard_knn2_keys_dev(self, d_queries: int, nq: int, d_keys_out: int, stream: int = 0):
+        """d_keys_out: 2 * nq uint32 keys for a binary engine, 2 * nq uint64 keys (4 * nq uint32 words) for a float engine."""
         self._check(self._lib.lcd_shard_knn2_keys_dev(self._h, C.c_void_p(d_queries), nq, C.c_void_p(d_keys_out), C.c_void_p(stream or None)))
 
     def shard_resolve_score_dev(self, d_queries: int, n_frames: int, nq: int, d_keys_gathered: int, n_ranks: int, d_row_ids: int,
                                 total_rows: int, last_word_id: int, d_sig_ids: int, ns: int, n_total: int, d_words_out: int,
                                 d_scores_out: int, incremental: bool = True, nndr: float = 0.8, cmp_new: bool = True, stream: int = 0):
+        """d_keys_gathered: n_ranks key sets of shard_knn2_keys_dev over n_frames * nq queries (uint32 pairs for binary engines, uint64
+        pairs for float engines)."""
         self._check(self._lib.lcd_shard_resolve_score_dev(
             self._h, C.c_void_p(d_queries), n_frames, nq, C.c_void_p(d_keys_gathered), n_ranks, C.c_void_p(d_row_ids), total_rows,
             last_word_id, int(incremental), float(nndr), int(cmp_new), C.c_void_p(d_sig_ids), ns, int(n_total),
@@ -813,6 +826,8 @@ class Engine:
     def shard_resolve_frames_dev(self, d_queries_all: int, frame0: int, n_frames: int, n_frames_total: int, nq: int, d_keys_gathered: int,
                                  n_ranks: int, d_row_ids: int, last_word_id: int, d_n_per_frame: int, d_words_out: int, incremental: bool = True,
                                  nndr: float = 0.8, cmp_new: bool = True, stream: int = 0):
+        """d_keys_gathered: n_ranks key sets of shard_knn2_keys_dev over n_frames_total * nq queries (uint32 pairs for binary engines,
+        uint64 pairs for float engines)."""
         self._check(self._lib.lcd_shard_resolve_frames_dev(
             self._h, C.c_void_p(d_queries_all), frame0, n_frames, n_frames_total, nq, C.c_void_p(d_keys_gathered), n_ranks, C.c_void_p(d_row_ids),
             last_word_id, int(incremental), float(nndr), int(cmp_new), C.c_void_p(d_n_per_frame or None), C.c_void_p(d_words_out),

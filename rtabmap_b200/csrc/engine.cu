@@ -32,6 +32,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <mutex>
 #include <string>
 #include <unordered_map>
@@ -797,8 +798,8 @@ int launch_resolve(lcd_engine * e, const ResolveArgs & a, int n_frames, cudaStre
 			else LCD_CUDA(e, cudaFuncSetAttribute(resolve_l2_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem32)));
 		}
 		prof_mark(e, LCD_PROF_RESOLVE, s);
-		if (e->nw == 64) resolve_l2_kernel<64><<<n_frames, kL2ResolveThreads, smem32, s>>>(a, e->d_partial64.p);
-		else resolve_l2_kernel<128><<<n_frames, kL2ResolveThreads, smem32, s>>>(a, e->d_partial64.p);
+		if (e->nw == 64) resolve_l2_kernel<64><<<n_frames, kL2ResolveThreads, smem32, s>>>(a, a.partial64);
+		else resolve_l2_kernel<128><<<n_frames, kL2ResolveThreads, smem32, s>>>(a, a.partial64);
 		prof_mark(e, LCD_PROF_RESOLVE, s);
 		LCD_CHECK_LAUNCH(e);
 		return LCD_OK;
@@ -1031,6 +1032,7 @@ int localize_dev(lcd_engine * e, const uint32_t * d_q, int n_frames, int nq, int
 	a.nq_frame = d_nq_frame;
 	a.nq_total = nq_total;
 	a.partial = e->d_partial.p;
+	a.partial64 = e->d_partial64.p;
 	a.n_chunks = n_chunks;
 	a.row_ids = e->row_ids.p;
 	a.incremental = incremental;
@@ -1522,6 +1524,7 @@ static int quantize_dev(lcd_engine * e, const uint32_t * d_q, int rows, int n_va
 	a.nq_total = rows;
 	a.nq_frame = n_valid < 0 ? d_n_valid : nullptr;
 	a.partial = e->d_partial.p;
+	a.partial64 = e->d_partial64.p;
 	a.n_chunks = n_chunks;
 	a.row_ids = e->row_ids.p;
 	a.incremental = incremental;
@@ -1599,6 +1602,7 @@ int lcd_dict_find_nn(lcd_engine * e, const void * queries, int nq, int increment
 	a.nq = nq;
 	a.nq_total = nq;
 	a.partial = e->d_partial.p;
+	a.partial64 = e->d_partial64.p;
 	a.n_chunks = n_chunks;
 	a.row_ids = e->row_ids.p;
 	a.incremental = incremental;
@@ -3362,18 +3366,35 @@ int lcd_shard_set_row_offset(lcd_engine * e, int global_row_offset)
 	return LCD_OK;
 }
 
+// Sharded key sets: per query two u32 keys (dist << 22 | global row) for binary descriptors, two u64 keys (float bits of the distance
+// << 32 | global row) for float descriptors; all-ones = none.  Buffers stay typed uint32_t: a float key pair is four words.
+static int shard_key_words(const lcd_engine * e) { return e->f32 ? 4 : 2; }
+
+// merge of the n_chunks partial top-2 sets run_knn left behind into one key pair per query
+static int shard_merge_keys(lcd_engine * e, int n_chunks, int nq, uint32_t * d_keys_out, cudaStream_t s)
+{
+	if (e->f32) knn2_merge64_kernel<<<(nq + 255) / 256, 256, 0, s>>>(e->d_partial64.p, n_chunks, nq, reinterpret_cast<ulonglong2 *>(d_keys_out));
+	else knn2_merge_kernel<<<(nq + 255) / 256, 256, 0, s>>>(e->d_partial.p, n_chunks, nq, d_keys_out);
+	LCD_CHECK_LAUNCH(e);
+	return LCD_OK;
+}
+
+// the resolve reads its keys from `keys` (gathered key sets), starting at query `q0`
+static void shard_set_keys(const lcd_engine * e, ResolveArgs & a, const uint32_t * keys, size_t q0)
+{
+	if (e->f32) a.partial64 = reinterpret_cast<const ulonglong2 *>(keys) + q0;
+	else a.partial = reinterpret_cast<const uint2 *>(keys) + q0;
+}
+
 int lcd_shard_knn2_keys_dev(lcd_engine * e, const void * d_queries, int nq, uint32_t * d_keys_out, void * stream)
 {
 	if (!e) return LCD_ERR_INVALID;
-	LCD_TRY(require_binary(e, "lcd_shard_knn2_keys_dev"));
 	LCD_TRY(set_device(e));
 	if (!d_queries || nq <= 0 || !d_keys_out) LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
 	int n_chunks = 0;
 	LCD_TRY(run_knn(e, static_cast<const uint32_t *>(d_queries), nq, e->n_indexed, &n_chunks, s));
-	knn2_merge_kernel<<<(nq + 255) / 256, 256, 0, s>>>(e->d_partial.p, n_chunks, nq, d_keys_out);
-	LCD_CHECK_LAUNCH(e);
-	return LCD_OK;
+	return shard_merge_keys(e, n_chunks, nq, d_keys_out, s);
 }
 
 int lcd_shard_resolve_score_dev(lcd_engine * e, const void * d_queries, int n_frames, int nq_per_frame,
@@ -3382,7 +3403,6 @@ int lcd_shard_resolve_score_dev(lcd_engine * e, const void * d_queries, int n_fr
                                 int * d_word_ids_out, long long * d_scores_out, void * stream)
 {
 	if (!e) return LCD_ERR_INVALID;
-	LCD_TRY(require_binary(e, "lcd_shard_resolve_score_dev"));
 	LCD_TRY(set_device(e));
 	if (!d_queries || !d_keys_gathered || !d_row_ids || n_frames <= 0 || n_ranks <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
@@ -3393,7 +3413,7 @@ int lcd_shard_resolve_score_dev(lcd_engine * e, const void * d_queries, int n_fr
 	a.queries = static_cast<const uint32_t *>(d_queries);
 	a.nq = nq_per_frame;
 	a.nq_total = n_frames * nq_per_frame;
-	a.partial = reinterpret_cast<const uint2 *>(d_keys_gathered);
+	shard_set_keys(e, a, d_keys_gathered, 0);
 	a.n_chunks = n_ranks;
 	a.row_ids = d_row_ids;
 	a.incremental = incremental;
@@ -3424,7 +3444,6 @@ int lcd_shard_resolve_frames_dev(lcd_engine * e, const void * d_queries_all, int
                                  float nndr, int new_words_compared_together, const int * d_n_per_frame, int * d_word_ids_out, void * stream)
 {
 	if (!e) return LCD_ERR_INVALID;
-	LCD_TRY(require_binary(e, "lcd_shard_resolve_frames_dev"));
 	LCD_TRY(set_device(e));
 	if (!d_queries_all || !d_keys_gathered || !d_row_ids || !d_word_ids_out || n_frames <= 0 || n_ranks <= 0 || frame0 < 0 ||
 	    frame0 + n_frames > n_frames_total)
@@ -3435,7 +3454,7 @@ int lcd_shard_resolve_frames_dev(lcd_engine * e, const void * d_queries_all, int
 	a.queries = static_cast<const uint32_t *>(d_queries_all) + static_cast<size_t>(frame0) * nq_per_frame * e->nw;
 	a.nq = nq_per_frame;
 	a.nq_total = n_frames_total * nq_per_frame;                                     // stride between the gathered key sets
-	a.partial = reinterpret_cast<const uint2 *>(d_keys_gathered) + static_cast<size_t>(frame0) * nq_per_frame;
+	shard_set_keys(e, a, d_keys_gathered, static_cast<size_t>(frame0) * nq_per_frame);
 	a.n_chunks = n_ranks;
 	a.row_ids = d_row_ids;
 	a.incremental = incremental;
@@ -3638,24 +3657,22 @@ int lcd_shard_comm_destroy(lcd_engine * e)
 	return LCD_OK;
 }
 
-int lcd_shard_process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d_images, int width, int height, int channels, const void * d_depth,
-                                 int depth_type, const lcd_orb_params * op, int incremental, float nndr, int new_words_compared_together,
-                                 const int * d_sig_ids, int ns, int n_total, const int * d_row_ids_global, int last_word_id,
-                                 const lcd_verify_params * vp, int * d_word_ids_out, float * d_likelihood_out, void * stream)
+// The exchange body of one sharded step, shared by lcd_shard_process_frames_dev and lcd_shard_localize_batch_dev.  desc: the n_frames
+// local frames of `cap` descriptor rows each (e->nw * 4 bytes per row); n_local: valid rows of each local frame, or nullptr (full frames).
+// `detect` runs first on the compute stream and produces desc / n_local (ORB); `finish` runs after the likelihood of the local frames
+// (verification).  Either may be empty.  Keys are exchanged as two u32 (binary) or two u64 (float) per query.
+using ShardHook = std::function<int(cudaStream_t)>;
+
+static int shard_step(lcd_engine * e, int n_frames, int cap, const uint8_t * desc, const int * n_local, const ShardHook & detect, const ShardHook & finish,
+                      int incremental, float nndr, int new_words_compared_together, const int * d_sig_ids, int ns, int n_total,
+                      const int * d_row_ids_global, int last_word_id, int * d_word_ids_out, float * d_likelihood_out, cudaStream_t s)
 {
-	if (!e) return LCD_ERR_INVALID;
-	LCD_TRY(require_binary(e, "lcd_shard_process_frames_dev"));
-	LCD_TRY(set_device(e));
-	if (!e->comm) LCD_FAIL(e, LCD_ERR_STATE, "no communicator: call lcd_shard_comm_init first");
-	if (!d_images || n_frames <= 0 || !op || !d_sig_ids || ns <= 0 || !d_row_ids_global || !d_likelihood_out)
-		LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
-	if (e->cfg.desc_dim != 32) LCD_FAIL(e, LCD_ERR_INVALID, "ORB descriptors need an engine with 32-byte binary descriptors");
-	const int cap = op->n_features;
-	if (cap <= 0 || cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "Kp/MaxFeatures must be 1..%d", kMaxFrameQueries);
 	const NcclApi & nc = nccl_api();
-	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
 	cudaStream_t c = e->comm_stream;
 	const int G = e->sh_ranks, R = e->sh_rank;
+	const size_t row_bytes = static_cast<size_t>(e->nw) * 4;
+	const size_t kw = shard_key_words(e);                               // u32 words of one query's key pair
+	const ncclDataType_t key_type = e->f32 ? ncclUint64 : ncclUint32; // two keys of this type per query
 	// The dictionary search runs on two halves of the local batch, so that the descriptor all-gather of the second half and the key
 	// exchange of the first run under a search kernel.  The merge + NNDR stage is a one-CTA-per-frame kernel that takes as long for half a
 	// batch as for a whole one, so it runs once on the whole batch and its exchange (word ids) is exposed: measured cheaper than splitting.
@@ -3673,20 +3690,14 @@ int lcd_shard_process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d
 	const int score_frames[2] = {s_parts == 2 ? (n_frames + 1) / 2 : n_frames, s_parts == 2 ? n_frames / 2 : 0};
 	const int score_f0[2] = {0, score_frames[0]};
 	const size_t rows = static_cast<size_t>(n_frames) * cap;
-	LCD_CUDA(e, e->o_kp.reserve(rows, 0, false, s));
-	LCD_CUDA(e, e->o_desc.reserve(rows * 32, 0, false, s));
-	LCD_CUDA(e, e->o_xyz.reserve(rows * 3, 0, false, s));
-	LCD_CUDA(e, e->o_uv.reserve(rows * 2, 0, false, s));
-	LCD_CUDA(e, e->o_n.reserve(n_frames, 0, false, s));
-	LCD_CUDA(e, e->sh_n_all.reserve(static_cast<size_t>(G) * n_frames, 0, false, s));
-	LCD_CUDA(e, e->d_like.reserve(static_cast<size_t>(n_frames) * ns, 0, false, s));
+	if (n_local) LCD_CUDA(e, e->sh_n_all.reserve(static_cast<size_t>(G) * n_frames, 0, false, s));
 	for (int h = 0; h < n_parts; ++h)
 	{
 		const size_t pr = static_cast<size_t>(part_frames[h]) * cap; // descriptor rows of this part on one rank
-		LCD_CUDA(e, e->sh_desc_all[h].reserve(pr * 32 * G, 0, false, s));
-		LCD_CUDA(e, e->sh_keys[h].reserve(pr * 2 * G, 0, false, s));
+		LCD_CUDA(e, e->sh_desc_all[h].reserve(pr * row_bytes * G, 0, false, s));
+		LCD_CUDA(e, e->sh_keys[h].reserve(pr * kw * G, 0, false, s));
 	}
-	LCD_CUDA(e, e->sh_keys_mine[0].reserve(rows * 2 * G, 0, false, s)); // [rank][local frame][feature]: both halves land in one array
+	LCD_CUDA(e, e->sh_keys_mine[0].reserve(rows * kw * G, 0, false, s)); // [rank][local frame][feature]: both halves land in one array
 	LCD_CUDA(e, e->sh_words_loc[0].reserve(rows, 0, false, s));
 	LCD_CUDA(e, e->sh_words_all[0].reserve(rows * G, 0, false, s));
 	for (int h = 0; h < s_parts; ++h)
@@ -3710,7 +3721,6 @@ int lcd_shard_process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d
 		if (cudaEventElapsedTime(&ms, e->sh_tr[0], e->sh_tr[1]) == cudaSuccess) fprintf(stderr, " end=%.3f", ms);
 		fprintf(stderr, "\n");
 	}
-	LCD_CUDA(e, zero_fill_async(e->o_desc.p, rows * 32, s)); // padding rows of short frames must hold defined bytes
 	if (e->sh_trace) LCD_CUDA(e, cudaEventRecord(e->sh_tr[0], s));
 	if (e->sh_trace == 2 && e->sh_ring_step < 16) LCD_CUDA(e, cudaEventRecord(e->sh_ring[(e->sh_ring_step * 2 + 0) * 9 + 8], s));
 	// the communication stream starts behind everything already queued on the compute stream
@@ -3718,18 +3728,18 @@ int lcd_shard_process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d
 	LCD_CUDA(e, cudaStreamWaitEvent(c, e->sh_ev[0][7], 0));
 
 	host_t[0] = std::chrono::steady_clock::now();
-	// phase 1: detect + describe the local frames in one pass (splitting detection costs more than the 30-50 us all-gather it would hide),
-	// then all-gather the descriptors part by part (and the keypoint counts): the second part's exchange runs under the first part's search
-	LCD_TRY(orb_run(e, n_frames, d_images, width, height, channels, d_depth, depth_type, op, cap, e->o_kp.p, e->o_desc.p, e->o_xyz.p, e->o_uv.p, e->o_n.p, s, 0,
-	                n_frames));
+	// phase 1: the local descriptors (detected here in one pass when `detect` is given: splitting detection costs more than the 30-50 us
+	// all-gather it would hide), then all-gather of the descriptors part by part (and of the per-frame counts): the second part's exchange
+	// runs under the first part's search
+	if (detect) LCD_TRY(detect(s));
 	for (int h = 0; h < n_parts; ++h)
 	{
 		LCD_TRY(shard_record(e, h, 0, s));
 		LCD_CUDA(e, cudaStreamWaitEvent(c, e->sh_ev[h][0], 0));
 		const size_t pr = static_cast<size_t>(part_frames[h]) * cap;
 		LCD_NCCL(e, nc.GroupStart());
-		LCD_NCCL(e, nc.AllGather(e->o_desc.p + static_cast<size_t>(part_f0[h]) * cap * 32, e->sh_desc_all[h].p, pr * 32, ncclUint8, e->comm, c));
-		if (h == n_parts - 1) LCD_NCCL(e, nc.AllGather(e->o_n.p, e->sh_n_all.p, n_frames, ncclInt32, e->comm, c));
+		LCD_NCCL(e, nc.AllGather(desc + static_cast<size_t>(part_f0[h]) * cap * row_bytes, e->sh_desc_all[h].p, pr * row_bytes, ncclUint8, e->comm, c));
+		if (h == n_parts - 1 && n_local) LCD_NCCL(e, nc.AllGather(n_local, e->sh_n_all.p, n_frames, ncclInt32, e->comm, c));
 		LCD_NCCL(e, nc.GroupEnd());
 		LCD_TRY(shard_record(e, h, 1, c));
 	}
@@ -3742,15 +3752,14 @@ int lcd_shard_process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d
 		LCD_CUDA(e, cudaStreamWaitEvent(s, e->sh_ev[h][1], 0));
 		int n_chunks = 0;
 		LCD_TRY(run_knn(e, reinterpret_cast<const uint32_t *>(e->sh_desc_all[h].p), nq_all, e->n_indexed, &n_chunks, s));
-		knn2_merge_kernel<<<(nq_all + 255) / 256, 256, 0, s>>>(e->d_partial.p, n_chunks, nq_all, e->sh_keys[h].p);
-		LCD_CHECK_LAUNCH(e);
+		LCD_TRY(shard_merge_keys(e, n_chunks, nq_all, e->sh_keys[h].p, s));
 		LCD_TRY(shard_record(e, h, 2, s));
 		LCD_CUDA(e, cudaStreamWaitEvent(c, e->sh_ev[h][2], 0));
 		LCD_NCCL(e, nc.GroupStart());
 		for (int p = 0; p < G; ++p)
 		{
-			LCD_NCCL(e, nc.Send(e->sh_keys[h].p + static_cast<size_t>(p) * pr * 2, pr * 2, ncclUint32, p, e->comm, c));
-			LCD_NCCL(e, nc.Recv(e->sh_keys_mine[0].p + (static_cast<size_t>(p) * rows + static_cast<size_t>(part_f0[h]) * cap) * 2, pr * 2, ncclUint32, p, e->comm, c));
+			LCD_NCCL(e, nc.Send(e->sh_keys[h].p + static_cast<size_t>(p) * pr * kw, pr * 2, key_type, p, e->comm, c));
+			LCD_NCCL(e, nc.Recv(e->sh_keys_mine[0].p + (static_cast<size_t>(p) * rows + static_cast<size_t>(part_f0[h]) * cap) * kw, pr * 2, key_type, p, e->comm, c));
 		}
 		LCD_NCCL(e, nc.GroupEnd());
 		LCD_TRY(shard_record(e, h, 3, c));
@@ -3762,10 +3771,10 @@ int lcd_shard_process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d
 		const size_t pr = static_cast<size_t>(tail_frames[h]) * cap;
 		LCD_CUDA(e, cudaStreamWaitEvent(s, e->sh_ev[t_parts == 2 ? h : n_parts - 1][3], 0));
 		ResolveArgs a{};
-		a.queries = reinterpret_cast<const uint32_t *>(e->o_desc.p) + static_cast<size_t>(tail_f0[h]) * cap * e->nw;
+		a.queries = reinterpret_cast<const uint32_t *>(desc) + static_cast<size_t>(tail_f0[h]) * cap * e->nw;
 		a.nq = cap;
 		a.nq_total = static_cast<int>(rows);                       // stride between the G key sets
-		a.partial = reinterpret_cast<const uint2 *>(e->sh_keys_mine[0].p) + static_cast<size_t>(tail_f0[h]) * cap;
+		shard_set_keys(e, a, e->sh_keys_mine[0].p, static_cast<size_t>(tail_f0[h]) * cap);
 		a.n_chunks = G;
 		a.row_ids = d_row_ids_global;
 		a.incremental = incremental;
@@ -3773,7 +3782,7 @@ int lcd_shard_process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d
 		a.cmp_new = new_words_compared_together;
 		a.last_word_id = last_word_id;
 		a.word_ids_out = e->sh_words_loc[h].p;
-		a.nq_frame = e->o_n.p + tail_f0[h];
+		a.nq_frame = n_local ? n_local + tail_f0[h] : nullptr;
 		LCD_TRY(launch_resolve(e, a, tail_frames[h], s));
 		if (d_word_ids_out)
 			LCD_CUDA(e, cudaMemcpyAsync(d_word_ids_out + static_cast<size_t>(tail_f0[h]) * cap, e->sh_words_loc[h].p, pr * sizeof(int), cudaMemcpyDeviceToDevice, s));
@@ -3809,7 +3818,7 @@ int lcd_shard_process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d
 		LCD_TRY(shard_record(e, h, 7, c));
 	}
 	host_t[4] = std::chrono::steady_clock::now();
-	// phase 5: likelihood of the local frames, verification of their top hypothesis
+	// phase 5: likelihood of the local frames (then `finish`: verification of their top hypothesis)
 	for (int h = 0; h < s_parts; ++h)
 	{
 		const int n = score_frames[h] * ns;
@@ -3817,9 +3826,7 @@ int lcd_shard_process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d
 		fixed_to_float_kernel<<<(n + 255) / 256, 256, 0, s>>>(e->sh_scores_loc[h].p, n, d_likelihood_out + static_cast<size_t>(score_f0[h]) * ns);
 		LCD_CHECK_LAUNCH(e);
 	}
-	if (vp)
-		LCD_TRY(verify_top_dev(e, reinterpret_cast<const uint32_t *>(e->o_desc.p), e->o_uv.p, n_frames, cap, d_likelihood_out, d_sig_ids, ns, vp, s, e->o_n.p,
-		                       e->o_xyz.p));
+	if (finish) LCD_TRY(finish(s));
 	if (e->sh_trace)
 	{
 		LCD_CUDA(e, cudaEventRecord(e->sh_tr[1], s));
@@ -3858,6 +3865,58 @@ int lcd_shard_process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d
 		}
 	}
 	return LCD_OK;
+}
+
+int lcd_shard_process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d_images, int width, int height, int channels, const void * d_depth,
+                                 int depth_type, const lcd_orb_params * op, int incremental, float nndr, int new_words_compared_together,
+                                 const int * d_sig_ids, int ns, int n_total, const int * d_row_ids_global, int last_word_id,
+                                 const lcd_verify_params * vp, int * d_word_ids_out, float * d_likelihood_out, void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(require_binary(e, "lcd_shard_process_frames_dev"));
+	LCD_TRY(set_device(e));
+	if (!e->comm) LCD_FAIL(e, LCD_ERR_STATE, "no communicator: call lcd_shard_comm_init first");
+	if (!d_images || n_frames <= 0 || !op || !d_sig_ids || ns <= 0 || !d_row_ids_global || !d_likelihood_out)
+		LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
+	if (e->cfg.desc_dim != 32) LCD_FAIL(e, LCD_ERR_INVALID, "ORB descriptors need an engine with 32-byte binary descriptors");
+	const int cap = op->n_features;
+	if (cap <= 0 || cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "Kp/MaxFeatures must be 1..%d", kMaxFrameQueries);
+	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	const size_t rows = static_cast<size_t>(n_frames) * cap;
+	LCD_CUDA(e, e->o_kp.reserve(rows, 0, false, s));
+	LCD_CUDA(e, e->o_desc.reserve(rows * 32, 0, false, s));
+	LCD_CUDA(e, e->o_xyz.reserve(rows * 3, 0, false, s));
+	LCD_CUDA(e, e->o_uv.reserve(rows * 2, 0, false, s));
+	LCD_CUDA(e, e->o_n.reserve(n_frames, 0, false, s));
+	LCD_CUDA(e, e->d_like.reserve(static_cast<size_t>(n_frames) * ns, 0, false, s));
+	LCD_CUDA(e, zero_fill_async(e->o_desc.p, rows * 32, s)); // padding rows of short frames must hold defined bytes
+	// detect + describe the local frames, and after the likelihood verify their top hypothesis
+	const ShardHook orb = [&](cudaStream_t st) {
+		return orb_run(e, n_frames, d_images, width, height, channels, d_depth, depth_type, op, cap, e->o_kp.p, e->o_desc.p, e->o_xyz.p, e->o_uv.p, e->o_n.p,
+		               st, 0, n_frames);
+	};
+	const ShardHook verify = [&](cudaStream_t st) {
+		return vp ? verify_top_dev(e, reinterpret_cast<const uint32_t *>(e->o_desc.p), e->o_uv.p, n_frames, cap, d_likelihood_out, d_sig_ids, ns, vp, st,
+		                           e->o_n.p, e->o_xyz.p)
+		          : LCD_OK;
+	};
+	return shard_step(e, n_frames, cap, e->o_desc.p, e->o_n.p, orb, verify, incremental, nndr, new_words_compared_together, d_sig_ids, ns, n_total,
+	                  d_row_ids_global, last_word_id, d_word_ids_out, d_likelihood_out, s);
+}
+
+int lcd_shard_localize_batch_dev(lcd_engine * e, const void * d_queries, int n_frames, int nq_per_frame, int incremental, float nndr,
+                                 int new_words_compared_together, const int * d_sig_ids, int ns, int n_total, const int * d_row_ids_global,
+                                 int last_word_id, int * d_word_ids_out, float * d_likelihood_out, void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (!e->comm) LCD_FAIL(e, LCD_ERR_STATE, "no communicator: call lcd_shard_comm_init first");
+	if (!d_queries || n_frames <= 0 || !d_sig_ids || ns <= 0 || !d_row_ids_global || !d_likelihood_out)
+		LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
+	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
+	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	return shard_step(e, n_frames, nq_per_frame, static_cast<const uint8_t *>(d_queries), nullptr, ShardHook(), ShardHook(), incremental, nndr,
+	                  new_words_compared_together, d_sig_ids, ns, n_total, d_row_ids_global, last_word_id, d_word_ids_out, d_likelihood_out, s);
 }
 
 int lcd_shard_finalize_dev(lcd_engine * e, const long long * d_scores, int n, float * d_likelihood_out, void * stream)

@@ -104,6 +104,22 @@ __global__ void knn2_l2_decode_kernel(const ulonglong2 * __restrict__ partial, i
 	d2[qi] = k2 == kKey64None ? -1.0f : key64_dist(k2);
 }
 
+// lcd_shard_knn2_keys_dev for float descriptors: merge the splits (n_splits of the exact kernel, 1 of the fp16 filter path) into one
+// key pair per query, in the order of the unsharded merge, so that ties go to the lowest global row
+__global__ void knn2_merge64_kernel(const ulonglong2 * __restrict__ partial, int n_splits, int nq, ulonglong2 * __restrict__ out)
+{
+	const int qi = blockIdx.x * blockDim.x + threadIdx.x;
+	if (qi >= nq) return;
+	unsigned long long k1 = kKey64None, k2 = kKey64None;
+	for (int c = 0; c < n_splits; ++c)
+	{
+		const ulonglong2 p = partial[static_cast<size_t>(c) * nq + qi];
+		top2_insert64(k1, k2, p.x);
+		top2_insert64(k1, k2, p.y);
+	}
+	out[qi] = make_ulonglong2(k1, k2);
+}
+
 // The decision on the multimap<float,int> fullResults of one descriptor (VWDictionary.cpp:1162-1219): candidates in insertion
 // order a1, a2 (index hits), n1, n2 (hits among this frame's new words); strict '<' keeps the earlier entry on ties.
 __device__ __forceinline__ bool nndr_decide64(unsigned long long a1, unsigned long long a2, unsigned long long n1, unsigned long long n2,

@@ -33,6 +33,7 @@ struct ResolveArgs
 	const int * nq_frame;     // valid descriptors of each frame (<= nq), or nullptr (= nq for all)
 	int nq_total;             // n_frames*nq (stride of `partial`)
 	const uint2 * partial;    // [n_chunks][nq_total] top-2 keys per vocabulary chunk / per rank
+	const ulonglong2 * partial64; // the same for float descriptors: 64-bit keys (l2_path.cuh)
 	int n_chunks;
 	const int * row_ids; // global row -> word id
 	int incremental;     // Kp/IncrementalDictionary
