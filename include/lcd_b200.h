@@ -257,6 +257,51 @@ int lcd_localize_batch_dev(lcd_engine * e, const void * d_queries, int n_frames,
                            const int * d_sig_ids, int ns, int n_total,
                            int * d_word_ids_out, float * d_likelihood_out, void * stream);
 
+/* ---- similarity likelihood: Memory::computeLikelihood with Kp/TfIdfLikelihoodUsed=false --------------------------
+ * The other branch of computeLikelihood (Memory.cpp:2179-2214): Signature::compareTo (Signature.cpp:250-288) of the query
+ * against every listed id, in list order.  Global-descriptor pipelines (Mem/GlobalDescriptorStrategy, PyDescriptor), the
+ * memory of OdometryMono and rehearsal (Mem/RehearsalSimilarity, Memory.cpp:4218-4266) use it.  For each id s:
+ *   s <= 0 (the virtual place)                          -> 0
+ *   query and s both carry a global descriptor          -> (float)(((double)dot(q, s) + 1.0f) / 2.0f)
+ *   otherwise, valid(x) = number of x's word ids > 0:
+ *     valid(q) == 0 or valid(s) == 0 (bad signature)    -> 0
+ *     else                                              -> (float)pairs / (float)max(valid(q), valid(s))
+ * pairs = sum over the shared word ids of min(count in q, count in s), what EpipolarGeometry::findPairs counts
+ * (EpipolarGeometry.h:119-151); valid(s) = the references the index holds for s (lcd_index_get_refs counts).  The word-pair value
+ * is exact.  Word ids <= 0 never pair: findPairs tests id >= 0 and would pair id 0, which the quantiser never puts into a
+ * signature (new and matched words are > 0, unquantised features get distinct negative ids).
+ * The dot product is one fp32 fused multiply-add chain in ascending dimension order: the same bits for a (query, signature)
+ * whatever the batch, the frame's position, ns or the entry point, within gamma_D * sum |q_i s_i| of the exact value
+ * (gamma_D = D u / (1 - D u), u = 2^-24).  OpenCV's cv::Mat::dot is dispatched per CPU, so no single reference bit pattern exists.
+ * Sharded engines (lcd_shard_set_row_offset != 0) get LCD_ERR_STATE from every call of this group.
+ *
+ * Global descriptors: Signature::sensorData().globalDescriptors(), type 1, one per signature, fp32 [n][dim] row-major.  The
+ * dimension is fixed by the first add; a later add with another dimension is LCD_ERR_INVALID.  Adding an id that has a
+ * descriptor replaces it; freed rows are reused before the store grows. */
+int lcd_gdesc_add(lcd_engine * e, const int * sig_ids, int n, int dim, const float * data);
+int lcd_gdesc_remove(lcd_engine * e, const int * sig_ids, int n);
+int lcd_gdesc_count(const lcd_engine * e);
+int lcd_gdesc_dim(const lcd_engine * e); /* 0 before the first add */
+/* Memory::computeLikelihood with Kp/TfIdfLikelihoodUsed=false for one query signature (with ns = 1 also Memory::rehearsal's
+ * compareTo, Memory.cpp:4245): query_word_ids[nq] its words (any order, duplicates and ids <= 0 allowed; nq may be 0),
+ * query_gdesc[lcd_gdesc_dim(e)] its global descriptor or NULL, sig_ids[ns], likelihood_out[ns].  Returns LCD_ERR_INVALID
+ * ("Global descriptors should be normalized!", the reference's UASSERT) when a global-descriptor value is < 0; the values are
+ * written all the same. */
+int lcd_index_similarity(lcd_engine * e, const int * query_word_ids, int nq, const float * query_gdesc,
+                         const int * sig_ids, int ns, float * likelihood_out);
+/* lcd_localize_batch semantics (quantise n_frames frames without mutation) followed by the similarity likelihood of every frame
+ * against sig_ids[ns]: gdesc[n_frames][lcd_gdesc_dim(e)] the frames' global descriptors or NULL, word_ids_out[n_frames*nq_per_frame],
+ * likelihood_out[n_frames*ns] (either output may be NULL).  LCD_ERR_INVALID as lcd_index_similarity when a value is < 0. */
+int lcd_localize_similarity_batch(lcd_engine * e, const void * queries, int n_frames, int nq_per_frame, int incremental, float nndr,
+                                  int new_words_compared_together, const float * gdesc, const int * sig_ids, int ns,
+                                  int * word_ids_out, float * likelihood_out);
+/* The same on device pointers, asynchronous on `stream` (NULL = the engine's stream).  It does not check the values: a caller
+ * that needs the UASSERT looks for values < 0 itself.  Similarity followed by verification is this call, then lcd_verify_top_dev
+ * on d_likelihood_out (any likelihood rows work there), then lcd_process_fetch. */
+int lcd_localize_similarity_batch_dev(lcd_engine * e, const void * d_queries, int n_frames, int nq_per_frame, int incremental,
+                                      float nndr, int new_words_compared_together, const float * d_gdesc, const int * d_sig_ids,
+                                      int ns, int * d_word_ids_out, float * d_likelihood_out, void * stream);
+
 /* ---- geometric verification: Memory::computeTransform ----------------------------------
  * Batched verification of n_pairs (FROM = old signature with 3-D points, TO = new signature with
  * 2-D keypoints) hypotheses.  Buffers are [n_pairs][cap] row-major; n_from/n_to give the valid

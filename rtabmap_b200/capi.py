@@ -143,6 +143,13 @@ SIGNATURES = {
     "lcd_bayes_reset": (_I, [_P]),
     "lcd_localize_batch": (_I, [_P, _P, _I, _I, _I, _F, _I, _P, _I, _I, _P, _P]),
     "lcd_localize_batch_dev": (_I, [_P, _P, _I, _I, _I, _F, _I, _P, _I, _I, _P, _P, _P]),
+    "lcd_gdesc_add": (_I, [_P, _P, _I, _I, _P]),
+    "lcd_gdesc_remove": (_I, [_P, _P, _I]),
+    "lcd_gdesc_count": (_I, [_P]),
+    "lcd_gdesc_dim": (_I, [_P]),
+    "lcd_index_similarity": (_I, [_P, _P, _I, _P, _P, _I, _P]),
+    "lcd_localize_similarity_batch": (_I, [_P, _P, _I, _I, _I, _F, _I, _P, _P, _I, _P, _P]),
+    "lcd_localize_similarity_batch_dev": (_I, [_P, _P, _I, _I, _I, _F, _I, _P, _P, _I, _P, _P, _P]),
     "lcd_match_pairs": (_I, [_P, _I, _I, _P, _P, _P, _P, _F, _P, _P]),
     "lcd_verify_batch": (_I, [_P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "lcd_pnp_ransac": (_I, [_P, _P, _P, _I, _P, _P, _I, _P, _P, _I, _I, _F, _I, _I, _I, _F, _P, _P]),
@@ -507,6 +514,73 @@ class Engine:
                                                       int(cmp_new), C.c_void_p(d_sig_ids), ns, int(n_total),
                                                       C.c_void_p(d_words_out or None), C.c_void_p(d_like_out or None),
                                                       C.c_void_p(stream or None)))
+
+    # -- similarity likelihood (Memory::computeLikelihood with Kp/TfIdfLikelihoodUsed=false) -----------------
+    def gdesc_add(self, sig_ids, desc):
+        """Store one global descriptor (type 1) per signature: desc [n, dim] float32.  Replaces an existing one; the first add fixes dim."""
+        s = _i32(sig_ids)
+        d = np.ascontiguousarray(desc, np.float32)
+        if d.ndim != 2 or d.shape[0] != len(s):
+            raise LcdError(-1, f"global descriptors must be [{len(s)}, dim] float32, got {d.shape}")
+        self._check(self._lib.lcd_gdesc_add(self._h, _ptr(s), len(s), d.shape[1], _ptr(d)))
+
+    def gdesc_remove(self, sig_ids):
+        """Drop the global descriptors of these signatures (ids without one are ignored); their rows are reused by later adds."""
+        s = _i32(sig_ids)
+        self._check(self._lib.lcd_gdesc_remove(self._h, _ptr(s), len(s)))
+
+    def gdesc_count(self) -> int:
+        """Number of signatures that carry a global descriptor."""
+        return int(self._lib.lcd_gdesc_count(self._h))
+
+    def gdesc_dim(self) -> int:
+        """Dimension of the stored global descriptors (0 before the first add)."""
+        return int(self._lib.lcd_gdesc_dim(self._h))
+
+    def _gdesc_rows(self, g, n: int):
+        if g is None:
+            return None
+        g = np.ascontiguousarray(g, np.float32).reshape(n, -1)
+        if g.shape[1] != self.gdesc_dim():
+            raise LcdError(-1, f"query global descriptors must have {self.gdesc_dim()} dimensions, got {g.shape[1]}")
+        return g
+
+    def similarity(self, query_word_ids, sig_ids, query_gdesc=None) -> np.ndarray:
+        """Signature::compareTo of one query signature (its word ids, optionally its global descriptor) against every id of
+        sig_ids: the similarity branch of Memory::computeLikelihood, and with one id Memory::rehearsal's comparison.  Returns
+        float32 [len(sig_ids)]."""
+        w = _i32(query_word_ids).reshape(-1)
+        s = _i32(sig_ids)
+        g = self._gdesc_rows(query_gdesc, 1)
+        out = np.zeros(len(s), np.float32)
+        self._check(self._lib.lcd_index_similarity(self._h, _ptr(w) if len(w) else None, len(w), _ptr(g), _ptr(s), len(s), _ptr(out)))
+        return out
+
+    def localize_similarity_batch(self, queries, n_frames: int, sig_ids, gdesc=None, incremental: bool = True, nndr: float = 0.8,
+                                  cmp_new: bool = True, want_words: bool = True):
+        """localize_batch with the similarity likelihood: quantise n_frames frames without changing the engine, then compare each
+        frame (its words, and its global descriptor when gdesc [n_frames, dim] is given) with every id of sig_ids.
+        Returns (word ids [n_frames, nq] or None, likelihood [n_frames, len(sig_ids)])."""
+        q = self._desc(queries)
+        assert len(q) % n_frames == 0
+        nq = len(q) // n_frames
+        s = _i32(sig_ids)
+        g = self._gdesc_rows(gdesc, n_frames)
+        words = np.zeros((n_frames, nq), np.int32) if want_words else None
+        like = np.zeros((n_frames, len(s)), np.float32)
+        self._check(self._lib.lcd_localize_similarity_batch(self._h, _ptr(q), n_frames, nq, int(incremental), float(nndr), int(cmp_new),
+                                                             _ptr(g), _ptr(s), len(s), _ptr(words), _ptr(like)))
+        return words, like
+
+    def localize_similarity_batch_dev(self, d_queries: int, n_frames: int, nq: int, d_sig_ids: int, ns: int, d_gdesc: int = 0,
+                                      d_words_out: int = 0, d_like_out: int = 0, incremental: bool = True, nndr: float = 0.8,
+                                      cmp_new: bool = True, stream: int = 0):
+        """localize_similarity_batch on device pointers (d_gdesc [n_frames, gdesc_dim()] float32 or 0), asynchronous on `stream`.
+        Does not check that global-descriptor values are >= 0."""
+        self._check(self._lib.lcd_localize_similarity_batch_dev(self._h, C.c_void_p(d_queries), n_frames, nq, int(incremental), float(nndr),
+                                                                 int(cmp_new), C.c_void_p(d_gdesc or None), C.c_void_p(d_sig_ids), ns,
+                                                                 C.c_void_p(d_words_out or None), C.c_void_p(d_like_out or None),
+                                                                 C.c_void_p(stream or None)))
 
     # -- geometric verification -----------------------------------------------------------------
     def _pairs(self, desc_from, desc_to, n_from, n_to):

@@ -17,6 +17,7 @@
 #include "nn_tensor_f32.cuh"
 #include "resolve.cuh"
 #include "score.cuh"
+#include "similarity.cuh"
 #include "bayes.cuh"
 #include "verify.cuh"
 #include "match_bf.cuh"
@@ -277,6 +278,8 @@ struct lcd_engine
 	DevBuf<int> ni;
 	std::vector<int> h_ni;
 	std::unordered_map<int, std::vector<std::pair<int, int>>> sig_words; // sig -> sorted (word,count)
+	DevBuf<int> nvalid;      // by signature id: valid(s) of Signature::compareTo = sum of the signature's posting counts
+	std::vector<int> h_nvalid; // = the sum of its sig_words counts; same size as h_ni
 	long long total_refs = 0;
 
 	// --- scratch
@@ -288,6 +291,7 @@ struct lcd_engine
 	DevBuf<int> d_word_ids, d_n_new, d_in_ids;
 	DevBuf<int> uq_count, uq_word, uq_prefix;
 	DevBuf<float> uq_idf;
+	DevBuf<int> uq_mult, q_valid; // similarity likelihood: query multiplicity of each unique word, valid(q) of each frame
 	DevBuf<long long> acc;
 	int acc_stride = 0;
 	DevBuf<int> d_sig_ids;
@@ -317,6 +321,11 @@ struct lcd_engine
 	DevBuf<int> st_n, st_slot_of_sig;
 	std::vector<int> h_slot_of_sig, free_slots;
 	int st_cap = 0, st_slots = 0;
+	// global descriptors (SensorData::globalDescriptors(), type 1, one per signature): rows [slot][gd_dim], the signature store's slot scheme
+	DevBuf<float> gd_rows, gd_query, gd_dot;
+	DevBuf<int> gd_slot_of_sig;
+	std::vector<int> h_gd_slot_of_sig, gd_free;
+	int gd_dim = 0, gd_slots = 0;
 	DevBuf<int> d_hyp_id, d_hyp_slot;
 	// ORB workspace
 	DevBuf<uint8_t> o_img, o_gray, o_mask, o_blur, o_desc;
@@ -473,7 +482,9 @@ int ensure_sigs(lcd_engine * e, int max_sig)
 		const size_t old = e->h_ni.size();
 		const size_t ncap = std::max(need, old + old / 2 + 1024);
 		LCD_CUDA(e, e->ni.reserve(ncap, old, true, e->stream));
+		LCD_CUDA(e, e->nvalid.reserve(e->ni.cap, old, true, e->stream));
 		e->h_ni.resize(e->ni.cap, 0);
+		e->h_nvalid.resize(e->ni.cap, 0);
 	}
 	return LCD_OK;
 }
@@ -828,12 +839,17 @@ int launch_resolve(lcd_engine * e, const ResolveArgs & a, int n_frames, cudaStre
 	return LCD_OK;
 }
 
-int ensure_uq(lcd_engine * e, int n_frames, int nq, cudaStream_t s)
+int ensure_uq(lcd_engine * e, int n_frames, int nq, cudaStream_t s, bool pairs = false)
 {
 	LCD_CUDA(e, e->uq_count.reserve(n_frames, 0, false, s));
 	LCD_CUDA(e, e->uq_word.reserve(static_cast<size_t>(n_frames) * nq, 0, false, s));
 	LCD_CUDA(e, e->uq_prefix.reserve(static_cast<size_t>(n_frames) * (nq + 1), 0, false, s));
 	LCD_CUDA(e, e->uq_idf.reserve(static_cast<size_t>(n_frames) * nq, 0, false, s));
+	if (pairs)
+	{
+		LCD_CUDA(e, e->uq_mult.reserve(static_cast<size_t>(n_frames) * nq, 0, false, s));
+		LCD_CUDA(e, e->q_valid.reserve(n_frames, 0, false, s));
+	}
 	return LCD_OK;
 }
 
@@ -850,7 +866,15 @@ void fill_prep(lcd_engine * e, ResolveArgs & a, float n_total, int self_ref)
 	a.uq_idf = e->uq_idf.p;
 }
 
-int launch_score(lcd_engine * e, int n_frames, int nq, cudaStream_t s)
+// the preparation of the similarity likelihood's word pairs (after fill_prep; ensure_uq(..., pairs = true))
+void fill_pairs(lcd_engine * e, ResolveArgs & a)
+{
+	a.pairs = 1;
+	a.uq_mult = e->uq_mult.p;
+	a.q_valid = e->q_valid.p;
+}
+
+int launch_score(lcd_engine * e, int n_frames, int nq, cudaStream_t s, bool pairs = false)
 {
 	ScoreArgs sa;
 	sa.nq = nq;
@@ -858,6 +882,7 @@ int launch_score(lcd_engine * e, int n_frames, int nq, cudaStream_t s)
 	sa.uq_word = e->uq_word.p;
 	sa.uq_prefix = e->uq_prefix.p;
 	sa.uq_idf = e->uq_idf.p;
+	sa.uq_mult = e->uq_mult.p;
 	sa.post_off = e->post_off.p;
 	sa.postings = e->postings.p;
 	sa.ni = e->ni.p;
@@ -866,7 +891,8 @@ int launch_score(lcd_engine * e, int n_frames, int nq, cudaStream_t s)
 	sa.acc_stride = e->acc_stride;
 	dim3 grid(e->score_blocks, n_frames);
 	prof_mark(e, LCD_PROF_SCORE, s);
-	score_kernel<<<grid, kScoreThreads, (nq + 1) * sizeof(int), s>>>(sa);
+	if (pairs) score_kernel<true><<<grid, kScoreThreads, (nq + 1) * sizeof(int), s>>>(sa);
+	else score_kernel<false><<<grid, kScoreThreads, (nq + 1) * sizeof(int), s>>>(sa);
 	prof_mark(e, LCD_PROF_SCORE, s);
 	LCD_CHECK_LAUNCH(e);
 	return LCD_OK;
@@ -925,6 +951,7 @@ int add_refs_impl(lcd_engine * e, int sig_id, const int * word_ids, int n)
 	merged.reserve(sw.size() + ids.size());
 	size_t si = 0;
 	size_t extra = 0;
+	int added = 0; // references that reach the index (words the dictionary holds)
 	for (size_t i = 0; i < ids.size();)
 	{
 		size_t j = i;
@@ -962,12 +989,15 @@ int add_refs_impl(lcd_engine * e, int sig_id, const int * word_ids, int n)
 			op.newlen = ++e->h_len[word];
 		}
 		e->total_refs += cnt;
+		added += cnt;
 		ops.push_back(op);
 	}
 	while (si < sw.size()) merged.push_back(sw[si++]);
 	sw.swap(merged);
 	e->h_ni[sig_id] += n;
 	LCD_CUDA(e, cudaMemcpyAsync(e->ni.p + sig_id, &e->h_ni[sig_id], sizeof(int), cudaMemcpyHostToDevice, e->stream));
+	e->h_nvalid[sig_id] += added;
+	LCD_CUDA(e, cudaMemcpyAsync(e->nvalid.p + sig_id, &e->h_nvalid[sig_id], sizeof(int), cudaMemcpyHostToDevice, e->stream));
 	if (extra)
 	{
 		LCD_TRY(ensure_postings(e, extra));
@@ -1015,11 +1045,44 @@ int check_queries(lcd_engine * e, const void * q, int nq)
 	return LCD_OK;
 }
 
-// quantise + score of n_frames independent frames on device buffers, no mutation
+// The similarity likelihood (Memory::computeLikelihood with Kp/TfIdfLikelihoodUsed=false) of n_frames frames whose word pairs the
+// resolve / prep kernel prepared (fill_pairs): word pairs, the global-descriptor dot products where the frames carry a descriptor
+// (d_gdesc [n_frames][gd_dim], or nullptr), then Signature::compareTo per (frame, k) into d_like [n_frames][ns].
+int launch_similarity(lcd_engine * e, int n_frames, int nq, const float * d_gdesc, const int * d_sig_ids, int ns, float * d_like, cudaStream_t s)
+{
+	LCD_TRY(launch_score(e, n_frames, nq, s, true));
+	const bool gd = d_gdesc && e->gd_slots > static_cast<int>(e->gd_free.size());
+	if (gd)
+	{
+		LCD_CUDA(e, e->gd_dot.reserve(static_cast<size_t>(n_frames) * ns, 0, false, s));
+		GdescArgs g{d_gdesc, n_frames, e->gd_rows.p, e->gd_dim, e->gd_slot_of_sig.p, static_cast<int>(e->h_gd_slot_of_sig.size()), d_sig_ids, ns,
+		            e->gd_dot.p};
+		prof_mark(e, LCD_PROF_SCORE, s);
+		gdesc_dot_kernel<<<dim3((ns + kGdBN - 1) / kGdBN, (n_frames + kGdBM - 1) / kGdBM), kGdThreads, 0, s>>>(g);
+		prof_mark(e, LCD_PROF_SCORE, s);
+		LCD_CHECK_LAUNCH(e);
+	}
+	SimilarityArgs f{e->acc.p, e->acc_stride, e->nvalid.p, static_cast<int>(e->h_nvalid.size()), e->q_valid.p, gd ? e->gd_dot.p : nullptr,
+	                 e->gd_slot_of_sig.p, static_cast<int>(e->h_gd_slot_of_sig.size()), d_sig_ids, ns, d_like};
+	similarity_finalize_kernel<<<dim3((ns + 255) / 256, n_frames), 256, 0, s>>>(f);
+	LCD_CHECK_LAUNCH(e);
+	return LCD_OK;
+}
+
+// which branch of Memory::computeLikelihood localize_dev scores with (Kp/TfIdfLikelihoodUsed)
+enum class LikelihoodKind
+{
+	TfIdf,
+	Similarity
+};
+
+// quantise + score of n_frames independent frames on device buffers, no mutation.  kind = Similarity: d_gdesc [n_frames][gd_dim] are
+// the frames' global descriptors (nullptr = none) and n_total is not used.
 int localize_dev(lcd_engine * e, const uint32_t * d_q, int n_frames, int nq, int incremental, float nndr, int cmp_new,
                  const int * d_sig_ids, int ns, int n_total, int * d_word_ids_out, float * d_like_out, cudaStream_t s,
-                 const int * d_nq_frame = nullptr)
+                 const int * d_nq_frame = nullptr, LikelihoodKind kind = LikelihoodKind::TfIdf, const float * d_gdesc = nullptr)
 {
+	const bool sim = kind == LikelihoodKind::Similarity;
 	if (e->n_indexed == 0 && !incremental) LCD_FAIL(e, LCD_ERR_STATE, "Dictionary mode is set to fixed but no words are in it!");
 	LCD_TRY(require_unsharded(e, "localisation on one engine"));
 	const int nq_total = n_frames * nq;
@@ -1045,12 +1108,14 @@ int localize_dev(lcd_engine * e, const uint32_t * d_q, int n_frames, int nq, int
 	a.pending_ids = nullptr;
 	if (score)
 	{
-		LCD_TRY(ensure_uq(e, n_frames, nq, s));
+		LCD_TRY(ensure_uq(e, n_frames, nq, s, sim));
 		LCD_TRY(ensure_acc(e, n_frames));
 		LCD_CUDA(e, zero_fill_async(e->acc.p, static_cast<size_t>(e->acc_stride) * n_frames * sizeof(long long), s));
 		fill_prep(e, a, static_cast<float>(n_total), 1);
+		if (sim) fill_pairs(e, a);
 	}
 	LCD_TRY(launch_resolve(e, a, n_frames, s));
+	if (score && sim) return launch_similarity(e, n_frames, nq, d_gdesc, d_sig_ids, ns, d_like_out, s);
 	if (score)
 	{
 		LCD_TRY(launch_score(e, n_frames, nq, s));
@@ -1287,6 +1352,7 @@ int lcd_dict_remove_words(lcd_engine * e, const int * ids, int n)
 	LCD_TRY(set_device(e));
 	bool pending_hit = false;
 	std::vector<int> zero_ids;
+	std::unordered_set<int> nvalid_changed;
 	for (int i = 0; i < n; ++i)
 	{
 		auto it = e->id2row.find(ids[i]);
@@ -1311,7 +1377,12 @@ int lcd_dict_remove_words(lcd_engine * e, const int * ids, int n)
 				if (sw == e->sig_words.end()) continue;
 				auto & v = sw->second;
 				auto pos = std::lower_bound(v.begin(), v.end(), std::make_pair(ids[i], 0));
-				if (pos != v.end() && pos->first == ids[i]) v.erase(pos);
+				if (pos != v.end() && pos->first == ids[i])
+				{
+					e->h_nvalid[pc.x] -= pos->second;
+					nvalid_changed.insert(pc.x);
+					v.erase(pos);
+				}
 			}
 			e->h_len[ids[i]] = 0;
 			zero_ids.push_back(ids[i]);
@@ -1320,6 +1391,10 @@ int lcd_dict_remove_words(lcd_engine * e, const int * ids, int n)
 	for (int id : zero_ids)
 	{
 		LCD_CUDA(e, cudaMemsetAsync(e->post_len.p + id, 0, sizeof(int), e->stream));
+	}
+	for (int sig : nvalid_changed)
+	{
+		LCD_CUDA(e, cudaMemcpyAsync(e->nvalid.p + sig, &e->h_nvalid[sig], sizeof(int), cudaMemcpyHostToDevice, e->stream));
 	}
 	if (pending_hit)
 	{
@@ -1423,9 +1498,11 @@ int lcd_dict_clear(lcd_engine * e)
 	std::fill(e->h_len.begin(), e->h_len.end(), 0);
 	std::fill(e->h_cap.begin(), e->h_cap.end(), 0);
 	std::fill(e->h_ni.begin(), e->h_ni.end(), 0);
+	std::fill(e->h_nvalid.begin(), e->h_nvalid.end(), 0);
 	if (e->post_len.p) LCD_CUDA(e, cudaMemsetAsync(e->post_len.p, 0, e->post_len.cap * sizeof(int), e->stream));
 	if (e->post_off.p) LCD_CUDA(e, cudaMemsetAsync(e->post_off.p, 0, e->post_off.cap * sizeof(uint32_t), e->stream));
 	if (e->ni.p) LCD_CUDA(e, cudaMemsetAsync(e->ni.p, 0, e->ni.cap * sizeof(int), e->stream));
+	if (e->nvalid.p) LCD_CUDA(e, cudaMemsetAsync(e->nvalid.p, 0, e->nvalid.cap * sizeof(int), e->stream));
 	e->post_used = 0;
 	e->sig_words.clear();
 	e->total_refs = 0;
@@ -1647,6 +1724,8 @@ int lcd_index_remove_sig(lcd_engine * e, int sig_id)
 	{
 		e->h_ni[sig_id] = 0;
 		LCD_CUDA(e, cudaMemsetAsync(e->ni.p + sig_id, 0, sizeof(int), e->stream));
+		e->h_nvalid[sig_id] = 0;
+		LCD_CUDA(e, cudaMemsetAsync(e->nvalid.p + sig_id, 0, sizeof(int), e->stream));
 	}
 	if (!ops.empty())
 	{
@@ -1723,6 +1802,7 @@ int lcd_index_load_csr(lcd_engine * e, const int * word_ids, int nw, const int64
 			buf[w++] = make_int2(sig[p], cnt[p]);
 			e->sig_words[sig[p]].emplace_back(word, cnt[p]);
 			e->h_ni[sig[p]] += cnt[p];
+			e->h_nvalid[sig[p]] += cnt[p];
 			e->total_refs += cnt[p];
 		}
 	}
@@ -1733,6 +1813,7 @@ int lcd_index_load_csr(lcd_engine * e, const int * word_ids, int nw, const int64
 	LCD_CUDA(e, cudaMemcpyAsync(e->post_off.p, e->h_off.data(), (static_cast<size_t>(max_word) + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
 	LCD_CUDA(e, cudaMemcpyAsync(e->post_len.p, e->h_len.data(), (static_cast<size_t>(max_word) + 1) * sizeof(int), cudaMemcpyHostToDevice, e->stream));
 	LCD_CUDA(e, cudaMemcpyAsync(e->ni.p, e->h_ni.data(), (static_cast<size_t>(max_sig) + 1) * sizeof(int), cudaMemcpyHostToDevice, e->stream));
+	LCD_CUDA(e, cudaMemcpyAsync(e->nvalid.p, e->h_nvalid.data(), (static_cast<size_t>(max_sig) + 1) * sizeof(int), cudaMemcpyHostToDevice, e->stream));
 	LCD_CUDA(e, cudaStreamSynchronize(e->stream));
 	return LCD_OK;
 }
@@ -1994,6 +2075,191 @@ int lcd_localize_batch(lcd_engine * e, const void * queries, int n_frames, int n
 		LCD_CUDA(e, cudaMemcpyAsync(likelihood_out, e->d_like.p, static_cast<size_t>(n_frames) * ns * sizeof(float), cudaMemcpyDeviceToHost, s));
 	LCD_CUDA(e, cudaStreamSynchronize(s));
 	return LCD_OK;
+}
+
+// ---- similarity likelihood: Memory::computeLikelihood with Kp/TfIdfLikelihoodUsed=false ----------------------------------------
+int lcd_gdesc_count(const lcd_engine * e) { return e ? e->gd_slots - static_cast<int>(e->gd_free.size()) : 0; }
+int lcd_gdesc_dim(const lcd_engine * e) { return e ? e->gd_dim : 0; }
+
+int lcd_gdesc_add(lcd_engine * e, const int * sig_ids, int n, int dim, const float * data)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(require_unsharded(e, "lcd_gdesc_add"));
+	if (n <= 0) return LCD_OK;
+	if (!sig_ids || !data) LCD_FAIL(e, LCD_ERR_INVALID, "null global descriptors");
+	if (dim <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "global descriptors need at least one dimension, got %d", dim);
+	if (e->gd_dim != 0 && dim != e->gd_dim) LCD_FAIL(e, LCD_ERR_INVALID, "global descriptors of this engine have %d dimensions, got %d", e->gd_dim, dim);
+	int max_id = 0;
+	for (int i = 0; i < n; ++i)
+	{
+		if (sig_ids[i] <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "signature id must be positive");
+		max_id = std::max(max_id, sig_ids[i]);
+	}
+	LCD_TRY(set_device(e));
+	cudaStream_t s = e->stream;
+	e->gd_dim = dim;
+	if (static_cast<size_t>(max_id) + 1 > e->h_gd_slot_of_sig.size())
+	{
+		const size_t old = e->h_gd_slot_of_sig.size();
+		e->h_gd_slot_of_sig.resize(std::max<size_t>(max_id + 1, old + old / 2 + 1024), -1);
+	}
+	// a signature that has a descriptor keeps its slot (replace); freed slots are reused before the store grows
+	const size_t prev_slots = static_cast<size_t>(e->gd_slots);
+	std::vector<int> slots(n);
+	bool contiguous = true;
+	for (int i = 0; i < n; ++i)
+	{
+		int slot = e->h_gd_slot_of_sig[sig_ids[i]];
+		if (slot < 0)
+		{
+			if (!e->gd_free.empty())
+			{
+				slot = e->gd_free.back();
+				e->gd_free.pop_back();
+			}
+			else slot = e->gd_slots++;
+		}
+		slots[i] = slot;
+		if (i > 0 && slots[i] != slots[i - 1] + 1) contiguous = false;
+		e->h_gd_slot_of_sig[sig_ids[i]] = slot;
+	}
+	const size_t row = static_cast<size_t>(dim);
+	LCD_CUDA(e, e->gd_rows.reserve(static_cast<size_t>(e->gd_slots) * row, prev_slots * row, false, s));
+	if (contiguous)
+		LCD_CUDA(e, cudaMemcpyAsync(e->gd_rows.p + static_cast<size_t>(slots[0]) * row, data, row * n * sizeof(float), cudaMemcpyHostToDevice, s));
+	else
+		for (int i = 0; i < n; ++i)
+			LCD_CUDA(e, cudaMemcpyAsync(e->gd_rows.p + static_cast<size_t>(slots[i]) * row, data + static_cast<size_t>(i) * row, row * sizeof(float),
+			                            cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, e->gd_slot_of_sig.reserve(e->h_gd_slot_of_sig.size(), 0, false, s));
+	LCD_CUDA(e, cudaMemcpyAsync(e->gd_slot_of_sig.p, e->h_gd_slot_of_sig.data(), e->h_gd_slot_of_sig.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, cudaStreamSynchronize(s));
+	return LCD_OK;
+}
+
+int lcd_gdesc_remove(lcd_engine * e, const int * sig_ids, int n)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(require_unsharded(e, "lcd_gdesc_remove"));
+	if (n <= 0) return LCD_OK;
+	if (!sig_ids) LCD_FAIL(e, LCD_ERR_INVALID, "null signature ids");
+	LCD_TRY(set_device(e));
+	bool changed = false;
+	for (int i = 0; i < n; ++i)
+	{
+		const int id = sig_ids[i];
+		if (id <= 0 || id >= static_cast<int>(e->h_gd_slot_of_sig.size()) || e->h_gd_slot_of_sig[id] < 0) continue;
+		e->gd_free.push_back(e->h_gd_slot_of_sig[id]);
+		e->h_gd_slot_of_sig[id] = -1;
+		changed = true;
+	}
+	if (!changed) return LCD_OK;
+	LCD_CUDA(e, cudaMemcpyAsync(e->gd_slot_of_sig.p, e->h_gd_slot_of_sig.data(), e->h_gd_slot_of_sig.size() * sizeof(int), cudaMemcpyHostToDevice, e->stream));
+	LCD_CUDA(e, cudaStreamSynchronize(e->stream));
+	return LCD_OK;
+}
+
+// UASSERT_MSG(dotProd>=0, ...) of Signature::compareTo (Signature.cpp:264); word-pair values are never negative
+static int check_normalized(lcd_engine * e, const float * like, size_t n)
+{
+	for (size_t i = 0; i < n; ++i)
+		if (!(like[i] >= 0.0f)) LCD_FAIL(e, LCD_ERR_INVALID, "Global descriptors should be normalized!");
+	return LCD_OK;
+}
+
+int lcd_index_similarity(lcd_engine * e, const int * query_word_ids, int nq, const float * query_gdesc, const int * sig_ids, int ns,
+                         float * likelihood_out)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	LCD_TRY(require_unsharded(e, "lcd_index_similarity"));
+	if (nq < 0 || (nq > 0 && !query_word_ids)) LCD_FAIL(e, LCD_ERR_INVALID, "The signature is null");
+	if (!sig_ids || ns <= 0 || !likelihood_out) LCD_FAIL(e, LCD_ERR_INVALID, "ids list is empty");
+	if (nq > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "at most %d words per signature", kMaxFrameQueries);
+	cudaStream_t s = e->stream;
+	const int nq1 = std::max(nq, 1); // a signature without words (global descriptor only) is prepared as one invalid id
+	LCD_CUDA(e, e->d_in_ids.reserve(nq1, 0, false, s));
+	LCD_CUDA(e, e->d_sig_ids.reserve(ns, 0, false, s));
+	LCD_CUDA(e, e->d_like.reserve(ns, 0, false, s));
+	if (nq > 0) LCD_CUDA(e, cudaMemcpyAsync(e->d_in_ids.p, query_word_ids, nq * sizeof(int), cudaMemcpyHostToDevice, s));
+	else LCD_CUDA(e, cudaMemsetAsync(e->d_in_ids.p, 0, sizeof(int), s));
+	LCD_CUDA(e, cudaMemcpyAsync(e->d_sig_ids.p, sig_ids, ns * sizeof(int), cudaMemcpyHostToDevice, s));
+	const float * d_g = nullptr;
+	if (query_gdesc && e->gd_dim > 0)
+	{
+		LCD_CUDA(e, e->gd_query.reserve(e->gd_dim, 0, false, s));
+		LCD_CUDA(e, cudaMemcpyAsync(e->gd_query.p, query_gdesc, e->gd_dim * sizeof(float), cudaMemcpyHostToDevice, s));
+		d_g = e->gd_query.p;
+	}
+	LCD_TRY(ensure_uq(e, 1, nq1, s, true));
+	LCD_TRY(ensure_acc(e, 1));
+	LCD_CUDA(e, cudaMemsetAsync(e->acc.p, 0, static_cast<size_t>(e->acc_stride) * sizeof(long long), s));
+	ResolveArgs a{};
+	a.nq = nq1;
+	fill_prep(e, a, 0.0f, 0);
+	fill_pairs(e, a);
+	int nq_pad = 32;
+	while (nq_pad < nq1) nq_pad <<= 1;
+	prep_from_ids_kernel<<<1, kResolveThreads, nq_pad * sizeof(uint32_t), s>>>(e->d_in_ids.p, a);
+	LCD_CHECK_LAUNCH(e);
+	LCD_TRY(launch_similarity(e, 1, nq1, d_g, e->d_sig_ids.p, ns, e->d_like.p, s));
+	LCD_CUDA(e, cudaMemcpyAsync(likelihood_out, e->d_like.p, ns * sizeof(float), cudaMemcpyDeviceToHost, s));
+	LCD_CUDA(e, cudaStreamSynchronize(s));
+	return check_normalized(e, likelihood_out, static_cast<size_t>(ns));
+}
+
+int lcd_localize_similarity_batch_dev(lcd_engine * e, const void * d_queries, int n_frames, int nq_per_frame, int incremental, float nndr,
+                                      int new_words_compared_together, const float * d_gdesc, const int * d_sig_ids, int ns,
+                                      int * d_word_ids_out, float * d_likelihood_out, void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	LCD_TRY(require_unsharded(e, "lcd_localize_similarity_batch_dev"));
+	if (!d_queries || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "Descriptors size is null!");
+	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
+	if (d_likelihood_out && (!d_sig_ids || ns <= 0)) LCD_FAIL(e, LCD_ERR_INVALID, "ids list is empty");
+	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	return localize_dev(e, static_cast<const uint32_t *>(d_queries), n_frames, nq_per_frame, incremental, nndr, new_words_compared_together,
+	                    d_sig_ids, ns, 0, d_word_ids_out, d_likelihood_out, s, nullptr, LikelihoodKind::Similarity, e->gd_dim > 0 ? d_gdesc : nullptr);
+}
+
+int lcd_localize_similarity_batch(lcd_engine * e, const void * queries, int n_frames, int nq_per_frame, int incremental, float nndr,
+                                  int new_words_compared_together, const float * gdesc, const int * sig_ids, int ns,
+                                  int * word_ids_out, float * likelihood_out)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	LCD_TRY(require_unsharded(e, "lcd_localize_similarity_batch"));
+	if (!queries || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "Descriptors size is null!");
+	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
+	if (likelihood_out && (!sig_ids || ns <= 0)) LCD_FAIL(e, LCD_ERR_INVALID, "ids list is empty");
+	cudaStream_t s = e->stream;
+	const size_t nq_total = static_cast<size_t>(n_frames) * nq_per_frame;
+	LCD_CUDA(e, e->d_queries.reserve(nq_total * e->nw, 0, false, s));
+	LCD_CUDA(e, cudaMemcpyAsync(e->d_queries.p, queries, nq_total * e->nw * 4, cudaMemcpyHostToDevice, s));
+	if (word_ids_out) LCD_CUDA(e, e->d_word_ids.reserve(nq_total, 0, false, s));
+	const float * d_g = nullptr;
+	if (likelihood_out)
+	{
+		LCD_CUDA(e, e->d_sig_ids.reserve(ns, 0, false, s));
+		LCD_CUDA(e, e->d_like.reserve(static_cast<size_t>(n_frames) * ns, 0, false, s));
+		LCD_CUDA(e, cudaMemcpyAsync(e->d_sig_ids.p, sig_ids, ns * sizeof(int), cudaMemcpyHostToDevice, s));
+		if (gdesc && e->gd_dim > 0)
+		{
+			const size_t ng = static_cast<size_t>(n_frames) * e->gd_dim;
+			LCD_CUDA(e, e->gd_query.reserve(ng, 0, false, s));
+			LCD_CUDA(e, cudaMemcpyAsync(e->gd_query.p, gdesc, ng * sizeof(float), cudaMemcpyHostToDevice, s));
+			d_g = e->gd_query.p;
+		}
+	}
+	LCD_TRY(localize_dev(e, e->d_queries.p, n_frames, nq_per_frame, incremental, nndr, new_words_compared_together, e->d_sig_ids.p,
+	                     likelihood_out ? ns : 0, 0, word_ids_out ? e->d_word_ids.p : nullptr, likelihood_out ? e->d_like.p : nullptr, s, nullptr,
+	                     LikelihoodKind::Similarity, d_g));
+	if (word_ids_out) LCD_CUDA(e, cudaMemcpyAsync(word_ids_out, e->d_word_ids.p, nq_total * sizeof(int), cudaMemcpyDeviceToHost, s));
+	if (likelihood_out)
+		LCD_CUDA(e, cudaMemcpyAsync(likelihood_out, e->d_like.p, static_cast<size_t>(n_frames) * ns * sizeof(float), cudaMemcpyDeviceToHost, s));
+	LCD_CUDA(e, cudaStreamSynchronize(s));
+	return likelihood_out ? check_normalized(e, likelihood_out, static_cast<size_t>(n_frames) * ns) : LCD_OK;
 }
 
 // ---- detect (ORB) ------------------------------------------------------------------------------

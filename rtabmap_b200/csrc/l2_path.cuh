@@ -351,6 +351,7 @@ resolve_l2_kernel(const ResolveArgs a, const ulonglong2 * __restrict__ partial64
 	}
 
 	// 3. word ids in creation order, and the created words into the not-indexed tail of the vocabulary (single-frame quantise)
+	int n_valid = 0;
 	for (int i = tid; i < nq; i += blockDim.x)
 	{
 		int wid;
@@ -365,6 +366,7 @@ resolve_l2_kernel(const ResolveArgs a, const ulonglong2 * __restrict__ partial64
 		}
 		if (a.word_ids_out) a.word_ids_out[pbase + i] = wid;
 		sbuf[i] = sv;
+		n_valid += wid > 0;
 	}
 	for (int i = nq + tid; i < nq_pad; i += blockDim.x)
 	{
@@ -382,6 +384,7 @@ resolve_l2_kernel(const ResolveArgs a, const ulonglong2 * __restrict__ partial64
 		}
 	}
 	if (tid == 0 && a.n_new_out) a.n_new_out[frame] = (a.find_only ? 0 : n_new);
+	if (a.q_valid) cta_count_store(n_valid, a.q_valid + frame);
 	__syncthreads();
 	if (a.do_prep) score_prep(sbuf, nq_pad, cap, a, frame);
 }

@@ -56,7 +56,23 @@ struct ResolveArgs
 	int * uq_word;        // [n_frames][nq]    unique matched word ids, ascending
 	int * uq_prefix;      // [n_frames][nq+1]  exclusive scan of posting lengths to walk
 	float * uq_idf;       // [n_frames][nq]    log10(N/nw)
+	// similarity likelihood (Memory.cpp:2179-2214): the per-word payload is the query's multiplicity of the word instead of the idf,
+	// and every posting is walked (TF-IDF skips the words whose idf is 0)
+	int pairs;
+	int * uq_mult;        // [n_frames][nq]    multiplicity of each unique word (pairs only)
+	int * q_valid;        // [n_frames]        valid(q): the frame's word ids > 0 (pairs only, else nullptr)
 };
+
+// Writes the CTA-wide sum of every thread's `mine` to *out (thread 0).  All threads of the CTA must call it.
+__device__ inline void cta_count_store(int mine, int * out)
+{
+	__shared__ int s_count;
+	if (threadIdx.x == 0) s_count = 0;
+	__syncthreads();
+	if (mine) atomicAdd(&s_count, mine);
+	__syncthreads();
+	if (threadIdx.x == 0) *out = s_count;
+}
 
 // Outcome of the multimap<float,int> fullResults of one descriptor.
 // a1,a2: index hits (packed keys), n1,n2: hits among this frame's new words (dist<<22|k).
@@ -135,6 +151,7 @@ __host__ __device__ inline size_t resolve_smem_bytes(int nq)
 
 // TF-IDF preparation from a list of candidate word ids in sbuf[0..n_pad) (kSortNone = skip):
 // sort, unique, per-word posting length + idf, exclusive scan.  Used by both entry kernels.
+// With a.pairs the payload is the word's multiplicity in the list and the whole posting list is walked.
 __device__ void score_prep(uint32_t * sbuf, int n_pad, int nq, const ResolveArgs & a, int frame)
 {
 	const int tid = threadIdx.x;
@@ -169,6 +186,7 @@ __device__ void score_prep(uint32_t * sbuf, int n_pad, int nq, const ResolveArgs
 		int * uqw = a.uq_word + static_cast<size_t>(frame) * nq;
 		int * uqp = a.uq_prefix + static_cast<size_t>(frame) * (nq + 1);
 		float * uqi = a.uq_idf + static_cast<size_t>(frame) * nq;
+		int * uqm = a.pairs ? a.uq_mult + static_cast<size_t>(frame) * nq : nullptr;
 		for (int c = 0; c < n_pad; c += 32)
 		{
 			const int i = c + lane;
@@ -177,17 +195,28 @@ __device__ void score_prep(uint32_t * sbuf, int n_pad, int nq, const ResolveArgs
 			const uint32_t m = __ballot_sync(0xFFFFFFFFu, f);
 			int len = 0;
 			float idf = 0.0f;
+			int mult = 0;
 			if (f)
 			{
 				const int id = static_cast<int>(v);
 				const int plen = id < a.id_cap ? a.post_len[id] : 0;
-				const float nw = static_cast<float>(plen + a.self_ref);
-				if (nw > 0.0f)
+				if (a.pairs)
 				{
-					// logNnw = log10(N/nw) on floats (Memory.cpp:2266)
-					idf = static_cast<float>(log10(static_cast<double>(__fdiv_rn(a.n_total, nw))));
+					int j = i + 1;
+					while (j < n_pad && sbuf[j] == v) ++j;
+					mult = j - i;
+					len = plen;
 				}
-				len = idf != 0.0f ? plen : 0;
+				else
+				{
+					const float nw = static_cast<float>(plen + a.self_ref);
+					if (nw > 0.0f)
+					{
+						// logNnw = log10(N/nw) on floats (Memory.cpp:2266)
+						idf = static_cast<float>(log10(static_cast<double>(__fdiv_rn(a.n_total, nw))));
+					}
+					len = idf != 0.0f ? plen : 0;
+				}
 			}
 			// inclusive scan of len across the warp
 			int incl = len;
@@ -201,7 +230,8 @@ __device__ void score_prep(uint32_t * sbuf, int n_pad, int nq, const ResolveArgs
 			{
 				const int k = base + __popc(m & ((1u << lane) - 1u));
 				uqw[k] = static_cast<int>(v);
-				uqi[k] = idf;
+				if (uqm) uqm[k] = mult;
+				else uqi[k] = idf;
 				uqp[k] = run + incl - len;
 			}
 			run += __shfl_sync(0xFFFFFFFFu, incl, 31);
@@ -413,6 +443,7 @@ resolve_kernel(const ResolveArgs a)
 	}
 
 	// 3. word ids (VWDictionary::getNextId = ++_lastWordId in creation order)
+	int n_valid = 0;
 	for (int i = tid; i < nq; i += blockDim.x)
 	{
 		int wid;
@@ -444,6 +475,7 @@ resolve_kernel(const ResolveArgs a)
 		}
 		if (a.word_ids_out) a.word_ids_out[pbase + i] = wid;
 		sbuf[i] = sv;
+		n_valid += wid > 0;
 	}
 	for (int i = nq + tid; i < nq_pad; i += blockDim.x)
 	{
@@ -451,6 +483,7 @@ resolve_kernel(const ResolveArgs a)
 		if (i < cap && a.word_ids_out) a.word_ids_out[pbase + i] = 0; // padding rows of a short frame
 	}
 	if (tid == 0 && a.n_new_out) a.n_new_out[frame] = n_new;
+	if (a.q_valid) cta_count_store(n_valid, a.q_valid + frame); // new words count too: they are ids > 0 of the query signature
 	__syncthreads();
 
 	// 4. unique matched words -> idf + posting extents for the scoring kernel
@@ -468,11 +501,14 @@ prep_from_ids_kernel(const int * __restrict__ word_ids, const ResolveArgs a)
 	while (nq_pad < nq) nq_pad <<= 1;
 	uint32_t * sbuf = reinterpret_cast<uint32_t *>(smem_raw);
 	const int frame = blockIdx.x;
+	int n_valid = 0;
 	for (int i = threadIdx.x; i < nq_pad; i += blockDim.x)
 	{
 		int w = i < nq ? word_ids[static_cast<size_t>(frame) * nq + i] : 0;
 		sbuf[i] = w > 0 ? static_cast<uint32_t>(w) : kSortNone;
+		n_valid += w > 0;
 	}
+	if (a.q_valid) cta_count_store(n_valid, a.q_valid + frame);
 	__syncthreads();
 	score_prep(sbuf, nq_pad, nq, a, frame);
 }

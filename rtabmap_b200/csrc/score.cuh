@@ -30,6 +30,7 @@ struct ScoreArgs
 	const int * uq_word;    // [n_frames][nq]
 	const int * uq_prefix;  // [n_frames][nq+1]
 	const float * uq_idf;   // [n_frames][nq]
+	const int * uq_mult;    // [n_frames][nq] query multiplicity of each word (PAIRS)
 	const uint32_t * post_off; // by word id
 	const int2 * postings;     // (signature id, count)
 	const int * ni;            // by signature id
@@ -39,6 +40,10 @@ struct ScoreArgs
 };
 
 // grid = (blocks_per_frame, n_frames)
+// PAIRS = false: the TF-IDF term of every posting.  PAIRS = true: the word pairs of Signature::compareTo (Signature.cpp:278-284),
+// acc[frame][sig] += min(count in the query, count in the signature) = EpipolarGeometry::findPairs summed over the shared ids
+// (EpipolarGeometry.h:119-151); integer, hence exact and independent of the order.
+template <bool PAIRS>
 __global__ void __launch_bounds__(kScoreThreads)
 score_kernel(const ScoreArgs a)
 {
@@ -58,6 +63,7 @@ score_kernel(const ScoreArgs a)
 	__syncthreads();
 	const int * uqw = a.uq_word + static_cast<size_t>(frame) * a.nq;
 	const float * uqi = a.uq_idf + static_cast<size_t>(frame) * a.nq;
+	const int * uqm = a.uq_mult + static_cast<size_t>(frame) * a.nq;
 	long long * acc = a.acc + static_cast<size_t>(frame) * a.acc_stride;
 
 	int p = begin + threadIdx.x;
@@ -77,10 +83,15 @@ score_kernel(const ScoreArgs a)
 	{
 		while (s_prefix[lo + 1] <= p) ++lo; // p < total = prefix[nuq]: stops at lo < nuq
 		const int word = uqw[lo];
-		const float idf = uqi[lo];
 		const int2 ref = a.postings[static_cast<size_t>(a.post_off[word]) + (p - s_prefix[lo])];
-		if (ref.x > 0 && ref.x < a.sig_cap)
+		if constexpr (PAIRS)
 		{
+			if (ref.x > 0 && ref.x < a.sig_cap)
+				atomicAdd(reinterpret_cast<unsigned long long *>(acc + ref.x), static_cast<unsigned long long>(min(uqm[lo], ref.y)));
+		}
+		else if (ref.x > 0 && ref.x < a.sig_cap)
+		{
+			const float idf = uqi[lo];
 			const float ni = static_cast<float>(a.ni[ref.x]);
 			if (ni != 0.0f)
 			{
