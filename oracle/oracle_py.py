@@ -1,5 +1,5 @@
-"""ctypes binding of oracle/liboracle.so (restatement) and oracle/_ref/libref_flann.so
-(the reference's own rtflann, compiled from /root/reference by oracle/Makefile).
+"""ctypes binding of oracle/liboracle.so (restatement), oracle/_ref/libref_flann.so (the reference's own rtflann) and
+oracle/_ref/libref_bayes.so (the reference's own BayesFilter.cpp), the last two compiled from /root/reference by oracle/Makefile.
 
 TEST INFRASTRUCTURE ONLY: checker for tests/, smoke() and bench.py's CPU baseline.
 """
@@ -15,10 +15,12 @@ import numpy as np
 HERE = Path(__file__).resolve().parent
 LIB = HERE / "liboracle.so"
 REF_LIB = HERE / "_ref" / "libref_flann.so"
+REF_BAYES_LIB = HERE / "_ref" / "libref_bayes.so"
 REFERENCE_ROOT = Path("/root/reference")
 
 _lib = None
 _ref = None
+_ref_bayes = None
 _P = C.c_void_p
 _I = C.c_int
 _F = C.c_float
@@ -33,11 +35,11 @@ def _reference_present() -> bool:
 
 
 def build(with_ref: bool = True) -> None:
-    """Compile liboracle.so (always) and _ref/libref_flann.so (when /root/reference is present)."""
+    """Compile liboracle.so (always) and _ref/libref_flann.so, _ref/libref_bayes.so (when /root/reference is present)."""
     srcs = [HERE / "oracle.cpp", HERE / "oracle_verify.cpp", HERE / "pnp_math.h"]
     if not LIB.exists() or LIB.stat().st_mtime < max(s.stat().st_mtime for s in srcs):
         subprocess.run(["make", "-C", str(HERE), "liboracle.so"], check=True, capture_output=True)
-    if with_ref and not REF_LIB.exists() and _reference_present():
+    if with_ref and not (REF_LIB.exists() and REF_BAYES_LIB.exists()) and _reference_present():
         subprocess.run(["make", "-C", str(HERE), "ref"], check=True, capture_output=True)
 
 
@@ -98,6 +100,31 @@ def ref_lib():
         R.ref_flann_knn2_l2.argtypes = [_P, _I, _I, _P, _I, _P, _P]
         _ref = R
     return _ref
+
+
+def ref_bayes_lib():
+    """The reference's compiled BayesFilter, or None when it has not been built (no /root/reference)."""
+    global _ref_bayes
+    if _ref_bayes is None:
+        if not REF_BAYES_LIB.exists():
+            if _reference_present():
+                build(with_ref=True)
+            else:
+                return None
+        R = C.CDLL(str(REF_BAYES_LIB))
+        R.ref_bayes_create.restype = _P
+        R.ref_bayes_create.argtypes = [C.c_char_p, _F, _I]
+        R.ref_bayes_destroy.argtypes = [_P]
+        R.ref_bayes_set_graph.argtypes = [_P, _P, _I, _P, _P, _P, _P, _I]
+        R.ref_bayes_compute_posterior.argtypes = [_P, _P, _P, _I, _P]
+        R.ref_bayes_compute_posterior.restype = _I
+        R.ref_bayes_reset.argtypes = [_P]
+        R.ref_bayes_get_prediction_lc.argtypes = [_P, _P, _I]
+        R.ref_bayes_get_prediction_lc.restype = _I
+        R.ref_bayes_generate_prediction.argtypes = [_P, _P, _I, _P]
+        R.ref_bayes_generate_prediction.restype = _I
+        _ref_bayes = R
+    return _ref_bayes
 
 
 def _p(a):
@@ -453,3 +480,60 @@ def verify_pair_repeat(desc_from, xyz_from, desc_to, uv_to, K4, xyz_to=None, nnd
                                    C.byref(ni), _p(r), _p(tv), _p(T), _p(cov), C.byref(sp))
     return {"ok": bool(ok), "matches": mids[:nm.value].copy(), "inliers": iids[:ni.value].copy(), "rvec": r, "tvec": tv, "transform": T.reshape(3, 4),
             "covariance": cov.reshape(6, 6), "second_pass": bool(sp.value)}
+
+
+# ---------------------------------------------------------------- the reference's BayesFilter (ref_bayes.cpp)
+class RefBayesFilter:
+    """rtabmap::BayesFilter compiled from the reference (Bayes/FullPredictionUpdate=true).  `prediction_lc` is the Bayes/PredictionLC
+    string as a user writes it (None keeps the reference's default); the graph is loaded with set_graph before each call."""
+
+    def __init__(self, prediction_lc: str | None = None, virtual_place_prior: float = 0.9):
+        self.R = ref_bayes_lib()
+        if self.R is None:
+            raise RuntimeError("oracle/_ref/libref_bayes.so is not built")
+        self.h = self.R.ref_bayes_create(None if prediction_lc is None else prediction_lc.encode(), float(virtual_place_prior), 1)
+        if not self.h:
+            raise RuntimeError("BayesFilter construction failed")
+
+    def __del__(self):
+        if getattr(self, "h", None):
+            self.R.ref_bayes_destroy(self.h)
+            self.h = None
+
+    def set_graph(self, tables: dict, stm=()):
+        """tables: {place id: {neighbour id: margin}} as Memory::getNeighborsId returns it; stm: ids in the short-term memory."""
+        ids = sorted(tables)
+        ptr = [0]
+        nid, mar = [], []
+        for i in ids:
+            for k, m in sorted(tables[i].items()):
+                nid.append(k)
+                mar.append(m)
+            ptr.append(len(nid))
+        a_ids, a_nid, a_mar, a_stm = _i32(ids), _i32(nid), _i32(mar), _i32(sorted(stm))
+        a_ptr = np.array(ptr, np.int64)
+        self.R.ref_bayes_set_graph(self.h, _p(a_ids), len(a_ids), _p(a_ptr), _p(a_nid), _p(a_mar), _p(a_stm), len(a_stm))
+
+    def compute_posterior(self, ids, likelihood) -> np.ndarray:
+        i = _i32(ids)
+        like = np.ascontiguousarray(likelihood, np.float32)
+        out = np.zeros(len(i), np.float32)
+        if self.R.ref_bayes_compute_posterior(self.h, _p(i), _p(like), len(i), _p(out)) != 0:
+            raise RuntimeError("BayesFilter::computePosterior failed")
+        return out
+
+    def reset(self):
+        self.R.ref_bayes_reset(self.h)
+
+    def prediction_lc(self) -> np.ndarray:
+        out = np.zeros(64, np.float64)
+        n = self.R.ref_bayes_get_prediction_lc(self.h, _p(out), len(out))
+        return out[:n].copy()
+
+    def generate_prediction(self, ids) -> np.ndarray:
+        """BayesFilter::generatePrediction: the dense float matrix P[row, col]."""
+        i = _i32(ids)
+        P = np.zeros((len(i), len(i)), np.float32)
+        if self.R.ref_bayes_generate_prediction(self.h, _p(i), len(i), _p(P)) != 0:
+            raise RuntimeError("BayesFilter::generatePrediction failed")
+        return P

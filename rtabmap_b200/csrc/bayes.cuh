@@ -5,9 +5,11 @@
 // matrix (400 MB at 10 000 places) and multiplies it with the last posterior on the CPU.  A column of that matrix is
 //     the LC value of every graph neighbour of the place (by margin)  +  one uniform value in every other row  +  the virtual-place row,
 // i.e. sparse + rank one, so the product is   prior[r] = U + P[r][0] post[0] + sum over columns c that list r of (P[r][c] - u_c) post[c]
-// with U = sum_c u_c post[c]: O(neighbours) instead of O(S^2).  Arithmetic follows the reference's float statements column by column;
-// the two places where it accumulates S values sequentially (the uniform fill of normalize, the posterior sum) are evaluated in
-// double, so results agree with the dense float product to ~1e-6 relative (north_star tolerance for float work: 1e-4).
+// with U = sum_c u_c post[c]: O(neighbours) instead of O(S^2).  Every column (its listed values, delta, uniform value, scale and
+// epsilon cut) is bit-equal to the reference's float statements, including normalize's column sum, which adds the uniform value to a
+// float once per filled row (repeated_fadd reproduces that loop without running it).  Only the product with the last posterior and
+// the posterior sum are evaluated in double, so results agree with the dense float product to ~1e-6 relative (tolerance for float
+// work: 1e-4).
 #pragma once
 #include "common.cuh"
 
@@ -43,6 +45,7 @@ struct BayesArgs
 __global__ void bayes_last_kernel(const BayesArgs a)
 {
 	const int r = blockIdx.x * blockDim.x + threadIdx.x;
+	if (r < 3) a.sums[r] = 0.0; // before the bound check: with fewer than 3 places the sums would keep the last call's values
 	if (r >= a.n) return;
 	float v = a.n_prev == 0 ? 1.0f : 0.0f;
 	const int id = a.ids[r];
@@ -56,7 +59,33 @@ __global__ void bayes_last_kernel(const BayesArgs a)
 	if (lo < a.n_prev && a.prev_ids[lo] == id) v = a.prev_post[lo];
 	a.last[r] = v;
 	a.prior[r] = 0.0;
-	if (r < 3) a.sums[r] = 0.0;
+}
+
+// s + value + value + ... (times adds, each rounded to nearest float) as normalize's fill loop computes it (BayesFilter.cpp:457-464),
+// in a few steps per binade of s instead of one per add.  Inside one binade every add moves s by the same number of ulps, once one add
+// inside the binade has been made: a round-half-even tie leaves the last bit even, and from an even s every later tie resolves the
+// same way.  So after a literal add that stays in its binade, the run of adds that keeps s below the next power of two is one step.
+// Adds that cross a binade, and sums below FLT_MIN, are made literally.  When an add leaves s unchanged (value under half an ulp, or a
+// tie onto the even s) no later add can move it.
+__host__ __device__ inline float repeated_fadd(float s, const float value, int times)
+{
+	while (times > 0)
+	{
+		const float before = s;
+		s = s + value;
+		--times;
+		if (s == before) break;
+		if (times == 0 || !(before >= 1.17549435e-38f) || ilogbf(s) != ilogbf(before)) continue;
+		const int e = ilogbf(s);
+		const int m = static_cast<int>(ldexpf(s, 23 - e));              // significand as an integer in [2^23, 2^24)
+		const int d = static_cast<int>(ldexpf((s + value) - s, 23 - e)); // ulps of the next add (exact difference)
+		if (d == 0) break;
+		const int fit = (0xFFFFFF - m) / d;                              // adds whose result stays below 2^(e+1)
+		const int k = times < fit ? times : fit;
+		s = ldexpf(static_cast<float>(m + k * d), e - 23);
+		times -= k;
+	}
+	return s;
 }
 
 // one thread per column: addNeighborProb + normalize without materialising the column
@@ -74,11 +103,14 @@ __global__ void bayes_columns_kernel(const BayesArgs a)
 	const int first = a.vp_used ? 1 : 0;
 	float s = 0.f;
 	int n_nonzero = 0;
+	bool diag_zero = false;
 	for (int e = a.col_ptr[c]; e < a.col_ptr[c + 1]; ++e)
 	{
 		const float v = static_cast<float>(a.lc[a.nbr_level[e] + 1]);
 		s = __fadd_rn(s, v);
-		n_nonzero += (v != 0.f && a.nbr_row[e] >= first) ? 1 : 0;
+		if (a.nbr_row[e] < first) continue;
+		if (v != 0.f) ++n_nonzero;
+		else if (a.nbr_row[e] == c) diag_zero = true;
 	}
 	float delta = 0.f;
 	const double lc0 = a.lc[0];
@@ -87,7 +119,8 @@ __global__ void bayes_columns_kernel(const BayesArgs a)
 		delta = static_cast<float>(static_cast<double>(a.total) - lc0 - static_cast<double>(s));
 		s = __fadd_rn(s, delta);
 	}
-	// NB: a diagonal whose list value is 0 becomes non-zero through delta; the list always holds the place itself at margin 0
+	// the fill below sees the diagonal after delta: a place whose own (margin-0) value is 0 is not filled once delta made it non-zero
+	if (diag_zero && delta != 0.f) ++n_nonzero;
 	float other = 0.f;
 	if (a.total < 1.f) other = __fsub_rn(1.0f, a.total);
 	float value = 0.f;
@@ -95,7 +128,7 @@ __global__ void bayes_columns_kernel(const BayesArgs a)
 	{
 		value = __fdiv_rn(other, static_cast<float>(a.n - 1));
 		const int zeros = (a.n - first) - n_nonzero;
-		s = static_cast<float>(static_cast<double>(s) + static_cast<double>(zeros) * static_cast<double>(value));
+		s = repeated_fadd(s, value, zeros);
 	}
 	const float max_norm = static_cast<float>(1.0 - (a.vp_used ? lc0 : 0.0));
 	float scale = 1.f;
