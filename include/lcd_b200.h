@@ -475,6 +475,96 @@ int lcd_map_frame(lcd_engine * e, int sig_id, int incremental, float nndr, int n
 int lcd_verify_top_dev(lcd_engine * e, const void * d_queries, const float * d_uv, int n_frames, int nq_per_frame,
                        const float * d_likelihood, const int * d_sig_ids, int ns, const lcd_verify_params * vp, void * stream);
 
+/* ---- the loop-closure decision of many localisation clients (Mem/IncrementalMemory=false) -----------------------------------
+ * A relocalisation service runs one rtabmap::Rtabmap per camera (a client) against one frozen map.  Each client has its own Bayes
+ * filter state (BayesFilter::_posterior) and its own last highest hypothesis (Rtabmap::_highestHypothesis); the map, and with it the
+ * prediction matrix, is shared.  These calls replace, for B clients at once, what Rtabmap::process does with one frame's raw
+ * likelihood in localisation mode: adjustLikelihood (Rtabmap.cpp:2119-2121), BayesFilter::computePosterior (:2133), the hypothesis
+ * selection and its checks (:2143-2233), and the verification of the accepted hypothesis with its rejections (:3133-3191).
+ * Proximity detection, the epipolar check (Rtabmap/VerifyLoopClosureHypothesis), retrieval and the graph walk stay the caller's.
+ *
+ * replaces: BayesFilter::BayesFilter + BayesFilter::reset (BayesFilter.cpp:43-68, :140-143) and Rtabmap's _highestHypothesis = (0, 0)
+ * (Rtabmap.cpp:467, :1094) for n_clients clients at once; calling it again resets every client.  LCD_ERR_CAPACITY when the device
+ * cannot hold the state. */
+int lcd_clients_create(lcd_engine * e, int n_clients);
+/* BayesFilter::reset + _highestHypothesis = (0, 0) of the listed clients */
+int lcd_clients_reset(lcd_engine * e, const int * clients, int n);
+/* The working memory the clients localise against: ids[n] ascending, ids[0] the virtual place (a negative id: Memory keeps it in the
+ * working memory, Memory.cpp:592), and the neighbour tables, Bayes/PredictionLC and Bayes/VirtualPlacePriorThr exactly as
+ * lcd_bayes_compute_posterior takes them (same checks).  The prediction's columns are computed here, once per map, bit-equal to
+ * lcd_bayes_compute_posterior's.  A client's last posterior is re-keyed to the current places when that client next computes
+ * (updatePosterior, BayesFilter.cpp:712-737), not when the map changes: a place it did not have starts from 0 (from 1 for every place
+ * when its state is empty), a place that left is dropped, and a place that left and came back while the client computed nothing keeps
+ * its value, as in the reference.  A call that fails (bad tables: LCD_ERR_INVALID; no device memory for the tables or for the clients'
+ * posteriors over the new map: LCD_ERR_CAPACITY) changes nothing: the previous map, or no map, stays in place. */
+int lcd_clients_set_map(lcd_engine * e, const int * ids, int n, const int64_t * col_ptr, const int * nbr_row, const int * nbr_level,
+                        const double * prediction_lc, int n_lc, float virtual_place_prior);
+
+typedef struct lcd_decide_params {
+	int virtual_place_ratio;         /* Rtabmap/VirtualPlaceLikelihoodRatio (0; 0 or 1)                                       */
+	float loop_thr;                  /* Rtabmap/LoopThr (0.11; [0, 1])                                                        */
+	float aggressive_loop_thr;       /* RGBD/AggressiveLoopThr (0.05; [0, 1]): used by LCD_FRAME_AGGRESSIVE frames when lower   */
+	float loop_ratio;                /* Rtabmap/LoopRatio (0; [0, 1])                                                         */
+	float max_loop_closure_distance; /* RGBD/MaxLoopClosureDistance (0 = off; >= 0, metres)                                   */
+} lcd_decide_params;
+
+/* frame flags: conditions the caller evaluates, because it owns the signature and the odometry cache */
+#define LCD_FRAME_SKIP 1       /* bad signature, intermediate node or empty working memory (Rtabmap.cpp:1994-1999): the likelihood row
+                                  is ignored, the posterior is untouched, highest = (0, 0) */
+#define LCD_FRAME_HOLD 2       /* small displacement or too fast movement (:2229-2233): the posterior is untouched, highest = the
+                                  client's last highest hypothesis */
+#define LCD_FRAME_AGGRESSIVE 4 /* the conditions of :2173-2177 hold (not localised yet, RGB-D SLAM mode, old map present) */
+
+/* decision statuses */
+#define LCD_DECIDE_SKIPPED 0            /* LCD_FRAME_SKIP */
+#define LCD_DECIDE_HELD 1               /* LCD_FRAME_HOLD */
+#define LCD_DECIDE_NO_HYPOTHESIS 2      /* no real place has a posterior > 0 (:2162) */
+#define LCD_DECIDE_UNDER_THRESHOLD 3    /* value < threshold */
+#define LCD_DECIDE_UNDER_RATIO 4        /* value < threshold and value < loop_ratio x last value (:2215-2222) */
+#define LCD_DECIDE_SINGLE_HYPOTHESIS 5  /* the posterior has <= 2 entries and the threshold is > 0 (:2188-2192) */
+#define LCD_DECIDE_RATIO 6              /* value < loop_ratio x last value (:2197-2201) */
+#define LCD_DECIDE_LAST_NULL 7          /* loop_ratio > 0 and the last value is 0 (:2202-2205) */
+#define LCD_DECIDE_ACCEPTED 8           /* _loopClosureHypothesis = highest (:2206-2210) */
+#define LCD_DECIDE_VERIFY_REJECTED 9    /* accepted, then Memory::computeTransform failed (:3156-3161) */
+#define LCD_DECIDE_DISTANCE_REJECTED 10 /* accepted and registered, transform norm > max_loop_closure_distance (:3162-3167) */
+
+typedef struct lcd_decision {
+	int highest_id;      /* _highestHypothesis.first after this frame (the client's new last highest hypothesis) */
+	float highest_value; /* _highestHypothesis.second: 1 - posterior(virtual place) */
+	int loop_id;         /* _loopClosureHypothesis.first: the accepted (and, after verification, registered) place, else 0 */
+	int status;          /* LCD_DECIDE_* */
+} lcd_decision;
+
+/* For each of n_frames frames, on the device: Rtabmap::adjustLikelihood of d_likelihood[n_frames][ns] (raw likelihood rows over the
+ * map's real places in ascending id order, as lcd_localize_batch_dev, lcd_localize_similarity_batch_dev and
+ * lcd_shard_localize_batch_dev write them; ns must equal the map's real places), BayesFilter::computePosterior of the frame's client
+ * (the client's state becomes the new posterior; d_posterior_out[n_frames][ns+1], element 0 the virtual place, may be NULL; rows of
+ * skipped or held frames are not written), then the hypothesis selection of Rtabmap.cpp:2143-2226: the real place with the largest
+ * posterior, scanned in descending id order with a strict '>' from (0, 0) (ties go to the highest id), its value replaced by
+ * 1 - posterior(virtual place); if its id is > 0, threshold loop_thr (aggressive_loop_thr for LCD_FRAME_AGGRESSIVE frames when lower);
+ * at or over the threshold the single-hypothesis, ratio and last-null rejections in that order, else accepted.  clients[n_frames] and
+ * frame_flags[n_frames] are host arrays, read before the call returns; a client appears at most once per call.  A client's posterior
+ * is the same bits whatever the batch size, its position in the batch and the other clients in it.  Results stay on the device:
+ * lcd_decide_fetch copies the decisions back, lcd_process_fetch the accepted ids (0 = none), lcd_verify_decided_dev verifies them. */
+int lcd_decide_batch_dev(lcd_engine * e, const float * d_likelihood, int n_frames, int ns, const int * clients, const int * frame_flags,
+                         const lcd_decide_params * dp, float * d_posterior_out, void * stream);
+/* decisions of the first n_frames frames of the last decision call (and its verification, when it ran): out[n_frames]; synchronises */
+int lcd_decide_fetch(lcd_engine * e, int n_frames, lcd_decision * out);
+/* replaces: Memory::computeTransform(_loopClosureHypothesis.first, signature) (Rtabmap.cpp:3133-3191) for the frames whose last
+ * decision was accepted (the other frames are not verified: ok = 0, no matches).  A failed registration becomes
+ * LCD_DECIDE_VERIFY_REJECTED, a transform longer than max_loop_closure_distance (> 0) LCD_DECIDE_DISTANCE_REJECTED; both clear loop_id,
+ * and the client's last highest hypothesis is left as it is.  d_queries / d_uv as lcd_process_batch_dev; n_frames must be the last
+ * decision's.  Results through lcd_process_fetch (hypothesis = the final loop id) and lcd_decide_fetch. */
+int lcd_verify_decided_dev(lcd_engine * e, const void * d_queries, const float * d_uv, int n_frames, int nq_per_frame,
+                           const lcd_verify_params * vp, void * stream);
+/* lcd_process_batch_dev with the decision: quantise + score against the map's real places (word ids and likelihood bit-identical to
+ * lcd_localize_batch_dev with those ids), lcd_decide_batch_dev, lcd_verify_decided_dev.  Binary engines only; sharded engines get
+ * LCD_ERR_STATE (a sharded rank calls lcd_decide_batch_dev on the rows lcd_shard_localize_batch_dev wrote). */
+int lcd_process_decide_batch_dev(lcd_engine * e, const void * d_queries, const float * d_uv, int n_frames, int nq_per_frame,
+                                 int incremental, float nndr, int new_words_compared_together, int ns, int n_total,
+                                 const lcd_verify_params * vp, const int * clients, const int * frame_flags, const lcd_decide_params * dp,
+                                 int * d_word_ids_out, float * d_likelihood_out, float * d_posterior_out, void * stream);
+
 /* ---- word-range sharding across GPUs (SURVEY.md §8(e)) ---------------------------
  * Each rank owns the words whose row (in ascending id order) falls in its range; rows
  * are numbered globally: set the global row offset of this shard so that packed top-2

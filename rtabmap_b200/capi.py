@@ -90,6 +90,25 @@ class VerifyResult(C.Structure):
     ]
 
 
+class DecideParams(C.Structure):
+    """lcd_decide_params (Rtabmap/VirtualPlaceLikelihoodRatio, Rtabmap/LoopThr, RGBD/AggressiveLoopThr, Rtabmap/LoopRatio,
+    RGBD/MaxLoopClosureDistance)."""
+    _fields_ = [
+        ("virtual_place_ratio", C.c_int),
+        ("loop_thr", C.c_float),
+        ("aggressive_loop_thr", C.c_float),
+        ("loop_ratio", C.c_float),
+        ("max_loop_closure_distance", C.c_float),
+    ]
+
+
+# frame flags and decision statuses of lcd_decide_batch_dev (lcd_b200.h)
+FRAME_SKIP, FRAME_HOLD, FRAME_AGGRESSIVE = 1, 2, 4
+DECIDE_STATUS = ("skipped", "held", "no hypothesis", "under threshold", "under ratio", "single hypothesis", "ratio", "last null", "accepted",
+                 "verification rejected", "distance rejected")
+DECISION_DTYPE = np.dtype([("highest_id", np.int32), ("highest_value", np.float32), ("loop_id", np.int32), ("status", np.int32)])
+
+
 def library_path() -> Path:
     return _build.LIB
 
@@ -170,6 +189,13 @@ SIGNATURES = {
     "lcd_map_detect_async": (_I, [_P, _P, _I, _I, _I, _P, _I, _P]),
     "lcd_map_frame": (_I, [_P, _I, _I, _F, _I, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     "lcd_verify_top_dev": (_I, [_P, _P, _P, _I, _I, _P, _P, _I, _P, _P]),
+    "lcd_clients_create": (_I, [_P, _I]),
+    "lcd_clients_reset": (_I, [_P, _P, _I]),
+    "lcd_clients_set_map": (_I, [_P, _P, _I, _P, _P, _P, _P, _I, _F]),
+    "lcd_decide_batch_dev": (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _P]),
+    "lcd_decide_fetch": (_I, [_P, _I, _P]),
+    "lcd_verify_decided_dev": (_I, [_P, _P, _P, _I, _I, _P, _P]),
+    "lcd_process_decide_batch_dev": (_I, [_P, _P, _P, _I, _I, _I, _F, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P]),
     "lcd_shard_set_row_offset": (_I, [_P, _I]),
     "lcd_shard_knn2_keys_dev": (_I, [_P, _P, _I, _P, _P]),
     "lcd_shard_resolve_score_dev": (_I, [_P, _P, _I, _I, _P, _I, _P, _I, _I, _I, _F, _I, _P, _I, _I, _P, _P, _P]),
@@ -846,6 +872,67 @@ class Engine:
         """lcd_verify_result records written by process_fetch_async into a uint8 array -> the dictionaries process_fetch returns"""
         res = (VerifyResult * n_frames).from_buffer_copy(buf[: n_frames * C.sizeof(VerifyResult)].tobytes())
         return Engine._results(res, n_frames)
+
+    # -- the loop-closure decision of many localisation clients ----------------------------------------------------
+    @staticmethod
+    def decide_params(virtual_place_ratio: int = 0, loop_thr: float = 0.11, aggressive_loop_thr: float = 0.05, loop_ratio: float = 0.0,
+                      max_loop_closure_distance: float = 0.0) -> DecideParams:
+        """lcd_decide_params with the reference's defaults."""
+        return DecideParams(int(virtual_place_ratio), float(loop_thr), float(aggressive_loop_thr), float(loop_ratio), float(max_loop_closure_distance))
+
+    def clients_create(self, n_clients: int):
+        """State for n_clients localisation clients, all empty (BayesFilter::reset, last highest hypothesis (0, 0)); again: resets all."""
+        self._check(self._lib.lcd_clients_create(self._h, int(n_clients)))
+
+    def clients_reset(self, clients):
+        """BayesFilter::reset and last highest hypothesis (0, 0) for the listed clients."""
+        c = _i32(clients)
+        self._check(self._lib.lcd_clients_reset(self._h, _ptr(c), len(c)))
+
+    def clients_set_map(self, ids, col_ptr, nbr_row, nbr_level, prediction_lc, virtual_place_prior: float = 0.9):
+        """The map every client localises against: ids ascending with ids[0] the virtual place, neighbour tables and Bayes/PredictionLC as
+        bayes_compute_posterior takes them.  The prediction's columns are computed once here."""
+        i = _i32(ids)
+        cp = np.ascontiguousarray(col_ptr, np.int64)
+        r = _i32(nbr_row)
+        lv = _i32(nbr_level)
+        lc = np.ascontiguousarray(prediction_lc, np.float64)
+        self._check(self._lib.lcd_clients_set_map(self._h, _ptr(i), len(i), _ptr(cp), _ptr(r), _ptr(lv), _ptr(lc), len(lc), float(virtual_place_prior)))
+
+    def decide_batch_dev(self, d_likelihood: int, n_frames: int, ns: int, clients, frame_flags, dp: DecideParams, d_posterior_out: int = 0,
+                         stream: int = 0):
+        """adjustLikelihood + the posterior of each frame's client + Rtabmap::process's hypothesis selection and checks, for raw likelihood
+        rows d_likelihood[n_frames][ns] on the device; d_posterior_out[n_frames][ns+1] or 0.  clients / frame_flags: one per frame (host)."""
+        c = _i32(clients)
+        f = _i32(frame_flags)
+        if len(c) != n_frames or len(f) != n_frames:
+            raise LcdError(-1, f"clients and frame_flags need {n_frames} entries")
+        self._check(self._lib.lcd_decide_batch_dev(self._h, C.c_void_p(d_likelihood), int(n_frames), int(ns), _ptr(c), _ptr(f), C.byref(dp),
+                                                    C.c_void_p(d_posterior_out or None), C.c_void_p(stream or None)))
+
+    def decide_fetch(self, n_frames: int) -> np.ndarray:
+        """The last decision's lcd_decision records as a structured array (highest_id, highest_value, loop_id, status)."""
+        out = np.zeros(n_frames, DECISION_DTYPE)
+        self._check(self._lib.lcd_decide_fetch(self._h, int(n_frames), _ptr(out)))
+        return out
+
+    def verify_decided_dev(self, d_queries: int, d_uv: int, n_frames: int, nq: int, vp: "VerifyParams", stream: int = 0):
+        """Memory::computeTransform of the accepted hypotheses of the last decision, and the verification / distance rejections."""
+        self._check(self._lib.lcd_verify_decided_dev(self._h, C.c_void_p(d_queries), C.c_void_p(d_uv), int(n_frames), int(nq), C.byref(vp),
+                                                      C.c_void_p(stream or None)))
+
+    def process_decide_batch_dev(self, d_queries: int, d_uv: int, n_frames: int, nq: int, ns: int, n_total: int, vp: "VerifyParams", clients,
+                                 frame_flags, dp: DecideParams, d_words_out: int = 0, d_like_out: int = 0, d_posterior_out: int = 0,
+                                 incremental: bool = True, nndr: float = 0.8, cmp_new: bool = True, stream: int = 0):
+        """Quantise + score against the map's real places, decide, verify the accepted hypotheses (binary, unsharded engines)."""
+        c = _i32(clients)
+        f = _i32(frame_flags)
+        if len(c) != n_frames or len(f) != n_frames:
+            raise LcdError(-1, f"clients and frame_flags need {n_frames} entries")
+        self._check(self._lib.lcd_process_decide_batch_dev(self._h, C.c_void_p(d_queries), C.c_void_p(d_uv), int(n_frames), int(nq), int(incremental),
+                                                            float(nndr), int(cmp_new), int(ns), int(n_total), C.byref(vp), _ptr(c), _ptr(f),
+                                                            C.byref(dp), C.c_void_p(d_words_out or None), C.c_void_p(d_like_out or None),
+                                                            C.c_void_p(d_posterior_out or None), C.c_void_p(stream or None)))
 
     # -- word-range sharding ----------------------------------------------------------------------
     @staticmethod

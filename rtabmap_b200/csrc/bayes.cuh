@@ -42,22 +42,28 @@ struct BayesArgs
 	float * post;             // [n] output
 };
 
+// updatePosterior (:712-737) for one place: its value in the last posterior (ids ascending), 0 for a place the last posterior did not
+// have, 1 for every place when the last posterior is empty
+__device__ inline float bayes_rekey(const int * prev_ids, const float * prev_post, int n_prev, int id)
+{
+	float v = n_prev == 0 ? 1.0f : 0.0f;
+	int lo = 0, hi = n_prev;
+	while (lo < hi)
+	{
+		const int mid = (lo + hi) >> 1;
+		if (prev_ids[mid] < id) lo = mid + 1;
+		else hi = mid;
+	}
+	if (lo < n_prev && prev_ids[lo] == id) v = prev_post[lo];
+	return v;
+}
+
 __global__ void bayes_last_kernel(const BayesArgs a)
 {
 	const int r = blockIdx.x * blockDim.x + threadIdx.x;
 	if (r < 3) a.sums[r] = 0.0; // before the bound check: with fewer than 3 places the sums would keep the last call's values
 	if (r >= a.n) return;
-	float v = a.n_prev == 0 ? 1.0f : 0.0f;
-	const int id = a.ids[r];
-	int lo = 0, hi = a.n_prev;
-	while (lo < hi)
-	{
-		const int mid = (lo + hi) >> 1;
-		if (a.prev_ids[mid] < id) lo = mid + 1;
-		else hi = mid;
-	}
-	if (lo < a.n_prev && a.prev_ids[lo] == id) v = a.prev_post[lo];
-	a.last[r] = v;
+	a.last[r] = bayes_rekey(a.prev_ids, a.prev_post, a.n_prev, a.ids[r]);
 	a.prior[r] = 0.0;
 }
 
@@ -88,18 +94,16 @@ __host__ __device__ inline float repeated_fadd(float s, const float value, int t
 	return s;
 }
 
-// one thread per column: addNeighborProb + normalize without materialising the column
-__global__ void bayes_columns_kernel(const BayesArgs a)
+// addNeighborProb + normalize of column c without materialising it: the uniform value of its unlisted rows (after scaling and the
+// epsilon cut), its scale (negative: renormalised, the epsilon cut applies to the listed entries too) and the mass added to its diagonal
+struct BayesColumn
 {
-	const int c = blockIdx.x * blockDim.x + threadIdx.x;
-	if (c >= a.n) return;
-	if (a.ids[c] < 0)
-	{
-		a.col_u[c] = 0.f;
-		a.col_scale[c] = 1.f;
-		a.col_delta[c] = 0.f;
-		return;
-	}
+	float u, scale, delta;
+};
+
+__device__ inline BayesColumn bayes_column(const BayesArgs & a, int c)
+{
+	if (a.ids[c] < 0) return BayesColumn{0.f, 1.f, 0.f};
 	const int first = a.vp_used ? 1 : 0;
 	float s = 0.f;
 	int n_nonzero = 0;
@@ -137,14 +141,46 @@ __global__ void bayes_columns_kernel(const BayesArgs a)
 		scale = __fdiv_rn(max_norm, s);
 		value = __fmul_rn(value, scale);
 		if (value < a.eps) value = 0.f;
-		a.col_scale[c] = -scale; // negative: "renormalised" (the epsilon cut applies to the listed entries too)
+		return BayesColumn{value, -scale, delta};
 	}
-	else a.col_scale[c] = 1.f;
-	a.col_u[c] = value;
-	a.col_delta[c] = delta;
-	if (scale == 1.f && a.col_scale[c] < 0.f) a.col_scale[c] = -1.f;
+	return BayesColumn{value, 1.f, delta};
+}
+
+// P[r][c] of listed entry e (row r of column c), the columns' values already in col_u / col_scale / col_delta
+__device__ inline float bayes_entry_value(const BayesArgs & a, int e, int c, int r)
+{
+	float v = static_cast<float>(a.lc[a.nbr_level[e] + 1]);
+	if (r == c) v = __fadd_rn(v, a.col_delta[c]);
+	const float sc = a.col_scale[c];
+	float pv = v;
+	if (v == 0.f) pv = a.col_u[c]; // a listed neighbour with a zero LC value is filled like any other zero row (already scaled)
+	else if (sc < 0.f)
+	{
+		pv = __fmul_rn(v, -sc);
+		if (pv < a.eps) pv = 0.f;
+	}
+	return pv;
+}
+
+// the virtual-place row and column (:375-411, :482-487): P[0][0], and P[r][0] of every real place r
+__device__ inline float bayes_vp_p00(float vpp, int n) { return vpp > 0.f ? (n > 1 ? vpp : 1.0f) : (n > 1 ? static_cast<float>(1.0 / n) : 1.0f); }
+__device__ inline float bayes_vp_pr0(float vpp, int n)
+{
+	return vpp > 0.f ? static_cast<float>((1.0 - static_cast<double>(vpp)) / (n - 1)) : static_cast<float>(1.0 / n);
+}
+
+// one thread per column: the column's values, and its share of U and of the real places' last-posterior sum
+__global__ void bayes_columns_kernel(const BayesArgs a)
+{
+	const int c = blockIdx.x * blockDim.x + threadIdx.x;
+	if (c >= a.n) return;
+	const BayesColumn col = bayes_column(a, c);
+	a.col_u[c] = col.u;
+	a.col_scale[c] = col.scale;
+	a.col_delta[c] = col.delta;
+	if (a.ids[c] < 0) return;
 	// U: the uniform part of this column reaches every row >= first
-	const double up = static_cast<double>(value) * static_cast<double>(a.last[c]);
+	const double up = static_cast<double>(col.u) * static_cast<double>(a.last[c]);
 	if (up != 0.0) atomicAdd(&a.sums[0], up);
 	atomicAdd(&a.sums[1], static_cast<double>(a.last[c]));
 }
@@ -158,17 +194,7 @@ __global__ void bayes_scatter_kernel(const BayesArgs a, int nnz, const int * __r
 	const int r = a.nbr_row[e];
 	const int first = a.vp_used ? 1 : 0;
 	if (r < first) return; // the virtual-place row is set by the model, not by neighbours
-	float v = static_cast<float>(a.lc[a.nbr_level[e] + 1]);
-	if (r == c) v = __fadd_rn(v, a.col_delta[c]);
-	const float sc = a.col_scale[c];
-	float pv = v;
-	const bool was_zero = v == 0.f;
-	if (was_zero) pv = a.col_u[c]; // a listed neighbour with a zero LC value is filled like any other zero row (already scaled)
-	else if (sc < 0.f)
-	{
-		pv = __fmul_rn(v, -sc);
-		if (pv < a.eps) pv = 0.f;
-	}
+	const float pv = bayes_entry_value(a, e, c, r);
 	const double d = (static_cast<double>(pv) - static_cast<double>(a.col_u[c])) * static_cast<double>(a.last[c]);
 	if (d != 0.0) atomicAdd(&a.prior[r], d);
 }
@@ -187,7 +213,7 @@ __global__ void bayes_update_kernel(const BayesArgs a)
 		if (a.vp_used && r == 0)
 		{
 			// row 0: P[0][0] = vpp (or 1 for a single place, or 1/n when vpp == 0), P[0][c] = lc[0] for every real place
-			float p00 = a.vpp > 0.f ? (a.n > 1 ? a.vpp : 1.0f) : (a.n > 1 ? static_cast<float>(1.0 / a.n) : 1.0f);
+			const float p00 = bayes_vp_p00(a.vpp, a.n);
 			prior = static_cast<double>(p00) * last0 + static_cast<double>(static_cast<float>(a.lc[0])) * a.sums[1]; // sums[1]: real places only
 		}
 		else
@@ -195,7 +221,7 @@ __global__ void bayes_update_kernel(const BayesArgs a)
 			prior = a.prior[r] + a.sums[0];
 			if (a.vp_used)
 			{
-				const float pr0 = a.vpp > 0.f ? static_cast<float>((1.0 - static_cast<double>(a.vpp)) / (a.n - 1)) : static_cast<float>(1.0 / a.n);
+				const float pr0 = bayes_vp_pr0(a.vpp, a.n);
 				prior += static_cast<double>(pr0) * last0;
 			}
 			(void)first;

@@ -19,6 +19,7 @@
 #include "score.cuh"
 #include "similarity.cuh"
 #include "bayes.cuh"
+#include "decide.cuh"
 #include "verify.cuh"
 #include "match_bf.cuh"
 #include "orb.cuh"
@@ -34,6 +35,8 @@
 #include <cstdlib>
 #include <cstring>
 #include <functional>
+#include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <unordered_map>
@@ -306,6 +309,40 @@ struct lcd_engine
 	DevBuf<float> by_like, by_last, by_u, by_scale, by_delta, by_post, by_state_post;
 	DevBuf<double> by_lc, by_prior, by_sums;
 	int by_n_state = 0;
+	// the loop-closure decision of many localisation clients against one map (lcd_clients_* / lcd_decide_*, decide.cuh)
+	struct MapVersion
+	{
+		DevBuf<int> ids; // ascending place ids, ids[0] = the virtual place
+		int n = 0;
+	};
+	std::map<int, std::unique_ptr<MapVersion>> dc_versions; // the current map and every map whose ids a client's last posterior is keyed to
+	int dc_map_ver = -1, dc_next_ver = 0, dc_n = 0;
+	struct MapTables
+	{
+		DevBuf<float> u;      // [n] uniform value of every column of the prediction
+		DevBuf<int> tptr;     // [n+1] listed entries by row
+		DevBuf<int> tcol;     // [nt] their columns
+		DevBuf<double> tval;  // [nt] P[r][c] - u_c
+	};
+	std::unique_ptr<MapTables> dc_tables; // the current map's; replaced as a whole by lcd_clients_set_map
+	double dc_lc0 = 0.0;
+	float dc_vpp = 0.f;
+	int dc_clients = 0;
+	std::vector<int> dc_ver;              // per client: the map version its last posterior is keyed to (-1 = empty state)
+	DevBuf<float> dc_post;                // [client][dc_stride] last posterior of every client
+	size_t dc_stride = 0;
+	DevBuf<int> dc_hi_id;                 // [client] last highest hypothesis
+	DevBuf<float> dc_hi_val;
+	PinBuf<long long> dc_h_tab;           // per-call frame tables, staged for the upload
+	cudaEvent_t dc_h_ev = nullptr;        // the last upload from dc_h_tab
+	DevBuf<long long> dc_tab;
+	std::vector<int> dc_active;           // clients whose posterior the call being launched computes
+	DevBuf<float> dc_adj, dc_last_t, dc_post_t;
+	DevBuf<double> dc_part_u, dc_part_s1, dc_part_p, dc_sums;
+	DevBuf<Decision> dc_dec;
+	int dc_last_frames = 0;               // frames of the last decision (0: none)
+	bool dc_hyp_valid = false;            // d_hyp_id / d_hyp_slot hold the last decision's accepted hypotheses
+	float dc_max_dist = 0.f;              // RGBD/MaxLoopClosureDistance of the last decision
 	// verification scratch
 	DevBuf<uint32_t> v_df, v_dt;
 	DevBuf<float> v_xyz, v_uv, v_obj, v_img, v_T, v_xyz_to, v_obj_to;
@@ -1253,6 +1290,7 @@ void lcd_destroy(lcd_engine * e)
 		if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
 		for (cudaEvent_t ev : e->copy_events) cudaEventDestroy(ev);
 		if (e->copy_fence) cudaEventDestroy(e->copy_fence);
+		if (e->dc_h_ev) cudaEventDestroy(e->dc_h_ev);
 		for (int i = 0; i < 4; ++i)
 		{
 			if (e->aux_stream[i]) cudaStreamDestroy(e->aux_stream[i]);
@@ -1913,12 +1951,12 @@ int lcd_bayes_reset(lcd_engine * e)
 	return LCD_OK;
 }
 
-int lcd_bayes_compute_posterior(lcd_engine * e, const int * ids, const float * likelihood, int n, const int64_t * col_ptr, const int * nbr_row,
-                                const int * nbr_level, const double * prediction_lc, int n_lc, float virtual_place_prior, float * posterior_out)
+// The checks lcd_bayes_compute_posterior and lcd_clients_set_map share, and what they derive: cp = col_ptr as int, ecol = the column of every
+// listed entry, total / eps = _totalPredictionLCValues / _predictionEpsilon.
+static int check_bayes_tables(lcd_engine * e, const int * ids, int n, const int64_t * col_ptr, const int * nbr_row, const int * nbr_level,
+                              const double * prediction_lc, int n_lc, float virtual_place_prior, std::vector<int> & cp, std::vector<int> & ecol,
+                              float & total, double & eps)
 {
-	if (!e) return LCD_ERR_INVALID;
-	LCD_TRY(set_device(e));
-	if (!ids || !likelihood || n <= 0 || !posterior_out) LCD_FAIL(e, LCD_ERR_INVALID, "likelihood is empty!");
 	if (!prediction_lc || n_lc < 2) LCD_FAIL(e, LCD_ERR_INVALID, "Prediction is not valid!");
 	if (!col_ptr) LCD_FAIL(e, LCD_ERR_INVALID, "null neighbour table");
 	if (!(virtual_place_prior >= 0.f && virtual_place_prior <= 1.f)) LCD_FAIL(e, LCD_ERR_INVALID, "Bayes/VirtualPlacePriorThr must be in [0, 1]");
@@ -1927,7 +1965,8 @@ int lcd_bayes_compute_posterior(lcd_engine * e, const int * ids, const float * l
 	if (ids[0] == 0) LCD_FAIL(e, LCD_ERR_INVALID, "id 0 is invalid");
 	const int64_t nnz = col_ptr[n];
 	if (col_ptr[0] != 0 || nnz < 0 || nnz > 0x7FFFFFFF) LCD_FAIL(e, LCD_ERR_INVALID, "bad neighbour table");
-	std::vector<int> cp(n + 1), ecol(static_cast<size_t>(nnz));
+	cp.assign(n + 1, 0);
+	ecol.assign(static_cast<size_t>(nnz), 0);
 	for (int c = 0; c < n; ++c)
 	{
 		if (col_ptr[c + 1] < col_ptr[c]) LCD_FAIL(e, LCD_ERR_INVALID, "col_ptr must be non-decreasing");
@@ -1946,8 +1985,7 @@ int lcd_bayes_compute_posterior(lcd_engine * e, const int * ids, const float * l
 	}
 	cp[n] = static_cast<int>(nnz);
 	// _totalPredictionLCValues / _predictionEpsilon as setPredictionLC computes them (float sum of the doubles, smallest value)
-	float total = 0.f;
-	double eps = prediction_lc[0];
+	eps = prediction_lc[0];
 	for (int j = 0; j < n_lc; ++j)
 	{
 		if (prediction_lc[j] < 0.0 || prediction_lc[j] > 1.0) LCD_FAIL(e, LCD_ERR_INVALID, "The prediction is not valid (values must be between >0 && <=1)");
@@ -1955,6 +1993,20 @@ int lcd_bayes_compute_posterior(lcd_engine * e, const int * ids, const float * l
 	}
 	total = 0.f;
 	for (int j = 0; j < n_lc; ++j) total = static_cast<float>(static_cast<double>(total) + prediction_lc[j]); // float += double
+	return LCD_OK;
+}
+
+int lcd_bayes_compute_posterior(lcd_engine * e, const int * ids, const float * likelihood, int n, const int64_t * col_ptr, const int * nbr_row,
+                                const int * nbr_level, const double * prediction_lc, int n_lc, float virtual_place_prior, float * posterior_out)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (!ids || !likelihood || n <= 0 || !posterior_out) LCD_FAIL(e, LCD_ERR_INVALID, "likelihood is empty!");
+	std::vector<int> cp, ecol;
+	float total = 0.f;
+	double eps = 0.0;
+	LCD_TRY(check_bayes_tables(e, ids, n, col_ptr, nbr_row, nbr_level, prediction_lc, n_lc, virtual_place_prior, cp, ecol, total, eps));
+	const int64_t nnz = col_ptr[n];
 	cudaStream_t s = e->stream;
 	const size_t nz = static_cast<size_t>(std::max<int64_t>(nnz, 1));
 	LCD_CUDA(e, e->by_ids.reserve(n, 0, false, s));
@@ -3276,6 +3328,7 @@ static int verify_top_dev(lcd_engine * e, const uint32_t * d_q, const float * d_
 	if (e->st_cap == 0) LCD_FAIL(e, LCD_ERR_STATE, "the signature store is empty: nothing to verify against");
 	LCD_CUDA(e, e->d_hyp_id.reserve(n_frames, 0, false, s));
 	LCD_CUDA(e, e->d_hyp_slot.reserve(n_frames, 0, false, s));
+	e->dc_hyp_valid = false; // the arg-max replaces the hypotheses of the last decision
 	argmax_hypothesis_kernel<<<n_frames, 256, 0, s>>>(d_like, ns, d_sig_ids, e->st_slot_of_sig.p, static_cast<int>(e->h_slot_of_sig.size()),
 	                                                  e->d_hyp_id.p, e->d_hyp_slot.p);
 	LCD_CHECK_LAUNCH(e);
@@ -3622,6 +3675,412 @@ int lcd_process_batch(lcd_engine * e, const void * queries, const float * uv, in
 	if (results) return verify_download(e, n_frames, 0, results, nullptr, nullptr, s);
 	LCD_CUDA(e, cudaStreamSynchronize(s));
 	return LCD_OK;
+}
+
+// ---- the loop-closure decision of many localisation clients (decide.cuh) -----------------------------------------
+static_assert(sizeof(Decision) == sizeof(lcd_decision), "decision layout");
+
+// drop the map versions that neither the current map nor any client's last posterior uses (the device must be idle)
+static void prune_map_versions(lcd_engine * e)
+{
+	for (auto it = e->dc_versions.begin(); it != e->dc_versions.end();)
+	{
+		const int v = it->first;
+		const bool held = v == e->dc_map_ver || std::find(e->dc_ver.begin(), e->dc_ver.end(), v) != e->dc_ver.end();
+		it = held ? std::next(it) : e->dc_versions.erase(it);
+	}
+}
+
+int lcd_clients_create(lcd_engine * e, int n_clients)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (n_clients <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "n_clients must be > 0");
+	LCD_CUDA(e, cudaDeviceSynchronize());
+	cudaStream_t s = e->stream;
+	const size_t n = static_cast<size_t>(n_clients);
+	if (e->dc_hi_id.reserve(n, 0, false, s) != cudaSuccess || e->dc_hi_val.reserve(n, 0, false, s) != cudaSuccess ||
+	    (e->dc_stride && e->dc_post.reserve(n * e->dc_stride, 0, false, s) != cudaSuccess))
+	{
+		cudaGetLastError();
+		e->dc_clients = 0;
+		e->dc_ver.clear();
+		LCD_FAIL(e, LCD_ERR_CAPACITY, "no device memory for the state of %d clients", n_clients);
+	}
+	LCD_CUDA(e, cudaMemsetAsync(e->dc_hi_id.p, 0, n * sizeof(int), s));
+	LCD_CUDA(e, cudaMemsetAsync(e->dc_hi_val.p, 0, n * sizeof(float), s));
+	LCD_CUDA(e, cudaStreamSynchronize(s));
+	e->dc_clients = n_clients;
+	e->dc_ver.assign(n, -1);
+	e->dc_last_frames = 0;
+	e->dc_hyp_valid = false;
+	prune_map_versions(e);
+	return LCD_OK;
+}
+
+int lcd_clients_reset(lcd_engine * e, const int * clients, int n)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (e->dc_clients <= 0) LCD_FAIL(e, LCD_ERR_STATE, "no clients: call lcd_clients_create first");
+	if (n <= 0) return LCD_OK;
+	if (!clients) LCD_FAIL(e, LCD_ERR_INVALID, "null client list");
+	for (int i = 0; i < n; ++i)
+		if (clients[i] < 0 || clients[i] >= e->dc_clients) LCD_FAIL(e, LCD_ERR_INVALID, "client %d is out of range [0, %d)", clients[i], e->dc_clients);
+	LCD_CUDA(e, cudaDeviceSynchronize());
+	cudaStream_t s = e->stream;
+	LCD_CUDA(e, e->d_i1.reserve(n, 0, false, s));
+	LCD_CUDA(e, cudaMemcpyAsync(e->d_i1.p, clients, n * sizeof(int), cudaMemcpyHostToDevice, s));
+	decide_reset_clients_kernel<<<(n + 255) / 256, 256, 0, s>>>(e->d_i1.p, n, e->dc_hi_id.p, e->dc_hi_val.p);
+	LCD_CHECK_LAUNCH(e);
+	LCD_CUDA(e, cudaStreamSynchronize(s));
+	for (int i = 0; i < n; ++i) e->dc_ver[clients[i]] = -1;
+	prune_map_versions(e);
+	return LCD_OK;
+}
+
+int lcd_clients_set_map(lcd_engine * e, const int * ids, int n, const int64_t * col_ptr, const int * nbr_row, const int * nbr_level,
+                        const double * prediction_lc, int n_lc, float virtual_place_prior)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (!ids || n <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "ids list is empty");
+	if (ids[0] >= 0) LCD_FAIL(e, LCD_ERR_INVALID, "ids[0] must be the virtual place (a negative id): the working memory always holds it");
+	std::vector<int> cp, ecol;
+	float total = 0.f;
+	double eps = 0.0;
+	LCD_TRY(check_bayes_tables(e, ids, n, col_ptr, nbr_row, nbr_level, prediction_lc, n_lc, virtual_place_prior, cp, ecol, total, eps));
+	const int64_t nnz = col_ptr[n];
+	// the listed entries by row: row r gathers (P[r][c] - u_c) last[c] over the columns c that list it, in ascending c
+	std::vector<int> tptr(n + 1, 0);
+	for (int64_t k = 0; k < nnz; ++k)
+		if (nbr_row[k] >= 1) ++tptr[nbr_row[k] + 1];
+	for (int r = 0; r < n; ++r) tptr[r + 1] += tptr[r];
+	const int nt = tptr[n];
+	std::vector<int> tentry(std::max(nt, 1)), tcol(std::max(nt, 1)), fill(tptr.begin(), tptr.end() - 1);
+	for (int64_t k = 0; k < nnz; ++k)
+	{
+		const int r = nbr_row[k];
+		if (r < 1) continue;
+		tentry[fill[r]] = static_cast<int>(k);
+		tcol[fill[r]++] = ecol[static_cast<size_t>(k)];
+	}
+	// Everything the new map needs is built in new buffers; the engine switches to it only after the last step that can fail, so a failed
+	// call leaves the previous map (or no map) in place.  The single-client path's per-call buffers serve as scratch for the column pass.
+	cudaStream_t s = e->stream;
+	auto ver = std::make_unique<lcd_engine::MapVersion>();
+	auto tab = std::make_unique<lcd_engine::MapTables>();
+	ver->n = n;
+	DevBuf<double> d_lc;
+	DevBuf<int> d_tentry;
+	const size_t nz = static_cast<size_t>(std::max<int64_t>(nnz, 1)), ntz = static_cast<size_t>(std::max(nt, 1));
+	// the scratch buffers below may be in use by queued work of the single-client path
+	LCD_CUDA(e, cudaStreamSynchronize(s));
+	if (ver->ids.reserve(n, 0, false, s) != cudaSuccess || e->by_colptr.reserve(n + 1, 0, false, s) != cudaSuccess ||
+	    e->by_row.reserve(nz, 0, false, s) != cudaSuccess || e->by_level.reserve(nz, 0, false, s) != cudaSuccess ||
+	    e->by_scale.reserve(n, 0, false, s) != cudaSuccess || e->by_delta.reserve(n, 0, false, s) != cudaSuccess ||
+	    d_lc.reserve(n_lc, 0, false, s) != cudaSuccess || d_tentry.reserve(ntz, 0, false, s) != cudaSuccess ||
+	    tab->u.reserve(n, 0, false, s) != cudaSuccess || tab->tptr.reserve(n + 1, 0, false, s) != cudaSuccess ||
+	    tab->tcol.reserve(ntz, 0, false, s) != cudaSuccess || tab->tval.reserve(ntz, 0, false, s) != cudaSuccess)
+	{
+		cudaGetLastError();
+		LCD_FAIL(e, LCD_ERR_CAPACITY, "no device memory for a map of %d places and %d listed entries", n, nt);
+	}
+	LCD_CUDA(e, cudaMemcpyAsync(ver->ids.p, ids, n * sizeof(int), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, cudaMemcpyAsync(e->by_colptr.p, cp.data(), (n + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
+	if (nnz)
+	{
+		LCD_CUDA(e, cudaMemcpyAsync(e->by_row.p, nbr_row, nnz * sizeof(int), cudaMemcpyHostToDevice, s));
+		LCD_CUDA(e, cudaMemcpyAsync(e->by_level.p, nbr_level, nnz * sizeof(int), cudaMemcpyHostToDevice, s));
+	}
+	LCD_CUDA(e, cudaMemcpyAsync(d_lc.p, prediction_lc, n_lc * sizeof(double), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, cudaMemcpyAsync(tab->tptr.p, tptr.data(), (n + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
+	if (nt)
+	{
+		LCD_CUDA(e, cudaMemcpyAsync(d_tentry.p, tentry.data(), nt * sizeof(int), cudaMemcpyHostToDevice, s));
+		LCD_CUDA(e, cudaMemcpyAsync(tab->tcol.p, tcol.data(), nt * sizeof(int), cudaMemcpyHostToDevice, s));
+	}
+	BayesArgs a{};
+	a.n = n;
+	a.vp_used = 1;
+	a.ids = ver->ids.p;
+	a.col_ptr = e->by_colptr.p;
+	a.nbr_row = e->by_row.p;
+	a.nbr_level = e->by_level.p;
+	a.lc = d_lc.p;
+	a.n_lc = n_lc;
+	a.total = total;
+	a.eps = static_cast<float>(eps);
+	a.vpp = virtual_place_prior;
+	a.col_u = tab->u.p;
+	a.col_scale = e->by_scale.p;
+	a.col_delta = e->by_delta.p;
+	decide_map_columns_kernel<<<(n + 255) / 256, 256, 0, s>>>(a);
+	LCD_CHECK_LAUNCH(e);
+	if (nt)
+	{
+		decide_entry_values_kernel<<<(nt + 255) / 256, 256, 0, s>>>(a, nt, d_tentry.p, tab->tcol.p, tab->tval.p);
+		LCD_CHECK_LAUNCH(e);
+	}
+	// the clients' posteriors keep their ids (re-keyed when each client next computes); their rows grow to the largest map
+	DevBuf<float> grown;
+	const size_t stride = std::max(e->dc_stride, static_cast<size_t>(n));
+	if (stride > e->dc_stride && e->dc_clients > 0)
+	{
+		if (grown.reserve(static_cast<size_t>(e->dc_clients) * stride, 0, false, s) != cudaSuccess)
+		{
+			cudaGetLastError();
+			LCD_FAIL(e, LCD_ERR_CAPACITY, "no device memory for the posteriors of %d clients over %d places", e->dc_clients, n);
+		}
+		// kernels of the last decision (on any stream) may still write the posteriors being copied
+		LCD_CUDA(e, cudaDeviceSynchronize());
+		if (e->dc_stride)
+			LCD_CUDA(e, cudaMemcpy2DAsync(grown.p, stride * sizeof(float), e->dc_post.p, e->dc_stride * sizeof(float), e->dc_stride * sizeof(float),
+			                              e->dc_clients, cudaMemcpyDeviceToDevice, s));
+	}
+	LCD_CUDA(e, cudaStreamSynchronize(s));
+	// kernels of the last decision may still read the tables this call replaces
+	LCD_CUDA(e, cudaDeviceSynchronize());
+	// commit: nothing below can fail
+	if (grown.p)
+	{
+		std::swap(grown.p, e->dc_post.p);
+		std::swap(grown.cap, e->dc_post.cap);
+	}
+	e->dc_stride = stride;
+	e->dc_tables = std::move(tab);
+	e->dc_map_ver = e->dc_next_ver++;
+	e->dc_versions[e->dc_map_ver] = std::move(ver);
+	e->dc_n = n;
+	e->dc_lc0 = prediction_lc[0];
+	e->dc_vpp = virtual_place_prior;
+	prune_map_versions(e);
+	return LCD_OK;
+}
+
+static int check_decide_params(lcd_engine * e, const lcd_decide_params * dp)
+{
+	if (!dp) LCD_FAIL(e, LCD_ERR_INVALID, "null decision parameters");
+	if (dp->virtual_place_ratio != 0 && dp->virtual_place_ratio != 1) LCD_FAIL(e, LCD_ERR_INVALID, "Rtabmap/VirtualPlaceLikelihoodRatio must be 0 or 1");
+	if (!(dp->loop_thr >= 0.f && dp->loop_thr <= 1.f)) LCD_FAIL(e, LCD_ERR_INVALID, "Rtabmap/LoopThr must be in [0, 1]");
+	if (!(dp->aggressive_loop_thr >= 0.f && dp->aggressive_loop_thr <= 1.f)) LCD_FAIL(e, LCD_ERR_INVALID, "RGBD/AggressiveLoopThr must be in [0, 1]");
+	if (!(dp->loop_ratio >= 0.f && dp->loop_ratio <= 1.f)) LCD_FAIL(e, LCD_ERR_INVALID, "Rtabmap/LoopRatio must be in [0, 1]");
+	if (!(dp->max_loop_closure_distance >= 0.f && std::isfinite(dp->max_loop_closure_distance)))
+		LCD_FAIL(e, LCD_ERR_INVALID, "RGBD/MaxLoopClosureDistance must be >= 0");
+	return LCD_OK;
+}
+
+// checks of one decision call and the upload of its frame tables (before any kernel of the call is queued)
+static int decide_prepare(lcd_engine * e, int n_frames, int ns, const int * clients, const int * frame_flags, const lcd_decide_params * dp,
+                          cudaStream_t s)
+{
+	if (e->dc_clients <= 0) LCD_FAIL(e, LCD_ERR_STATE, "no clients: call lcd_clients_create first");
+	if (e->dc_map_ver < 0) LCD_FAIL(e, LCD_ERR_STATE, "no map: call lcd_clients_set_map first");
+	LCD_TRY(check_decide_params(e, dp));
+	if (n_frames <= 0 || !clients || !frame_flags) LCD_FAIL(e, LCD_ERR_INVALID, "no frames");
+	if (ns <= 0 || ns != e->dc_n - 1) LCD_FAIL(e, LCD_ERR_INVALID, "ns = %d, but the map holds %d real places", ns, e->dc_n - 1);
+	std::vector<char> seen(e->dc_clients, 0);
+	e->dc_active.clear();
+	for (int f = 0; f < n_frames; ++f)
+	{
+		const int c = clients[f];
+		if (c < 0 || c >= e->dc_clients) LCD_FAIL(e, LCD_ERR_INVALID, "client %d of frame %d is out of range [0, %d)", c, f, e->dc_clients);
+		if (seen[c]) LCD_FAIL(e, LCD_ERR_INVALID, "client %d appears more than once in one call", c);
+		seen[c] = 1;
+		if (!(frame_flags[f] & (kDcFlagSkip | kDcFlagHold))) e->dc_active.push_back(f);
+	}
+	const int B = static_cast<int>(e->dc_active.size());
+	const size_t words = 2 * static_cast<size_t>(n_frames) + 4 * static_cast<size_t>(B);
+	if (!e->dc_h_ev) LCD_CUDA(e, cudaEventCreateWithFlags(&e->dc_h_ev, cudaEventDisableTiming));
+	else LCD_CUDA(e, cudaEventSynchronize(e->dc_h_ev)); // the staging buffer of the last call has been copied
+	LCD_CUDA(e, e->dc_h_tab.reserve(words));
+	long long * h = e->dc_h_tab.p;
+	for (int f = 0; f < n_frames; ++f)
+	{
+		h[f] = clients[f];
+		h[n_frames + f] = frame_flags[f];
+	}
+	long long * hb = h + 2 * n_frames;
+	for (int b = 0; b < B; ++b)
+	{
+		const int f = e->dc_active[b], c = clients[f], v = e->dc_ver[c];
+		const lcd_engine::MapVersion * mv = v >= 0 ? e->dc_versions.at(v).get() : nullptr;
+		hb[b] = f;
+		hb[B + b] = c;
+		hb[2 * B + b] = mv ? mv->n : 0;
+		hb[3 * B + b] = static_cast<long long>(reinterpret_cast<uintptr_t>(mv ? mv->ids.p : nullptr));
+		e->dc_active[b] = c;
+	}
+	LCD_CUDA(e, e->dc_tab.reserve(words, 0, false, s));
+	LCD_CUDA(e, cudaMemcpyAsync(e->dc_tab.p, h, words * sizeof(long long), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, cudaEventRecord(e->dc_h_ev, s));
+	return LCD_OK;
+}
+
+// adjustLikelihood, the posterior of every frame that computes one, the hypothesis selection and checks
+static int decide_launch(lcd_engine * e, const float * d_like, int n_frames, int ns, const lcd_decide_params * dp, float * d_post_out, cudaStream_t s)
+{
+	const int n = e->dc_n, B = static_cast<int>(e->dc_active.size());
+	const lcd_engine::MapTables & t = *e->dc_tables;
+	DecideMap m{n, e->dc_versions.at(e->dc_map_ver)->ids.p, t.u.p, t.tptr.p, t.tcol.p, t.tval.p, e->dc_lc0, e->dc_vpp};
+	const long long * tab = e->dc_tab.p;
+	LCD_CUDA(e, e->dc_adj.reserve(static_cast<size_t>(n_frames) * n, 0, false, s));
+	adjust_likelihood_kernel<<<n_frames, kAdjustThreads, 0, s>>>(d_like, ns, dp->virtual_place_ratio, e->dc_adj.p);
+	LCD_CHECK_LAUNCH(e);
+	if (B > 0)
+	{
+		const int n_cc = (n + kDcColChunk - 1) / kDcColChunk, n_rc = (n + kDcRowChunk - 1) / kDcRowChunk;
+		const size_t nb = static_cast<size_t>(n) * B;
+		LCD_CUDA(e, e->dc_last_t.reserve(nb, 0, false, s));
+		LCD_CUDA(e, e->dc_post_t.reserve(nb, 0, false, s));
+		LCD_CUDA(e, e->dc_part_u.reserve(static_cast<size_t>(n_cc) * B, 0, false, s));
+		LCD_CUDA(e, e->dc_part_s1.reserve(static_cast<size_t>(n_cc) * B, 0, false, s));
+		LCD_CUDA(e, e->dc_part_p.reserve(static_cast<size_t>(n_rc) * B, 0, false, s));
+		LCD_CUDA(e, e->dc_sums.reserve(3 * static_cast<size_t>(B), 0, false, s));
+		DecideBatch d{};
+		d.B = B;
+		d.frame = tab + 2 * n_frames;
+		d.client = d.frame + B;
+		d.prev_n = d.client + B;
+		d.prev_ids = d.prev_n + B;
+		d.cl_post = e->dc_post.p;
+		d.stride = static_cast<long long>(e->dc_stride);
+		d.adj = e->dc_adj.p;
+		d.last_t = e->dc_last_t.p;
+		d.post_t = e->dc_post_t.p;
+		d.part_u = e->dc_part_u.p;
+		d.part_s1 = e->dc_part_s1.p;
+		d.part_p = e->dc_part_p.p;
+		d.u = e->dc_sums.p;
+		d.s1 = e->dc_sums.p + B;
+		d.psum = e->dc_sums.p + 2 * B;
+		const int threads = std::min(kDcThreads, (B + 31) / 32 * 32);
+		decide_last_kernel<<<static_cast<unsigned>((nb + 255) / 256), 256, 0, s>>>(m, d);
+		LCD_CHECK_LAUNCH(e);
+		decide_columns_kernel<<<n_cc, threads, 0, s>>>(m, d);
+		LCD_CHECK_LAUNCH(e);
+		decide_sum_chunks_kernel<<<(B + 127) / 128, 128, 0, s>>>(d.part_u, n_cc, B, d.u);
+		LCD_CHECK_LAUNCH(e);
+		decide_sum_chunks_kernel<<<(B + 127) / 128, 128, 0, s>>>(d.part_s1, n_cc, B, d.s1);
+		LCD_CHECK_LAUNCH(e);
+		decide_rows_kernel<<<n_rc, threads, 0, s>>>(m, d);
+		LCD_CHECK_LAUNCH(e);
+		decide_sum_chunks_kernel<<<(B + 127) / 128, 128, 0, s>>>(d.part_p, n_rc, B, d.psum);
+		LCD_CHECK_LAUNCH(e);
+		decide_normalize_kernel<<<dim3((n + 31) / 32, (B + 31) / 32), dim3(32, 8), 0, s>>>(m, d, e->dc_post.p, d_post_out);
+		LCD_CHECK_LAUNCH(e);
+	}
+	LCD_CUDA(e, e->dc_dec.reserve(n_frames, 0, false, s));
+	LCD_CUDA(e, e->d_hyp_id.reserve(n_frames, 0, false, s));
+	LCD_CUDA(e, e->d_hyp_slot.reserve(n_frames, 0, false, s));
+	DecideSelect a{};
+	a.n_frames = n_frames;
+	a.client = tab;
+	a.flags = tab + n_frames;
+	a.cl_post = e->dc_post.p;
+	a.stride = static_cast<long long>(e->dc_stride);
+	a.hi_id = e->dc_hi_id.p;
+	a.hi_val = e->dc_hi_val.p;
+	a.loop_thr = dp->loop_thr;
+	a.aggressive_loop_thr = dp->aggressive_loop_thr;
+	a.loop_ratio = dp->loop_ratio;
+	a.sig_slot = e->st_slot_of_sig.p;
+	a.slot_cap = e->st_slot_of_sig.p ? static_cast<int>(e->h_slot_of_sig.size()) : 0;
+	a.dec = e->dc_dec.p;
+	a.hyp_id = e->d_hyp_id.p;
+	a.hyp_slot = e->d_hyp_slot.p;
+	decide_select_kernel<<<n_frames, 256, 0, s>>>(m, a);
+	LCD_CHECK_LAUNCH(e);
+	// the clients that computed now hold posteriors keyed to the current map
+	for (int c : e->dc_active) e->dc_ver[c] = e->dc_map_ver;
+	e->dc_last_frames = n_frames;
+	e->dc_hyp_valid = true;
+	e->dc_max_dist = dp->max_loop_closure_distance;
+	return LCD_OK;
+}
+
+int lcd_decide_batch_dev(lcd_engine * e, const float * d_likelihood, int n_frames, int ns, const int * clients, const int * frame_flags,
+                         const lcd_decide_params * dp, float * d_posterior_out, void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (!d_likelihood) LCD_FAIL(e, LCD_ERR_INVALID, "likelihood is empty");
+	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	LCD_TRY(decide_prepare(e, n_frames, ns, clients, frame_flags, dp, s));
+	return decide_launch(e, d_likelihood, n_frames, ns, dp, d_posterior_out, s);
+}
+
+int lcd_decide_fetch(lcd_engine * e, int n_frames, lcd_decision * out)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (!out || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null output");
+	if (e->dc_last_frames == 0) LCD_FAIL(e, LCD_ERR_STATE, "no decision: run lcd_decide_batch_dev first");
+	if (n_frames > e->dc_last_frames) LCD_FAIL(e, LCD_ERR_INVALID, "the last decision has %d frames", e->dc_last_frames);
+	LCD_CUDA(e, cudaDeviceSynchronize());
+	LCD_CUDA(e, cudaMemcpy(out, e->dc_dec.p, n_frames * sizeof(lcd_decision), cudaMemcpyDeviceToHost));
+	return LCD_OK;
+}
+
+// Memory::computeTransform of every accepted hypothesis of the last decision (store slot -1: not verified), then the rejections of
+// Rtabmap.cpp:3156-3167
+static int verify_decided(lcd_engine * e, const uint32_t * d_q, const float * d_uv, int n_frames, int nq, const lcd_verify_params * vp, cudaStream_t s)
+{
+	if (!vp) LCD_FAIL(e, LCD_ERR_INVALID, "null verification parameters");
+	if (vp->iterations > kMaxRansacIters) LCD_FAIL(e, LCD_ERR_CAPACITY, "Vis/Iterations > %d", kMaxRansacIters);
+	if (e->st_cap == 0) LCD_FAIL(e, LCD_ERR_STATE, "the signature store is empty: nothing to verify against");
+	if (e->dc_last_frames == 0 || !e->dc_hyp_valid) LCD_FAIL(e, LCD_ERR_STATE, "no decision to verify: run lcd_decide_batch_dev first");
+	if (n_frames != e->dc_last_frames) LCD_FAIL(e, LCD_ERR_INVALID, "the last decision has %d frames, not %d", e->dc_last_frames, n_frames);
+	const int cap = std::max(e->st_cap, nq);
+	MatchSrc src{e->st_desc.p, e->st_xyz.p, e->st_n.p, e->d_hyp_slot.p, e->st_cap, d_q, d_uv, nullptr, nq, nq, nullptr};
+	LCD_TRY(launch_match(e, n_frames, cap, vp->nndr, false, s, &src));
+	LCD_TRY(launch_pnp(e, n_frames, cap, vp, s));
+	LCD_TRY(launch_second_pass(e, n_frames, cap, vp, s, &src));
+	decide_verified_kernel<<<(n_frames + 127) / 128, 128, 0, s>>>(n_frames, e->v_ok.p, e->v_T.p, e->dc_max_dist, e->dc_dec.p, e->d_hyp_id.p);
+	LCD_CHECK_LAUNCH(e);
+	return LCD_OK;
+}
+
+int lcd_verify_decided_dev(lcd_engine * e, const void * d_queries, const float * d_uv, int n_frames, int nq_per_frame, const lcd_verify_params * vp,
+                           void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(require_binary(e, "lcd_verify_decided_dev"));
+	LCD_TRY(set_device(e));
+	if (!d_queries || !d_uv || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "Descriptors size is null!");
+	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
+	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	return verify_decided(e, static_cast<const uint32_t *>(d_queries), d_uv, n_frames, nq_per_frame, vp, s);
+}
+
+int lcd_process_decide_batch_dev(lcd_engine * e, const void * d_queries, const float * d_uv, int n_frames, int nq_per_frame, int incremental,
+                                 float nndr, int new_words_compared_together, int ns, int n_total, const lcd_verify_params * vp, const int * clients,
+                                 const int * frame_flags, const lcd_decide_params * dp, int * d_word_ids_out, float * d_likelihood_out,
+                                 float * d_posterior_out, void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(require_binary(e, "lcd_process_decide_batch_dev"));
+	LCD_TRY(require_unsharded(e, "lcd_process_decide_batch_dev"));
+	LCD_TRY(set_device(e));
+	if (!d_queries || !d_uv || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "Descriptors size is null!");
+	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
+	if (!vp) LCD_FAIL(e, LCD_ERR_INVALID, "null verification parameters");
+	if (vp->iterations > kMaxRansacIters) LCD_FAIL(e, LCD_ERR_CAPACITY, "Vis/Iterations > %d", kMaxRansacIters);
+	if (e->st_cap == 0) LCD_FAIL(e, LCD_ERR_STATE, "the signature store is empty: nothing to verify against");
+	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	LCD_TRY(decide_prepare(e, n_frames, ns, clients, frame_flags, dp, s));
+	float * d_like = d_likelihood_out;
+	if (!d_like)
+	{
+		LCD_CUDA(e, e->d_like.reserve(static_cast<size_t>(n_frames) * ns, 0, false, s));
+		d_like = e->d_like.p;
+	}
+	const uint32_t * d_q = static_cast<const uint32_t *>(d_queries);
+	const int * d_sig_ids = e->dc_versions.at(e->dc_map_ver)->ids.p + 1; // the map's real places, ascending
+	LCD_TRY(localize_dev(e, d_q, n_frames, nq_per_frame, incremental, nndr, new_words_compared_together, d_sig_ids, ns, n_total, d_word_ids_out,
+	                     d_like, s));
+	LCD_TRY(decide_launch(e, d_like, n_frames, ns, dp, d_posterior_out, s));
+	return verify_decided(e, d_q, d_uv, n_frames, nq_per_frame, vp, s);
 }
 
 // ---- word-range sharding ---------------------------------------------------------------------
