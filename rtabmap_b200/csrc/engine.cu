@@ -356,6 +356,10 @@ struct lcd_engine
 	DevBuf<uint32_t> st_desc;
 	DevBuf<float> st_xyz;
 	DevBuf<int> st_n, st_slot_of_sig;
+	// each row's temporary FROM dictionary of the matching kernel (verify.cuh, from_dict_build_kernel), built on first use for the
+	// (nf, Vis/CorNNDR) of the call: word of each descriptor, creator of each word [slot][st_cap], and what it was built for [slot]
+	DevBuf<uint16_t> st_kof, st_creator;
+	DevBuf<FromDictTag> st_ftag;
 	std::vector<int> h_slot_of_sig, free_slots;
 	int st_cap = 0, st_slots = 0;
 	// global descriptors (SensorData::globalDescriptors(), type 1, one per signature): rows [slot][gd_dim], the signature store's slot scheme
@@ -2803,18 +2807,32 @@ static int launch_match(lcd_engine * e, int n_pairs, int cap, float nndr, bool w
 	a.n_match = e->v_nm.p;
 	a.from_ids = want_ids ? e->v_fid.p : nullptr;
 	a.to_ids = want_ids ? e->v_tid.p : nullptr;
-	const size_t smem = match_smem_bytes(cap, e->nw);
+	// FROM rows of the signature store: their temporary dictionaries are cached next to the store (from_dict_build_kernel)
+	const bool from_store = src && src->from_slot && src->desc_from == e->st_desc.p;
+	FromDictArgs fa{};
+	if (from_store)
+	{
+		a.from_tag = e->st_ftag.p;
+		a.from_kof = e->st_kof.p;
+		a.from_creator = e->st_creator.p;
+		fa = FromDictArgs{src->desc_from, src->n_from, src->from_slot, src->cap_from, std::min(cap, src->cap_from), nndr, e->st_ftag.p, e->st_kof.p, e->st_creator.p};
+	}
+	const size_t smem = match_smem_bytes(cap, e->nw), smem_fd = from_dict_smem_bytes(fa.rows, e->nw);
 	if (smem > static_cast<size_t>(e->smem_optin)) LCD_FAIL(e, LCD_ERR_CAPACITY, "cap %d needs %zu B of shared memory", cap, smem);
-#define LCD_MATCH_CASE(NW_)                                                                                             \
-	case NW_:                                                                                                           \
-	{                                                                                                                   \
-		auto kern = pair_match_kernel<NW_>;                                                                             \
-		if (smem > 48 * 1024)                                                                                           \
-			LCD_CUDA(e, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem))); \
-		prof_mark(e, LCD_PROF_MATCH, s);                                                                                \
-		kern<<<n_pairs, kResolveThreads, smem, s>>>(a);                                                                 \
-		prof_mark(e, LCD_PROF_MATCH, s);                                                                                \
-		break;                                                                                                          \
+#define LCD_MATCH_CASE(NW_)                                                                                                 \
+	case NW_:                                                                                                               \
+	{                                                                                                                       \
+		auto kern = pair_match_kernel<NW_>;                                                                                 \
+		auto kern_fd = from_dict_build_kernel<NW_>;                                                                         \
+		if (smem > 40 * 1024) /* static shared memory counts against the default 48 KB too */                             \
+			LCD_CUDA(e, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));     \
+		if (smem_fd > 40 * 1024)                                                                                            \
+			LCD_CUDA(e, cudaFuncSetAttribute(kern_fd, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_fd))); \
+		prof_mark(e, LCD_PROF_MATCH, s);                                                                                    \
+		if (from_store) kern_fd<<<n_pairs, kResolveThreads, smem_fd, s>>>(fa);                                              \
+		kern<<<n_pairs, kResolveThreads, smem, s>>>(a);                                                                     \
+		prof_mark(e, LCD_PROF_MATCH, s);                                                                                    \
+		break;                                                                                                              \
 	}
 	switch (e->nw)
 	{
@@ -3263,12 +3281,17 @@ int lcd_sig_add_batch(lcd_engine * e, const int * sig_ids, int n_sigs, int cap, 
 	LCD_CUDA(e, e->st_desc.reserve(static_cast<size_t>(e->st_slots) * cap * e->nw, prev_slots * cap * e->nw, false, s));
 	LCD_CUDA(e, e->st_xyz.reserve(static_cast<size_t>(e->st_slots) * cap * 3, prev_slots * cap * 3, false, s));
 	LCD_CUDA(e, e->st_n.reserve(static_cast<size_t>(e->st_slots), prev_slots, true, s));
+	LCD_CUDA(e, e->st_kof.reserve(static_cast<size_t>(e->st_slots) * cap, prev_slots * cap, false, s));
+	LCD_CUDA(e, e->st_creator.reserve(static_cast<size_t>(e->st_slots) * cap, prev_slots * cap, false, s));
+	LCD_CUDA(e, e->st_ftag.reserve(static_cast<size_t>(e->st_slots), prev_slots, false, s));
 	const size_t drow = static_cast<size_t>(cap) * e->nw * 4, xrow = static_cast<size_t>(cap) * 3 * sizeof(float);
+	// a written row's cached FROM dictionary is stale (0xFF..: nf = -1 matches no call)
 	if (contiguous)
 	{
 		LCD_CUDA(e, cudaMemcpyAsync(e->st_desc.p + static_cast<size_t>(slots[0]) * cap * e->nw, desc, drow * n_sigs, cudaMemcpyHostToDevice, s));
 		LCD_CUDA(e, cudaMemcpyAsync(e->st_xyz.p + static_cast<size_t>(slots[0]) * cap * 3, xyz, xrow * n_sigs, cudaMemcpyHostToDevice, s));
 		LCD_CUDA(e, cudaMemcpyAsync(e->st_n.p + slots[0], n, n_sigs * sizeof(int), cudaMemcpyHostToDevice, s));
+		LCD_CUDA(e, cudaMemsetAsync(e->st_ftag.p + slots[0], 0xFF, n_sigs * sizeof(FromDictTag), s));
 	}
 	else
 	{
@@ -3277,6 +3300,7 @@ int lcd_sig_add_batch(lcd_engine * e, const int * sig_ids, int n_sigs, int cap, 
 			LCD_CUDA(e, cudaMemcpyAsync(e->st_desc.p + static_cast<size_t>(slots[i]) * cap * e->nw, static_cast<const char *>(desc) + drow * i, drow, cudaMemcpyHostToDevice, s));
 			LCD_CUDA(e, cudaMemcpyAsync(e->st_xyz.p + static_cast<size_t>(slots[i]) * cap * 3, xyz + static_cast<size_t>(i) * cap * 3, xrow, cudaMemcpyHostToDevice, s));
 			LCD_CUDA(e, cudaMemcpyAsync(e->st_n.p + slots[i], n + i, sizeof(int), cudaMemcpyHostToDevice, s));
+			LCD_CUDA(e, cudaMemsetAsync(e->st_ftag.p + slots[i], 0xFF, sizeof(FromDictTag), s));
 		}
 	}
 	LCD_CUDA(e, e->st_slot_of_sig.reserve(e->h_slot_of_sig.size(), 0, false, s));
@@ -3296,6 +3320,7 @@ int lcd_sig_remove(lcd_engine * e, int sig_id)
 	const int minus1 = -1;
 	LCD_CUDA(e, cudaMemcpyAsync(e->st_slot_of_sig.p + sig_id, &minus1, sizeof(int), cudaMemcpyHostToDevice, e->stream));
 	LCD_CUDA(e, cudaMemsetAsync(e->st_n.p + slot, 0, sizeof(int), e->stream));
+	LCD_CUDA(e, cudaMemsetAsync(e->st_ftag.p + slot, 0xFF, sizeof(FromDictTag), e->stream));
 	LCD_CUDA(e, cudaStreamSynchronize(e->stream));
 	return LCD_OK;
 }

@@ -24,6 +24,16 @@ constexpr int kPnpChunk = 128;      // RANSAC hypotheses evaluated per chunk (on
 constexpr int kVerifyThreads = 256; // threads of the CTA: the second half helps with the inlier counts, LM sums and error passes
 constexpr int kMaxRansacIters = 320;
 
+// What a signature-store row's cached FROM dictionary was built for.  The temporary dictionary of addNewWords(descriptorsFrom) is a
+// function of the row's first nf descriptors and Vis/CorNNDR alone, so the matching kernel reuses it while both are those of the call.
+struct FromDictTag
+{
+	int nf;             // -1: stale (the row was written or freed since)
+	int n_dict;
+	uint32_t nndr_bits; // Vis/CorNNDR as float bits
+	int unused;
+};
+
 struct MatchArgs
 {
 	const uint32_t * desc_from; // [n_from_rows][cap_from][NW]
@@ -39,6 +49,10 @@ struct MatchArgs
 	int cap_to;                 // row stride of the TO arrays
 	int cap;                    // stride of the outputs and size of the shared-memory arrays (>= both)
 	float nndr; // Vis/CorNNDR
+	// FROM dictionaries cached per signature-store row (from_slot only, else nullptr): see from_dict_build_kernel
+	const FromDictTag * from_tag;  // [n_from_rows]
+	const uint16_t * from_kof;     // [n_from_rows][cap_from]
+	const uint16_t * from_creator; // [n_from_rows][cap_from]
 	// outputs
 	float * obj;       // [n_pairs][cap][3]
 	float * img;       // [n_pairs][cap][2]
@@ -51,9 +65,135 @@ struct MatchArgs
 	int * to_ids;      // [n_pairs][cap] or nullptr
 };
 
+// ---- TO x dictionary 2-NN of the matching kernel on the tensor cores ------------------------------------------------------------
+// A descriptor bit b is the s8 value 1 - 2b, so the s32 dot product of two descriptors is 32*NW - 2*hamming: exact integers, as in
+// nn_tensor.cuh.  mma.m16n8k32 gives each thread (group g = lane / 4, tig = lane % 4) the k positions 4*tig..4*tig+3 (a0, a1, b0) and
+// 16+4*tig..19+4*tig (a2, a3, b1) of a k-step.  The order of k inside a dot product is free as long as A and B agree, so those eight
+// positions are the eight bits of byte 4*ks + tig of the packed descriptor: low nibble -> a0/a1/b0, high nibble -> a2/a3/b1.  The
+// queries (A) are expanded in registers per k-step; the dictionary (B) is expanded to s8 in shared memory, kScanWords words at a time.
+constexpr int kScanNJ = 4;                 // n8 tiles (dictionary words / 8) per accumulator set of a warp: 16 registers (1024 threads: 64 each)
+constexpr int kScanWords = 64;             // dictionary words expanded per pass
+// 32-bit words per expanded dictionary word: 32*NW s8 + 32 bytes of padding, so the lds.64 of the 8 groups x 4 threads of a warp
+// fall on 32 different banks in each half-warp
+__host__ __device__ constexpr int scan_stride_words(int nw) { return 8 * nw + 8; }
+__host__ __device__ constexpr size_t scan_tile_bytes(int nw) { return static_cast<size_t>(kScanWords) * scan_stride_words(nw) * 4; }
+
 __host__ __device__ inline size_t match_smem_bytes(int cap, int nw)
 {
-	return static_cast<size_t>(cap) * (4 + 4 + 4 + 2 + 2 + 1 + 1 + 4 + 4 + 2 + 2) + 2 * static_cast<size_t>(cap) * nw * 4 + 128;
+	return scan_tile_bytes(nw) + static_cast<size_t>(cap) * (4 + 4 + 4 + 2 + 2 + 1 + 1 + 4 + 4 + 2 + 2) + 2 * static_cast<size_t>(cap) * nw * 4 + 128;
+}
+
+// the four bits of a nibble as four s8 values 1 - 2b (byte j = bit j)
+__device__ __forceinline__ uint32_t pm1_nibble(uint32_t n)
+{
+	return ((n * 0x00204081u) & 0x01010101u) * 0xFEu + 0x01010101u;
+}
+
+__device__ __forceinline__ void mma_s8_m16n8k32(int (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1)
+{
+	asm("mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+	    : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
+	    : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+
+// For every query j < nt: merges the two nearest dictionary words, as keys (d << kKeyShift) + k, into sa1[j] / sa2[j].  The keys are
+// the ones a scan of k = 0..n_dict-1 with top2_insert produces: distinct per k, so the smaller k wins a tie whatever the order.
+// Warp w owns the 16-query tiles w, w + 32, ...; per pass it multiplies them by kScanWords expanded words.  All threads must call it.
+// Not inlined: with the matching kernel's live values around it, the 64 registers of a 1024-thread CTA spill.
+template <int NW>
+__device__ __noinline__ void to_dict_knn2_mma(const uint32_t * __restrict__ q, int nt, const uint32_t * __restrict__ dict, int n_dict, uint32_t * __restrict__ stile,
+                                 uint32_t * sa1, uint32_t * sa2)
+{
+	constexpr int S = scan_stride_words(NW);
+	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
+	const int g = lane >> 2, tig = lane & 3;
+	const int n_mt = (nt + 15) >> 4;
+	for (int w0 = 0; w0 < n_dict; w0 += kScanWords)
+	{
+		__syncthreads(); // the previous pass is consumed
+		for (int i = tid; i < kScanWords * NW; i += blockDim.x)
+		{
+			const int w = i / NW, v = i % NW;
+			const uint32_t x = w0 + w < n_dict ? dict[static_cast<size_t>(w0 + w) * NW + v] : 0u;
+			uint4 * dst = reinterpret_cast<uint4 *>(stile + w * S + v * 8); // packed byte 4v + b -> s8 bytes 8(4v + b) .. +7
+			dst[0] = make_uint4(pm1_nibble(x & 0xFu), pm1_nibble((x >> 4) & 0xFu), pm1_nibble((x >> 8) & 0xFu), pm1_nibble((x >> 12) & 0xFu));
+			dst[1] = make_uint4(pm1_nibble((x >> 16) & 0xFu), pm1_nibble((x >> 20) & 0xFu), pm1_nibble((x >> 24) & 0xFu), pm1_nibble(x >> 28));
+		}
+		__syncthreads();
+		const int n_valid = min(kScanWords, n_dict - w0);
+		for (int mt = warp; mt < n_mt; mt += nwarps)
+		{
+			const int r0 = mt * 16 + g, r1 = r0 + 8;
+			const uint32_t * q0 = q + static_cast<size_t>(min(r0, nt - 1)) * NW; // rows past nt compute on a real row; dropped below
+			const uint32_t * q1 = q + static_cast<size_t>(min(r1, nt - 1)) * NW;
+			uint32_t k1a = kKeyNone, k2a = kKeyNone, k1b = kKeyNone, k2b = kKeyNone;
+#pragma unroll 1
+			for (int n0 = 0; n0 < n_valid; n0 += 8 * kScanNJ)
+			{
+				int acc[kScanNJ][4];
+#pragma unroll
+				for (int j = 0; j < kScanNJ; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0;
+#pragma unroll 4
+				for (int ks = 0; ks < NW; ++ks)
+				{
+					const uint32_t x0 = q0[ks] >> (8 * tig), x1 = q1[ks] >> (8 * tig);
+					const uint32_t a0 = pm1_nibble(x0 & 0xFu), a1 = pm1_nibble(x1 & 0xFu), a2 = pm1_nibble((x0 >> 4) & 0xFu), a3 = pm1_nibble((x1 >> 4) & 0xFu);
+#pragma unroll
+					for (int j = 0; j < kScanNJ; ++j)
+					{
+						const uint2 b = *reinterpret_cast<const uint2 *>(stile + (n0 + j * 8 + g) * S + ks * 8 + tig * 2);
+						mma_s8_m16n8k32(acc[j], a0, a1, a2, a3, b.x, b.y);
+					}
+				}
+				// c0 / c1: row r0, words 2 tig and 2 tig + 1 of the n8 tile; c2 / c3: row r1.  key = ((32 NW - dot) / 2 << kKeyShift) + k
+#pragma unroll
+				for (int j = 0; j < kScanNJ; ++j)
+				{
+#pragma unroll
+					for (int e = 0; e < 2; ++e)
+					{
+						const int kl = n0 + j * 8 + tig * 2 + e;
+						if (kl < n_valid)
+						{
+							const uint32_t base = (static_cast<uint32_t>(32 * NW) << (kKeyShift - 1)) + static_cast<uint32_t>(w0 + kl);
+							top2_insert(k1a, k2a, base - (static_cast<uint32_t>(acc[j][e]) << (kKeyShift - 1)));
+							top2_insert(k1b, k2b, base - (static_cast<uint32_t>(acc[j][2 + e]) << (kKeyShift - 1)));
+						}
+					}
+				}
+			}
+#pragma unroll
+			for (int o = 1; o < 4; o <<= 1)
+			{
+				const uint32_t oa1 = __shfl_xor_sync(0xFFFFFFFFu, k1a, o), oa2 = __shfl_xor_sync(0xFFFFFFFFu, k2a, o);
+				const uint32_t ob1 = __shfl_xor_sync(0xFFFFFFFFu, k1b, o), ob2 = __shfl_xor_sync(0xFFFFFFFFu, k2b, o);
+				top2_insert(k1a, k2a, oa1);
+				top2_insert(k1a, k2a, oa2);
+				top2_insert(k1b, k2b, ob1);
+				top2_insert(k1b, k2b, ob2);
+			}
+			if (tig == 0)
+			{
+				// the same warp owns these rows in every pass: no barrier between the passes' merges
+				if (r0 < nt)
+				{
+					uint32_t u1 = sa1[r0], u2 = sa2[r0];
+					top2_insert(u1, u2, k1a);
+					top2_insert(u1, u2, k2a);
+					sa1[r0] = u1;
+					sa2[r0] = u2;
+				}
+				if (r1 < nt)
+				{
+					uint32_t u1 = sa1[r1], u2 = sa2[r1];
+					top2_insert(u1, u2, k1b);
+					top2_insert(u1, u2, k2b);
+					sa1[r1] = u1;
+					sa2[r1] = u2;
+				}
+			}
+		}
+	}
 }
 
 // phase clocks of the matching kernel: diagnostics only, compiled in with -DLCD_DEBUG_PHASES
@@ -64,6 +204,89 @@ __device__ long long g_match_dbg[8];
 #define MATCH_PHASE(k) do { } while (0)
 #endif
 
+// FROM side: addNewWords(descriptorsFrom, 1) on an empty dictionary.  Copies the nf descriptors of F to sdesc; on return L[k] is the
+// descriptor that created word k and rank[i] the word of descriptor i.  Returns the number of words.  All threads must call it.
+template <int NW>
+__device__ int from_dictionary(const uint32_t * F, int nf, uint32_t * sdesc, uint32_t * sa1, uint32_t * sa2, int * res, uint16_t * L,
+                               uint16_t * rank, uint8_t * flag, uint8_t * flag2, int * s_nL, float nndr)
+{
+	const int tid = threadIdx.x;
+	for (int i = tid; i < nf * NW; i += blockDim.x) sdesc[i] = F[i]; // the scans re-read every descriptor ~nf/32 times
+	for (int i = tid; i < nf; i += blockDim.x)
+	{
+		sa1[i] = kKeyNone;
+		sa2[i] = kKeyNone;
+		flag[i] = 1;
+		res[i] = 0;
+	}
+	__syncthreads();
+	int n_dict = 0;
+	if (nf > 0) n_dict = resolve_rounds<NW>(sdesc, nf, sa1, sa2, res, L, rank, flag, flag2, s_nL, nndr, 1);
+	__syncthreads();
+	for (int i = tid; i < nf; i += blockDim.x)
+		if (!flag[i]) rank[i] = static_cast<uint16_t>(-1 - res[i]);
+	__syncthreads();
+	return n_dict;
+}
+
+struct FromDictArgs
+{
+	const uint32_t * desc;  // signature store [slots][cap_from][NW]
+	const int * n;          // [slots]
+	const int * slot;       // [n_pairs] row of each pair (-1 = none)
+	int cap_from;
+	int rows;               // min(cap of the call, cap_from): size of the shared-memory arrays
+	float nndr;
+	FromDictTag * tag;      // [slots]
+	uint16_t * kof;         // [slots][cap_from]
+	uint16_t * creator;     // [slots][cap_from]
+};
+
+__host__ __device__ inline size_t from_dict_smem_bytes(int rows, int nw)
+{
+	return static_cast<size_t>(rows) * (static_cast<size_t>(nw) * 4 + 4 + 4 + 4 + 2 + 2 + 1 + 1) + 128;
+}
+
+// Builds the FROM dictionary of each pair's store row unless it is cached for this nf and NNDR already or an earlier pair of the batch
+// has the same row (frames often share a hypothesis).  One CTA per pair, launched before pair_match_kernel on the same stream.
+template <int NW>
+__global__ void __launch_bounds__(kResolveThreads)
+from_dict_build_kernel(const FromDictArgs a)
+{
+	extern __shared__ __align__(128) unsigned char smem_raw[];
+	const int rows = a.rows;
+	uint32_t * sdesc = reinterpret_cast<uint32_t *>(smem_raw); // [rows][NW]
+	uint32_t * sa1 = sdesc + static_cast<size_t>(rows) * NW;
+	uint32_t * sa2 = sa1 + rows;
+	int * res = reinterpret_cast<int *>(sa2 + rows);
+	uint16_t * L = reinterpret_cast<uint16_t *>(res + rows);
+	uint16_t * rank = L + rows;
+	uint8_t * flag = reinterpret_cast<uint8_t *>(rank + rows);
+	uint8_t * flag2 = flag + rows;
+	__shared__ int s_nL, s_build;
+	const int pair = blockIdx.x, slot = a.slot[pair];
+	if (slot < 0) return;
+	const int nf = min(a.n[slot], rows);
+	const uint32_t nndr_bits = __float_as_uint(a.nndr);
+	if (threadIdx.x == 0)
+	{
+		const FromDictTag t = a.tag[slot];
+		int build = t.nf != nf || t.nndr_bits != nndr_bits;
+		for (int p = 0; p < pair && build; ++p)
+			if (a.slot[p] == slot) build = 0;
+		s_build = build;
+	}
+	__syncthreads();
+	if (!s_build) return;
+	const size_t base = static_cast<size_t>(slot) * a.cap_from;
+	const int n_dict = from_dictionary<NW>(a.desc + base * NW, nf, sdesc, sa1, sa2, res, L, rank, flag, flag2, &s_nL, a.nndr);
+	for (int i = threadIdx.x; i < nf; i += blockDim.x) a.kof[base + i] = rank[i];
+	for (int k = threadIdx.x; k < n_dict; k += blockDim.x) a.creator[base + k] = L[k];
+	__threadfence();
+	__syncthreads();
+	if (threadIdx.x == 0) a.tag[slot] = FromDictTag{nf, n_dict, nndr_bits, 0};
+}
+
 template <int NW>
 __global__ void __launch_bounds__(kResolveThreads)
 pair_match_kernel(const MatchArgs a)
@@ -71,7 +294,8 @@ pair_match_kernel(const MatchArgs a)
 	MATCH_PHASE(0);
 	extern __shared__ __align__(128) unsigned char smem_raw[];
 	const int cap = a.cap;
-	uint32_t * dict = reinterpret_cast<uint32_t *>(smem_raw);             // [cap][NW] words of the temporary dictionary
+	uint32_t * stile = reinterpret_cast<uint32_t *>(smem_raw);           // [kScanWords][scan_stride_words(NW)] s8 words of the TO scan
+	uint32_t * dict = stile + scan_tile_bytes(NW) / 4;                    // [cap][NW] words of the temporary dictionary
 	uint32_t * sdesc = dict + static_cast<size_t>(cap) * NW;              // [cap][NW] the side being quantised (FROM, then TO)
 	uint32_t * sa1 = sdesc + static_cast<size_t>(cap) * NW;               // [cap]
 	uint32_t * sa2 = sa1 + cap;
@@ -97,33 +321,38 @@ pair_match_kernel(const MatchArgs a)
 	const uint32_t * F = a.desc_from + fbase * NW;
 	const uint32_t * T = a.desc_to + tbase * NW;
 
-	// ---- FROM side: addNewWords(descriptorsFrom, 1) on an empty dictionary -------------------
-	for (int i = tid; i < nf * NW; i += blockDim.x) sdesc[i] = F[i];   // the scans below re-read every descriptor ~nf/32 times
-	for (int i = tid; i < nf; i += blockDim.x)
+	// ---- FROM side: addNewWords(descriptorsFrom, 1) on an empty dictionary, or the store row's cached result -------------------
+	__shared__ int s_cached;
+	if (tid == 0)
 	{
-		sa1[i] = kKeyNone;
-		sa2[i] = kKeyNone;
-		flag[i] = 1;
-		res[i] = 0;
+		const FromDictTag * t = a.from_tag && frow >= 0 ? a.from_tag + frow : nullptr;
+		s_cached = t && t->nf == nf && t->nndr_bits == __float_as_uint(a.nndr) ? t->n_dict : -1;
 	}
 	__syncthreads();
-	int n_dict = 0;
-	if (nf > 0) n_dict = resolve_rounds<NW>(sdesc, nf, sa1, sa2, res, L, rank, flag, flag2, &s_nL, a.nndr, 1);
-	__syncthreads();
+	const bool cached = s_cached >= 0;
+	int n_dict;
+	if (cached)
+	{
+		n_dict = s_cached;
+		for (int i = tid; i < nf; i += blockDim.x) rank[i] = a.from_kof[fbase + i];
+		for (int k = tid; k < n_dict; k += blockDim.x) L[k] = a.from_creator[fbase + k];
+		__syncthreads();
+	}
+	else n_dict = from_dictionary<NW>(F, nf, sdesc, sa1, sa2, res, L, rank, flag, flag2, &s_nL, a.nndr);
 	MATCH_PHASE(1);
 	for (int k = tid; k < n_dict; k += blockDim.x)
 	{
 		cntF[k] = 0;
 		cntT[k] = 0;
 		uint32_t q[NW];
-		load_desc<NW>(sdesc, L[k], q);
+		load_desc<NW>(cached ? F : sdesc, L[k], q);
 #pragma unroll
 		for (int v = 0; v < NW; ++v) dict[static_cast<size_t>(k) * NW + v] = q[v];
 	}
 	__syncthreads();
 	for (int i = tid; i < nf; i += blockDim.x)
 	{
-		const int k = flag[i] ? rank[i] : (-1 - res[i]);
+		const int k = rank[i];
 		atomicAdd(&cntF[k], 1);
 		idxF[k] = static_cast<uint16_t>(i);
 		if (a.from_ids) a.from_ids[base + i] = k + 1;
@@ -134,30 +363,17 @@ pair_match_kernel(const MatchArgs a)
 	// ---- TO side: update(); addNewWords(descriptorsTo, 2) --------------------------------------
 	__syncthreads();
 	for (int i = tid; i < nt * NW; i += blockDim.x) sdesc[i] = T[i];
+	for (int j = tid; j < nt; j += blockDim.x)
+	{
+		sa1[j] = kKeyNone;
+		sa2[j] = kKeyNone;
+	}
+	__syncthreads();
+	to_dict_knn2_mma<NW>(sdesc, nt, dict, n_dict, stile, sa1, sa2);
 	__syncthreads();
 	for (int j = tid; j < nt; j += blockDim.x)
 	{
-		uint32_t q[NW];
-		load_desc<NW>(sdesc, j, q);
-		uint32_t k1 = kKeyNone, k2 = kKeyNone;
-		for (int k = 0; k < n_dict; ++k)
-		{
-			const uint4 * row = reinterpret_cast<const uint4 *>(dict + static_cast<size_t>(k) * NW);
-			uint32_t w[NW];
-#pragma unroll
-			for (int v = 0; v < NW / 4; ++v)
-			{
-				const uint4 x = row[v];
-				w[4 * v] = x.x;
-				w[4 * v + 1] = x.y;
-				w[4 * v + 2] = x.z;
-				w[4 * v + 3] = x.w;
-			}
-			const uint32_t d = hamming<NW, 2>(q, w); // carry-save tree: 5 POPC instead of 8 for 256-bit descriptors
-			top2_insert(k1, k2, (d << kKeyShift) + static_cast<uint32_t>(k));
-		}
-		sa1[j] = k1;
-		sa2[j] = k2;
+		const uint32_t k1 = sa1[j], k2 = sa2[j];
 		int bt;
 		flag[j] = nndr_decide(k1, k2, kKeyNone, kKeyNone, a.nndr, bt) ? 1 : 0;
 		res[j] = static_cast<int>(k1 & kKeyRowMask);
