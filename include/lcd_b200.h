@@ -481,7 +481,8 @@ int lcd_verify_top_dev(lcd_engine * e, const void * d_queries, const float * d_u
  * prediction matrix, is shared.  These calls replace, for B clients at once, what Rtabmap::process does with one frame's raw
  * likelihood in localisation mode: adjustLikelihood (Rtabmap.cpp:2119-2121), BayesFilter::computePosterior (:2133), the hypothesis
  * selection and its checks (:2143-2233), and the verification of the accepted hypothesis with its rejections (:3133-3191).
- * Proximity detection, the epipolar check (Rtabmap/VerifyLoopClosureHypothesis), retrieval and the graph walk stay the caller's.
+ * The epipolar check (VhEp/Enabled) is lcd_decide_epipolar_dev, run between the decision and its verification.  Proximity detection,
+ * retrieval and the graph walk stay the caller's.
  *
  * replaces: BayesFilter::BayesFilter + BayesFilter::reset (BayesFilter.cpp:43-68, :140-143) and Rtabmap's _highestHypothesis = (0, 0)
  * (Rtabmap.cpp:467, :1094) for n_clients clients at once; calling it again resets every client.  LCD_ERR_CAPACITY when the device
@@ -639,10 +640,73 @@ int lcd_shard_localize_batch_dev(lcd_engine * e, const void * d_queries, int n_f
                                  const int * d_sig_ids, int ns, int n_total, const int * d_row_ids_global, int last_word_id,
                                  int * d_word_ids_out, float * d_likelihood_out, void * stream);
 
+/* ---- epipolar verification of loop-closure hypotheses (VhEp/Enabled) ---------------------------------------------------------
+ * EpipolarGeometry::check(A, B) (corelib/src/EpipolarGeometry.cpp:65-102) of a new signature A and a hypothesis B, from word ids and
+ * keypoints alone (no depth, any descriptor type): findPairsUnique, the word ids >= 0 found exactly once in A and once in B, in
+ * ascending id order; then cv::findFundamentalMat(FM_RANSAC, ransac_param1, ransac_param2) on their keypoints as OpenCV 4.13 runs it
+ * (7 points: the 7-point kernel alone, mask all ones; 8-14: LMeDS; >= 15: RANSAC with 7-point samples, 1000 iterations at most); the
+ * check passes with at least match_count_min inliers.  Where the reference itself fails, the check is a rejection: findFundamentalMat
+ * returns no matrix (the reference asserts on the empty Mat), or OpenCV raises.  OpenCV raises when its 7-point kernel returns -1
+ * models: the four coefficients of the determinant polynomial are exactly zero, which collinear points can cause.  raised flags the
+ * inputs where the coefficients as computed here are exactly zero; they are not OpenCV's bits, so OpenCV raises on some inputs that
+ * raised does not flag (53 of the 640 sets of the test corpus, all with many collinear points). */
+typedef struct lcd_epipolar_params {
+	int match_count_min;  /* VhEp/MatchCountMin (8) */
+	double ransac_param1; /* VhEp/RansacParam1 (3): distance threshold, compared squared; <= 0 -> 3 as in findFundamentalMat */
+	double ransac_param2; /* VhEp/RansacParam2 (0.99): confidence; outside (DBL_EPSILON, 1 - DBL_EPSILON) -> 0.99 */
+} lcd_epipolar_params;
+
+#define LCD_EPIPOLAR_NONE 0   /* fewer than 7 pairs or fewer than match_count_min: no fundamental matrix */
+#define LCD_EPIPOLAR_7POINT 1 /* exactly 7 pairs */
+#define LCD_EPIPOLAR_LMEDS 2  /* 8-14 pairs */
+#define LCD_EPIPOLAR_RANSAC 3 /* 15 pairs or more */
+
+typedef struct lcd_epipolar_result {
+	int checked;        /* 1: the pair was checked */
+	int ok;             /* EpipolarGeometry::check */
+	int n_pairs;        /* findPairsUnique pairs */
+	int n_inliers;      /* uSum(status) (0 when no matrix) */
+	int method;         /* LCD_EPIPOLAR_* */
+	int found;          /* findFundamentalMat returned a matrix (0 also where OpenCV raises) */
+	int iterations_run; /* registrator iterations executed (0 for 7 pairs) */
+	int raised;         /* a sample's 7-point kernel returned -1 models, where OpenCV raises (see above); a rejection here */
+	double F[9];        /* the returned matrix, row-major (7 pairs: the first solution); zeros when none */
+} lcd_epipolar_result;
+
+/* EpipolarGeometry::check for n_pairs explicit (A = new, B = old) signatures.  ids_*[n_pairs][cap] word ids, uv_*[n_pairs][cap][2]
+ * keypoints (row i = word i), n_*[n_pairs] rows used; out[n_pairs]; status_out[n_pairs][cap] (optional) the inlier mask in pair order.
+ * LCD_ERR_INVALID for a count outside [0, cap]; LCD_ERR_CAPACITY for cap > 4096. */
+int lcd_epipolar_check_batch(lcd_engine * e, int n_pairs, int cap, const int * ids_a, const float * uv_a, const int * n_a,
+                             const int * ids_b, const float * uv_b, const int * n_b, const lcd_epipolar_params * p,
+                             lcd_epipolar_result * out, uint8_t * status_out);
+
+/* The stored places' words for the check inside the decision: Signature::getWords() / getWordsKpts() of each signature, word_ids[n_sigs][cap]
+ * and uv[n_sigs][cap][2] (row i = word i), n[n_sigs] rows used.  A store of its own (no descriptors, no depth), so RGB-only callers and
+ * float engines can fill it; adding an id again replaces its row, and slots of removed ids are reused.  LCD_ERR_INVALID for an id <= 0
+ * or a count outside [0, cap]; LCD_ERR_CAPACITY for cap > 4096. */
+int lcd_sig_words_add_batch(lcd_engine * e, const int * sig_ids, int n_sigs, int cap, const int * word_ids, const float * uv, const int * n);
+int lcd_sig_words_remove(lcd_engine * e, int sig_id);
+int lcd_sig_words_count(const lcd_engine * e);
+
+#define LCD_DECIDE_EPIPOLAR_REJECTED 11 /* value over the threshold, EpipolarGeometry::check failed (Rtabmap.cpp:2193-2196) */
+
+/* VhEp/Enabled on the last decision (Rtabmap.cpp:2193, between the single-hypothesis and the ratio rejections): every frame whose status
+ * is ACCEPTED, RATIO or LAST_NULL is checked against its highest hypothesis in the word store (a hypothesis not stored is a signature
+ * without words: 0 pairs).  A failed check makes the frame LCD_DECIDE_EPIPOLAR_REJECTED with loop id 0 and no hypothesis left for
+ * lcd_verify_decided_dev; highest_id / highest_value stay.  A frame that passes keeps its status.  d_word_ids[n_frames][nq_per_frame]
+ * (the frame's words, e.g. from lcd_localize_batch_dev), d_uv[n_frames][nq_per_frame][2], d_n_per_frame[n_frames]: device pointers.
+ * Composition: a likelihood call, lcd_decide_batch_dev, lcd_decide_epipolar_dev, then optionally lcd_verify_decided_dev.
+ * LCD_ERR_STATE without a decision; LCD_ERR_INVALID when n_frames differs from the last decision's; LCD_ERR_CAPACITY for
+ * nq_per_frame > 4096. */
+int lcd_decide_epipolar_dev(lcd_engine * e, const int * d_word_ids, const float * d_uv, const int * d_n_per_frame, int n_frames,
+                            int nq_per_frame, const lcd_epipolar_params * p, void * stream);
+/* the per-frame check results of the last lcd_decide_epipolar_dev (checked = 0: the frame did not reach the check) */
+int lcd_epipolar_fetch(lcd_engine * e, int n_frames, lcd_epipolar_result * out);
+
 /* ---- measurement hooks ---------------------------------------------------------------
  * Optional per-kernel timing with CUDA events recorded on the launching stream around
  * every launch of kernel class `which` (0 = dictionary NN, 1 = resolve, 2 = score, 3 = pair
- * matching, 4 = PnP RANSAC, 5 = all ORB kernels).
+ * matching, 4 = PnP RANSAC, 5 = all ORB kernels, 6 = the epipolar check).
  * lcd_profile_read synchronises, returns the summed device time and the launch count
  * since the last reset. */
 #define LCD_PROF_NN 0
@@ -651,6 +715,7 @@ int lcd_shard_localize_batch_dev(lcd_engine * e, const void * d_queries, int n_f
 #define LCD_PROF_MATCH 3
 #define LCD_PROF_PNP 4
 #define LCD_PROF_ORB 5
+#define LCD_PROF_EPIPOLAR 6
 int lcd_profile_enable(lcd_engine * e, int on);
 int lcd_profile_read(lcd_engine * e, int which, double * total_ms, long long * launches);
 int lcd_profile_reset(lcd_engine * e);

@@ -102,10 +102,27 @@ class DecideParams(C.Structure):
     ]
 
 
+class EpipolarParams(C.Structure):
+    """lcd_epipolar_params (VhEp/MatchCountMin, VhEp/RansacParam1, VhEp/RansacParam2)."""
+    _fields_ = [("match_count_min", C.c_int), ("ransac_param1", C.c_double), ("ransac_param2", C.c_double)]
+
+
+class EpipolarResult(C.Structure):
+    _fields_ = [
+        ("checked", C.c_int), ("ok", C.c_int), ("n_pairs", C.c_int), ("n_inliers", C.c_int), ("method", C.c_int), ("found", C.c_int),
+        ("iterations_run", C.c_int), ("raised", C.c_int), ("F", C.c_double * 9),
+    ]
+
+
+def _epi_dict(r: EpipolarResult) -> dict:
+    return {"checked": r.checked, "ok": r.ok, "n_pairs": r.n_pairs, "n_inliers": r.n_inliers, "method": r.method, "found": r.found,
+            "iterations_run": r.iterations_run, "raised": r.raised, "F": np.array(r.F[:], np.float64).reshape(3, 3)}
+
+
 # frame flags and decision statuses of lcd_decide_batch_dev (lcd_b200.h)
 FRAME_SKIP, FRAME_HOLD, FRAME_AGGRESSIVE = 1, 2, 4
 DECIDE_STATUS = ("skipped", "held", "no hypothesis", "under threshold", "under ratio", "single hypothesis", "ratio", "last null", "accepted",
-                 "verification rejected", "distance rejected")
+                 "verification rejected", "distance rejected", "epipolar rejected")
 DECISION_DTYPE = np.dtype([("highest_id", np.int32), ("highest_value", np.float32), ("loop_id", np.int32), ("status", np.int32)])
 
 
@@ -208,6 +225,12 @@ SIGNATURES = {
     "lcd_shard_comm_destroy": (_I, [_P]),
     "lcd_shard_process_frames_dev": (_I, [_P, _I, _P, _I, _I, _I, _P, _I, _P, _I, _F, _I, _P, _I, _I, _P, _I, _P, _P, _P, _P]),
     "lcd_shard_localize_batch_dev": (_I, [_P, _P, _I, _I, _I, _F, _I, _P, _I, _I, _P, _I, _P, _P, _P]),
+    "lcd_epipolar_check_batch": (_I, [_P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "lcd_sig_words_add_batch": (_I, [_P, _P, _I, _I, _P, _P, _P]),
+    "lcd_sig_words_remove": (_I, [_P, _I]),
+    "lcd_sig_words_count": (_I, [_P]),
+    "lcd_decide_epipolar_dev": (_I, [_P, _P, _P, _P, _I, _I, _P, _P]),
+    "lcd_epipolar_fetch": (_I, [_P, _I, _P]),
     "lcd_profile_enable": (_I, [_P, _I]),
     "lcd_profile_read": (_I, [_P, _I, _P, _P]),
     "lcd_profile_reset": (_I, [_P]),
@@ -909,6 +932,55 @@ class Engine:
             raise LcdError(-1, f"clients and frame_flags need {n_frames} entries")
         self._check(self._lib.lcd_decide_batch_dev(self._h, C.c_void_p(d_likelihood), int(n_frames), int(ns), _ptr(c), _ptr(f), C.byref(dp),
                                                     C.c_void_p(d_posterior_out or None), C.c_void_p(stream or None)))
+
+    def sig_words_add_batch(self, sig_ids, word_ids, uv, n):
+        """The stored places' words and keypoints for the epipolar check: word_ids [k, cap] int32, uv [k, cap, 2] float32, n [k]."""
+        s = _i32(sig_ids)
+        w = np.ascontiguousarray(word_ids, np.int32)
+        k, cap = w.shape
+        u = np.ascontiguousarray(uv, np.float32).reshape(k, cap, 2)
+        nn = _i32(n)
+        if len(s) != k or len(nn) != k:
+            raise LcdError(-1, f"{k} signatures need {k} ids and counts")
+        self._check(self._lib.lcd_sig_words_add_batch(self._h, _ptr(s), k, cap, _ptr(w), _ptr(u), _ptr(nn)))
+
+    def sig_words_remove(self, sig_id: int):
+        self._check(self._lib.lcd_sig_words_remove(self._h, int(sig_id)))
+
+    @property
+    def sig_words_count(self) -> int:
+        return int(self._lib.lcd_sig_words_count(self._h))
+
+    def decide_epipolar_dev(self, d_word_ids: int, d_uv: int, d_n_per_frame: int, n_frames: int, nq_per_frame: int, match_count_min: int = 8,
+                            ransac_param1: float = 3.0, ransac_param2: float = 0.99, stream: int = 0):
+        """VhEp/Enabled on the last decision (device pointers: word ids [n_frames][nq], uv [n_frames][nq][2], counts [n_frames])."""
+        p = EpipolarParams(int(match_count_min), float(ransac_param1), float(ransac_param2))
+        self._check(self._lib.lcd_decide_epipolar_dev(self._h, C.c_void_p(d_word_ids), C.c_void_p(d_uv), C.c_void_p(d_n_per_frame),
+                                                       int(n_frames), int(nq_per_frame), C.byref(p), C.c_void_p(stream or None)))
+
+    def epipolar_fetch(self, n_frames: int):
+        out = (EpipolarResult * n_frames)()
+        self._check(self._lib.lcd_epipolar_fetch(self._h, int(n_frames), out))
+        return [_epi_dict(r) for r in out]
+
+    def epipolar_check_batch(self, ids_a, uv_a, n_a, ids_b, uv_b, n_b, match_count_min: int = 8, ransac_param1: float = 3.0,
+                             ransac_param2: float = 0.99, with_status: bool = False):
+        """EpipolarGeometry::check of n pairs (A = new, B = old).  ids_* [n, cap] int32, uv_* [n, cap, 2] float32, n_* [n].  Returns a
+        list of dicts (ok, n_pairs, n_inliers, method, found, iterations_run, raised, F) and, with with_status, the [n, cap] masks."""
+        ids_a = np.ascontiguousarray(ids_a, np.int32)
+        n, cap = ids_a.shape
+        ids_b = np.ascontiguousarray(ids_b, np.int32).reshape(n, cap)
+        uv_a = np.ascontiguousarray(uv_a, np.float32).reshape(n, cap, 2)
+        uv_b = np.ascontiguousarray(uv_b, np.float32).reshape(n, cap, 2)
+        n_a = np.ascontiguousarray(n_a, np.int32).reshape(n)
+        n_b = np.ascontiguousarray(n_b, np.int32).reshape(n)
+        p = EpipolarParams(int(match_count_min), float(ransac_param1), float(ransac_param2))
+        out = (EpipolarResult * n)()
+        status = np.zeros((n, cap), np.uint8) if with_status else None
+        self._check(self._lib.lcd_epipolar_check_batch(self._h, n, cap, _ptr(ids_a), _ptr(uv_a), _ptr(n_a), _ptr(ids_b), _ptr(uv_b), _ptr(n_b),
+                                                       C.byref(p), out, _ptr(status) if status is not None else None))
+        res = [_epi_dict(r) for r in out]
+        return (res, status) if with_status else res
 
     def decide_fetch(self, n_frames: int) -> np.ndarray:
         """The last decision's lcd_decision records as a structured array (highest_id, highest_value, loop_id, status)."""

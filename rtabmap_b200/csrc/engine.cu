@@ -21,6 +21,7 @@
 #include "bayes.cuh"
 #include "decide.cuh"
 #include "verify.cuh"
+#include "epipolar.cuh"
 #include "match_bf.cuh"
 #include "orb.cuh"
 
@@ -346,6 +347,19 @@ struct lcd_engine
 	// verification scratch
 	DevBuf<uint32_t> v_df, v_dt;
 	DevBuf<float> v_xyz, v_uv, v_obj, v_img, v_T, v_xyz_to, v_obj_to;
+	// epipolar check scratch
+	DevBuf<int> ep_ids_a, ep_ids_b, ep_n, ep_res;
+	DevBuf<float> ep_uv_a, ep_uv_b;
+	DevBuf<double> ep_F;
+	DevBuf<uint8_t> ep_status;
+	DevBuf<int> ep_slot, ep_skip;
+	int ep_last_frames = 0; // frames of the last lcd_decide_epipolar_dev (0: none)
+	// word store of the stored places for the epipolar check: Signature::getWords() / getWordsKpts() by row
+	DevBuf<int> ws_ids, ws_n, ws_slot_of_sig;
+	DevBuf<float> ws_uv;
+	int ws_cap = 0, ws_rows = 0;
+	std::vector<int> h_ws_slot_of_sig, ws_free;
+	int ws_count = 0;
 	DevBuf<double> v_cov6;
 	DevBuf<ulonglong2> bf_keys_a, bf_keys_b;
 	DevBuf<unsigned long long> bf_best;
@@ -386,7 +400,7 @@ struct lcd_engine
 	{
 		std::vector<cudaEvent_t> ev; // start/stop pairs
 		size_t used = 0;
-	} prof[6];
+	} prof[7];
 
 	// tuning knobs (env: LCD_NN_CTAS_PER_SM, LCD_NN_TQ, LCD_NN_VARIANT, LCD_SCORE_BLOCKS)
 	int nn_ctas_per_sm = 2, nn_tq = 8, nn_variant = 2, score_blocks = 32;
@@ -1332,7 +1346,7 @@ int lcd_profile_reset(lcd_engine * e)
 
 int lcd_profile_read(lcd_engine * e, int which, double * total_ms, long long * launches)
 {
-	if (!e || which < 0 || which > 5) return LCD_ERR_INVALID;
+	if (!e || which < 0 || which > 6) return LCD_ERR_INVALID;
 	LCD_TRY(set_device(e));
 	LCD_CUDA(e, cudaDeviceSynchronize());
 	auto & p = e->prof[which];
@@ -3133,6 +3147,231 @@ int lcd_pnp_ransac(lcd_engine * e, const float * object_points, const float * im
 	}
 	return lcd_pnp_ransac_batch(e, 1, n, object_points, image_points, &n, K, dist_coeffs, n_dist, rvec, tvec, use_extrinsic_guess, iterations,
 	                            reproj_error, min_inliers, flags, refine_iterations, refine_sigma, inliers_out, n_inliers_out, nullptr);
+}
+
+// ---- EpipolarGeometry::check of explicit signature pairs ------------------------------------------------
+} // extern "C"
+static int launch_epipolar(lcd_engine * e, int n_pairs, EpiArgs & a, const lcd_epipolar_params * p, cudaStream_t s)
+{
+	const size_t smem = epi_smem_bytes(std::max(a.cap_a, a.cap_b));
+	if (smem > static_cast<size_t>(e->smem_optin)) LCD_FAIL(e, LCD_ERR_CAPACITY, "%d words per side need %zu B of shared memory", std::max(a.cap_a, a.cap_b), smem);
+	LCD_CUDA(e, e->ep_res.reserve(static_cast<size_t>(n_pairs) * 8, 0, false, s));
+	LCD_CUDA(e, e->ep_F.reserve(static_cast<size_t>(n_pairs) * 9, 0, false, s));
+	a.match_count_min = p->match_count_min;
+	// findFundamentalMat's own resets of a threshold <= 0 and of a confidence outside (DBL_EPSILON, 1 - DBL_EPSILON)
+	a.thr = p->ransac_param1 <= 0 ? 3. : p->ransac_param1;
+	a.conf = (p->ransac_param2 < 2.220446049250313e-16 || p->ransac_param2 > 1 - 2.220446049250313e-16) ? 0.99 : p->ransac_param2;
+	a.res = e->ep_res.p;
+	a.F = e->ep_F.p;
+	if (smem > 48 * 1024)
+		LCD_CUDA(e, cudaFuncSetAttribute(epipolar_check_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+	prof_mark(e, LCD_PROF_EPIPOLAR, s);
+	epipolar_check_kernel<<<n_pairs, kEpiThreads, smem, s>>>(a);
+	prof_mark(e, LCD_PROF_EPIPOLAR, s);
+	LCD_CHECK_LAUNCH(e);
+	return LCD_OK;
+}
+
+static void epipolar_results(int n, const int * hr, const double * hF, lcd_epipolar_result * out)
+{
+	for (int i = 0; i < n; ++i)
+	{
+		const int * r = hr + static_cast<size_t>(i) * 8;
+		lcd_epipolar_result & o = out[i];
+		o.checked = r[0];
+		o.ok = r[1];
+		o.n_pairs = r[2];
+		o.n_inliers = r[3];
+		o.method = r[4];
+		o.found = r[5];
+		o.iterations_run = r[6];
+		o.raised = r[7];
+		for (int k = 0; k < 9; ++k) o.F[k] = hF[static_cast<size_t>(i) * 9 + k];
+	}
+}
+extern "C" {
+int lcd_epipolar_check_batch(lcd_engine * e, int n_pairs, int cap, const int * ids_a, const float * uv_a, const int * n_a, const int * ids_b,
+                             const float * uv_b, const int * n_b, const lcd_epipolar_params * p, lcd_epipolar_result * out, uint8_t * status_out)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (n_pairs <= 0 || cap <= 0 || !ids_a || !uv_a || !n_a || !ids_b || !uv_b || !n_b || !p || !out)
+		LCD_FAIL(e, LCD_ERR_INVALID, "null or empty epipolar input");
+	if (cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "at most %d words per signature", kMaxFrameQueries);
+	for (int i = 0; i < n_pairs; ++i)
+		if (n_a[i] < 0 || n_a[i] > cap || n_b[i] < 0 || n_b[i] > cap)
+			LCD_FAIL(e, LCD_ERR_INVALID, "pair %d has %d / %d words (cap %d)", i, n_a[i], n_b[i], cap);
+	cudaStream_t s = e->stream;
+	const size_t rows = static_cast<size_t>(n_pairs) * cap;
+	LCD_CUDA(e, e->ep_ids_a.reserve(rows, 0, false, s));
+	LCD_CUDA(e, e->ep_ids_b.reserve(rows, 0, false, s));
+	LCD_CUDA(e, e->ep_uv_a.reserve(rows * 2, 0, false, s));
+	LCD_CUDA(e, e->ep_uv_b.reserve(rows * 2, 0, false, s));
+	LCD_CUDA(e, e->ep_n.reserve(static_cast<size_t>(n_pairs) * 2, 0, false, s));
+	if (status_out) LCD_CUDA(e, e->ep_status.reserve(rows, 0, false, s));
+	LCD_CUDA(e, cudaMemcpyAsync(e->ep_ids_a.p, ids_a, rows * sizeof(int), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, cudaMemcpyAsync(e->ep_ids_b.p, ids_b, rows * sizeof(int), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, cudaMemcpyAsync(e->ep_uv_a.p, uv_a, rows * 2 * sizeof(float), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, cudaMemcpyAsync(e->ep_uv_b.p, uv_b, rows * 2 * sizeof(float), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, cudaMemcpyAsync(e->ep_n.p, n_a, n_pairs * sizeof(int), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, cudaMemcpyAsync(e->ep_n.p + n_pairs, n_b, n_pairs * sizeof(int), cudaMemcpyHostToDevice, s));
+	EpiArgs a{};
+	a.ids_a = e->ep_ids_a.p;
+	a.uv_a = e->ep_uv_a.p;
+	a.n_a = e->ep_n.p;
+	a.ids_b = e->ep_ids_b.p;
+	a.uv_b = e->ep_uv_b.p;
+	a.n_b = e->ep_n.p + n_pairs;
+	a.cap_a = a.cap_b = cap;
+	a.status = status_out ? e->ep_status.p : nullptr;
+	a.status_cap = cap;
+	LCD_TRY(launch_epipolar(e, n_pairs, a, p, s));
+	std::vector<int> hr(static_cast<size_t>(n_pairs) * 8);
+	std::vector<double> hF(static_cast<size_t>(n_pairs) * 9);
+	LCD_CUDA(e, cudaMemcpyAsync(hr.data(), e->ep_res.p, hr.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+	LCD_CUDA(e, cudaMemcpyAsync(hF.data(), e->ep_F.p, hF.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+	if (status_out) LCD_CUDA(e, cudaMemcpyAsync(status_out, e->ep_status.p, rows, cudaMemcpyDeviceToHost, s));
+	LCD_CUDA(e, cudaStreamSynchronize(s));
+	epipolar_results(n_pairs, hr.data(), hF.data(), out);
+	return LCD_OK;
+}
+
+int lcd_sig_words_add_batch(lcd_engine * e, const int * sig_ids, int n_sigs, int cap, const int * word_ids, const float * uv, const int * n)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (n_sigs <= 0 || cap <= 0 || !sig_ids || !word_ids || !uv || !n) LCD_FAIL(e, LCD_ERR_INVALID, "null or empty word store input");
+	if (cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "at most %d words per signature", kMaxFrameQueries);
+	int max_id = 0;
+	for (int i = 0; i < n_sigs; ++i)
+	{
+		if (sig_ids[i] <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "signature id %d is not > 0", sig_ids[i]);
+		if (n[i] < 0 || n[i] > cap) LCD_FAIL(e, LCD_ERR_INVALID, "signature %d has %d words (cap %d)", sig_ids[i], n[i], cap);
+		max_id = std::max(max_id, sig_ids[i]);
+	}
+	cudaStream_t s = e->stream;
+	if (cap > e->ws_cap && e->ws_rows > 0)
+	{
+		// wider rows: re-lay the stored rows out at the new stride
+		DevBuf<int> ids2;
+		DevBuf<float> uv2;
+		LCD_CUDA(e, ids2.reserve(static_cast<size_t>(e->ws_rows) * cap, 0, false, s));
+		LCD_CUDA(e, uv2.reserve(static_cast<size_t>(e->ws_rows) * cap * 2, 0, false, s));
+		LCD_CUDA(e, cudaMemcpy2DAsync(ids2.p, cap * sizeof(int), e->ws_ids.p, e->ws_cap * sizeof(int), e->ws_cap * sizeof(int), e->ws_rows,
+		                              cudaMemcpyDeviceToDevice, s));
+		LCD_CUDA(e, cudaMemcpy2DAsync(uv2.p, cap * 2 * sizeof(float), e->ws_uv.p, e->ws_cap * 2 * sizeof(float), e->ws_cap * 2 * sizeof(float),
+		                              e->ws_rows, cudaMemcpyDeviceToDevice, s));
+		LCD_CUDA(e, cudaStreamSynchronize(s));
+		std::swap(e->ws_ids.p, ids2.p);
+		std::swap(e->ws_ids.cap, ids2.cap);
+		std::swap(e->ws_uv.p, uv2.p);
+		std::swap(e->ws_uv.cap, uv2.cap);
+	}
+	e->ws_cap = std::max(e->ws_cap, cap);
+	if (static_cast<size_t>(max_id) + 1 > e->h_ws_slot_of_sig.size())
+		e->h_ws_slot_of_sig.resize(std::max<size_t>(max_id + 1, e->h_ws_slot_of_sig.size() * 3 / 2 + 1024), -1);
+	std::vector<int> slots(n_sigs);
+	for (int i = 0; i < n_sigs; ++i)
+	{
+		int slot = e->h_ws_slot_of_sig[sig_ids[i]];
+		if (slot < 0)
+		{
+			if (!e->ws_free.empty())
+			{
+				slot = e->ws_free.back();
+				e->ws_free.pop_back();
+			}
+			else
+				slot = e->ws_rows++;
+			e->h_ws_slot_of_sig[sig_ids[i]] = slot;
+			++e->ws_count;
+		}
+		slots[i] = slot;
+	}
+	const size_t wc = e->ws_cap;
+	LCD_CUDA(e, e->ws_ids.reserve(static_cast<size_t>(e->ws_rows) * wc, e->ws_ids.cap, false, s));
+	LCD_CUDA(e, e->ws_uv.reserve(static_cast<size_t>(e->ws_rows) * wc * 2, e->ws_uv.cap, false, s));
+	LCD_CUDA(e, e->ws_n.reserve(e->ws_rows, e->ws_n.cap, false, s));
+	for (int i = 0; i < n_sigs; ++i)
+	{
+		const size_t r = slots[i];
+		LCD_CUDA(e, cudaMemcpyAsync(e->ws_ids.p + r * wc, word_ids + static_cast<size_t>(i) * cap, n[i] * sizeof(int), cudaMemcpyHostToDevice, s));
+		LCD_CUDA(e, cudaMemcpyAsync(e->ws_uv.p + r * wc * 2, uv + static_cast<size_t>(i) * cap * 2, n[i] * 2 * sizeof(float), cudaMemcpyHostToDevice, s));
+		LCD_CUDA(e, cudaMemcpyAsync(e->ws_n.p + r, n + i, sizeof(int), cudaMemcpyHostToDevice, s));
+	}
+	LCD_CUDA(e, e->ws_slot_of_sig.reserve(e->h_ws_slot_of_sig.size(), 0, false, s));
+	LCD_CUDA(e, cudaMemcpyAsync(e->ws_slot_of_sig.p, e->h_ws_slot_of_sig.data(), e->h_ws_slot_of_sig.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, cudaStreamSynchronize(s));
+	return LCD_OK;
+}
+
+int lcd_sig_words_remove(lcd_engine * e, int sig_id)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (sig_id <= 0 || sig_id >= static_cast<int>(e->h_ws_slot_of_sig.size()) || e->h_ws_slot_of_sig[sig_id] < 0) return LCD_OK;
+	e->ws_free.push_back(e->h_ws_slot_of_sig[sig_id]);
+	e->h_ws_slot_of_sig[sig_id] = -1;
+	--e->ws_count;
+	const int minus1 = -1;
+	LCD_CUDA(e, cudaMemcpy(e->ws_slot_of_sig.p + sig_id, &minus1, sizeof(int), cudaMemcpyHostToDevice));
+	return LCD_OK;
+}
+
+int lcd_sig_words_count(const lcd_engine * e) { return e ? e->ws_count : 0; }
+
+int lcd_decide_epipolar_dev(lcd_engine * e, const int * d_word_ids, const float * d_uv, const int * d_n_per_frame, int n_frames, int nq_per_frame,
+                            const lcd_epipolar_params * p, void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (e->dc_last_frames == 0) LCD_FAIL(e, LCD_ERR_STATE, "no decision to check: run lcd_decide_batch_dev first");
+	if (!d_word_ids || !d_uv || !d_n_per_frame || !p) LCD_FAIL(e, LCD_ERR_INVALID, "null epipolar input");
+	if (n_frames != e->dc_last_frames) LCD_FAIL(e, LCD_ERR_INVALID, "the last decision has %d frames, not %d", e->dc_last_frames, n_frames);
+	if (nq_per_frame <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "nq_per_frame %d", nq_per_frame);
+	if (nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "at most %d words per frame", kMaxFrameQueries);
+	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	LCD_CUDA(e, e->ep_slot.reserve(n_frames, 0, false, s));
+	LCD_CUDA(e, e->ep_skip.reserve(n_frames, 0, false, s));
+	LCD_CUDA(e, e->ws_n.reserve(1, 0, true, s)); // an empty store: every hypothesis is a signature without words
+	LCD_CUDA(e, e->ws_ids.reserve(1, 0, false, s));
+	LCD_CUDA(e, e->ws_uv.reserve(2, 0, false, s));
+	epi_decide_prep_kernel<<<(n_frames + 127) / 128, 128, 0, s>>>(n_frames, e->dc_dec.p, e->ws_slot_of_sig.p,
+	                                                                 static_cast<int>(e->h_ws_slot_of_sig.size()), e->ep_slot.p, e->ep_skip.p);
+	LCD_CHECK_LAUNCH(e);
+	EpiArgs a{};
+	a.ids_a = d_word_ids;
+	a.uv_a = d_uv;
+	a.n_a = d_n_per_frame;
+	a.ids_b = e->ws_ids.p;
+	a.uv_b = e->ws_uv.p;
+	a.n_b = e->ws_n.p;
+	a.slot_b = e->ep_slot.p;
+	a.skip = e->ep_skip.p;
+	a.cap_a = nq_per_frame;
+	a.cap_b = std::max(e->ws_cap, 1);
+	LCD_TRY(launch_epipolar(e, n_frames, a, p, s));
+	epi_decide_apply_kernel<<<(n_frames + 127) / 128, 128, 0, s>>>(n_frames, e->ep_res.p, e->dc_dec.p, e->dc_hyp_valid ? e->d_hyp_id.p : nullptr,
+	                                                                  e->dc_hyp_valid ? e->d_hyp_slot.p : nullptr);
+	LCD_CHECK_LAUNCH(e);
+	e->ep_last_frames = n_frames;
+	return LCD_OK;
+}
+
+int lcd_epipolar_fetch(lcd_engine * e, int n_frames, lcd_epipolar_result * out)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (!out || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null output");
+	if (e->ep_last_frames == 0) LCD_FAIL(e, LCD_ERR_STATE, "no epipolar decision: run lcd_decide_epipolar_dev first");
+	if (n_frames > e->ep_last_frames) LCD_FAIL(e, LCD_ERR_INVALID, "the last epipolar decision has %d frames", e->ep_last_frames);
+	std::vector<int> hr(static_cast<size_t>(n_frames) * 8);
+	std::vector<double> hF(static_cast<size_t>(n_frames) * 9);
+	LCD_CUDA(e, cudaDeviceSynchronize());
+	LCD_CUDA(e, cudaMemcpy(hr.data(), e->ep_res.p, hr.size() * sizeof(int), cudaMemcpyDeviceToHost));
+	LCD_CUDA(e, cudaMemcpy(hF.data(), e->ep_F.p, hF.size() * sizeof(double), cudaMemcpyDeviceToHost));
+	epipolar_results(n_frames, hr.data(), hF.data(), out);
+	return LCD_OK;
 }
 
 // ---- brute-force matching of two descriptor sets: cv::BFMatcher ----------------------------------------

@@ -16,6 +16,7 @@
 #pragma once
 #include "common.cuh"
 #include "pnp_device.cuh"
+#include "ransac.cuh"
 #include "resolve.cuh"
 
 namespace lcd {
@@ -645,20 +646,6 @@ __host__ __device__ inline size_t pnp_smem_bytes(int cap)
 	return static_cast<size_t>(cap) * (12 + 8 + 4 + 4 + 2 + 2 + 1) + kMaxRansacIters * (6 * 2) + kPnpChunk * (4 + 6 * 8) + (28 * 32 + 32) * 8 + 1024;
 }
 
-__device__ inline int ransac_update_num_iters(double p, double ep, int modelPoints, int maxIters)
-{
-	p = fmax(p, 0.);
-	p = fmin(p, 1.);
-	ep = fmax(ep, 0.);
-	ep = fmin(ep, 1.);
-	double num = fmax(1. - p, 2.2250738585072014e-308);
-	double denom = 1. - pow(1. - ep, static_cast<double>(modelPoints));
-	if (denom < 2.2250738585072014e-308) return 0;
-	num = log(num);
-	denom = log(denom);
-	return denom >= 0 || -num >= maxIters * (-denom) ? maxIters : static_cast<int>(nearbyint(num / denom));
-}
-
 // block-wide sum of NV doubles per thread; result valid in all threads (via smem)
 template <int NV>
 __device__ inline void block_sum(double (&v)[NV], double * s_red /* [NV * 32] */, double * s_out /* [NV] */)
@@ -925,8 +912,7 @@ pnp_ransac_kernel(const PnpArgs a)
 					int idx_i;
 					for (;;)
 					{
-						state = static_cast<unsigned long long>(static_cast<unsigned>(state)) * 4164903690ull + static_cast<unsigned>(state >> 32);
-						idx_i = static_cast<int>(static_cast<unsigned>(state) % static_cast<unsigned>(n));
+						idx_i = cv_rng_uniform(state, n);
 						int j;
 						for (j = 0; j < i; ++j)
 							if (idx_i == sidx[it * 6 + j]) break;
