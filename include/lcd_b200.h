@@ -481,8 +481,8 @@ int lcd_verify_top_dev(lcd_engine * e, const void * d_queries, const float * d_u
  * prediction matrix, is shared.  These calls replace, for B clients at once, what Rtabmap::process does with one frame's raw
  * likelihood in localisation mode: adjustLikelihood (Rtabmap.cpp:2119-2121), BayesFilter::computePosterior (:2133), the hypothesis
  * selection and its checks (:2143-2233), and the verification of the accepted hypothesis with its rejections (:3133-3191).
- * The epipolar check (VhEp/Enabled) is lcd_decide_epipolar_dev, run between the decision and its verification.  Proximity detection,
- * retrieval and the graph walk stay the caller's.
+ * The epipolar check (VhEp/Enabled) is lcd_decide_epipolar_dev, run between the decision and its verification; proximity detection by
+ * space is lcd_decide_proximity_dev, run after it.  Retrieval and the graph optimisation stay the caller's.
  *
  * replaces: BayesFilter::BayesFilter + BayesFilter::reset (BayesFilter.cpp:43-68, :140-143) and Rtabmap's _highestHypothesis = (0, 0)
  * (Rtabmap.cpp:467, :1094) for n_clients clients at once; calling it again resets every client.  LCD_ERR_CAPACITY when the device
@@ -555,7 +555,10 @@ int lcd_decide_fetch(lcd_engine * e, int n_frames, lcd_decision * out);
  * decision was accepted (the other frames are not verified: ok = 0, no matches).  A failed registration becomes
  * LCD_DECIDE_VERIFY_REJECTED, a transform longer than max_loop_closure_distance (> 0) LCD_DECIDE_DISTANCE_REJECTED; both clear loop_id,
  * and the client's last highest hypothesis is left as it is.  d_queries / d_uv as lcd_process_batch_dev; n_frames must be the last
- * decision's.  Results through lcd_process_fetch (hypothesis = the final loop id) and lcd_decide_fetch. */
+ * decision's.  Results through lcd_process_fetch (hypothesis = the final loop id) and lcd_decide_fetch.  After lcd_decide_proximity_dev,
+ * a frame whose accepted place a proximity detection registered keeps LCD_DECIDE_ACCEPTED but is not registered again: lcd_process_fetch
+ * reports it with ok = 0 and no matches, and its transform is that of the lcd_proximity_fetch path with link_type
+ * LCD_PROXIMITY_LINK_GLOBAL (the reference adds that link with the proximity transform, Rtabmap.cpp:2902-2913, :3134). */
 int lcd_verify_decided_dev(lcd_engine * e, const void * d_queries, const float * d_uv, int n_frames, int nq_per_frame,
                            const lcd_verify_params * vp, void * stream);
 /* lcd_process_batch_dev with the decision: quantise + score against the map's real places (word ids and likelihood bit-identical to
@@ -703,10 +706,91 @@ int lcd_decide_epipolar_dev(lcd_engine * e, const int * d_word_ids, const float 
 /* the per-frame check results of the last lcd_decide_epipolar_dev (checked = 0: the frame did not reach the check) */
 int lcd_epipolar_fetch(lcd_engine * e, int n_frames, lcd_epipolar_result * out);
 
+/* ---- proximity detection by space (RGBD/ProximityBySpace) of many localisation clients --------------------------------------------
+ * Rtabmap::process, Rtabmap.cpp:2698-2934, in localisation mode, for every frame of the last decision at once.
+ *
+ * The optimised poses of the map set by lcd_clients_set_map (Rtabmap::_optimizedPoses): ids[n] the map's real places in the same ascending
+ * order (anything else: LCD_ERR_INVALID), poses[n][12] each place's rtabmap::Transform 3x4 row-major (a value that is not finite:
+ * LCD_ERR_INVALID, the reference asserts there, Graph.cpp:2278), and each place's neighbour links in CSR form: nbr_ids[nbr_ptr[i] ..
+ * nbr_ptr[i+1]) the places its kNeighbor / kNeighborMerged links point to (Signature::getLinks of those types, the links
+ * Memory::getNeighborsId follows with ignoreLoopIds, Memory.cpp:1824-1845, and Memory::getNeighborLinks returns, :1521-1560).  Links to
+ * places that are not in the map cannot join a path and are dropped.  Intermediate nodes (weight -1, Rtabmap/CreateIntermediateNodes)
+ * are not supported.  A failed call (LCD_ERR_CAPACITY: no device memory) keeps the previous poses; a later lcd_clients_set_map makes
+ * them stale and lcd_decide_proximity_dev returns LCD_ERR_STATE until poses are set for the new map. */
+int lcd_clients_set_map_poses(lcd_engine * e, const int * ids, int n, const float * poses, const int64_t * nbr_ptr, const int * nbr_ids);
+
+typedef struct lcd_proximity_params {
+	float local_radius;              /* RGBD/LocalRadius (10 m; > 0) */
+	float angle;                     /* RGBD/ProximityAngle (45 degrees; 0 = no angle filter) */
+	int max_paths;                   /* RGBD/ProximityMaxPaths (3; 1..16: <= 0, unlimited in the reference, is LCD_ERR_CAPACITY) */
+	int max_graph_depth;             /* RGBD/ProximityMaxGraphDepth (50; 0 = unlimited) */
+	float path_filtering_radius;     /* RGBD/ProximityPathFilteringRadius (1 m; <= 0 = off) */
+	float max_loop_closure_distance; /* RGBD/MaxLoopClosureDistance (0 = off): caps the filtering radius (Rtabmap.cpp:2822-2826) */
+	const lcd_verify_params * verify; /* the registrations' parameters */
+} lcd_proximity_params;
+
+#define LCD_PROXIMITY_OFF 0      /* the frame's enabled flag was 0 */
+#define LCD_PROXIMITY_RAN 1
+#define LCD_PROXIMITY_CAPACITY 2 /* more than 1024 places inside RGBD/LocalRadius: the frame was not segmented, its decision is untouched */
+#define LCD_PROXIMITY_LINK_LOCAL 1  /* Link::kLocalSpaceClosure */
+#define LCD_PROXIMITY_LINK_GLOBAL 2 /* Link::kGlobalClosure: the accepted place is the global hypothesis (:2902-2906) */
+#define LCD_DECIDE_PROXIMITY_SUPPRESSED 12 /* accepted, then a proximity detection was made near it on another place (:3193-3196) */
+
+typedef struct lcd_proximity_path {
+	float likelihood;  /* NearestPathKey (Rtabmap.cpp:1147-1176) of the path: its highest adjusted likelihood, */
+	int id;            /*   the place that has it (ties: the smaller distance), */
+	float distance;    /*   and (currentPoseInv * pose).getNormSquared() of that place */
+	int candidate_id;  /* the place the registration was attempted with */
+	int accepted;      /* registered, and the inverted transform's norm within the filtering radius */
+	int link_type;     /* LCD_PROXIMITY_LINK_* of the link the reference adds, 0 when not accepted */
+	lcd_verify_result result; /* Memory::computeTransform(candidate, frame) */
+} lcd_proximity_path;
+
+typedef struct lcd_proximity_result {
+	int status;        /* LCD_PROXIMITY_* */
+	int n_nearest;     /* places inside RGBD/LocalRadius (graph::findNearestNodes) */
+	int n_paths;       /* paths of Rtabmap::getPaths */
+	int n_attempts;    /* registrations attempted (localVisualPathsChecked) */
+	int suppressed_id; /* loopIdSuppressedByProximity (0: none) */
+	lcd_proximity_path paths[16]; /* the first n_attempts, in the order they were attempted */
+} lcd_proximity_result;
+
+/* Proximity detection on the last decision, after lcd_decide_batch_dev (and lcd_decide_epipolar_dev) and before lcd_verify_decided_dev.
+ * Per frame with enabled[f] != 0 (the caller's check of Rtabmap.cpp:2698-2723: RGBD/ProximityBySpace, RGB-D SLAM mode, weight >= 0,
+ * Rtabmap/StartNewMapOnLoopClosure, optimiser iterations, small displacement / too fast movement), frame_poses[f][12] the frame's
+ * optimised pose (host arrays):
+ *  1. graph::findNearestNodes(frame, poses, local_radius) (Graph.cpp:2239-2325): squared distances in float, x + y then + z, places with
+ *     a squared distance < local_radius^2 (rtflann's radius result sets), ids >= 1.  In localisation mode the graph-depth filter of
+ *     Rtabmap.cpp:2740-2789 does not run (Memory::isIncremental() is false) and no map place is in the short-term memory (:2773): the
+ *     map's places are loaded into the working memory (Memory.cpp:262-272), the short-term memory holds the session's own frames (:1263).
+ *  2. Rtabmap::getPaths (Rtabmap.cpp:5303-5382): the nearest place not in a path yet, Memory::getNeighborsId(it, max_graph_depth, ...)
+ *     over neighbour links and through places within the radius only, then the reached places not in a path yet, in ascending id order,
+ *     each admitted when it is the first or links to a place already admitted (one reachable only through a higher id waits for a later
+ *     path).
+ *  3. The paths' NearestPathKey from the decision's adjusted likelihood (0 for skipped or held frames, which computed none).
+ *  4. The paths in descending key order (:2827-2934): graph::findNearestPoses with the radius and RGBD/ProximityAngle, the key's place
+ *     when its likelihood is > 0 and it passed, else the nearest place left; attempted when closer than the filtering radius, until
+ *     max_paths attempts.  The frame is never linked to a map place, so signature->hasLink does not fire.
+ * All attempts of the batch are then registered in one launch (store rows as FROM, the frame's d_queries / d_uv rows as TO, as
+ * lcd_verify_decided_dev takes them, null guess: RGBD/ProximityOdomGuess = false).  A registration is accepted when it succeeds and the
+ * inverted transform's norm is within the filtering radius.  When the frame's decision is accepted and its place lies within the radius,
+ * an accepted detection on it keeps the decision (its transform is the proximity path's; lcd_verify_decided_dev skips the frame), one on
+ * another place makes it LCD_DECIDE_PROXIMITY_SUPPRESSED with loop id 0 (:2894-2911, :3193-3196).  Float transform inverses are
+ * computed as [R^T | -R^T t]; the reference's Eigen inverse may differ in the last bits.
+ * The registrations read row f of d_queries / d_uv for frame f in place (no copy); slots not attempted register nothing.
+ * Binary engines only.  LCD_ERR_STATE without a decision, without poses for the current map, with an empty signature store, when the
+ * decision already had its proximity step, or when it was already verified (lcd_verify_decided_dev, lcd_process_decide_batch_dev: the
+ * proximity step comes first, as in the reference); LCD_ERR_INVALID for n_frames other than the decision's, bad parameters or a pose that
+ * is not finite; LCD_ERR_CAPACITY for max_paths outside 1..16 or nq_per_frame > 4096. */
+int lcd_decide_proximity_dev(lcd_engine * e, const void * d_queries, const float * d_uv, int n_frames, int nq_per_frame, const float * frame_poses,
+                             const int * enabled, const lcd_proximity_params * pp, void * stream);
+/* the per-frame results of the last lcd_decide_proximity_dev; synchronises */
+int lcd_proximity_fetch(lcd_engine * e, int n_frames, lcd_proximity_result * out);
+
 /* ---- measurement hooks ---------------------------------------------------------------
  * Optional per-kernel timing with CUDA events recorded on the launching stream around
  * every launch of kernel class `which` (0 = dictionary NN, 1 = resolve, 2 = score, 3 = pair
- * matching, 4 = PnP RANSAC, 5 = all ORB kernels, 6 = the epipolar check).
+ * matching, 4 = PnP RANSAC, 5 = all ORB kernels, 6 = the epipolar check, 7 = the proximity candidate kernel).
  * lcd_profile_read synchronises, returns the summed device time and the launch count
  * since the last reset. */
 #define LCD_PROF_NN 0
@@ -716,6 +800,7 @@ int lcd_epipolar_fetch(lcd_engine * e, int n_frames, lcd_epipolar_result * out);
 #define LCD_PROF_PNP 4
 #define LCD_PROF_ORB 5
 #define LCD_PROF_EPIPOLAR 6
+#define LCD_PROF_PROXIMITY 7
 int lcd_profile_enable(lcd_engine * e, int on);
 int lcd_profile_read(lcd_engine * e, int which, double * total_ms, long long * launches);
 int lcd_profile_reset(lcd_engine * e);

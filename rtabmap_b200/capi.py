@@ -119,10 +119,36 @@ def _epi_dict(r: EpipolarResult) -> dict:
             "iterations_run": r.iterations_run, "raised": r.raised, "F": np.array(r.F[:], np.float64).reshape(3, 3)}
 
 
+class ProximityParams(C.Structure):
+    """lcd_proximity_params (RGBD/LocalRadius, RGBD/ProximityAngle in degrees, RGBD/ProximityMaxPaths, RGBD/ProximityMaxGraphDepth,
+    RGBD/ProximityPathFilteringRadius, RGBD/MaxLoopClosureDistance, the registrations' lcd_verify_params)."""
+    _fields_ = [
+        ("local_radius", C.c_float), ("angle", C.c_float), ("max_paths", C.c_int), ("max_graph_depth", C.c_int),
+        ("path_filtering_radius", C.c_float), ("max_loop_closure_distance", C.c_float), ("verify", C.POINTER(VerifyParams)),
+    ]
+
+
+class ProximityPath(C.Structure):
+    _fields_ = [
+        ("likelihood", C.c_float), ("id", C.c_int), ("distance", C.c_float), ("candidate_id", C.c_int), ("accepted", C.c_int),
+        ("link_type", C.c_int), ("result", VerifyResult),
+    ]
+
+
+class ProximityResult(C.Structure):
+    _fields_ = [
+        ("status", C.c_int), ("n_nearest", C.c_int), ("n_paths", C.c_int), ("n_attempts", C.c_int), ("suppressed_id", C.c_int),
+        ("paths", ProximityPath * 16),
+    ]
+
+
 # frame flags and decision statuses of lcd_decide_batch_dev (lcd_b200.h)
 FRAME_SKIP, FRAME_HOLD, FRAME_AGGRESSIVE = 1, 2, 4
 DECIDE_STATUS = ("skipped", "held", "no hypothesis", "under threshold", "under ratio", "single hypothesis", "ratio", "last null", "accepted",
-                 "verification rejected", "distance rejected", "epipolar rejected")
+                 "verification rejected", "distance rejected", "epipolar rejected", "proximity suppressed")
+# lcd_proximity_result.status and lcd_proximity_path.link_type
+PROXIMITY_OFF, PROXIMITY_RAN, PROXIMITY_CAPACITY = 0, 1, 2
+LINK_LOCAL_SPACE, LINK_GLOBAL = 1, 2
 DECISION_DTYPE = np.dtype([("highest_id", np.int32), ("highest_value", np.float32), ("loop_id", np.int32), ("status", np.int32)])
 
 
@@ -231,6 +257,9 @@ SIGNATURES = {
     "lcd_sig_words_count": (_I, [_P]),
     "lcd_decide_epipolar_dev": (_I, [_P, _P, _P, _P, _I, _I, _P, _P]),
     "lcd_epipolar_fetch": (_I, [_P, _I, _P]),
+    "lcd_clients_set_map_poses": (_I, [_P, _P, _I, _P, _P, _P]),
+    "lcd_decide_proximity_dev": (_I, [_P, _P, _P, _I, _I, _P, _P, _P, _P]),
+    "lcd_proximity_fetch": (_I, [_P, _I, _P]),
     "lcd_profile_enable": (_I, [_P, _I]),
     "lcd_profile_read": (_I, [_P, _I, _P, _P]),
     "lcd_profile_reset": (_I, [_P]),
@@ -1005,6 +1034,48 @@ class Engine:
                                                             float(nndr), int(cmp_new), int(ns), int(n_total), C.byref(vp), _ptr(c), _ptr(f),
                                                             C.byref(dp), C.c_void_p(d_words_out or None), C.c_void_p(d_like_out or None),
                                                             C.c_void_p(d_posterior_out or None), C.c_void_p(stream or None)))
+
+    def clients_set_map_poses(self, ids, poses, nbr_ptr, nbr_ids):
+        """The optimised pose of every real place of the current map (ids ascending as set_map's, poses [n, 3, 4] float32) and its
+        neighbour links in CSR form (nbr_ptr [n+1], nbr_ids: the linked places' ids)."""
+        i = _i32(ids)
+        p = np.ascontiguousarray(poses, np.float32).reshape(len(i), 12)
+        cp = np.ascontiguousarray(nbr_ptr, np.int64)
+        nb = _i32(nbr_ids) if len(nbr_ids) else np.zeros(1, np.int32)
+        self._check(self._lib.lcd_clients_set_map_poses(self._h, _ptr(i), len(i), _ptr(p), _ptr(cp), _ptr(nb)))
+
+    @staticmethod
+    def proximity_params(vp: "VerifyParams", local_radius: float = 10.0, angle: float = 45.0, max_paths: int = 3, max_graph_depth: int = 50,
+                         path_filtering_radius: float = 1.0, max_loop_closure_distance: float = 0.0) -> ProximityParams:
+        """lcd_proximity_params with the reference's defaults; vp must outlive the call that uses them."""
+        return ProximityParams(float(local_radius), float(angle), int(max_paths), int(max_graph_depth), float(path_filtering_radius),
+                               float(max_loop_closure_distance), C.pointer(vp))
+
+    def decide_proximity_dev(self, d_queries: int, d_uv: int, n_frames: int, nq: int, frame_poses, enabled, pp: ProximityParams,
+                             stream: int = 0):
+        """Proximity detection by space on the last decision: frame_poses [n_frames, 3, 4] and enabled [n_frames] (host), the frames'
+        descriptors and keypoints on the device as verify_decided_dev takes them."""
+        p = np.ascontiguousarray(frame_poses, np.float32).reshape(-1)
+        en = _i32(enabled)
+        if len(p) != 12 * n_frames or len(en) != n_frames:
+            raise LcdError(-1, f"frame_poses and enabled need {n_frames} entries")
+        self._check(self._lib.lcd_decide_proximity_dev(self._h, C.c_void_p(d_queries), C.c_void_p(d_uv), int(n_frames), int(nq), _ptr(p),
+                                                        _ptr(en), C.byref(pp), C.c_void_p(stream or None)))
+
+    def proximity_fetch(self, n_frames: int):
+        """The last proximity step's per-frame records: dicts with status, n_nearest, n_paths, suppressed_id and the attempted paths."""
+        out = (ProximityResult * n_frames)()
+        self._check(self._lib.lcd_proximity_fetch(self._h, int(n_frames), out))
+        recs = []
+        for r in out:
+            paths = []
+            for j in range(r.n_attempts):
+                q = r.paths[j]
+                paths.append({"likelihood": np.float32(q.likelihood), "id": q.id, "distance": np.float32(q.distance), "candidate_id": q.candidate_id,
+                              "accepted": bool(q.accepted), "link_type": q.link_type, "result": self._results([q.result], 1)[0]})
+            recs.append({"status": r.status, "n_nearest": r.n_nearest, "n_paths": r.n_paths, "n_attempts": r.n_attempts,
+                         "suppressed_id": r.suppressed_id, "paths": paths})
+        return recs
 
     # -- word-range sharding ----------------------------------------------------------------------
     @staticmethod

@@ -299,12 +299,13 @@ __global__ void decide_select_kernel(const DecideMap m, const DecideSelect a)
 }
 
 // Rtabmap.cpp:3156-3167 after the verification of the accepted hypotheses: a failed registration, or (max_dist > 0) a transform longer
-// than RGBD/MaxLoopClosureDistance, rejects the loop closure (the last highest hypothesis is left as it is)
+// than RGBD/MaxLoopClosureDistance, rejects the loop closure (the last highest hypothesis is left as it is).  skip (may be null): frames
+// whose hypothesis a proximity detection already registered (proximity.cuh), which keep their decision.
 __global__ void decide_verified_kernel(int n_frames, const int * __restrict__ ok, const float * __restrict__ T, float max_dist,
-                                       Decision * __restrict__ dec, int * __restrict__ hyp_id)
+                                       Decision * __restrict__ dec, int * __restrict__ hyp_id, const unsigned char * __restrict__ skip)
 {
 	const int f = blockIdx.x * blockDim.x + threadIdx.x;
-	if (f >= n_frames || dec[f].status != kDcAccepted) return;
+	if (f >= n_frames || dec[f].status != kDcAccepted || (skip && skip[f])) return;
 	int status = kDcAccepted;
 	if (!ok[f]) status = kDcVerifyRejected;
 	else if (max_dist > 0.f)

@@ -22,6 +22,7 @@
 #include "decide.cuh"
 #include "verify.cuh"
 #include "epipolar.cuh"
+#include "proximity.cuh"
 #include "match_bf.cuh"
 #include "orb.cuh"
 
@@ -344,6 +345,24 @@ struct lcd_engine
 	int dc_last_frames = 0;               // frames of the last decision (0: none)
 	bool dc_hyp_valid = false;            // d_hyp_id / d_hyp_slot hold the last decision's accepted hypotheses
 	float dc_max_dist = 0.f;              // RGBD/MaxLoopClosureDistance of the last decision
+	std::vector<int> dc_h_ids;            // the current map's ids (host copy)
+	// proximity detection by space (lcd_clients_set_map_poses / lcd_decide_proximity_dev, proximity.cuh)
+	struct MapPoses
+	{
+		DevBuf<float> poses;  // [n][12] optimised pose of every real place
+		DevBuf<int> nbr_ptr;  // [n+1] neighbour links by row
+		DevBuf<int> nbr_row;  // their target rows
+	};
+	std::unique_ptr<MapPoses> px_map;     // the poses of map version px_ver
+	int px_ver = -1;
+	DevBuf<float> px_frame_pose;
+	DevBuf<int> px_enabled, px_slot, px_row, px_nto;
+	DevBuf<ProxRecord> px_rec;
+	DevBuf<PackedVerifyResult> px_res;
+	DevBuf<unsigned char> px_skip;
+	int px_last_frames = 0, px_max_paths = 0;
+	bool px_valid = false;                // px_skip belongs to the last decision
+	bool dc_verified = false;             // the last decision went through lcd_verify_decided_dev
 	// verification scratch
 	DevBuf<uint32_t> v_df, v_dt;
 	DevBuf<float> v_xyz, v_uv, v_obj, v_img, v_T, v_xyz_to, v_obj_to;
@@ -400,7 +419,7 @@ struct lcd_engine
 	{
 		std::vector<cudaEvent_t> ev; // start/stop pairs
 		size_t used = 0;
-	} prof[7];
+	} prof[8];
 
 	// tuning knobs (env: LCD_NN_CTAS_PER_SM, LCD_NN_TQ, LCD_NN_VARIANT, LCD_SCORE_BLOCKS)
 	int nn_ctas_per_sm = 2, nn_tq = 8, nn_variant = 2, score_blocks = 32;
@@ -1346,7 +1365,7 @@ int lcd_profile_reset(lcd_engine * e)
 
 int lcd_profile_read(lcd_engine * e, int which, double * total_ms, long long * launches)
 {
-	if (!e || which < 0 || which > 6) return LCD_ERR_INVALID;
+	if (!e || which < 0 || which > 7) return LCD_ERR_INVALID;
 	LCD_TRY(set_device(e));
 	LCD_CUDA(e, cudaDeviceSynchronize());
 	auto & p = e->prof[which];
@@ -2763,6 +2782,7 @@ struct MatchSrc
 	int n_to_all;
 	int cap_to;
 	const float * xyz_to; // 3-D points of the TO side (words3B) or nullptr
+	const int * to_row = nullptr; // TO row of each pair (nullptr: the pair's own row)
 };
 
 static int launch_match(lcd_engine * e, int n_pairs, int cap, float nndr, bool want_ids, cudaStream_t s, const MatchSrc * src = nullptr)
@@ -2793,6 +2813,7 @@ static int launch_match(lcd_engine * e, int n_pairs, int cap, float nndr, bool w
 		a.n_to_all = src->n_to_all;
 		a.cap_to = src->cap_to;
 		a.xyz_to = src->xyz_to;
+		a.to_row = src->to_row;
 	}
 	else
 	{
@@ -2932,6 +2953,7 @@ static int launch_second_pass(lcd_engine * e, int n_pairs, int cap, const lcd_ve
 		a.n_to = src->n_to;
 		a.n_to_all = src->n_to_all;
 		a.cap_to = src->cap_to;
+		a.to_row = src->to_row;
 	}
 	else
 	{
@@ -4116,6 +4138,7 @@ int lcd_clients_set_map(lcd_engine * e, const int * ids, int n, const int64_t * 
 	e->dc_map_ver = e->dc_next_ver++;
 	e->dc_versions[e->dc_map_ver] = std::move(ver);
 	e->dc_n = n;
+	e->dc_h_ids.assign(ids, ids + n);
 	e->dc_lc0 = prediction_lc[0];
 	e->dc_vpp = virtual_place_prior;
 	prune_map_versions(e);
@@ -4259,6 +4282,9 @@ static int decide_launch(lcd_engine * e, const float * d_like, int n_frames, int
 	for (int c : e->dc_active) e->dc_ver[c] = e->dc_map_ver;
 	e->dc_last_frames = n_frames;
 	e->dc_hyp_valid = true;
+	e->px_valid = false;
+	e->px_last_frames = 0;
+	e->dc_verified = false;
 	e->dc_max_dist = dp->max_loop_closure_distance;
 	return LCD_OK;
 }
@@ -4300,8 +4326,10 @@ static int verify_decided(lcd_engine * e, const uint32_t * d_q, const float * d_
 	LCD_TRY(launch_match(e, n_frames, cap, vp->nndr, false, s, &src));
 	LCD_TRY(launch_pnp(e, n_frames, cap, vp, s));
 	LCD_TRY(launch_second_pass(e, n_frames, cap, vp, s, &src));
-	decide_verified_kernel<<<(n_frames + 127) / 128, 128, 0, s>>>(n_frames, e->v_ok.p, e->v_T.p, e->dc_max_dist, e->dc_dec.p, e->d_hyp_id.p);
+	decide_verified_kernel<<<(n_frames + 127) / 128, 128, 0, s>>>(n_frames, e->v_ok.p, e->v_T.p, e->dc_max_dist, e->dc_dec.p, e->d_hyp_id.p,
+	                                                             e->px_valid ? e->px_skip.p : nullptr);
 	LCD_CHECK_LAUNCH(e);
+	e->dc_verified = true;
 	return LCD_OK;
 }
 
@@ -4345,6 +4373,187 @@ int lcd_process_decide_batch_dev(lcd_engine * e, const void * d_queries, const f
 	                     d_like, s));
 	LCD_TRY(decide_launch(e, d_like, n_frames, ns, dp, d_posterior_out, s));
 	return verify_decided(e, d_q, d_uv, n_frames, nq_per_frame, vp, s);
+}
+
+// ---- proximity detection by space (proximity.cuh) ---------------------------------------------------------------------
+static_assert(sizeof(ProxPath) == 16, "lcd_proximity_path key layout");
+
+int lcd_clients_set_map_poses(lcd_engine * e, const int * ids, int n, const float * poses, const int64_t * nbr_ptr, const int * nbr_ids)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (e->dc_map_ver < 0) LCD_FAIL(e, LCD_ERR_STATE, "no map: call lcd_clients_set_map first");
+	if (!ids || !poses || !nbr_ptr || n != e->dc_n - 1) LCD_FAIL(e, LCD_ERR_INVALID, "n = %d, but the map holds %d real places", n, e->dc_n - 1);
+	for (int i = 0; i < n; ++i)
+		if (ids[i] != e->dc_h_ids[i + 1]) LCD_FAIL(e, LCD_ERR_INVALID, "ids[%d] = %d differs from the map's %d", i, ids[i], e->dc_h_ids[i + 1]);
+	for (size_t k = 0; k < 12 * static_cast<size_t>(n); ++k)
+		if (!std::isfinite(poses[k])) LCD_FAIL(e, LCD_ERR_INVALID, "the pose of place %d is not finite", ids[k / 12]);
+	if (nbr_ptr[0] != 0) LCD_FAIL(e, LCD_ERR_INVALID, "nbr_ptr[0] must be 0");
+	for (int i = 0; i < n; ++i)
+		if (nbr_ptr[i + 1] < nbr_ptr[i]) LCD_FAIL(e, LCD_ERR_INVALID, "nbr_ptr must not decrease");
+	if (nbr_ptr[n] > INT32_MAX || (nbr_ptr[n] > 0 && !nbr_ids)) LCD_FAIL(e, LCD_ERR_INVALID, "bad neighbour links");
+	// links to places outside the map (not in the working memory) can never join a path: they are dropped here
+	std::vector<int> ptr(n + 1, 0), row;
+	row.reserve(static_cast<size_t>(nbr_ptr[n]));
+	for (int i = 0; i < n; ++i)
+	{
+		for (int64_t k = nbr_ptr[i]; k < nbr_ptr[i + 1]; ++k)
+		{
+			const int * it = std::lower_bound(ids, ids + n, nbr_ids[k]);
+			if (it != ids + n && *it == nbr_ids[k]) row.push_back(static_cast<int>(it - ids));
+		}
+		ptr[i + 1] = static_cast<int>(row.size());
+	}
+	cudaStream_t s = e->stream;
+	auto m = std::make_unique<lcd_engine::MapPoses>();
+	if (m->poses.reserve(12 * static_cast<size_t>(n), 0, false, s) != cudaSuccess || m->nbr_ptr.reserve(n + 1, 0, false, s) != cudaSuccess ||
+	    m->nbr_row.reserve(std::max<size_t>(row.size(), 1), 0, false, s) != cudaSuccess)
+	{
+		cudaGetLastError();
+		LCD_FAIL(e, LCD_ERR_CAPACITY, "no device memory for the poses and links of %d places", n);
+	}
+	LCD_CUDA(e, cudaMemcpyAsync(m->poses.p, poses, 12 * static_cast<size_t>(n) * sizeof(float), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, cudaMemcpyAsync(m->nbr_ptr.p, ptr.data(), (n + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
+	if (!row.empty()) LCD_CUDA(e, cudaMemcpyAsync(m->nbr_row.p, row.data(), row.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, cudaStreamSynchronize(s));
+	// kernels of the last proximity step may still read the poses this call replaces
+	LCD_CUDA(e, cudaDeviceSynchronize());
+	e->px_map = std::move(m);
+	e->px_ver = e->dc_map_ver;
+	return LCD_OK;
+}
+
+// Memory::computeTransform(place, frame) of n_pairs arbitrary (frame row, place) pairs in one launch, with a null guess
+// (RGBD/ProximityOdomGuess = false): FROM = the store row d_slot[i] (-1: none) with its cached dictionary, TO = row d_row[i] of the frames'
+// d_q / d_uv (nq rows each), d_n_to[i] of its descriptors (0: the pair is not registered)
+static int verify_frame_pairs(lcd_engine * e, const uint32_t * d_q, const float * d_uv, int n_pairs, int nq, const int * d_row, const int * d_n_to,
+                              const int * d_slot, const lcd_verify_params * vp, cudaStream_t s)
+{
+	const int cap = std::max(e->st_cap, nq);
+	MatchSrc src{e->st_desc.p, e->st_xyz.p, e->st_n.p, d_slot, e->st_cap, d_q, d_uv, d_n_to, 0, nq, nullptr, d_row};
+	LCD_TRY(launch_match(e, n_pairs, cap, vp->nndr, false, s, &src));
+	LCD_TRY(launch_pnp(e, n_pairs, cap, vp, s));
+	return launch_second_pass(e, n_pairs, cap, vp, s, &src);
+}
+
+int lcd_decide_proximity_dev(lcd_engine * e, const void * d_queries, const float * d_uv, int n_frames, int nq_per_frame, const float * frame_poses,
+                             const int * enabled, const lcd_proximity_params * pp, void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(require_binary(e, "lcd_decide_proximity_dev"));
+	LCD_TRY(set_device(e));
+	if (!d_queries || !d_uv || !frame_poses || !enabled || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null or empty frame input");
+	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
+	if (!pp || !pp->verify) LCD_FAIL(e, LCD_ERR_INVALID, "null proximity or verification parameters");
+	const lcd_verify_params * vp = pp->verify;
+	if (vp->iterations > kMaxRansacIters) LCD_FAIL(e, LCD_ERR_CAPACITY, "Vis/Iterations > %d", kMaxRansacIters);
+	if (!(pp->local_radius > 0.f) || !std::isfinite(pp->local_radius)) LCD_FAIL(e, LCD_ERR_INVALID, "RGBD/LocalRadius must be > 0");
+	if (!(pp->angle >= 0.f) || !std::isfinite(pp->angle)) LCD_FAIL(e, LCD_ERR_INVALID, "RGBD/ProximityAngle must be >= 0");
+	if (pp->max_graph_depth < 0) LCD_FAIL(e, LCD_ERR_INVALID, "RGBD/ProximityMaxGraphDepth must be >= 0");
+	if (!std::isfinite(pp->path_filtering_radius) || !(pp->max_loop_closure_distance >= 0.f) || !std::isfinite(pp->max_loop_closure_distance))
+		LCD_FAIL(e, LCD_ERR_INVALID, "bad RGBD/ProximityPathFilteringRadius or RGBD/MaxLoopClosureDistance");
+	// <= 0 is "no limit" in the reference (Rtabmap.cpp:2829); at most kPxMaxPaths attempts per frame are supported
+	if (pp->max_paths <= 0 || pp->max_paths > kPxMaxPaths) LCD_FAIL(e, LCD_ERR_CAPACITY, "RGBD/ProximityMaxPaths must be 1..%d", kPxMaxPaths);
+	if (e->st_cap == 0) LCD_FAIL(e, LCD_ERR_STATE, "the signature store is empty: nothing to verify against");
+	if (e->dc_last_frames == 0 || !e->dc_hyp_valid) LCD_FAIL(e, LCD_ERR_STATE, "no decision: run lcd_decide_batch_dev first");
+	if (e->dc_verified) LCD_FAIL(e, LCD_ERR_STATE, "the decision was already verified: run proximity detection before lcd_verify_decided_dev");
+	if (n_frames != e->dc_last_frames) LCD_FAIL(e, LCD_ERR_INVALID, "the last decision has %d frames, not %d", e->dc_last_frames, n_frames);
+	if (!e->px_map || e->px_ver != e->dc_map_ver) LCD_FAIL(e, LCD_ERR_STATE, "no poses for the current map: call lcd_clients_set_map_poses");
+	if (e->px_last_frames) LCD_FAIL(e, LCD_ERR_STATE, "proximity detection already ran on this decision");
+	for (int k = 0; k < 12 * n_frames; ++k)
+		if (!std::isfinite(frame_poses[k])) LCD_FAIL(e, LCD_ERR_INVALID, "the pose of frame %d is not finite", k / 12);
+	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	const int mp = pp->max_paths, n_pairs = n_frames * mp;
+	LCD_CUDA(e, e->px_frame_pose.reserve(12 * static_cast<size_t>(n_frames), 0, false, s));
+	LCD_CUDA(e, e->px_enabled.reserve(n_frames, 0, false, s));
+	LCD_CUDA(e, e->px_rec.reserve(n_frames, 0, false, s));
+	LCD_CUDA(e, e->px_skip.reserve(n_frames, 0, false, s));
+	LCD_CUDA(e, e->px_slot.reserve(n_pairs, 0, false, s));
+	LCD_CUDA(e, e->px_row.reserve(n_pairs, 0, false, s));
+	LCD_CUDA(e, e->px_nto.reserve(n_pairs, 0, false, s));
+	LCD_CUDA(e, e->px_res.reserve(n_pairs, 0, false, s));
+	LCD_CUDA(e, cudaMemcpyAsync(e->px_frame_pose.p, frame_poses, 12 * static_cast<size_t>(n_frames) * sizeof(float), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, cudaMemcpyAsync(e->px_enabled.p, enabled, n_frames * sizeof(int), cudaMemcpyHostToDevice, s));
+	// RGBD/ProximityPathFilteringRadius, capped by RGBD/MaxLoopClosureDistance (Rtabmap.cpp:2822-2826)
+	float fr = pp->path_filtering_radius;
+	if (pp->max_loop_closure_distance > 0.f && (fr <= 0.f || pp->max_loop_closure_distance < fr)) fr = pp->max_loop_closure_distance;
+	ProxArgs a{};
+	a.n = e->dc_n - 1;
+	a.ids = e->dc_versions.at(e->dc_map_ver)->ids.p + 1;
+	a.poses = e->px_map->poses.p;
+	a.nbr_ptr = e->px_map->nbr_ptr.p;
+	a.nbr_row = e->px_map->nbr_row.p;
+	a.frame_pose = e->px_frame_pose.p;
+	a.enabled = e->px_enabled.p;
+	a.flags = e->dc_tab.p + n_frames;
+	a.adj = e->dc_adj.p;
+	a.dec = e->dc_dec.p;
+	a.sig_slot = e->st_slot_of_sig.p;
+	a.slot_cap = e->st_slot_of_sig.p ? static_cast<int>(e->h_slot_of_sig.size()) : 0;
+	a.radius = pp->local_radius;
+	// _proximityAngle *= M_PI/180.0f, a float (Rtabmap.cpp:609-612)
+	a.angle = static_cast<float>(static_cast<double>(pp->angle) * (M_PI / 180.0));
+	a.filter_radius = fr;
+	a.max_paths = mp;
+	a.max_depth = pp->max_graph_depth;
+	a.rec = e->px_rec.p;
+	a.pair_slot = e->px_slot.p;
+	a.pair_row = e->px_row.p;
+	a.pair_n_to = e->px_nto.p;
+	a.nq = nq_per_frame;
+	prof_mark(e, LCD_PROF_PROXIMITY, s);
+	proximity_paths_kernel<<<n_frames, kPxThreads, 0, s>>>(a);
+	prof_mark(e, LCD_PROF_PROXIMITY, s);
+	LCD_CHECK_LAUNCH(e);
+	LCD_TRY(verify_frame_pairs(e, static_cast<const uint32_t *>(d_queries), d_uv, n_pairs, nq_per_frame, e->px_row.p, e->px_nto.p, e->px_slot.p, vp, s));
+	pack_verify_results_kernel<<<(n_pairs + 127) / 128, 128, 0, s>>>(n_pairs, e->v_ok.p, e->v_nm.p, e->v_ninl.p, e->v_iters.p, e->v_rvec.p, e->v_tvec.p,
+	                                                                e->v_T.p, e->v_cov6.p, e->px_res.p);
+	LCD_CHECK_LAUNCH(e);
+	proximity_apply_kernel<<<(n_frames + 127) / 128, 128, 0, s>>>(n_frames, mp, fr, e->v_ok.p, e->v_T.p, e->px_rec.p, e->dc_dec.p, e->d_hyp_id.p,
+	                                                             e->d_hyp_slot.p, e->px_skip.p);
+	LCD_CHECK_LAUNCH(e);
+	e->px_last_frames = n_frames;
+	e->px_max_paths = mp;
+	e->px_valid = true;
+	return LCD_OK;
+}
+
+int lcd_proximity_fetch(lcd_engine * e, int n_frames, lcd_proximity_result * out)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (!out || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null output");
+	if (e->px_last_frames == 0) LCD_FAIL(e, LCD_ERR_STATE, "no proximity detection: run lcd_decide_proximity_dev first");
+	if (n_frames > e->px_last_frames) LCD_FAIL(e, LCD_ERR_INVALID, "the last proximity detection has %d frames", e->px_last_frames);
+	LCD_CUDA(e, cudaDeviceSynchronize());
+	const int mp = e->px_max_paths;
+	std::vector<ProxRecord> rec(n_frames);
+	std::vector<PackedVerifyResult> res(static_cast<size_t>(n_frames) * mp);
+	LCD_CUDA(e, cudaMemcpy(rec.data(), e->px_rec.p, n_frames * sizeof(ProxRecord), cudaMemcpyDeviceToHost));
+	LCD_CUDA(e, cudaMemcpy(res.data(), e->px_res.p, res.size() * sizeof(PackedVerifyResult), cudaMemcpyDeviceToHost));
+	for (int f = 0; f < n_frames; ++f)
+	{
+		const ProxRecord & r = rec[f];
+		lcd_proximity_result & o = out[f];
+		memset(&o, 0, sizeof(o));
+		o.status = r.status;
+		o.n_nearest = r.n_nearest;
+		o.n_paths = r.n_paths;
+		o.n_attempts = r.n_attempts;
+		o.suppressed_id = r.suppressed;
+		for (int j = 0; j < r.n_attempts; ++j)
+		{
+			lcd_proximity_path & p = o.paths[j];
+			p.likelihood = r.path[j].likelihood;
+			p.id = r.path[j].id;
+			p.distance = r.path[j].distance;
+			p.candidate_id = r.path[j].candidate;
+			p.accepted = r.accepted[j];
+			p.link_type = r.link_type[j];
+			memcpy(&p.result, &res[static_cast<size_t>(f) * mp + j], sizeof(lcd_verify_result));
+		}
+	}
+	return LCD_OK;
 }
 
 // ---- word-range sharding ---------------------------------------------------------------------

@@ -48,6 +48,7 @@ struct MatchArgs
 	const int * n_to;           // [n_pairs] or nullptr (= n_to_all)
 	int n_to_all;
 	int cap_to;                 // row stride of the TO arrays
+	const int * to_row;         // nullptr: TO row = pair; else the TO row of each pair
 	int cap;                    // stride of the outputs and size of the shared-memory arrays (>= both)
 	float nndr; // Vis/CorNNDR
 	// FROM dictionaries cached per signature-store row (from_slot only, else nullptr): see from_dict_build_kernel
@@ -318,7 +319,7 @@ pair_match_kernel(const MatchArgs a)
 	const int nt = min(a.n_to ? a.n_to[pair] : a.n_to_all, min(cap, a.cap_to));
 	const size_t base = static_cast<size_t>(pair) * cap;
 	const size_t fbase = static_cast<size_t>(frow >= 0 ? frow : 0) * a.cap_from;
-	const size_t tbase = static_cast<size_t>(pair) * a.cap_to;
+	const size_t tbase = static_cast<size_t>(a.to_row ? a.to_row[pair] : pair) * a.cap_to;
 	const uint32_t * F = a.desc_from + fbase * NW;
 	const uint32_t * T = a.desc_to + tbase * NW;
 
@@ -469,6 +470,7 @@ struct GuessMatchArgs
 	const int * n_to;
 	int n_to_all;
 	int cap_to;
+	const int * to_row;     // nullptr: TO row = pair
 	int cap;
 	const int * ok1;        // [n_pairs] first pass accepted
 	const double * rvec;    // [n_pairs][3] first-pass pose
@@ -513,7 +515,7 @@ guess_match_kernel(const GuessMatchArgs a)
 	const int nf = min(a.n_from[frow], min(cap, a.cap_from));
 	const int nt = min(a.n_to ? a.n_to[pair] : a.n_to_all, min(cap, a.cap_to));
 	const size_t base = static_cast<size_t>(pair) * cap;
-	const size_t fbase = static_cast<size_t>(frow) * a.cap_from, tbase = static_cast<size_t>(pair) * a.cap_to;
+	const size_t fbase = static_cast<size_t>(frow) * a.cap_from, tbase = static_cast<size_t>(a.to_row ? a.to_row[pair] : pair) * a.cap_to;
 	if (tid == 0)
 	{
 		rodrigues_v2m(rv, s_R, nullptr);
