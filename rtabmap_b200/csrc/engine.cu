@@ -467,8 +467,6 @@ struct lcd_engine
 	DevBuf<int> sh_n_all, sh_words_loc[2], sh_words_all[2];
 	DevBuf<uint32_t> sh_keys[2], sh_keys_mine[2];
 	DevBuf<long long> sh_scores[2], sh_scores_loc[2];
-	bool match_has_xyz_to = false; // verify_upload staged xyz_to for the next launch_match
-	bool pnp_has_obj_to = false;   // the last launch_match gathered obj_to for launch_pnp
 };
 
 #define LCD_FAIL(e, code, ...)                          \
@@ -2743,8 +2741,9 @@ long long lcd_debug_orb_buffer(lcd_engine * e, int which, void * out, long long 
 }
 
 // ---- geometric verification ------------------------------------------------------------------
+// Stages the host's pairs in the engine's verification buffers; src: those buffers, FROM and TO row = pair.
 static int verify_upload(lcd_engine * e, int n_pairs, int cap, const void * desc_from, const float * xyz_from, const int * n_from,
-                         const void * desc_to, const float * uv_to, const int * n_to, cudaStream_t s, const float * xyz_to = nullptr)
+                         const void * desc_to, const float * uv_to, const float * xyz_to, const int * n_to, cudaStream_t s, PairSource & src)
 {
 	const size_t rows = static_cast<size_t>(n_pairs) * cap;
 	LCD_CUDA(e, e->v_df.reserve(rows * e->nw, 0, false, s));
@@ -2766,26 +2765,12 @@ static int verify_upload(lcd_engine * e, int n_pairs, int cap, const void * desc
 		LCD_CUDA(e, e->v_xyz_to.reserve(rows * 3, 0, false, s));
 		LCD_CUDA(e, cudaMemcpyAsync(e->v_xyz_to.p, xyz_to, rows * 3 * sizeof(float), cudaMemcpyHostToDevice, s));
 	}
+	src = PairSource{{e->v_df.p, e->v_xyz.p, e->v_nf.p, nullptr, cap},
+	                 {e->v_dt.p, e->v_uv.p, xyz_to ? e->v_xyz_to.p : nullptr, e->v_nt.p, 0, cap, nullptr}};
 	return LCD_OK;
 }
 
-struct MatchSrc
-{
-	const uint32_t * desc_from;
-	const float * xyz_from;
-	const int * n_from;
-	const int * from_slot;
-	int cap_from;
-	const uint32_t * desc_to;
-	const float * uv_to;
-	const int * n_to;
-	int n_to_all;
-	int cap_to;
-	const float * xyz_to; // 3-D points of the TO side (words3B) or nullptr
-	const int * to_row = nullptr; // TO row of each pair (nullptr: the pair's own row)
-};
-
-static int launch_match(lcd_engine * e, int n_pairs, int cap, float nndr, bool want_ids, cudaStream_t s, const MatchSrc * src = nullptr)
+static int launch_match(lcd_engine * e, const PairSource & src, int n_pairs, int cap, float nndr, bool want_ids, cudaStream_t s)
 {
 	const size_t rows = static_cast<size_t>(n_pairs) * cap;
 	LCD_CUDA(e, e->v_obj.reserve(rows * 3, 0, false, s));
@@ -2800,38 +2785,9 @@ static int launch_match(lcd_engine * e, int n_pairs, int cap, float nndr, bool w
 		LCD_CUDA(e, e->v_tid.reserve(rows, 0, false, s));
 	}
 	MatchArgs a{};
-	if (src)
-	{
-		a.desc_from = src->desc_from;
-		a.xyz_from = src->xyz_from;
-		a.n_from = src->n_from;
-		a.from_slot = src->from_slot;
-		a.cap_from = src->cap_from;
-		a.desc_to = src->desc_to;
-		a.uv_to = src->uv_to;
-		a.n_to = src->n_to;
-		a.n_to_all = src->n_to_all;
-		a.cap_to = src->cap_to;
-		a.xyz_to = src->xyz_to;
-		a.to_row = src->to_row;
-	}
-	else
-	{
-		a.desc_from = e->v_df.p;
-		a.xyz_from = e->v_xyz.p;
-		a.n_from = e->v_nf.p;
-		a.from_slot = nullptr;
-		a.cap_from = cap;
-		a.desc_to = e->v_dt.p;
-		a.uv_to = e->v_uv.p;
-		a.n_to = e->v_nt.p;
-		a.n_to_all = 0;
-		a.cap_to = cap;
-		a.xyz_to = e->match_has_xyz_to ? e->v_xyz_to.p : nullptr;
-	}
-	if (a.xyz_to) LCD_CUDA(e, e->v_obj_to.reserve(rows * 3, 0, false, s));
-	a.obj_to = a.xyz_to ? e->v_obj_to.p : nullptr;
-	e->pnp_has_obj_to = a.xyz_to != nullptr;
+	a.src = src;
+	if (src.to.xyz) LCD_CUDA(e, e->v_obj_to.reserve(rows * 3, 0, false, s));
+	a.obj_to = src.to.xyz ? e->v_obj_to.p : nullptr;
 	a.cap = cap;
 	a.nndr = nndr;
 	a.obj = e->v_obj.p;
@@ -2843,14 +2799,14 @@ static int launch_match(lcd_engine * e, int n_pairs, int cap, float nndr, bool w
 	a.from_ids = want_ids ? e->v_fid.p : nullptr;
 	a.to_ids = want_ids ? e->v_tid.p : nullptr;
 	// FROM rows of the signature store: their temporary dictionaries are cached next to the store (from_dict_build_kernel)
-	const bool from_store = src && src->from_slot && src->desc_from == e->st_desc.p;
+	const bool from_store = src.from.slot && src.from.desc == e->st_desc.p;
 	FromDictArgs fa{};
 	if (from_store)
 	{
 		a.from_tag = e->st_ftag.p;
 		a.from_kof = e->st_kof.p;
 		a.from_creator = e->st_creator.p;
-		fa = FromDictArgs{src->desc_from, src->n_from, src->from_slot, src->cap_from, std::min(cap, src->cap_from), nndr, e->st_ftag.p, e->st_kof.p, e->st_creator.p};
+		fa = FromDictArgs{src.from.desc, src.from.n, src.from.slot, src.from.cap, std::min(cap, src.from.cap), nndr, e->st_ftag.p, e->st_kof.p, e->st_creator.p};
 	}
 	const size_t smem = match_smem_bytes(cap, e->nw), smem_fd = from_dict_smem_bytes(fa.rows, e->nw);
 	if (smem > static_cast<size_t>(e->smem_optin)) LCD_FAIL(e, LCD_ERR_CAPACITY, "cap %d needs %zu B of shared memory", cap, smem);
@@ -2881,8 +2837,9 @@ static int launch_match(lcd_engine * e, int n_pairs, int cap, float nndr, bool w
 	return LCD_OK;
 }
 
-static int launch_pnp(lcd_engine * e, int n_pairs, int cap, const lcd_verify_params * p, cudaStream_t s, bool gate_min_matches = true,
-                      bool want_cov = true)
+// obj_to: words3B of each correspondence (launch_match's v_obj_to) or nullptr
+static int launch_pnp(lcd_engine * e, int n_pairs, int cap, const lcd_verify_params * p, const float * obj_to, cudaStream_t s,
+                      bool gate_min_matches = true, bool want_cov = true)
 {
 	const size_t rows = static_cast<size_t>(n_pairs) * cap;
 	if (want_cov && p->var_median_ratio <= 1) LCD_FAIL(e, LCD_ERR_INVALID, "Vis/PnPVarianceMedianRatio must be > 1 (UASSERT in estimateMotion3DTo2D)");
@@ -2907,7 +2864,7 @@ static int launch_pnp(lcd_engine * e, int n_pairs, int cap, const lcd_verify_par
 	a.refine_iterations = p->refine_iterations;
 	a.refine_sigma = p->refine_sigma;
 	a.gate_min_matches = gate_min_matches ? 1 : 0;
-	a.obj_to = (want_cov && e->pnp_has_obj_to) ? e->v_obj_to.p : nullptr;
+	a.obj_to = obj_to;
 	a.var_median_ratio = p->var_median_ratio;
 	a.max_variance = p->max_variance;
 	a.split_linear = p->split_linear_cov;
@@ -2935,40 +2892,12 @@ static int launch_pnp(lcd_engine * e, int n_pairs, int cap, const lcd_verify_par
 }
 
 // Reg/RepeatOnce: the second registration pass of the pairs whose first pass succeeded (guess_match_kernel), then PnP again on all pairs
-// (pairs that keep their first-pass correspondences reproduce their first-pass result).  src as in launch_match.
-static int launch_second_pass(lcd_engine * e, int n_pairs, int cap, const lcd_verify_params * p, cudaStream_t s, const MatchSrc * src)
+// (pairs that keep their first-pass correspondences reproduce their first-pass result).  src and obj_to: those of the first pass.
+static int launch_second_pass(lcd_engine * e, const PairSource & src, int n_pairs, int cap, const lcd_verify_params * p, float * obj_to, cudaStream_t s)
 {
 	if (!p->repeat_once || p->guess_win_size <= 0 || p->image_width <= 0 || p->image_height <= 0) return LCD_OK;
 	GuessMatchArgs a{};
-	if (src)
-	{
-		a.desc_from = src->desc_from;
-		a.xyz_from = src->xyz_from;
-		a.n_from = src->n_from;
-		a.from_slot = src->from_slot;
-		a.cap_from = src->cap_from;
-		a.desc_to = src->desc_to;
-		a.uv_to = src->uv_to;
-		a.xyz_to = src->xyz_to;
-		a.n_to = src->n_to;
-		a.n_to_all = src->n_to_all;
-		a.cap_to = src->cap_to;
-		a.to_row = src->to_row;
-	}
-	else
-	{
-		a.desc_from = e->v_df.p;
-		a.xyz_from = e->v_xyz.p;
-		a.n_from = e->v_nf.p;
-		a.from_slot = nullptr;
-		a.cap_from = cap;
-		a.desc_to = e->v_dt.p;
-		a.uv_to = e->v_uv.p;
-		a.xyz_to = e->match_has_xyz_to ? e->v_xyz_to.p : nullptr;
-		a.n_to = e->v_nt.p;
-		a.n_to_all = 0;
-		a.cap_to = cap;
-	}
+	a.src = src;
 	a.cap = cap;
 	a.ok1 = e->v_ok.p;
 	a.rvec = e->v_rvec.p;
@@ -2980,7 +2909,7 @@ static int launch_second_pass(lcd_engine * e, int n_pairs, int cap, const lcd_ve
 	a.nndr = p->nndr;
 	a.obj = e->v_obj.p;
 	a.img = e->v_img.p;
-	a.obj_to = e->pnp_has_obj_to ? e->v_obj_to.p : nullptr;
+	a.obj_to = obj_to;
 	a.match_id = e->v_mid.p;
 	a.match_from = e->v_mfrom.p;
 	a.match_to = e->v_mto.p;
@@ -3007,7 +2936,35 @@ static int launch_second_pass(lcd_engine * e, int n_pairs, int cap, const lcd_ve
 	}
 #undef LCD_GUESS_CASE
 	LCD_CHECK_LAUNCH(e);
-	return launch_pnp(e, n_pairs, cap, p, s);
+	return launch_pnp(e, n_pairs, cap, p, obj_to, s);
+}
+
+// Memory::computeTransform of every pair: global matching, PnP, then the Reg/RepeatOnce pass.  cap: stride of the outputs, at least
+// both row strides of src.  The covariance takes words3B from src.to.xyz when it is set.
+static int register_pairs(lcd_engine * e, const PairSource & src, int n_pairs, int cap, const lcd_verify_params * vp, cudaStream_t s)
+{
+	LCD_TRY(launch_match(e, src, n_pairs, cap, vp->nndr, false, s));
+	float * obj_to = src.to.xyz ? e->v_obj_to.p : nullptr;
+	LCD_TRY(launch_pnp(e, n_pairs, cap, vp, obj_to, s));
+	return launch_second_pass(e, src, n_pairs, cap, vp, obj_to, s);
+}
+
+static int check_verify_params(lcd_engine * e, const lcd_verify_params * vp, bool need_store)
+{
+	if (!vp) LCD_FAIL(e, LCD_ERR_INVALID, "null verification parameters");
+	if (vp->iterations > kMaxRansacIters) LCD_FAIL(e, LCD_ERR_CAPACITY, "Vis/Iterations > %d", kMaxRansacIters);
+	if (need_store && e->st_cap == 0) LCD_FAIL(e, LCD_ERR_STATE, "the signature store is empty: nothing to verify against");
+	return LCD_OK;
+}
+
+// the per-pair verification outputs of the last registration as lcd_verify_result rows
+static int pack_verify_results(lcd_engine * e, int n, PackedVerifyResult * d_out, cudaStream_t s)
+{
+	static_assert(sizeof(PackedVerifyResult) == sizeof(lcd_verify_result), "PackedVerifyResult must mirror lcd_verify_result");
+	pack_verify_results_kernel<<<(n + 127) / 128, 128, 0, s>>>(n, e->v_ok.p, e->v_nm.p, e->v_ninl.p, e->v_iters.p, e->v_rvec.p, e->v_tvec.p, e->v_T.p,
+	                                                          e->v_cov6.p, d_out);
+	LCD_CHECK_LAUNCH(e);
+	return LCD_OK;
 }
 
 // copy the per-pair verification outputs back (cap = 0: skip the id arrays)
@@ -3022,14 +2979,11 @@ static int verify_download(lcd_engine * e, int n_pairs, int cap, lcd_verify_resu
 	}
 	LCD_CUDA(e, e->v_packed.reserve(n_pairs, 0, false, s));
 	LCD_CUDA(e, e->h_packed.reserve(n_pairs));
-	pack_verify_results_kernel<<<(n_pairs + 127) / 128, 128, 0, s>>>(n_pairs, e->v_ok.p, e->v_nm.p, e->v_ninl.p, e->v_iters.p, e->v_rvec.p, e->v_tvec.p,
-	                                                                e->v_T.p, e->v_cov6.p, e->v_packed.p);
-	LCD_CHECK_LAUNCH(e);
+	LCD_TRY(pack_verify_results(e, n_pairs, e->v_packed.p, s));
 	LCD_CUDA(e, cudaMemcpyAsync(e->h_packed.p, e->v_packed.p, n_pairs * sizeof(PackedVerifyResult), cudaMemcpyDeviceToHost, s));
 	if (cap > 0 && match_ids) LCD_CUDA(e, cudaMemcpyAsync(match_ids, e->v_mid.p, rows * sizeof(int), cudaMemcpyDeviceToHost, s));
 	if (cap > 0 && inlier_ids) LCD_CUDA(e, cudaMemcpyAsync(inlier_ids, e->v_inl_ids.p, rows * sizeof(int), cudaMemcpyDeviceToHost, s));
 	LCD_CUDA(e, cudaStreamSynchronize(s));
-	static_assert(sizeof(PackedVerifyResult) == sizeof(lcd_verify_result), "PackedVerifyResult must mirror lcd_verify_result");
 	memcpy(results, e->h_packed.p, n_pairs * sizeof(lcd_verify_result));
 	return LCD_OK;
 }
@@ -3049,9 +3003,9 @@ int lcd_match_pairs(lcd_engine * e, int n_pairs, int cap, const void * desc_from
 	LCD_TRY(set_device(e));
 	LCD_TRY(check_verify_args(e, n_pairs, cap, desc_from, desc_to, n_from, n_to));
 	cudaStream_t s = e->stream;
-	LCD_TRY(verify_upload(e, n_pairs, cap, desc_from, nullptr, n_from, desc_to, nullptr, n_to, s));
-	e->match_has_xyz_to = false;
-	LCD_TRY(launch_match(e, n_pairs, cap, nndr, true, s));
+	PairSource src;
+	LCD_TRY(verify_upload(e, n_pairs, cap, desc_from, nullptr, n_from, desc_to, nullptr, nullptr, n_to, s, src));
+	LCD_TRY(launch_match(e, src, n_pairs, cap, nndr, true, s));
 	const size_t rows = static_cast<size_t>(n_pairs) * cap;
 	if (from_ids) LCD_CUDA(e, cudaMemcpyAsync(from_ids, e->v_fid.p, rows * sizeof(int), cudaMemcpyDeviceToHost, s));
 	if (to_ids) LCD_CUDA(e, cudaMemcpyAsync(to_ids, e->v_tid.p, rows * sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -3068,13 +3022,11 @@ int lcd_verify_batch(lcd_engine * e, int n_pairs, int cap, const void * desc_fro
 	LCD_TRY(set_device(e));
 	LCD_TRY(check_verify_args(e, n_pairs, cap, desc_from, desc_to, n_from, n_to));
 	if (!xyz_from || !uv_to || !params || !results) LCD_FAIL(e, LCD_ERR_INVALID, "null verification argument");
-	if (params->iterations > kMaxRansacIters) LCD_FAIL(e, LCD_ERR_CAPACITY, "Vis/Iterations > %d", kMaxRansacIters);
+	LCD_TRY(check_verify_params(e, params, false));
 	cudaStream_t s = e->stream;
-	LCD_TRY(verify_upload(e, n_pairs, cap, desc_from, xyz_from, n_from, desc_to, uv_to, n_to, s, xyz_to));
-	e->match_has_xyz_to = xyz_to != nullptr;
-	LCD_TRY(launch_match(e, n_pairs, cap, params->nndr, false, s));
-	LCD_TRY(launch_pnp(e, n_pairs, cap, params, s));
-	LCD_TRY(launch_second_pass(e, n_pairs, cap, params, s, nullptr));
+	PairSource src;
+	LCD_TRY(verify_upload(e, n_pairs, cap, desc_from, xyz_from, n_from, desc_to, uv_to, xyz_to, n_to, s, src));
+	LCD_TRY(register_pairs(e, src, n_pairs, cap, params, s));
 	return verify_download(e, n_pairs, cap, results, match_ids, inlier_ids, s);
 }
 
@@ -3128,7 +3080,7 @@ int lcd_pnp_ransac_batch(lcd_engine * e, int n_sets, int cap, const float * obje
 	vp.cx = K[2];
 	vp.cy = K[5];
 	vp.var_median_ratio = 2;
-	LCD_TRY(launch_pnp(e, n_sets, cap, &vp, s, false, false));
+	LCD_TRY(launch_pnp(e, n_sets, cap, &vp, nullptr, s, false, false));
 	std::vector<double> hr(static_cast<size_t>(n_sets) * 3), ht(static_cast<size_t>(n_sets) * 3);
 	std::vector<int> hn(n_sets), hit(n_sets);
 	LCD_CUDA(e, cudaMemcpyAsync(hr.data(), e->v_rvec.p, hr.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
@@ -3435,7 +3387,8 @@ int lcd_match_bf(lcd_engine * e, int n_pairs, int cap, const void * desc_query, 
 	cudaStream_t s = e->stream;
 	const size_t rows = static_cast<size_t>(n_pairs) * cap;
 	// FROM buffers hold the train side, TO buffers the query side (cv::BFMatcher::match(queryDescriptors = TO, trainDescriptors = FROM))
-	LCD_TRY(verify_upload(e, n_pairs, cap, desc_train, nullptr, n_train, desc_query, nullptr, n_query, s));
+	PairSource staged;
+	LCD_TRY(verify_upload(e, n_pairs, cap, desc_train, nullptr, n_train, desc_query, nullptr, nullptr, n_query, s, staged));
 	LCD_CUDA(e, e->bf_keys_a.reserve(rows, 0, false, s));
 	LCD_CUDA(e, e->d_i1.reserve(rows, 0, false, s));
 	LCD_CUDA(e, e->d_f1.reserve(rows, 0, false, s));
@@ -3586,16 +3539,25 @@ int lcd_sig_remove(lcd_engine * e, int sig_id)
 	return LCD_OK;
 }
 
+// d_nq_frame: descriptors of each frame (nullptr: nq each); d_xyz_to: the frames' 3-D points (words3B) or nullptr
 static int verify_top_dev(lcd_engine * e, const uint32_t * d_q, const float * d_uv, int n_frames, int nq, const float * d_like,
-                          const int * d_sig_ids, int ns, const lcd_verify_params * vp, cudaStream_t s, const int * d_nq_frame = nullptr,
-                          const float * d_xyz_to = nullptr);
+                          const int * d_sig_ids, int ns, const lcd_verify_params * vp, cudaStream_t s, const int * d_nq_frame, const float * d_xyz_to)
+{
+	LCD_TRY(check_verify_params(e, vp, true));
+	LCD_CUDA(e, e->d_hyp_id.reserve(n_frames, 0, false, s));
+	LCD_CUDA(e, e->d_hyp_slot.reserve(n_frames, 0, false, s));
+	e->dc_hyp_valid = false; // the arg-max replaces the hypotheses of the last decision
+	argmax_hypothesis_kernel<<<n_frames, 256, 0, s>>>(d_like, ns, d_sig_ids, e->st_slot_of_sig.p, static_cast<int>(e->h_slot_of_sig.size()),
+	                                                  e->d_hyp_id.p, e->d_hyp_slot.p);
+	LCD_CHECK_LAUNCH(e);
+	const PairSource src{{e->st_desc.p, e->st_xyz.p, e->st_n.p, e->d_hyp_slot.p, e->st_cap}, {d_q, d_uv, d_xyz_to, d_nq_frame, nq, nq, nullptr}};
+	return register_pairs(e, src, n_frames, std::max(e->st_cap, nq), vp, s);
+}
 
 static int process_dev(lcd_engine * e, const uint32_t * d_q, const float * d_uv, int n_frames, int nq, int incremental, float nndr, int cmp_new,
                        const int * d_sig_ids, int ns, int n_total, const lcd_verify_params * vp, int * d_words, float * d_like, cudaStream_t s)
 {
-	if (!vp) LCD_FAIL(e, LCD_ERR_INVALID, "null verification parameters");
-	if (vp->iterations > kMaxRansacIters) LCD_FAIL(e, LCD_ERR_CAPACITY, "Vis/Iterations > %d", kMaxRansacIters);
-	if (e->st_cap == 0) LCD_FAIL(e, LCD_ERR_STATE, "the signature store is empty: nothing to verify against");
+	LCD_TRY(check_verify_params(e, vp, true));
 	if (!d_sig_ids || ns <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "ids list is empty");
 	if (!d_like)
 	{
@@ -3603,26 +3565,7 @@ static int process_dev(lcd_engine * e, const uint32_t * d_q, const float * d_uv,
 		d_like = e->d_like.p;
 	}
 	LCD_TRY(localize_dev(e, d_q, n_frames, nq, incremental, nndr, cmp_new, d_sig_ids, ns, n_total, d_words, d_like, s));
-	return verify_top_dev(e, d_q, d_uv, n_frames, nq, d_like, d_sig_ids, ns, vp, s);
-}
-
-static int verify_top_dev(lcd_engine * e, const uint32_t * d_q, const float * d_uv, int n_frames, int nq, const float * d_like,
-                          const int * d_sig_ids, int ns, const lcd_verify_params * vp, cudaStream_t s, const int * d_nq_frame, const float * d_xyz_to)
-{
-	if (!vp) LCD_FAIL(e, LCD_ERR_INVALID, "null verification parameters");
-	if (vp->iterations > kMaxRansacIters) LCD_FAIL(e, LCD_ERR_CAPACITY, "Vis/Iterations > %d", kMaxRansacIters);
-	if (e->st_cap == 0) LCD_FAIL(e, LCD_ERR_STATE, "the signature store is empty: nothing to verify against");
-	LCD_CUDA(e, e->d_hyp_id.reserve(n_frames, 0, false, s));
-	LCD_CUDA(e, e->d_hyp_slot.reserve(n_frames, 0, false, s));
-	e->dc_hyp_valid = false; // the arg-max replaces the hypotheses of the last decision
-	argmax_hypothesis_kernel<<<n_frames, 256, 0, s>>>(d_like, ns, d_sig_ids, e->st_slot_of_sig.p, static_cast<int>(e->h_slot_of_sig.size()),
-	                                                  e->d_hyp_id.p, e->d_hyp_slot.p);
-	LCD_CHECK_LAUNCH(e);
-	const int cap = std::max(e->st_cap, nq);
-	MatchSrc src{e->st_desc.p, e->st_xyz.p, e->st_n.p, e->d_hyp_slot.p, e->st_cap, d_q, d_uv, d_nq_frame, nq, nq, d_xyz_to};
-	LCD_TRY(launch_match(e, n_frames, cap, vp->nndr, false, s, &src));
-	LCD_TRY(launch_pnp(e, n_frames, cap, vp, s));
-	return launch_second_pass(e, n_frames, cap, vp, s, &src);
+	return verify_top_dev(e, d_q, d_uv, n_frames, nq, d_like, d_sig_ids, ns, vp, s, nullptr, nullptr);
 }
 
 int lcd_process_batch_dev(lcd_engine * e, const void * d_queries, const float * d_uv, int n_frames, int nq_per_frame, int incremental, float nndr,
@@ -3847,9 +3790,7 @@ int lcd_process_frames_submit(lcd_engine * e, int n_frames, const uint8_t * imag
 	{
 		LCD_CUDA(e, e->v_packed.reserve(n_frames, 0, false, s));
 		LCD_CUDA(e, f.res.reserve(n_frames));
-		pack_verify_results_kernel<<<(n_frames + 127) / 128, 128, 0, s>>>(n_frames, e->v_ok.p, e->v_nm.p, e->v_ninl.p, e->v_iters.p, e->v_rvec.p,
-		                                                                 e->v_tvec.p, e->v_T.p, e->v_cov6.p, e->v_packed.p);
-		LCD_CHECK_LAUNCH(e);
+		LCD_TRY(pack_verify_results(e, n_frames, e->v_packed.p, s));
 		LCD_CUDA(e, cudaMemcpyAsync(f.res.p, e->v_packed.p, n_frames * sizeof(PackedVerifyResult), cudaMemcpyDeviceToHost, s));
 		f.user_results = results;
 	}
@@ -3896,7 +3837,7 @@ int lcd_verify_top_dev(lcd_engine * e, const void * d_queries, const float * d_u
 	if (!d_queries || !d_uv || !d_likelihood || !d_sig_ids || n_frames <= 0 || ns <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
-	return verify_top_dev(e, static_cast<const uint32_t *>(d_queries), d_uv, n_frames, nq_per_frame, d_likelihood, d_sig_ids, ns, vp, s);
+	return verify_top_dev(e, static_cast<const uint32_t *>(d_queries), d_uv, n_frames, nq_per_frame, d_likelihood, d_sig_ids, ns, vp, s, nullptr, nullptr);
 }
 
 int lcd_process_fetch(lcd_engine * e, int n_frames, int * hypothesis_out, lcd_verify_result * results)
@@ -3921,12 +3862,9 @@ int lcd_process_fetch_async(lcd_engine * e, int n_frames, int * hypothesis_out, 
 	if (hypothesis_out) LCD_CUDA(e, cudaMemcpyAsync(hypothesis_out, e->d_hyp_id.p, n_frames * sizeof(int), cudaMemcpyDeviceToHost, s));
 	if (results)
 	{
-		static_assert(sizeof(PackedVerifyResult) == sizeof(lcd_verify_result), "packed result layout");
 		if (!e->v_ok.p || !e->d_hyp_id.p) LCD_FAIL(e, LCD_ERR_STATE, "no verification results on the device: run a step with verify parameters first");
 		LCD_CUDA(e, e->v_packed.reserve(n_frames, 0, false, s));
-		pack_verify_results_kernel<<<(n_frames + 127) / 128, 128, 0, s>>>(n_frames, e->v_ok.p, e->v_nm.p, e->v_ninl.p, e->v_iters.p, e->v_rvec.p, e->v_tvec.p,
-		                                                                 e->v_T.p, e->v_cov6.p, e->v_packed.p);
-		LCD_CHECK_LAUNCH(e);
+		LCD_TRY(pack_verify_results(e, n_frames, e->v_packed.p, s));
 		LCD_CUDA(e, cudaMemcpyAsync(results, e->v_packed.p, n_frames * sizeof(PackedVerifyResult), cudaMemcpyDeviceToHost, s));
 	}
 	return LCD_OK;
@@ -4316,16 +4254,11 @@ int lcd_decide_fetch(lcd_engine * e, int n_frames, lcd_decision * out)
 // Rtabmap.cpp:3156-3167
 static int verify_decided(lcd_engine * e, const uint32_t * d_q, const float * d_uv, int n_frames, int nq, const lcd_verify_params * vp, cudaStream_t s)
 {
-	if (!vp) LCD_FAIL(e, LCD_ERR_INVALID, "null verification parameters");
-	if (vp->iterations > kMaxRansacIters) LCD_FAIL(e, LCD_ERR_CAPACITY, "Vis/Iterations > %d", kMaxRansacIters);
-	if (e->st_cap == 0) LCD_FAIL(e, LCD_ERR_STATE, "the signature store is empty: nothing to verify against");
+	LCD_TRY(check_verify_params(e, vp, true));
 	if (e->dc_last_frames == 0 || !e->dc_hyp_valid) LCD_FAIL(e, LCD_ERR_STATE, "no decision to verify: run lcd_decide_batch_dev first");
 	if (n_frames != e->dc_last_frames) LCD_FAIL(e, LCD_ERR_INVALID, "the last decision has %d frames, not %d", e->dc_last_frames, n_frames);
-	const int cap = std::max(e->st_cap, nq);
-	MatchSrc src{e->st_desc.p, e->st_xyz.p, e->st_n.p, e->d_hyp_slot.p, e->st_cap, d_q, d_uv, nullptr, nq, nq, nullptr};
-	LCD_TRY(launch_match(e, n_frames, cap, vp->nndr, false, s, &src));
-	LCD_TRY(launch_pnp(e, n_frames, cap, vp, s));
-	LCD_TRY(launch_second_pass(e, n_frames, cap, vp, s, &src));
+	const PairSource src{{e->st_desc.p, e->st_xyz.p, e->st_n.p, e->d_hyp_slot.p, e->st_cap}, {d_q, d_uv, nullptr, nullptr, nq, nq, nullptr}};
+	LCD_TRY(register_pairs(e, src, n_frames, std::max(e->st_cap, nq), vp, s));
 	decide_verified_kernel<<<(n_frames + 127) / 128, 128, 0, s>>>(n_frames, e->v_ok.p, e->v_T.p, e->dc_max_dist, e->dc_dec.p, e->d_hyp_id.p,
 	                                                             e->px_valid ? e->px_skip.p : nullptr);
 	LCD_CHECK_LAUNCH(e);
@@ -4356,9 +4289,7 @@ int lcd_process_decide_batch_dev(lcd_engine * e, const void * d_queries, const f
 	LCD_TRY(set_device(e));
 	if (!d_queries || !d_uv || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "Descriptors size is null!");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
-	if (!vp) LCD_FAIL(e, LCD_ERR_INVALID, "null verification parameters");
-	if (vp->iterations > kMaxRansacIters) LCD_FAIL(e, LCD_ERR_CAPACITY, "Vis/Iterations > %d", kMaxRansacIters);
-	if (e->st_cap == 0) LCD_FAIL(e, LCD_ERR_STATE, "the signature store is empty: nothing to verify against");
+	LCD_TRY(check_verify_params(e, vp, true));
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
 	LCD_TRY(decide_prepare(e, n_frames, ns, clients, frame_flags, dp, s));
 	float * d_like = d_likelihood_out;
@@ -4423,19 +4354,6 @@ int lcd_clients_set_map_poses(lcd_engine * e, const int * ids, int n, const floa
 	return LCD_OK;
 }
 
-// Memory::computeTransform(place, frame) of n_pairs arbitrary (frame row, place) pairs in one launch, with a null guess
-// (RGBD/ProximityOdomGuess = false): FROM = the store row d_slot[i] (-1: none) with its cached dictionary, TO = row d_row[i] of the frames'
-// d_q / d_uv (nq rows each), d_n_to[i] of its descriptors (0: the pair is not registered)
-static int verify_frame_pairs(lcd_engine * e, const uint32_t * d_q, const float * d_uv, int n_pairs, int nq, const int * d_row, const int * d_n_to,
-                              const int * d_slot, const lcd_verify_params * vp, cudaStream_t s)
-{
-	const int cap = std::max(e->st_cap, nq);
-	MatchSrc src{e->st_desc.p, e->st_xyz.p, e->st_n.p, d_slot, e->st_cap, d_q, d_uv, d_n_to, 0, nq, nullptr, d_row};
-	LCD_TRY(launch_match(e, n_pairs, cap, vp->nndr, false, s, &src));
-	LCD_TRY(launch_pnp(e, n_pairs, cap, vp, s));
-	return launch_second_pass(e, n_pairs, cap, vp, s, &src);
-}
-
 int lcd_decide_proximity_dev(lcd_engine * e, const void * d_queries, const float * d_uv, int n_frames, int nq_per_frame, const float * frame_poses,
                              const int * enabled, const lcd_proximity_params * pp, void * stream)
 {
@@ -4446,7 +4364,7 @@ int lcd_decide_proximity_dev(lcd_engine * e, const void * d_queries, const float
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
 	if (!pp || !pp->verify) LCD_FAIL(e, LCD_ERR_INVALID, "null proximity or verification parameters");
 	const lcd_verify_params * vp = pp->verify;
-	if (vp->iterations > kMaxRansacIters) LCD_FAIL(e, LCD_ERR_CAPACITY, "Vis/Iterations > %d", kMaxRansacIters);
+	LCD_TRY(check_verify_params(e, vp, false));
 	if (!(pp->local_radius > 0.f) || !std::isfinite(pp->local_radius)) LCD_FAIL(e, LCD_ERR_INVALID, "RGBD/LocalRadius must be > 0");
 	if (!(pp->angle >= 0.f) || !std::isfinite(pp->angle)) LCD_FAIL(e, LCD_ERR_INVALID, "RGBD/ProximityAngle must be >= 0");
 	if (pp->max_graph_depth < 0) LCD_FAIL(e, LCD_ERR_INVALID, "RGBD/ProximityMaxGraphDepth must be >= 0");
@@ -4505,10 +4423,13 @@ int lcd_decide_proximity_dev(lcd_engine * e, const void * d_queries, const float
 	proximity_paths_kernel<<<n_frames, kPxThreads, 0, s>>>(a);
 	prof_mark(e, LCD_PROF_PROXIMITY, s);
 	LCD_CHECK_LAUNCH(e);
-	LCD_TRY(verify_frame_pairs(e, static_cast<const uint32_t *>(d_queries), d_uv, n_pairs, nq_per_frame, e->px_row.p, e->px_nto.p, e->px_slot.p, vp, s));
-	pack_verify_results_kernel<<<(n_pairs + 127) / 128, 128, 0, s>>>(n_pairs, e->v_ok.p, e->v_nm.p, e->v_ninl.p, e->v_iters.p, e->v_rvec.p, e->v_tvec.p,
-	                                                                e->v_T.p, e->v_cov6.p, e->px_res.p);
-	LCD_CHECK_LAUNCH(e);
+	// Memory::computeTransform(place, frame) of every attempted pair in one launch, with a null guess (RGBD/ProximityOdomGuess = false):
+	// FROM = the store row px_slot[i] (-1: none) with its cached dictionary, TO = row px_row[i] of the frames' descriptors, px_nto[i] of
+	// them (0: the pair is not registered)
+	const PairSource src{{e->st_desc.p, e->st_xyz.p, e->st_n.p, e->px_slot.p, e->st_cap},
+	                     {static_cast<const uint32_t *>(d_queries), d_uv, nullptr, e->px_nto.p, 0, nq_per_frame, e->px_row.p}};
+	LCD_TRY(register_pairs(e, src, n_pairs, std::max(e->st_cap, nq_per_frame), vp, s));
+	LCD_TRY(pack_verify_results(e, n_pairs, e->px_res.p, s));
 	proximity_apply_kernel<<<(n_frames + 127) / 128, 128, 0, s>>>(n_frames, mp, fr, e->v_ok.p, e->v_T.p, e->px_rec.p, e->dc_dec.p, e->d_hyp_id.p,
 	                                                             e->d_hyp_slot.p, e->px_skip.p);
 	LCD_CHECK_LAUNCH(e);

@@ -35,30 +35,57 @@ struct FromDictTag
 	int unused;
 };
 
+// Where the two signatures of each pair are read, for both matching passes.
+struct PairSource
+{
+	struct
+	{
+		const uint32_t * desc; // [n_from_rows][cap][NW]
+		const float * xyz;     // [n_from_rows][cap][3]   NaN = no depth
+		const int * n;         // [n_from_rows]
+		const int * slot;      // nullptr: FROM row = pair; else row of the signature store for each pair (-1 = none)
+		int cap;               // row stride of the FROM arrays
+	} from;
+	struct
+	{
+		const uint32_t * desc; // [n_to_rows][cap][NW]
+		const float * uv;      // [n_to_rows][cap][2]
+		const float * xyz;     // [n_to_rows][cap][3] or nullptr: Signature::getWords3 of the TO side (words3B of estimateMotion3DTo2D)
+		const int * n;         // [n_pairs] or nullptr (= n_all)
+		int n_all;
+		int cap;               // row stride of the TO arrays
+		const int * row;       // nullptr: TO row = pair; else the TO row of each pair
+	} to;
+
+	__device__ __forceinline__ int from_row(int pair) const { return from.slot ? from.slot[pair] : pair; }
+	// TO descriptors of the pair, at most cap (the call's) and the TO row stride
+	__device__ __forceinline__ int to_count(int pair, int cap) const { return min(to.n ? to.n[pair] : to.n_all, min(cap, to.cap)); }
+	__device__ __forceinline__ size_t to_base(int pair) const { return static_cast<size_t>(to.row ? to.row[pair] : pair) * to.cap; }
+};
+
+// words3B: the 3-D point of TO descriptor ti (TO row at tbase) to output row m of obj_to; nothing when obj_to is nullptr (no TO points)
+__device__ __forceinline__ void gather_obj_to(const PairSource & src, float * obj_to, size_t m, size_t tbase, int ti)
+{
+	if (!obj_to) return;
+	const float * r = src.to.xyz + (tbase + ti) * 3;
+	obj_to[m * 3 + 0] = r[0];
+	obj_to[m * 3 + 1] = r[1];
+	obj_to[m * 3 + 2] = r[2];
+}
+
 struct MatchArgs
 {
-	const uint32_t * desc_from; // [n_from_rows][cap_from][NW]
-	const float * xyz_from;     // [n_from_rows][cap_from][3]   NaN = no depth
-	const int * n_from;         // [n_from_rows]
-	const int * from_slot;      // nullptr: FROM row = pair; else row of the signature store for each pair (-1 = none)
-	int cap_from;               // row stride of the FROM arrays
-	const uint32_t * desc_to;   // [n_pairs][cap_to][NW]
-	const float * uv_to;        // [n_pairs][cap_to][2]
-	const float * xyz_to;       // [n_pairs][cap_to][3] or nullptr: Signature::getWords3 of the TO side (words3B of estimateMotion3DTo2D)
-	const int * n_to;           // [n_pairs] or nullptr (= n_to_all)
-	int n_to_all;
-	int cap_to;                 // row stride of the TO arrays
-	const int * to_row;         // nullptr: TO row = pair; else the TO row of each pair
-	int cap;                    // stride of the outputs and size of the shared-memory arrays (>= both)
+	PairSource src;
+	int cap;                    // stride of the outputs and size of the shared-memory arrays (>= both row strides)
 	float nndr; // Vis/CorNNDR
-	// FROM dictionaries cached per signature-store row (from_slot only, else nullptr): see from_dict_build_kernel
+	// FROM dictionaries cached per signature-store row (src.from.slot only, else nullptr): see from_dict_build_kernel
 	const FromDictTag * from_tag;  // [n_from_rows]
-	const uint16_t * from_kof;     // [n_from_rows][cap_from]
-	const uint16_t * from_creator; // [n_from_rows][cap_from]
+	const uint16_t * from_kof;     // [n_from_rows][src.from.cap]
+	const uint16_t * from_creator; // [n_from_rows][src.from.cap]
 	// outputs
 	float * obj;       // [n_pairs][cap][3]
 	float * img;       // [n_pairs][cap][2]
-	float * obj_to;    // [n_pairs][cap][3] 3-D point of the TO side for each correspondence (NaN = none); nullptr when xyz_to is
+	float * obj_to;    // [n_pairs][cap][3] 3-D point of the TO side for each correspondence (NaN = none); nullptr when src.to.xyz is
 	int * match_id;    // [n_pairs][cap]  word id of the correspondence (ascending)
 	int * match_from;  // [n_pairs][cap]  descriptor index in FROM
 	int * match_to;    // [n_pairs][cap]  descriptor index in TO
@@ -314,14 +341,14 @@ pair_match_kernel(const MatchArgs a)
 
 	const int tid = threadIdx.x;
 	const int pair = blockIdx.x;
-	const int frow = a.from_slot ? a.from_slot[pair] : pair;
-	const int nf = frow >= 0 ? min(a.n_from[frow], min(cap, a.cap_from)) : 0;
-	const int nt = min(a.n_to ? a.n_to[pair] : a.n_to_all, min(cap, a.cap_to));
+	const int frow = a.src.from_row(pair);
+	const int nf = frow >= 0 ? min(a.src.from.n[frow], min(cap, a.src.from.cap)) : 0;
+	const int nt = a.src.to_count(pair, cap);
 	const size_t base = static_cast<size_t>(pair) * cap;
-	const size_t fbase = static_cast<size_t>(frow >= 0 ? frow : 0) * a.cap_from;
-	const size_t tbase = static_cast<size_t>(a.to_row ? a.to_row[pair] : pair) * a.cap_to;
-	const uint32_t * F = a.desc_from + fbase * NW;
-	const uint32_t * T = a.desc_to + tbase * NW;
+	const size_t fbase = static_cast<size_t>(frow >= 0 ? frow : 0) * a.src.from.cap;
+	const size_t tbase = a.src.to_base(pair);
+	const uint32_t * F = a.src.from.desc + fbase * NW;
+	const uint32_t * T = a.src.to.desc + tbase * NW;
 
 	// ---- FROM side: addNewWords(descriptorsFrom, 1) on an empty dictionary, or the store row's cached result -------------------
 	__shared__ int s_cached;
@@ -406,7 +433,7 @@ pair_match_kernel(const MatchArgs a)
 		bool ok = cntF[k] == 1 && cntT[k] == 1;
 		if (ok)
 		{
-			const float * p = a.xyz_from + (fbase + idxF[k]) * 3;
+			const float * p = a.src.from.xyz + (fbase + idxF[k]) * 3;
 			ok = isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]);
 		}
 		flag[k] = ok ? 1 : 0;
@@ -427,20 +454,14 @@ pair_match_kernel(const MatchArgs a)
 	{
 		const int k = L[m];
 		const int fi = idxF[k], ti = idxT[k];
-		const float * p = a.xyz_from + (fbase + fi) * 3;
-		const float * q = a.uv_to + (tbase + ti) * 2;
+		const float * p = a.src.from.xyz + (fbase + fi) * 3;
+		const float * q = a.src.to.uv + (tbase + ti) * 2;
 		a.obj[(base + m) * 3 + 0] = p[0];
 		a.obj[(base + m) * 3 + 1] = p[1];
 		a.obj[(base + m) * 3 + 2] = p[2];
 		a.img[(base + m) * 2 + 0] = q[0];
 		a.img[(base + m) * 2 + 1] = q[1];
-		if (a.obj_to)
-		{
-			const float * r = a.xyz_to + (tbase + ti) * 3;
-			a.obj_to[(base + m) * 3 + 0] = r[0];
-			a.obj_to[(base + m) * 3 + 1] = r[1];
-			a.obj_to[(base + m) * 3 + 2] = r[2];
-		}
+		gather_obj_to(a.src, a.obj_to, base + m, tbase, ti);
 		a.match_id[base + m] = k + 1;
 		a.match_from[base + m] = fi;
 		a.match_to[base + m] = ti;
@@ -459,18 +480,7 @@ pair_match_kernel(const MatchArgs a)
 // Pairs whose first pass failed (or whose pose is the identity: "guess not set") keep their first-pass correspondences.
 struct GuessMatchArgs
 {
-	const uint32_t * desc_from;
-	const float * xyz_from;
-	const int * n_from;
-	const int * from_slot;
-	int cap_from;
-	const uint32_t * desc_to;
-	const float * uv_to;
-	const float * xyz_to;
-	const int * n_to;
-	int n_to_all;
-	int cap_to;
-	const int * to_row;     // nullptr: TO row = pair
+	PairSource src;
 	int cap;
 	const int * ok1;        // [n_pairs] first pass accepted
 	const double * rvec;    // [n_pairs][3] first-pass pose
@@ -510,12 +520,12 @@ guess_match_kernel(const GuessMatchArgs a)
 	const double * rv = a.rvec + pair * 3;
 	const double * tv = a.tvec + pair * 3;
 	if (rv[0] == 0.0 && rv[1] == 0.0 && rv[2] == 0.0 && tv[0] == 0.0 && tv[1] == 0.0 && tv[2] == 0.0) return; // guess.isIdentity(): global matching again
-	const int frow = a.from_slot ? a.from_slot[pair] : pair;
+	const int frow = a.src.from_row(pair);
 	if (frow < 0) return;
-	const int nf = min(a.n_from[frow], min(cap, a.cap_from));
-	const int nt = min(a.n_to ? a.n_to[pair] : a.n_to_all, min(cap, a.cap_to));
+	const int nf = min(a.src.from.n[frow], min(cap, a.src.from.cap));
+	const int nt = a.src.to_count(pair, cap);
 	const size_t base = static_cast<size_t>(pair) * cap;
-	const size_t fbase = static_cast<size_t>(frow) * a.cap_from, tbase = static_cast<size_t>(a.to_row ? a.to_row[pair] : pair) * a.cap_to;
+	const size_t fbase = static_cast<size_t>(frow) * a.src.from.cap, tbase = a.src.to_base(pair);
 	if (tid == 0)
 	{
 		rodrigues_v2m(rv, s_R, nullptr);
@@ -525,8 +535,8 @@ guess_match_kernel(const GuessMatchArgs a)
 	}
 	for (int j = tid; j < nt; j += blockDim.x)
 	{
-		s_uv[2 * j] = a.uv_to[(tbase + j) * 2];
-		s_uv[2 * j + 1] = a.uv_to[(tbase + j) * 2 + 1];
+		s_uv[2 * j] = a.src.to.uv[(tbase + j) * 2];
+		s_uv[2 * j + 1] = a.src.to.uv[(tbase + j) * 2 + 1];
 		claim[j] = 0x7FFFFFFF;
 	}
 	__syncthreads();
@@ -535,7 +545,7 @@ guess_match_kernel(const GuessMatchArgs a)
 	for (int i = tid; i < nf; i += blockDim.x)
 	{
 		int m = -1;
-		const float * X = a.xyz_from + (fbase + i) * 3;
+		const float * X = a.src.from.xyz + (fbase + i) * 3;
 		double pu, pv;
 		project_point(s_R, s_t, a.cam, X, pu, pv);
 		const float px = static_cast<float>(pu), py = static_cast<float>(pv);
@@ -545,7 +555,7 @@ guess_match_kernel(const GuessMatchArgs a)
 		if (inb && zc > 0.0f && isfinite(X[0]) && isfinite(X[1]) && isfinite(X[2]))
 		{
 			uint32_t q[NW];
-			load_desc<NW>(a.desc_from + fbase * NW, i, q);
+			load_desc<NW>(a.src.from.desc + fbase * NW, i, q);
 			int cnt = 0, b1 = -1;
 			uint32_t d1 = 0xFFFFFFFFu, d2 = 0xFFFFFFFFu;
 			for (int j = 0; j < nt; ++j)
@@ -555,7 +565,7 @@ guess_match_kernel(const GuessMatchArgs a)
 				if (!(dist < r2)) continue;
 				++cnt;
 				uint32_t w[NW];
-				load_desc<NW>(a.desc_to + tbase * NW, j, w);
+				load_desc<NW>(a.src.to.desc + tbase * NW, j, w);
 				const uint32_t d = hamming<NW, 0>(q, w);
 				if (d < d1)
 				{
@@ -591,19 +601,13 @@ guess_match_kernel(const GuessMatchArgs a)
 	for (int m = tid; m < nm; m += blockDim.x)
 	{
 		const int fi = L[m], ti = sel[fi];
-		const float * p = a.xyz_from + (fbase + fi) * 3;
+		const float * p = a.src.from.xyz + (fbase + fi) * 3;
 		a.obj[(base + m) * 3 + 0] = p[0];
 		a.obj[(base + m) * 3 + 1] = p[1];
 		a.obj[(base + m) * 3 + 2] = p[2];
 		a.img[(base + m) * 2 + 0] = s_uv[2 * ti];
 		a.img[(base + m) * 2 + 1] = s_uv[2 * ti + 1];
-		if (a.obj_to)
-		{
-			const float * r = a.xyz_to + (tbase + ti) * 3;
-			a.obj_to[(base + m) * 3 + 0] = r[0];
-			a.obj_to[(base + m) * 3 + 1] = r[1];
-			a.obj_to[(base + m) * 3 + 2] = r[2];
-		}
+		gather_obj_to(a.src, a.obj_to, base + m, tbase, ti);
 		a.match_id[base + m] = fi;
 		a.match_from[base + m] = fi;
 		a.match_to[base + m] = ti;
