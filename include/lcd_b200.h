@@ -346,10 +346,18 @@ int lcd_match_pairs(lcd_engine * e, int n_pairs, int cap, const void * desc_from
  * (:843-990) -> cv3::solvePnPRansac (opencv/solvepnp.cpp:112-417).  xyz_from: NaN where a keypoint has no depth.  xyz_to: the 3-D
  * points of the TO signature (words3B; NaN = none) or NULL when it has none — the covariance then comes from the 10 %-depth ray
  * model (image size set) or from the reprojection RMS (image size 0 x 0), as in the reference.
- * match_ids / inlier_ids [n_pairs*cap] (word ids, ascending / in inlier order) may be NULL. */
+ * match_ids / inlier_ids [n_pairs*cap] (word ids, ascending / in inlier order) may be NULL.
+ * cap (here, and max(store row size, nq) in the store-backed calls) is bounded by the matching kernel's shared memory, not by 4096:
+ * LCD_ERR_CAPACITY when its dynamic size (DESIGN.md §6) plus its static size exceeds the device's opt-in limit per block.  On an H100
+ * (232 448 B per block) the largest cap is 3540 for 16-byte descriptors, 2248 for 32-byte and 1233 for 64-byte ones (2560 B static).
+ * The refusal leaves the engine usable. */
 int lcd_verify_batch(lcd_engine * e, int n_pairs, int cap, const void * desc_from, const float * xyz_from, const int * n_from,
                      const void * desc_to, const float * uv_to, const float * xyz_to, const int * n_to,
                      const lcd_verify_params * params, lcd_verify_result * results, int * match_ids, int * inlier_ids);
+
+/* Static shared memory in bytes of a verification kernel at the engine's descriptor size: which = 0 pair matching, 1 matching with a
+ * guess (Reg/RepeatOnce), 2 PnP RANSAC, 3 FROM-dictionary build.  < 0 on error. */
+long long lcd_verify_static_smem(lcd_engine * e, int which);
 
 /* replaces: util3d::solvePnPRansac (util3d_motion_estimation.cpp:843-990; argument for argument: objectPoints, imagePoints,
  * cameraMatrix, distCoeffs, rvec, tvec, useExtrinsicGuess, iterationsCount, reprojectionError, minInliersCount, inliers, flags,

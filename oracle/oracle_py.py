@@ -372,6 +372,35 @@ def solve_pnp_iterative(X, uv, K4, rvec0, tvec0):
     return r, t
 
 
+def project_points(X, K4, rvec, tvec):
+    """cv::projectPoints of float points without distortion, in double (NaN points give NaN pixels): [n, 2] float64."""
+    X = np.ascontiguousarray(X, np.float32).reshape(-1, 3)
+    K4 = np.ascontiguousarray(K4, np.float64)
+    r = np.ascontiguousarray(rvec, np.float64)
+    t = np.ascontiguousarray(tvec, np.float64)
+    uv = np.zeros((max(len(X), 1), 2))
+    _vlib().orcv_project(_p(X), len(X), _p(K4), _p(r), _p(t), _p(uv))
+    return uv[:len(X)]
+
+
+def guess_match(desc_from, xyz_from, desc_to, uv_to, K4, rvec, tvec, image_size=(640, 480), guess_win_size=40, nndr=0.8):
+    """The correspondence search of the Reg/RepeatOnce pass (orcv_guess_match): for every FROM point the TO index it is matched to
+    (-1 none) under the guess (rvec, tvec), and the number of FROM points that project inside the image in front of the camera."""
+    L = _vlib()
+    t = 0 if desc_from.dtype == np.uint8 else 1
+    a = np.ascontiguousarray(desc_from)
+    b = np.ascontiguousarray(desc_to)
+    xa = np.ascontiguousarray(xyz_from, np.float32)
+    ub = np.ascontiguousarray(uv_to, np.float32)
+    K4 = np.ascontiguousarray(K4, np.float64)
+    r = np.ascontiguousarray(rvec, np.float64)
+    tv = np.ascontiguousarray(tvec, np.float64)
+    sel = np.zeros(max(len(a), 1), np.int32)
+    n_proj = L.orcv_guess_match(t, a.shape[1], _p(a), _p(xa), len(a), _p(b), _p(ub), len(b), _p(K4), _p(r), _p(tv), int(image_size[0]),
+                                int(image_size[1]), float(guess_win_size), float(nndr), _p(sel))
+    return sel[:len(a)].copy(), int(n_proj)
+
+
 def pnp_ransac(X, uv, K4, iterations=300, reproj=2.0, min_inliers=20, refine_iterations=1, refine_sigma=3.0, guess=None):
     """util3d::solvePnPRansac (cv3::solvePnPRansac + refinement): ok, rvec, tvec, inlier indices, iterations run."""
     L = _vlib()

@@ -214,6 +214,7 @@ SIGNATURES = {
     "lcd_localize_similarity_batch_dev": (_I, [_P, _P, _I, _I, _I, _F, _I, _P, _P, _I, _P, _P, _P]),
     "lcd_match_pairs": (_I, [_P, _I, _I, _P, _P, _P, _P, _F, _P, _P]),
     "lcd_verify_batch": (_I, [_P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "lcd_verify_static_smem": (C.c_longlong, [_P, _I]),
     "lcd_pnp_ransac": (_I, [_P, _P, _P, _I, _P, _P, _I, _P, _P, _I, _I, _F, _I, _I, _I, _F, _P, _P]),
     "lcd_pnp_ransac_batch": (_I, [_P, _I, _I, _P, _P, _P, _P, _P, _I, _P, _P, _I, _I, _F, _I, _I, _I, _F, _P, _P, _P]),
     "lcd_match_bf": (_I, [_P, _I, _I, _P, _P, _P, _P, _I, _P, _P, _P, _P]),
@@ -703,6 +704,14 @@ class Engine:
                         "transform": np.array(r.transform[:], np.float32).reshape(3, 4),
                         "covariance": np.array(r.covariance[:], np.float64).reshape(6, 6)})
         return out
+
+    def verify_static_smem(self, which: int) -> int:
+        """static shared memory in bytes of a verification kernel at the engine's descriptor size: 0 pair matching, 1 matching with a
+        guess, 2 PnP RANSAC, 3 FROM-dictionary build"""
+        n = self._lib.lcd_verify_static_smem(self._h, int(which))
+        if n < 0:
+            self._check(int(n))
+        return int(n)
 
     def pnp_ransac(self, object_points, image_points, K4, rvec=None, tvec=None, use_guess: bool = True, iterations: int = 300,
                    reproj_error: float = 2.0, min_inliers: int = 20, flags: int = 0, refine_iterations: int = 1, refine_sigma: float = 3.0,

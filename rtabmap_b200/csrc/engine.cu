@@ -2770,6 +2770,33 @@ static int verify_upload(lcd_engine * e, int n_pairs, int cap, const void * desc
 	return LCD_OK;
 }
 
+// Shared memory of one verification launch: LCD_ERR_CAPACITY unless the kernel's static shared memory plus dyn fits the device's
+// opt-in limit per block; raises the kernel's dynamic limit when the default 48 KB is exceeded.  A failed runtime call is taken off
+// the runtime's last error too, so the next launch check of the engine does not report it again.
+static int fit_smem(lcd_engine * e, const void * kern, size_t dyn, int cap)
+{
+	cudaFuncAttributes fa{};
+	cudaError_t c = cudaFuncGetAttributes(&fa, kern);
+	if (c != cudaSuccess)
+	{
+		cudaGetLastError();
+		LCD_FAIL(e, LCD_ERR_CUDA, "cudaFuncGetAttributes failed: %s", cudaGetErrorString(c));
+	}
+	const size_t need = fa.sharedSizeBytes + dyn;
+	if (need > static_cast<size_t>(e->smem_optin))
+		LCD_FAIL(e, LCD_ERR_CAPACITY, "cap %d needs %zu B of shared memory (%zu B static), the device allows %d", cap, need, fa.sharedSizeBytes, e->smem_optin);
+	if (need > 48 * 1024)
+	{
+		c = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(dyn));
+		if (c != cudaSuccess)
+		{
+			cudaGetLastError();
+			LCD_FAIL(e, LCD_ERR_CUDA, "cudaFuncSetAttribute(%zu B) failed: %s", dyn, cudaGetErrorString(c));
+		}
+	}
+	return LCD_OK;
+}
+
 static int launch_match(lcd_engine * e, const PairSource & src, int n_pairs, int cap, float nndr, bool want_ids, cudaStream_t s)
 {
 	const size_t rows = static_cast<size_t>(n_pairs) * cap;
@@ -2809,16 +2836,13 @@ static int launch_match(lcd_engine * e, const PairSource & src, int n_pairs, int
 		fa = FromDictArgs{src.from.desc, src.from.n, src.from.slot, src.from.cap, std::min(cap, src.from.cap), nndr, e->st_ftag.p, e->st_kof.p, e->st_creator.p};
 	}
 	const size_t smem = match_smem_bytes(cap, e->nw), smem_fd = from_dict_smem_bytes(fa.rows, e->nw);
-	if (smem > static_cast<size_t>(e->smem_optin)) LCD_FAIL(e, LCD_ERR_CAPACITY, "cap %d needs %zu B of shared memory", cap, smem);
 #define LCD_MATCH_CASE(NW_)                                                                                                 \
 	case NW_:                                                                                                               \
 	{                                                                                                                       \
 		auto kern = pair_match_kernel<NW_>;                                                                                 \
 		auto kern_fd = from_dict_build_kernel<NW_>;                                                                         \
-		if (smem > 40 * 1024) /* static shared memory counts against the default 48 KB too */                             \
-			LCD_CUDA(e, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));     \
-		if (smem_fd > 40 * 1024)                                                                                            \
-			LCD_CUDA(e, cudaFuncSetAttribute(kern_fd, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_fd))); \
+		LCD_TRY(fit_smem(e, reinterpret_cast<const void *>(kern), smem, cap));                                              \
+		if (from_store) LCD_TRY(fit_smem(e, reinterpret_cast<const void *>(kern_fd), smem_fd, cap));                        \
 		prof_mark(e, LCD_PROF_MATCH, s);                                                                                    \
 		if (from_store) kern_fd<<<n_pairs, kResolveThreads, smem_fd, s>>>(fa);                                              \
 		kern<<<n_pairs, kResolveThreads, smem, s>>>(a);                                                                     \
@@ -2881,9 +2905,7 @@ static int launch_pnp(lcd_engine * e, int n_pairs, int cap, const lcd_verify_par
 	static const int pnp_clocks = env_int("LCD_PNP_CLOCKS", 0); // diagnostics: phase clocks of the RANSAC kernel (lcd_debug_orb_buffer 7)
 	a.phase_clk = pnp_clocks ? e->v_clk.p : nullptr;
 	const size_t smem = pnp_smem_bytes(cap);
-	if (smem > static_cast<size_t>(e->smem_optin)) LCD_FAIL(e, LCD_ERR_CAPACITY, "cap %d needs %zu B of shared memory", cap, smem);
-	if (smem > 48 * 1024)
-		LCD_CUDA(e, cudaFuncSetAttribute(pnp_ransac_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+	LCD_TRY(fit_smem(e, reinterpret_cast<const void *>(pnp_ransac_kernel), smem, cap));
 	prof_mark(e, LCD_PROF_PNP, s);
 	pnp_ransac_kernel<<<n_pairs, kVerifyThreads, smem, s>>>(a);
 	prof_mark(e, LCD_PROF_PNP, s);
@@ -2915,13 +2937,11 @@ static int launch_second_pass(lcd_engine * e, const PairSource & src, int n_pair
 	a.match_to = e->v_mto.p;
 	a.n_match = e->v_nm.p;
 	const size_t smem = guess_smem_bytes(cap);
-	if (smem > static_cast<size_t>(e->smem_optin)) LCD_FAIL(e, LCD_ERR_CAPACITY, "cap %d needs %zu B of shared memory", cap, smem);
 #define LCD_GUESS_CASE(NW_)                                                                                              \
 	case NW_:                                                                                                            \
 	{                                                                                                                    \
 		auto kern = guess_match_kernel<NW_>;                                                                             \
-		if (smem > 48 * 1024)                                                                                            \
-			LCD_CUDA(e, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem))); \
+		LCD_TRY(fit_smem(e, reinterpret_cast<const void *>(kern), smem, cap));                                           \
 		prof_mark(e, LCD_PROF_MATCH, s);                                                                                 \
 		kern<<<n_pairs, 256, smem, s>>>(a);                                                                              \
 		prof_mark(e, LCD_PROF_MATCH, s);                                                                                 \
@@ -3030,6 +3050,31 @@ int lcd_verify_batch(lcd_engine * e, int n_pairs, int cap, const void * desc_fro
 	return verify_download(e, n_pairs, cap, results, match_ids, inlier_ids, s);
 }
 
+long long lcd_verify_static_smem(lcd_engine * e, int which)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(require_binary(e, "lcd_verify_static_smem"));
+	LCD_TRY(set_device(e));
+	const void * kern = nullptr;
+	switch (which * 100 + e->nw)
+	{
+	case 4: kern = reinterpret_cast<const void *>(pair_match_kernel<4>); break;
+	case 8: kern = reinterpret_cast<const void *>(pair_match_kernel<8>); break;
+	case 16: kern = reinterpret_cast<const void *>(pair_match_kernel<16>); break;
+	case 104: kern = reinterpret_cast<const void *>(guess_match_kernel<4>); break;
+	case 108: kern = reinterpret_cast<const void *>(guess_match_kernel<8>); break;
+	case 116: kern = reinterpret_cast<const void *>(guess_match_kernel<16>); break;
+	case 204: case 208: case 216: kern = reinterpret_cast<const void *>(pnp_ransac_kernel); break;
+	case 304: kern = reinterpret_cast<const void *>(from_dict_build_kernel<4>); break;
+	case 308: kern = reinterpret_cast<const void *>(from_dict_build_kernel<8>); break;
+	case 316: kern = reinterpret_cast<const void *>(from_dict_build_kernel<16>); break;
+	default: LCD_FAIL(e, LCD_ERR_INVALID, "no verification kernel %d", which);
+	}
+	cudaFuncAttributes fa{};
+	LCD_CUDA(e, cudaFuncGetAttributes(&fa, kern));
+	return static_cast<long long>(fa.sharedSizeBytes);
+}
+
 // ---- stand-alone PnP RANSAC: util3d::solvePnPRansac ------------------------------------------------
 static int check_pnp_camera(lcd_engine * e, const double K[9], const double * dist_coeffs, int n_dist, int flags)
 {
@@ -3128,7 +3173,7 @@ int lcd_pnp_ransac(lcd_engine * e, const float * object_points, const float * im
 static int launch_epipolar(lcd_engine * e, int n_pairs, EpiArgs & a, const lcd_epipolar_params * p, cudaStream_t s)
 {
 	const size_t smem = epi_smem_bytes(std::max(a.cap_a, a.cap_b));
-	if (smem > static_cast<size_t>(e->smem_optin)) LCD_FAIL(e, LCD_ERR_CAPACITY, "%d words per side need %zu B of shared memory", std::max(a.cap_a, a.cap_b), smem);
+	LCD_TRY(fit_smem(e, reinterpret_cast<const void *>(epipolar_check_kernel), smem, std::max(a.cap_a, a.cap_b)));
 	LCD_CUDA(e, e->ep_res.reserve(static_cast<size_t>(n_pairs) * 8, 0, false, s));
 	LCD_CUDA(e, e->ep_F.reserve(static_cast<size_t>(n_pairs) * 9, 0, false, s));
 	a.match_count_min = p->match_count_min;
@@ -3137,8 +3182,6 @@ static int launch_epipolar(lcd_engine * e, int n_pairs, EpiArgs & a, const lcd_e
 	a.conf = (p->ransac_param2 < 2.220446049250313e-16 || p->ransac_param2 > 1 - 2.220446049250313e-16) ? 0.99 : p->ransac_param2;
 	a.res = e->ep_res.p;
 	a.F = e->ep_F.p;
-	if (smem > 48 * 1024)
-		LCD_CUDA(e, cudaFuncSetAttribute(epipolar_check_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
 	prof_mark(e, LCD_PROF_EPIPOLAR, s);
 	epipolar_check_kernel<<<n_pairs, kEpiThreads, smem, s>>>(a);
 	prof_mark(e, LCD_PROF_EPIPOLAR, s);
