@@ -337,7 +337,8 @@ typedef struct lcd_verify_result {
 
 /* replaces: the global matching of RegistrationVis::computeTransformationImpl through a temporary
  * VWDictionary (RegistrationVis.cpp:1482-1503), Vis/CorNNType 0/3: from_ids/to_ids[n_pairs*cap] word
- * ids of every descriptor (ids start at 1 per pair). */
+ * ids of every descriptor (ids start at 1 per pair).  Binary engines only (LCD_ERR_INVALID on a float engine); the float matching is
+ * observable through lcd_verify_batch's match_ids / inlier_ids. */
 int lcd_match_pairs(lcd_engine * e, int n_pairs, int cap, const void * desc_from, const int * n_from,
                     const void * desc_to, const int * n_to, float nndr, int * from_ids, int * to_ids);
 
@@ -350,13 +351,19 @@ int lcd_match_pairs(lcd_engine * e, int n_pairs, int cap, const void * desc_from
  * cap (here, and max(store row size, nq) in the store-backed calls) is bounded by the matching kernel's shared memory, not by 4096:
  * LCD_ERR_CAPACITY when its dynamic size (DESIGN.md §6) plus its static size exceeds the device's opt-in limit per block.  On an H100
  * (232 448 B per block) the largest cap is 3540 for 16-byte descriptors, 2248 for 32-byte and 1233 for 64-byte ones (2560 B static).
- * The refusal leaves the engine usable. */
+ * The refusal leaves the engine usable.
+ * Float engines (LCD_DESC_F32, 64 or 128 floats; every registration call below, the store-backed ones included): the same temporary
+ * dictionary with squared L2 in place of Hamming (VWDictionary.cpp:1020-1028, NORM_L2SQR / rtflann L2), summed in rtflann's order
+ * (dist.h:158-166) for the dictionary and for the Reg/RepeatOnce pass's cv::BFMatcher(NORM_L2SQR) ranking, whose OpenCV SIMD order can
+ * differ in the last ulp (as lcd_match_bf).  Ties go to the first-created word.  Both sides are read from global memory and shared
+ * memory holds per-row scalars only, so every cap up to 4096 is accepted at 64-D and 128-D (largest dynamic size 37 B per row). */
 int lcd_verify_batch(lcd_engine * e, int n_pairs, int cap, const void * desc_from, const float * xyz_from, const int * n_from,
                      const void * desc_to, const float * uv_to, const float * xyz_to, const int * n_to,
                      const lcd_verify_params * params, lcd_verify_result * results, int * match_ids, int * inlier_ids);
 
 /* Static shared memory in bytes of a verification kernel at the engine's descriptor size: which = 0 pair matching, 1 matching with a
- * guess (Reg/RepeatOnce), 2 PnP RANSAC, 3 FROM-dictionary build.  < 0 on error. */
+ * guess (Reg/RepeatOnce), 2 PnP RANSAC, 3 FROM-dictionary build; on a float engine 0 is the kernel that resolves the TO side and assembles the
+ * correspondences (the TO x dictionary scan before it has only static shared memory).  < 0 on error. */
 long long lcd_verify_static_smem(lcd_engine * e, int which);
 
 /* replaces: util3d::solvePnPRansac (util3d_motion_estimation.cpp:843-990; argument for argument: objectPoints, imagePoints,
@@ -395,7 +402,8 @@ int lcd_match_bf(lcd_engine * e, int n_pairs, int cap, const void * desc_query, 
  * The per-node data Memory keeps for verification (Signature::getWordsDescriptors / getWords3,
  * corelib/include/rtabmap/core/Signature.h:155-164), resident in HBM so that the hypothesis picked
  * from the likelihood can be verified without a host round trip.
- * desc [n_sigs][cap][dim], xyz [n_sigs][cap][3] (NaN = no depth), n[n_sigs] valid rows. */
+ * desc [n_sigs][cap][dim] (bytes of a binary engine, floats of a float engine), xyz [n_sigs][cap][3] (NaN = no depth), n[n_sigs]
+ * valid rows. */
 int lcd_sig_add_batch(lcd_engine * e, const int * sig_ids, int n_sigs, int cap, const void * desc,
                       const float * xyz, const int * n);
 int lcd_sig_remove(lcd_engine * e, int sig_id);

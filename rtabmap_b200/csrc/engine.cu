@@ -393,6 +393,10 @@ struct lcd_engine
 	// (nf, Vis/CorNNDR) of the call: word of each descriptor, creator of each word [slot][st_cap], and what it was built for [slot]
 	DevBuf<uint16_t> st_kof, st_creator;
 	DevBuf<FromDictTag> st_ftag;
+	// float engines: the FROM dictionaries of host pairs [pair][cap] (stored rows use st_*) and the TO descriptors' two nearest words
+	DevBuf<uint16_t> v_kof, v_creator;
+	DevBuf<FromDictTag> v_ftag;
+	DevBuf<ulonglong2> v_keys64;
 	std::vector<int> h_slot_of_sig, free_slots;
 	int st_cap = 0, st_slots = 0;
 	// global descriptors (SensorData::globalDescriptors(), type 1, one per signature): rows [slot][gd_dim], the signature store's slot scheme
@@ -2797,6 +2801,42 @@ static int fit_smem(lcd_engine * e, const void * kern, size_t dyn, int cap)
 	return LCD_OK;
 }
 
+// Float descriptors: FROM dictionaries (cached per store row, or built per host pair), the TO x dictionary scan, then the TO new-word
+// loop and the correspondences (verify.cuh).  a: launch_match's arguments, with the store's FROM-dictionary cache when from_store.
+static int launch_match_l2(lcd_engine * e, const PairSource & src, int n_pairs, int cap, float nndr, bool from_store, MatchArgs a, cudaStream_t s)
+{
+	const bool d64 = e->nw == 64; // else 128
+	const auto kern_fd = d64 ? from_dict_l2_kernel<64> : from_dict_l2_kernel<128>;
+	const auto kern_scan = d64 ? to_dict_knn2_l2_kernel<64> : to_dict_knn2_l2_kernel<128>;
+	const auto kern = d64 ? pair_match_l2_kernel<64> : pair_match_l2_kernel<128>;
+	FromDictArgs fa{src.from.desc, src.from.n, src.from.slot, src.from.cap, std::min(cap, src.from.cap), nndr, e->st_ftag.p, e->st_kof.p, e->st_creator.p};
+	if (!from_store)
+	{
+		// host pairs: FROM row = pair (src.from.slot is nullptr), built on every call
+		const size_t frows = static_cast<size_t>(n_pairs) * src.from.cap;
+		LCD_CUDA(e, e->v_kof.reserve(frows, 0, false, s));
+		LCD_CUDA(e, e->v_creator.reserve(frows, 0, false, s));
+		LCD_CUDA(e, e->v_ftag.reserve(n_pairs, 0, false, s));
+		fa.tag = e->v_ftag.p;
+		fa.kof = e->v_kof.p;
+		fa.creator = e->v_creator.p;
+		a.from_tag = fa.tag;
+		a.from_kof = fa.kof;
+		a.from_creator = fa.creator;
+	}
+	LCD_CUDA(e, e->v_keys64.reserve(static_cast<size_t>(n_pairs) * cap, 0, false, s));
+	const size_t smem_fd = from_dict_l2_smem_bytes(fa.rows), smem = match_l2_smem_bytes(cap);
+	LCD_TRY(fit_smem(e, reinterpret_cast<const void *>(kern_fd), smem_fd, cap));
+	LCD_TRY(fit_smem(e, reinterpret_cast<const void *>(kern), smem, cap));
+	prof_mark(e, LCD_PROF_MATCH, s);
+	kern_fd<<<n_pairs, kL2ResolveThreads, smem_fd, s>>>(fa);
+	kern_scan<<<dim3(n_pairs, (cap + kL2ScanThreads - 1) / kL2ScanThreads), kL2ScanThreads, 0, s>>>(a, e->v_keys64.p);
+	kern<<<n_pairs, kL2ResolveThreads, smem, s>>>(a, e->v_keys64.p);
+	prof_mark(e, LCD_PROF_MATCH, s);
+	LCD_CHECK_LAUNCH(e);
+	return LCD_OK;
+}
+
 static int launch_match(lcd_engine * e, const PairSource & src, int n_pairs, int cap, float nndr, bool want_ids, cudaStream_t s)
 {
 	const size_t rows = static_cast<size_t>(n_pairs) * cap;
@@ -2835,6 +2875,7 @@ static int launch_match(lcd_engine * e, const PairSource & src, int n_pairs, int
 		a.from_creator = e->st_creator.p;
 		fa = FromDictArgs{src.from.desc, src.from.n, src.from.slot, src.from.cap, std::min(cap, src.from.cap), nndr, e->st_ftag.p, e->st_kof.p, e->st_creator.p};
 	}
+	if (e->f32) return launch_match_l2(e, src, n_pairs, cap, nndr, from_store, a, s);
 	const size_t smem = match_smem_bytes(cap, e->nw), smem_fd = from_dict_smem_bytes(fa.rows, e->nw);
 #define LCD_MATCH_CASE(NW_)                                                                                                 \
 	case NW_:                                                                                                               \
@@ -2937,21 +2978,23 @@ static int launch_second_pass(lcd_engine * e, const PairSource & src, int n_pair
 	a.match_to = e->v_mto.p;
 	a.n_match = e->v_nm.p;
 	const size_t smem = guess_smem_bytes(cap);
-#define LCD_GUESS_CASE(NW_)                                                                                              \
+#define LCD_GUESS_CASE(NW_, DESC_)                                                                                       \
 	case NW_:                                                                                                            \
 	{                                                                                                                    \
-		auto kern = guess_match_kernel<NW_>;                                                                             \
+		auto kern = guess_match_kernel<DESC_>;                                                                           \
 		LCD_TRY(fit_smem(e, reinterpret_cast<const void *>(kern), smem, cap));                                           \
 		prof_mark(e, LCD_PROF_MATCH, s);                                                                                 \
 		kern<<<n_pairs, 256, smem, s>>>(a);                                                                              \
 		prof_mark(e, LCD_PROF_MATCH, s);                                                                                 \
 		break;                                                                                                           \
 	}
-	switch (e->nw)
+	switch (e->nw) // 32-bit words per row: 4, 8, 16 binary; 64, 128 float
 	{
-		LCD_GUESS_CASE(4)
-		LCD_GUESS_CASE(8)
-		LCD_GUESS_CASE(16)
+		LCD_GUESS_CASE(4, HammingDesc<4>)
+		LCD_GUESS_CASE(8, HammingDesc<8>)
+		LCD_GUESS_CASE(16, HammingDesc<16>)
+		LCD_GUESS_CASE(64, L2Desc<64>)
+		LCD_GUESS_CASE(128, L2Desc<128>)
 	default: LCD_FAIL(e, LCD_ERR_INVALID, "unsupported descriptor size");
 	}
 #undef LCD_GUESS_CASE
@@ -3038,7 +3081,6 @@ int lcd_verify_batch(lcd_engine * e, int n_pairs, int cap, const void * desc_fro
                      lcd_verify_result * results, int * match_ids, int * inlier_ids)
 {
 	if (!e) return LCD_ERR_INVALID;
-	LCD_TRY(require_binary(e, "lcd_verify_batch"));
 	LCD_TRY(set_device(e));
 	LCD_TRY(check_verify_args(e, n_pairs, cap, desc_from, desc_to, n_from, n_to));
 	if (!xyz_from || !uv_to || !params || !results) LCD_FAIL(e, LCD_ERR_INVALID, "null verification argument");
@@ -3053,21 +3095,28 @@ int lcd_verify_batch(lcd_engine * e, int n_pairs, int cap, const void * desc_fro
 long long lcd_verify_static_smem(lcd_engine * e, int which)
 {
 	if (!e) return LCD_ERR_INVALID;
-	LCD_TRY(require_binary(e, "lcd_verify_static_smem"));
 	LCD_TRY(set_device(e));
 	const void * kern = nullptr;
-	switch (which * 100 + e->nw)
+	switch (which * 1000 + e->nw) // nw: 4, 8, 16 binary; 64, 128 float
 	{
 	case 4: kern = reinterpret_cast<const void *>(pair_match_kernel<4>); break;
 	case 8: kern = reinterpret_cast<const void *>(pair_match_kernel<8>); break;
 	case 16: kern = reinterpret_cast<const void *>(pair_match_kernel<16>); break;
-	case 104: kern = reinterpret_cast<const void *>(guess_match_kernel<4>); break;
-	case 108: kern = reinterpret_cast<const void *>(guess_match_kernel<8>); break;
-	case 116: kern = reinterpret_cast<const void *>(guess_match_kernel<16>); break;
-	case 204: case 208: case 216: kern = reinterpret_cast<const void *>(pnp_ransac_kernel); break;
-	case 304: kern = reinterpret_cast<const void *>(from_dict_build_kernel<4>); break;
-	case 308: kern = reinterpret_cast<const void *>(from_dict_build_kernel<8>); break;
-	case 316: kern = reinterpret_cast<const void *>(from_dict_build_kernel<16>); break;
+	case 1004: kern = reinterpret_cast<const void *>(guess_match_kernel<HammingDesc<4>>); break;
+	case 1008: kern = reinterpret_cast<const void *>(guess_match_kernel<HammingDesc<8>>); break;
+	case 1016: kern = reinterpret_cast<const void *>(guess_match_kernel<HammingDesc<16>>); break;
+	case 2004: case 2008: case 2016: kern = reinterpret_cast<const void *>(pnp_ransac_kernel); break;
+	case 3004: kern = reinterpret_cast<const void *>(from_dict_build_kernel<4>); break;
+	case 3008: kern = reinterpret_cast<const void *>(from_dict_build_kernel<8>); break;
+	case 3016: kern = reinterpret_cast<const void *>(from_dict_build_kernel<16>); break;
+	// float engines (nw = 64, 128 floats)
+	case 64: kern = reinterpret_cast<const void *>(pair_match_l2_kernel<64>); break;
+	case 128: kern = reinterpret_cast<const void *>(pair_match_l2_kernel<128>); break;
+	case 1064: kern = reinterpret_cast<const void *>(guess_match_kernel<L2Desc<64>>); break;
+	case 1128: kern = reinterpret_cast<const void *>(guess_match_kernel<L2Desc<128>>); break;
+	case 2064: case 2128: kern = reinterpret_cast<const void *>(pnp_ransac_kernel); break;
+	case 3064: kern = reinterpret_cast<const void *>(from_dict_l2_kernel<64>); break;
+	case 3128: kern = reinterpret_cast<const void *>(from_dict_l2_kernel<128>); break;
 	default: LCD_FAIL(e, LCD_ERR_INVALID, "no verification kernel %d", which);
 	}
 	cudaFuncAttributes fa{};
@@ -3494,7 +3543,6 @@ int lcd_sig_slots(const lcd_engine * e) { return e ? e->st_slots : 0; }
 int lcd_sig_add_batch(lcd_engine * e, const int * sig_ids, int n_sigs, int cap, const void * desc, const float * xyz, const int * n)
 {
 	if (!e) return LCD_ERR_INVALID;
-	LCD_TRY(require_binary(e, "lcd_sig_add_batch"));
 	if (n_sigs <= 0) return LCD_OK;
 	if (!sig_ids || !desc || !xyz || !n || cap <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null signature data");
 	if (cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "at most %d features per signature", kMaxFrameQueries);
@@ -3616,7 +3664,6 @@ int lcd_process_batch_dev(lcd_engine * e, const void * d_queries, const float * 
                           int * d_word_ids_out, float * d_likelihood_out, void * stream)
 {
 	if (!e) return LCD_ERR_INVALID;
-	LCD_TRY(require_binary(e, "lcd_process_batch_dev"));
 	LCD_TRY(set_device(e));
 	if (!d_queries || !d_uv || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "Descriptors size is null!");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
@@ -3875,7 +3922,6 @@ int lcd_verify_top_dev(lcd_engine * e, const void * d_queries, const float * d_u
                        const int * d_sig_ids, int ns, const lcd_verify_params * vp, void * stream)
 {
 	if (!e) return LCD_ERR_INVALID;
-	LCD_TRY(require_binary(e, "lcd_verify_top_dev"));
 	LCD_TRY(set_device(e));
 	if (!d_queries || !d_uv || !d_likelihood || !d_sig_ids || n_frames <= 0 || ns <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
@@ -3918,7 +3964,6 @@ int lcd_process_batch(lcd_engine * e, const void * queries, const float * uv, in
                       int * word_ids_out, float * likelihood_out, int * hypothesis_out, lcd_verify_result * results)
 {
 	if (!e) return LCD_ERR_INVALID;
-	LCD_TRY(require_binary(e, "lcd_process_batch"));
 	LCD_TRY(set_device(e));
 	if (!queries || !uv || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "Descriptors size is null!");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
@@ -4313,7 +4358,6 @@ int lcd_verify_decided_dev(lcd_engine * e, const void * d_queries, const float *
                            void * stream)
 {
 	if (!e) return LCD_ERR_INVALID;
-	LCD_TRY(require_binary(e, "lcd_verify_decided_dev"));
 	LCD_TRY(set_device(e));
 	if (!d_queries || !d_uv || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "Descriptors size is null!");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
@@ -4401,7 +4445,6 @@ int lcd_decide_proximity_dev(lcd_engine * e, const void * d_queries, const float
                              const int * enabled, const lcd_proximity_params * pp, void * stream)
 {
 	if (!e) return LCD_ERR_INVALID;
-	LCD_TRY(require_binary(e, "lcd_decide_proximity_dev"));
 	LCD_TRY(set_device(e));
 	if (!d_queries || !d_uv || !frame_poses || !enabled || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null or empty frame input");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);

@@ -180,7 +180,7 @@ __device__ int resolve_rounds_l2(const float * __restrict__ fq, int nq, const un
                                  uint16_t * L, uint16_t * rank, uint8_t * flag, int * s_nL, float nndr, int cmp_new)
 {
 	constexpr int kWarps = kL2ResolveThreads / 32;
-	__shared__ unsigned long long s_wk[kWarps][32][2]; // per warp, per descriptor of the chunk: best two among the created words it scanned
+	__shared__ __align__(16) unsigned long long s_wk[kWarps][32][2]; // per warp, per descriptor of the chunk: best two among the created words it scanned
 	__shared__ float s_dl[32][33];                     // s_dl[e][j] = distance between descriptors c0+e and c0+j of the current chunk
 	const int tid = threadIdx.x;
 	const int warp = tid >> 5, lane = tid & 31;

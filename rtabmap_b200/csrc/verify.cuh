@@ -15,6 +15,7 @@
 // over all points) and one thread then replays the sequential best/niters bookkeeping over the counts.
 #pragma once
 #include "common.cuh"
+#include "l2_path.cuh"
 #include "pnp_device.cuh"
 #include "ransac.cuh"
 #include "resolve.cuh"
@@ -469,6 +470,227 @@ pair_match_kernel(const MatchArgs a)
 	MATCH_PHASE(5);
 }
 
+// ---- pair matching of float descriptors (LCD_DESC_F32, 64-D / 128-D) ---------------------------------------------------------
+// The same temporary dictionary as from_dict_build_kernel + pair_match_kernel, with squared L2 summed in rtflann's order
+// (l2_path.cuh) in place of Hamming (VWDictionary.cpp:1020-1028: NORM_L2SQR / rtflann L2 for CV_32F).  A float row is 256 or 512
+// bytes, so both sides stay in global memory (L2-resident per pair) and shared memory holds per-row scalars only; the work is split
+// into three launches of at most 256 threads (the new-word loop, resolve_rounds_l2, is written for kL2ResolveThreads):
+//   from_dict_l2_kernel      FROM side, addNewWords(descriptorsFrom, 1): kof[i] = word of descriptor i, creator[k] = descriptor
+//                            that created word k, tag.n_dict.  Store rows: cached per row as the binary build; host pairs: per pair.
+//   to_dict_knn2_l2_kernel   TO side, the 2-NN of every TO descriptor over the FROM words, exact, keys pack64(d, k) (ties -> lowest k)
+//   pair_match_l2_kernel     TO side, the NNDR decision and the new-word loop of addNewWords(descriptorsTo, 2), then the
+//                            correspondences into exactly the outputs pair_match_kernel writes
+constexpr int kL2ScanThreads = 128; // TO descriptors per CTA of the 2-NN scan, one per thread (DIM floats in registers)
+constexpr int kL2ScanWords = 32;    // dictionary words staged per shared-memory tile of the scan
+
+__host__ __device__ inline size_t from_dict_l2_smem_bytes(int rows)
+{
+	return static_cast<size_t>(rows) * (8 + 8 + 4 + 2 + 2 + 1) + 128;
+}
+
+__host__ __device__ inline size_t match_l2_smem_bytes(int cap)
+{
+	return static_cast<size_t>(cap) * (8 + 8 + 4 + 4 + 4 + 2 + 2 + 2 + 2 + 1) + 128;
+}
+
+// One CTA per pair.  a.slot set: store rows, built unless cached for this nf and NNDR or built by an earlier pair of the batch (as
+// from_dict_build_kernel).  a.slot == nullptr: row = pair, always built (the host pairs of lcd_verify_batch).
+template <int DIM>
+__global__ void __launch_bounds__(kL2ResolveThreads)
+from_dict_l2_kernel(const FromDictArgs a)
+{
+	extern __shared__ __align__(128) unsigned char smem_raw[];
+	const int rows = a.rows;
+	unsigned long long * sa1 = reinterpret_cast<unsigned long long *>(smem_raw); // [rows] no index hits: the dictionary starts empty
+	unsigned long long * sa2 = sa1 + rows;
+	int * res = reinterpret_cast<int *>(sa2 + rows);
+	uint16_t * L = reinterpret_cast<uint16_t *>(res + rows);
+	uint16_t * rank = L + rows;
+	uint8_t * flag = reinterpret_cast<uint8_t *>(rank + rows);
+	__shared__ int s_nL, s_build;
+	const int pair = blockIdx.x, slot = a.slot ? a.slot[pair] : pair;
+	if (slot < 0) return;
+	const int nf = min(a.n[slot], rows);
+	const uint32_t nndr_bits = __float_as_uint(a.nndr);
+	if (threadIdx.x == 0)
+	{
+		int build = 1;
+		if (a.slot)
+		{
+			const FromDictTag t = a.tag[slot];
+			build = t.nf != nf || t.nndr_bits != nndr_bits;
+			for (int p = 0; p < pair && build; ++p)
+				if (a.slot[p] == slot) build = 0;
+		}
+		s_build = build;
+	}
+	__syncthreads();
+	if (!s_build) return;
+	const size_t base = static_cast<size_t>(slot) * a.cap_from;
+	for (int i = threadIdx.x; i < nf; i += blockDim.x)
+	{
+		sa1[i] = kKey64None;
+		sa2[i] = kKey64None;
+		flag[i] = 1;
+		res[i] = 0;
+	}
+	__syncthreads();
+	const int n_dict = resolve_rounds_l2<DIM>(reinterpret_cast<const float *>(a.desc) + base * DIM, nf, sa1, sa2, res, L, rank, flag, &s_nL, a.nndr, 1);
+	__syncthreads();
+	for (int i = threadIdx.x; i < nf; i += blockDim.x) a.kof[base + i] = flag[i] ? rank[i] : static_cast<uint16_t>(-1 - res[i]);
+	for (int k = threadIdx.x; k < n_dict; k += blockDim.x) a.creator[base + k] = L[k];
+	__threadfence();
+	__syncthreads();
+	if (threadIdx.x == 0) a.tag[slot] = FromDictTag{nf, n_dict, nndr_bits, 0};
+}
+
+// grid (n_pairs, ceil(cap / kL2ScanThreads)): pairs on x, which has no 65 535 limit, as in the other matching kernels.  keys[pair][j] = the two nearest FROM words of TO descriptor j.  The words are read
+// through a.from_creator from the FROM row, kL2ScanWords at a time into shared memory, and every thread compares its descriptor
+// with each of them (broadcast reads).
+template <int DIM>
+__global__ void __launch_bounds__(kL2ScanThreads)
+to_dict_knn2_l2_kernel(const MatchArgs a, ulonglong2 * __restrict__ keys)
+{
+	__shared__ __align__(16) float s_w[kL2ScanWords * DIM];
+	const int pair = blockIdx.x, tid = threadIdx.x;
+	const int nt = a.src.to_count(pair, a.cap);
+	const int j = blockIdx.y * kL2ScanThreads + tid;
+	if (blockIdx.y * kL2ScanThreads >= nt) return;
+	const int frow = a.src.from_row(pair);
+	const int n_dict = frow >= 0 ? a.from_tag[frow].n_dict : 0;
+	const size_t fbase = static_cast<size_t>(frow >= 0 ? frow : 0) * a.src.from.cap;
+	const float4 * F4 = reinterpret_cast<const float4 *>(a.src.from.desc + fbase * DIM);
+	const uint16_t * creator = a.from_creator + fbase;
+	float q[DIM];
+	{
+		const float4 * t4 = reinterpret_cast<const float4 *>(a.src.to.desc + (a.src.to_base(pair) + min(j, nt - 1)) * DIM);
+#pragma unroll
+		for (int v = 0; v < DIM / 4; ++v)
+		{
+			const float4 x = t4[v];
+			q[4 * v] = x.x;
+			q[4 * v + 1] = x.y;
+			q[4 * v + 2] = x.z;
+			q[4 * v + 3] = x.w;
+		}
+	}
+	unsigned long long k1 = kKey64None, k2 = kKey64None;
+	float4 * s_w4 = reinterpret_cast<float4 *>(s_w);
+	for (int w0 = 0; w0 < n_dict; w0 += kL2ScanWords)
+	{
+		const int nw = min(kL2ScanWords, n_dict - w0);
+		__syncthreads();
+		for (int i = tid; i < nw * (DIM / 4); i += kL2ScanThreads)
+			s_w4[i] = F4[static_cast<size_t>(creator[w0 + i / (DIM / 4)]) * (DIM / 4) + i % (DIM / 4)];
+		__syncthreads();
+		for (int r = 0; r < nw; ++r) top2_insert64(k1, k2, pack64(l2_reg_vs_stream<DIM>(q, s_w + r * DIM), static_cast<uint32_t>(w0 + r)));
+	}
+	if (j < nt) keys[static_cast<size_t>(pair) * a.cap + j] = make_ulonglong2(k1, k2);
+}
+
+// One CTA per pair, after to_dict_knn2_l2_kernel.  Dynamic shared memory: match_l2_smem_bytes(cap).
+template <int DIM>
+__global__ void __launch_bounds__(kL2ResolveThreads)
+pair_match_l2_kernel(const MatchArgs a, const ulonglong2 * __restrict__ keys)
+{
+	extern __shared__ __align__(128) unsigned char smem_raw[];
+	const int cap = a.cap;
+	unsigned long long * sa1 = reinterpret_cast<unsigned long long *>(smem_raw); // [cap] the TO descriptors' two nearest FROM words
+	unsigned long long * sa2 = sa1 + cap;
+	int * res = reinterpret_cast<int *>(sa2 + cap);
+	int * cntF = res + cap;
+	int * cntT = cntF + cap;
+	uint16_t * L = reinterpret_cast<uint16_t *>(cntT + cap);
+	uint16_t * rank = L + cap;
+	uint16_t * idxF = rank + cap;
+	uint16_t * idxT = idxF + cap;
+	uint8_t * flag = reinterpret_cast<uint8_t *>(idxT + cap);
+	__shared__ int s_nL;
+
+	const int tid = threadIdx.x;
+	const int pair = blockIdx.x;
+	const int frow = a.src.from_row(pair);
+	const int nf = frow >= 0 ? min(a.src.from.n[frow], min(cap, a.src.from.cap)) : 0;
+	const int nt = a.src.to_count(pair, cap);
+	const int n_dict = frow >= 0 ? a.from_tag[frow].n_dict : 0;
+	const size_t base = static_cast<size_t>(pair) * cap;
+	const size_t fbase = static_cast<size_t>(frow >= 0 ? frow : 0) * a.src.from.cap;
+	const size_t tbase = a.src.to_base(pair);
+
+	for (int k = tid; k < n_dict; k += blockDim.x)
+	{
+		cntF[k] = 0;
+		cntT[k] = 0;
+	}
+	for (int j = tid; j < nt; j += blockDim.x)
+	{
+		const ulonglong2 kk = keys[base + j];
+		sa1[j] = kk.x;
+		sa2[j] = kk.y;
+		int bt;
+		flag[j] = nndr_decide64(kk.x, kk.y, kKey64None, kKey64None, a.nndr, bt) ? 1 : 0;
+		res[j] = static_cast<int>(key64_row(kk.x));
+	}
+	__syncthreads();
+	for (int i = tid; i < nf; i += blockDim.x)
+	{
+		const int k = a.from_kof[fbase + i];
+		atomicAdd(&cntF[k], 1);
+		idxF[k] = static_cast<uint16_t>(i);
+	}
+	resolve_rounds_l2<DIM>(reinterpret_cast<const float *>(a.src.to.desc) + tbase * DIM, nt, sa1, sa2, res, L, rank, flag, &s_nL, a.nndr, 1);
+	__syncthreads();
+	for (int j = tid; j < nt; j += blockDim.x)
+	{
+		if (!flag[j] && res[j] >= 0)
+		{
+			atomicAdd(&cntT[res[j]], 1);
+			idxT[res[j]] = static_cast<uint16_t>(j);
+		}
+	}
+	__syncthreads();
+
+	// ---- correspondences: ids seen exactly once on each side, finite 3D, ascending id (as pair_match_kernel) ------------
+	for (int k = tid; k < n_dict; k += blockDim.x)
+	{
+		bool ok = cntF[k] == 1 && cntT[k] == 1;
+		if (ok)
+		{
+			const float * p = a.src.from.xyz + (fbase + idxF[k]) * 3;
+			ok = isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]);
+		}
+		flag[k] = ok ? 1 : 0;
+	}
+	__syncthreads();
+	if (tid < 32)
+	{
+		const int n = warp0_compact(flag, n_dict, L, rank);
+		if (tid == 0)
+		{
+			s_nL = n;
+			a.n_match[pair] = n;
+		}
+	}
+	__syncthreads();
+	const int nm = s_nL;
+	for (int m = tid; m < nm; m += blockDim.x)
+	{
+		const int k = L[m];
+		const int fi = idxF[k], ti = idxT[k];
+		const float * p = a.src.from.xyz + (fbase + fi) * 3;
+		const float * q = a.src.to.uv + (tbase + ti) * 2;
+		a.obj[(base + m) * 3 + 0] = p[0];
+		a.obj[(base + m) * 3 + 1] = p[1];
+		a.obj[(base + m) * 3 + 2] = p[2];
+		a.img[(base + m) * 2 + 0] = q[0];
+		a.img[(base + m) * 2 + 1] = q[1];
+		gather_obj_to(a.src, a.obj_to, base + m, tbase, ti);
+		a.match_id[base + m] = k + 1;
+		a.match_from[base + m] = fi;
+		a.match_to[base + m] = ti;
+	}
+}
+
 // ------------------------------------------------------------------- second pass: matching with a guess
 // Reg/RepeatOnce (Registration.cpp:221-229): when the first registration succeeded, RegistrationVis runs again with that transform
 // as the guess (RegistrationVis.cpp:1017-1070, :1225-1370, Vis/CorGuessMatchToProjection = false): the 3-D points of FROM are
@@ -501,7 +723,47 @@ struct GuessMatchArgs
 
 __host__ __device__ inline size_t guess_smem_bytes(int cap) { return static_cast<size_t>(cap) * (8 + 4 + 4 + 2 + 2 + 1) + 64; }
 
+// Descriptor kinds of the guess pass: the distance cv::BFMatcher ranks a FROM point's candidates by.  kWords: 32-bit words per row.
 template <int NW>
+struct HammingDesc // NORM_HAMMING; the FROM descriptor is held in registers
+{
+	static constexpr int kWords = NW;
+	using Dist = uint32_t;
+	static constexpr Dist kFar = 0xFFFFFFFFu;
+	struct Query
+	{
+		uint32_t w[NW];
+	};
+	__device__ __forceinline__ static void load(const uint32_t * base, int i, Query & q) { load_desc<NW>(base, i, q.w); }
+	__device__ __forceinline__ static Dist dist(const Query & q, const uint32_t * base, int j)
+	{
+		uint32_t w[NW];
+		load_desc<NW>(base, j, w);
+		return hamming<NW, 0>(q.w, w);
+	}
+};
+
+template <int DIM>
+struct L2Desc // NORM_L2SQR in rtflann's order; a 256 / 512-byte FROM descriptor is streamed from memory, not held in registers
+{
+	static constexpr int kWords = DIM;
+	using Dist = float;
+	static constexpr Dist kFar = INFINITY;
+	struct Query
+	{
+		const float * p;
+	};
+	__device__ __forceinline__ static void load(const uint32_t * base, int i, Query & q)
+	{
+		q.p = reinterpret_cast<const float *>(base) + static_cast<size_t>(i) * DIM;
+	}
+	__device__ __forceinline__ static Dist dist(const Query & q, const uint32_t * base, int j)
+	{
+		return l2_rtflann<DIM>(q.p, reinterpret_cast<const float *>(base) + static_cast<size_t>(j) * DIM);
+	}
+};
+
+template <class D>
 __global__ void __launch_bounds__(256)
 guess_match_kernel(const GuessMatchArgs a)
 {
@@ -554,19 +816,17 @@ guess_match_kernel(const GuessMatchArgs a)
 		const bool inb = isfinite(px) && !(px < 0.0f) && !(px >= wmax) && isfinite(py) && !(py < 0.0f) && !(py >= hmax);
 		if (inb && zc > 0.0f && isfinite(X[0]) && isfinite(X[1]) && isfinite(X[2]))
 		{
-			uint32_t q[NW];
-			load_desc<NW>(a.src.from.desc + fbase * NW, i, q);
+			typename D::Query q;
+			D::load(a.src.from.desc + fbase * D::kWords, i, q);
 			int cnt = 0, b1 = -1;
-			uint32_t d1 = 0xFFFFFFFFu, d2 = 0xFFFFFFFFu;
+			typename D::Dist d1 = D::kFar, d2 = D::kFar;
 			for (int j = 0; j < nt; ++j)
 			{
 				const float dx = __fsub_rn(px, s_uv[2 * j]), dy = __fsub_rn(py, s_uv[2 * j + 1]);
 				const float dist = __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy));
 				if (!(dist < r2)) continue;
 				++cnt;
-				uint32_t w[NW];
-				load_desc<NW>(a.src.to.desc + tbase * NW, j, w);
-				const uint32_t d = hamming<NW, 0>(q, w);
+				const typename D::Dist d = D::dist(q, a.src.to.desc + tbase * D::kWords, j);
 				if (d < d1)
 				{
 					d2 = d1;
