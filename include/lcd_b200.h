@@ -125,8 +125,35 @@ int lcd_orb_detect_describe_dev(lcd_engine * e, int n_frames, const uint8_t * d_
 int lcd_orb_overflow(lcd_engine * e);
 /* Which kernels the last detection used (bit flags; diagnostics for tests and benchmarks): 1 = FAST and blur tiles staged by TMA with a
  * tensor map (rows a multiple of 16 bytes), 2 = descriptors from shared-memory patches (rows a multiple of 4 bytes on every level, edge
- * threshold >= 19), 4 = vectorised gray / mask preparation (rows a multiple of 8 pixels, even height).  0 = the general kernels. */
+ * threshold >= 19), 4 = vectorised gray / mask preparation (rows a multiple of 8 pixels, even height), 8 = the GFTT/ORB detector
+ * (lcd_detector_set).  0 = the general kernels. */
 int lcd_orb_last_path(const lcd_engine * e);
+
+/* ---- detect: the detector of every image-level call -----------------------------------------
+ * LCD_DETECTOR_ORB (the default): Kp/DetectorStrategy=2, FAST corners on the ORB pyramid, as above.
+ * LCD_DETECTOR_GFTT_ORB: Kp/DetectorStrategy=8 (RTAB-Map's default), rtabmap::GFTT_ORB (Features2d.cpp:2141-2178, :2352-2356):
+ * cv::GFTTDetector(Kp/MaxFeatures, GFTT/QualityLevel, GFTT/MinDistance, GFTT/BlockSize, GFTT/UseHarrisDetector, GFTT/K) on the
+ * level-0 gray image and depth mask, then cv::ORB::compute on the kept corners (corners within ORB/EdgeThreshold of the border are
+ * dropped, the order is kept, descriptors are steered by the corners' angle of -1 degree).  Keypoints carry size = GFTT/BlockSize,
+ * angle = -1, response = the minimum eigenvalue, octave = 0.  lcd_orb_params still supplies n_features, edge_threshold, patch_size and
+ * the depth fields.  Once selected, lcd_orb_detect_describe[_dev], lcd_process_frames[_submit|_dev], lcd_map_detect_async and
+ * lcd_shard_process_frames_dev all detect GFTT/ORB.  Width and height must be even; more than 65 536 local maxima above the quality
+ * threshold in a frame truncate its candidate list, reported as for FAST (lcd_orb_overflow, LCD_ERR_CAPACITY). */
+#define LCD_DETECTOR_ORB 2
+#define LCD_DETECTOR_GFTT_ORB 8
+typedef struct lcd_gftt_params {
+	double quality_level; /* GFTT/QualityLevel (0.001): must be > 0 */
+	double min_distance;  /* GFTT/MinDistance (7): must be >= 0; below 1 no distance filter */
+	int block_size;       /* GFTT/BlockSize: 3 is the only value implemented */
+	int use_harris;       /* GFTT/UseHarrisDetector: 0 is the only value implemented */
+	double k;             /* GFTT/K (0.04): unused without the Harris detector */
+} lcd_gftt_params;
+/* Select the detector.  `params` is read for LCD_DETECTOR_GFTT_ORB (NULL = the defaults above) and ignored for LCD_DETECTOR_ORB.
+ * LCD_ERR_INVALID for an unknown detector, use_harris != 0, block_size != 3, quality_level <= 0 or a negative min_distance; the
+ * previous selection then stays. */
+int lcd_detector_set(lcd_engine * e, int detector, const lcd_gftt_params * params);
+/* The selected detector; `params` (may be NULL) receives its GFTT parameters. */
+int lcd_detector_get(const lcd_engine * e, lcd_gftt_params * params);
 
 /* ---- dictionary: VWDictionary ------------------------------------------------ */
 /* replaces: VWDictionary::addWord (VWDictionary.cpp:1554-1580) for n words whose ids

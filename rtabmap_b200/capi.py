@@ -54,6 +54,16 @@ class OrbParams(C.Structure):
     ]
 
 
+class GfttParams(C.Structure):
+    """lcd_gftt_params (GFTT/* parameters of the reference, Parameters.h:313-317)."""
+    _fields_ = [("quality_level", C.c_double), ("min_distance", C.c_double), ("block_size", C.c_int), ("use_harris", C.c_int), ("k", C.c_double)]
+
+
+# lcd_detector_set; depth type of a ready-made CV_8UC1 mask (lcd_b200.h)
+DETECTOR_ORB, DETECTOR_GFTT_ORB = 2, 8
+DEPTH_MASK_U8 = 3
+
+
 class VerifyParams(C.Structure):
     """lcd_verify_params (Vis/* parameters of the reference, corelib/include/rtabmap/core/Parameters.h:713-754)."""
     _fields_ = [
@@ -174,6 +184,8 @@ SIGNATURES = {
     "lcd_orb_detect_describe_dev": (_I, [_P, _I, _P, _I, _I, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P, _P]),
     "lcd_orb_overflow": (_I, [_P]),
     "lcd_orb_last_path": (_I, [_P]),
+    "lcd_detector_set": (_I, [_P, _I, _P]),
+    "lcd_detector_get": (_I, [_P, _P]),
     "lcd_dict_add_words": (_I, [_P, _P, _P, _I]),
     "lcd_dict_remove_words": (_I, [_P, _P, _I]),
     "lcd_dict_update": (_I, [_P]),
@@ -376,8 +388,9 @@ class Engine:
         return OrbParams(n_features, n_levels, scale_factor, edge_threshold, fast_threshold, patch_size, min_depth, max_depth, int(depth_as_mask),
                          *[float(k) for k in K4])
 
-    def orb_detect_describe(self, images, depth, params: "OrbParams", cap: int = 0):
-        """images [n,h,w] (gray) or [n,h,w,3] (BGR) uint8; depth [n,h,w] uint16 (mm) / float32 (m) / None.
+    def orb_detect_describe(self, images, depth, params: "OrbParams", cap: int = 0, depth_type: int = 0):
+        """images [n,h,w] (gray) or [n,h,w,3] (BGR) uint8; depth [n,h,w] uint16 (mm) / float32 (m) / None, or with
+        depth_type=DEPTH_MASK_U8 a ready-made uint8 mask (0 / non-zero).
         Returns per frame: (keypoints [k,6] float32 = x,y,size,angle,response,octave; desc [k,32]; xyz [k,3])."""
         img = np.ascontiguousarray(images, np.uint8)
         assert img.ndim in (3, 4)
@@ -386,7 +399,9 @@ class Engine:
         dtype = 0
         dptr = None
         if depth is not None:
-            if depth.dtype == np.uint16:
+            if depth_type == DEPTH_MASK_U8:
+                dtype, depth = DEPTH_MASK_U8, np.ascontiguousarray(depth, np.uint8)
+            elif depth.dtype == np.uint16:
                 dtype, depth = 1, np.ascontiguousarray(depth)
             else:
                 dtype, depth = 2, np.ascontiguousarray(depth, np.float32)
@@ -783,6 +798,20 @@ class Engine:
     def orb_last_path(self) -> int:
         """bit flags of the kernels the last detection used: 1 TMA tiles, 2 shared-memory patches, 4 vectorised preparation"""
         return self._lib.lcd_orb_last_path(self._h)
+
+    @staticmethod
+    def gftt_params(quality_level=0.001, min_distance=7.0, block_size=3, use_harris=False, k=0.04):
+        """GFTT/QualityLevel, GFTT/MinDistance, GFTT/BlockSize, GFTT/UseHarrisDetector, GFTT/K (the reference defaults)"""
+        return GfttParams(float(quality_level), float(min_distance), int(block_size), int(bool(use_harris)), float(k))
+
+    def set_detector(self, detector: int, params: "GfttParams" = None):
+        """DETECTOR_ORB (Kp/DetectorStrategy=2, the default) or DETECTOR_GFTT_ORB (8) for every image-level call of this engine"""
+        self._check(self._lib.lcd_detector_set(self._h, int(detector), C.byref(params) if params is not None else None))
+
+    def detector(self):
+        """(detector, GfttParams) currently selected"""
+        p = GfttParams()
+        return self._lib.lcd_detector_get(self._h, C.byref(p)), p
 
     def orb_overflow(self) -> bool:
         r = self._lib.lcd_orb_overflow(self._h)

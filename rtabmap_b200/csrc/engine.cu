@@ -25,6 +25,7 @@
 #include "proximity.cuh"
 #include "match_bf.cuh"
 #include "orb.cuh"
+#include "gftt.cuh"
 
 #include <cuda.h>
 #include <dlfcn.h>
@@ -415,6 +416,13 @@ struct lcd_engine
 	float gauss_sigma_loaded = -1.f;
 	int orb_tma_used = 0; // the last FAST launch staged its tiles through a tensor map
 	int orb_path = 0;     // lcd_orb_last_path flags of the last detection
+	int detector = LCD_DETECTOR_ORB; // lcd_detector_set: what orb_run detects
+	lcd_gftt_params gftt{0.001, 7.0, 3, 0, 0.04};
+	DevBuf<float> g_eig;
+	DevBuf<unsigned> g_max_key;
+	DevBuf<unsigned long long> g_keys;
+	DevBuf<int> g_count;
+	DevBuf<uint32_t> g_bitmap;
 	DevBuf<float> d_uv;
 
 	// measurement hooks (lcd_profile_*)
@@ -2391,6 +2399,210 @@ static int orb_geometry(lcd_engine * e, int width, int height, const lcd_orb_par
 	return LCD_OK;
 }
 
+// cv::getGaussianKernel(7, 2, CV_32F) into the blur kernels' constant taps, once per engine
+static int load_gauss7(lcd_engine * e, cudaStream_t s)
+{
+	if (e->gauss_sigma_loaded == 2.0f) return LCD_OK;
+	// exp(-x^2 / (2 sigma^2)) normalised in double, stored as float
+	double t[7], sum = 0;
+	for (int i = 0; i < 7; ++i)
+	{
+		t[i] = exp(-0.5 * (i - 3) * (i - 3) / 4.0);
+		sum += t[i];
+	}
+	float kf[7];
+	for (int i = 0; i < 7; ++i) kf[i] = static_cast<float>(t[i] / sum);
+	LCD_CUDA(e, cudaMemcpyToSymbolAsync(kOrbGauss7, kf, sizeof(kf), 0, cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, cudaStreamSynchronize(s));
+	e->gauss_sigma_loaded = 2.0f;
+	return LCD_OK;
+}
+
+// 3-D points and plain coordinates of the detected keypoints (pointers already at the first frame of the range)
+static int orb_lift(lcd_engine * e, int n_frames, int width, int height, const void * d_depth, int depth_type, const lcd_orb_params * p, int cap,
+                    const OrbKeypoint * d_kp, const int * d_n, float * d_xyz, float * d_uv, cudaStream_t s)
+{
+	if (d_xyz)
+	{
+		OrbXyzArgs a{};
+		a.depth = (depth_type != LCD_DEPTH_NONE && depth_type != LCD_DEPTH_MASK_U8) ? d_depth : nullptr;
+		a.depth_type = depth_type;
+		a.w = width;
+		a.h = height;
+		a.fx = p->fx;
+		a.fy = p->fy;
+		a.cx = p->cx;
+		a.cy = p->cy;
+		a.min_depth = p->min_depth;
+		a.max_depth = p->max_depth;
+		a.kps = d_kp;
+		a.n_kp = d_n;
+		a.cap = cap;
+		a.xyz = d_xyz;
+		dim3 grd((cap + 255) / 256, n_frames);
+		orb_xyz_kernel<<<grd, 256, 0, s>>>(a);
+		LCD_CHECK_LAUNCH(e);
+	}
+	if (d_uv)
+	{
+		dim3 grd((cap + 255) / 256, n_frames);
+		orb_uv_kernel<<<grd, 256, 0, s>>>(d_kp, d_n, cap, d_uv);
+		LCD_CHECK_LAUNCH(e);
+	}
+	return LCD_OK;
+}
+
+// GFTT/ORB (lcd_detector_set, Kp/DetectorStrategy=8): orb_run's inputs, outputs and frame ranges, one pyramid level.  Gray + mask
+// (orb_prepare*), corner map with the per-frame maximum, local maxima, per-frame sort, minDistance walk + ORB's border filter, then the
+// level-0 blur, the steered BRIEF descriptors and the 3-D points of the FAST path.
+static int gftt_run(lcd_engine * e, int n_frames, const uint8_t * d_images, int width, int height, int channels, const void * d_depth,
+                    int depth_type, const lcd_orb_params * p, int cap, OrbKeypoint * d_kp, uint8_t * d_desc, float * d_xyz, float * d_uv,
+                    int * d_n, cudaStream_t s, int frame0, int total_frames)
+{
+	if (total_frames <= 0) total_frames = frame0 + n_frames;
+	if (!p) LCD_FAIL(e, LCD_ERR_INVALID, "null ORB parameters");
+	lcd_orb_params p1 = *p;
+	p1.n_levels = 1; // cv::ORB::compute builds the levels its keypoints use: GFTT corners are all octave 0
+	OrbGeom g{};
+	LCD_TRY(orb_geometry(e, width, height, &p1, g));
+	if (width % 2 || height % 2) LCD_FAIL(e, LCD_ERR_INVALID, "GFTT/ORB needs an even image width and height");
+	if (channels != 1 && channels != 3) LCD_FAIL(e, LCD_ERR_INVALID, "images must be 8UC1 or 8UC3 (BGR)");
+	if (cap <= 0 || cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "cap must be 1..%d", kMaxFrameQueries);
+	if (!d_depth) depth_type = LCD_DEPTH_NONE;
+	if (depth_type < LCD_DEPTH_NONE || depth_type > LCD_DEPTH_MASK_U8) LCD_FAIL(e, LCD_ERR_INVALID, "unknown depth type %d", depth_type);
+	const bool use_mask = depth_type == LCD_DEPTH_MASK_U8 || (depth_type != LCD_DEPTH_NONE && p->depth_as_mask);
+	const size_t px = static_cast<size_t>(width) * height;
+	const size_t pyr = static_cast<size_t>(total_frames) * g.frame_stride;
+	LCD_CUDA(e, e->o_gray.reserve(pyr, 0, false, s));
+	LCD_CUDA(e, e->o_blur.reserve(pyr, 0, false, s));
+	if (use_mask) LCD_CUDA(e, e->o_mask.reserve(pyr, 0, false, s));
+	LCD_CUDA(e, e->g_eig.reserve(static_cast<size_t>(total_frames) * px, 0, false, s));
+	LCD_CUDA(e, e->g_max_key.reserve(total_frames, 0, false, s));
+	LCD_CUDA(e, e->g_count.reserve(total_frames, 0, false, s));
+	LCD_CUDA(e, e->g_keys.reserve(static_cast<size_t>(total_frames) * kGfttCandCap, 0, false, s));
+	const int bitmap_words = (width + 31) / 32;
+	const size_t bitmap_bytes = static_cast<size_t>(bitmap_words) * height * sizeof(uint32_t);
+	const bool bitmap_smem = bitmap_bytes <= static_cast<size_t>(kGfttBitmapSmem);
+	if (!bitmap_smem) LCD_CUDA(e, e->g_bitmap.reserve(static_cast<size_t>(total_frames) * bitmap_words * height, 0, false, s));
+	if (frame0 == 0)
+	{
+		LCD_CUDA(e, e->o_overflow.reserve(1, 0, true, s));
+		LCD_CUDA(e, zero_fill_async(e->o_overflow.p, sizeof(int), s));
+	}
+	if (!d_kp)
+	{
+		LCD_CUDA(e, e->o_kp.reserve(static_cast<size_t>(total_frames) * cap, 0, false, s));
+		d_kp = e->o_kp.p;
+	}
+	if (!d_n)
+	{
+		LCD_CUDA(e, e->o_n.reserve(total_frames, 0, false, s));
+		d_n = e->o_n.p;
+	}
+	d_images += static_cast<size_t>(frame0) * px * channels;
+	if (d_depth) d_depth = static_cast<const unsigned char *>(d_depth) + static_cast<size_t>(frame0) * px * (depth_elem_bytes(depth_type));
+	uint8_t * const w_gray = e->o_gray.p + static_cast<size_t>(frame0) * g.frame_stride;
+	uint8_t * const w_blur = e->o_blur.p + static_cast<size_t>(frame0) * g.frame_stride;
+	uint8_t * const w_mask = use_mask ? e->o_mask.p + static_cast<size_t>(frame0) * g.frame_stride : nullptr;
+	float * const w_eig = e->g_eig.p + static_cast<size_t>(frame0) * px;
+	unsigned * const w_max_key = e->g_max_key.p + frame0;
+	int * const w_count = e->g_count.p + frame0;
+	unsigned long long * const w_keys = e->g_keys.p + static_cast<size_t>(frame0) * kGfttCandCap;
+	uint32_t * const w_bitmap = bitmap_smem ? nullptr : e->g_bitmap.p + static_cast<size_t>(frame0) * bitmap_words * height;
+	d_kp += static_cast<size_t>(frame0) * cap;
+	d_n += frame0;
+	if (d_desc) d_desc += static_cast<size_t>(frame0) * cap * 32;
+	if (d_xyz) d_xyz += static_cast<size_t>(frame0) * cap * 3;
+	if (d_uv) d_uv += static_cast<size_t>(frame0) * cap * 2;
+	LCD_TRY(load_gauss7(e, s));
+	prof_mark(e, LCD_PROF_ORB, s);
+	LCD_CUDA(e, zero_fill_async(w_max_key, n_frames * sizeof(unsigned), s));
+	LCD_CUDA(e, zero_fill_async(w_count, n_frames * sizeof(int), s));
+	e->orb_path = 8;
+	{
+		OrbPrepArgs a{};
+		a.images = d_images;
+		a.channels = channels;
+		a.depth = use_mask ? d_depth : nullptr;
+		a.depth_type = depth_type;
+		a.min_depth = p->min_depth;
+		a.max_depth = p->max_depth;
+		a.gray = w_gray;
+		a.mask = w_mask;
+		a.g = g;
+		const bool aligned = ((reinterpret_cast<uintptr_t>(d_images) | reinterpret_cast<uintptr_t>(a.depth) | reinterpret_cast<uintptr_t>(w_gray) |
+		                       reinterpret_cast<uintptr_t>(w_mask)) & 15u) == 0 && g.frame_stride % 16 == 0;
+		if (width % 8 == 0 && aligned)
+		{
+			e->orb_path |= 4;
+			dim3 blk(16, 16), grd((width / 8 + 15) / 16, (height / 2 + 15) / 16, n_frames);
+			orb_prepare_vec_kernel<<<grd, blk, 0, s>>>(a);
+		}
+		else
+		{
+			dim3 blk(32, 8), grd(((width + 1) / 2 + 31) / 32, ((height + 1) / 2 + 7) / 8, n_frames);
+			orb_prepare_kernel<<<grd, blk, 0, s>>>(a);
+		}
+		LCD_CHECK_LAUNCH(e);
+	}
+	if (d_desc)
+	{
+		dim3 grd((width + kBlurTW - 1) / kBlurTW, (height + kBlurTH - 1) / kBlurTH, n_frames);
+		orb_blur_kernel<<<grd, 256, 0, s>>>(w_gray, w_blur, g, 0);
+		LCD_CHECK_LAUNCH(e);
+	}
+	{
+		GfttEigArgs a{w_gray, w_mask, width, height, g.frame_stride, w_eig, w_max_key};
+		gftt_eig_kernel<<<dim3((width + kGfttColTile - 1) / kGfttColTile, n_frames), 128, 0, s>>>(a);
+		LCD_CHECK_LAUNCH(e);
+	}
+	{
+		GfttCandArgs a{w_eig, w_mask, width, height, g.frame_stride, w_max_key, e->gftt.quality_level, w_keys, w_count, e->o_overflow.p};
+		gftt_cand_kernel<<<dim3((width + 31) / 32, (height + 7) / 8, n_frames), dim3(32, 8), 0, s>>>(a);
+		LCD_CHECK_LAUNCH(e);
+	}
+	{
+		const int smem = kGfttSortChunk * static_cast<int>(sizeof(unsigned long long));
+		LCD_CUDA(e, cudaFuncSetAttribute(gftt_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+		gftt_sort_kernel<<<n_frames, 1024, smem, s>>>(w_keys, w_count);
+		LCD_CHECK_LAUNCH(e);
+	}
+	{
+		GfttSelectArgs a{};
+		a.keys = w_keys;
+		a.count = w_count;
+		a.w = width;
+		a.h = height;
+		a.min_distance = e->gftt.min_distance;
+		a.max_corners = p->n_features;
+		a.edge = p->edge_threshold;
+		a.bitmap_words = bitmap_words;
+		a.bitmap = w_bitmap;
+		a.kps = d_kp;
+		a.n_kp = d_n;
+		a.cap = cap;
+		const int smem = (bitmap_smem && a.min_distance >= 1.0) ? static_cast<int>(bitmap_bytes) : 0;
+		LCD_CUDA(e, cudaFuncSetAttribute(gftt_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kGfttBitmapSmem));
+		gftt_select_kernel<<<n_frames, 256, smem, s>>>(a);
+		LCD_CHECK_LAUNCH(e);
+	}
+	if (d_desc)
+	{
+		dim3 grd((cap + kOrbDescribeKp - 1) / kOrbDescribeKp, n_frames);
+		if (g.edge >= kOrbPatchR && width % 4 == 0)
+		{
+			e->orb_path |= 2;
+			orb_describe_patch_kernel<<<grd, 256, 0, s>>>(w_blur, g, d_kp, d_n, cap, d_desc);
+		}
+		else
+			orb_describe_kernel<<<grd, 256, 0, s>>>(w_gray, w_blur, g, d_kp, d_n, cap, d_desc);
+		LCD_CHECK_LAUNCH(e);
+	}
+	LCD_TRY(orb_lift(e, n_frames, width, height, d_depth, depth_type, p, cap, d_kp, d_n, d_xyz, d_uv, s));
+	prof_mark(e, LCD_PROF_ORB, s);
+	return LCD_OK;
+}
+
 // Detect + describe frames [frame0, frame0 + n_frames) of a batch of total_frames (total_frames = 0: the range is the whole
 // batch).  Every input, workspace and output pointer addresses frame 0 of the batch; ranges are independent, so the host
 // path runs them chunk by chunk while the next chunk's images are still on their way over PCIe.
@@ -2398,6 +2610,9 @@ static int orb_run(lcd_engine * e, int n_frames, const uint8_t * d_images, int w
                    int depth_type, const lcd_orb_params * p, int cap, OrbKeypoint * d_kp, uint8_t * d_desc, float * d_xyz, float * d_uv,
                    int * d_n, cudaStream_t s, int frame0 = 0, int total_frames = 0)
 {
+	if (e->detector == LCD_DETECTOR_GFTT_ORB)
+		return gftt_run(e, n_frames, d_images, width, height, channels, d_depth, depth_type, p, cap, d_kp, d_desc, d_xyz, d_uv, d_n, s, frame0,
+		                total_frames);
 	if (total_frames <= 0) total_frames = frame0 + n_frames;
 	OrbGeom g{};
 	LCD_TRY(orb_geometry(e, width, height, p, g));
@@ -2449,21 +2664,7 @@ static int orb_run(lcd_engine * e, int n_frames, const uint8_t * d_images, int w
 	if (d_desc) d_desc += static_cast<size_t>(frame0) * cap * 32;
 	if (d_xyz) d_xyz += static_cast<size_t>(frame0) * cap * 3;
 	if (d_uv) d_uv += static_cast<size_t>(frame0) * cap * 2;
-	if (e->gauss_sigma_loaded != 2.0f)
-	{
-		// cv::getGaussianKernel(7, 2, CV_32F): exp(-x^2 / (2 sigma^2)) normalised in double, stored as float
-		double t[7], sum = 0;
-		for (int i = 0; i < 7; ++i)
-		{
-			t[i] = exp(-0.5 * (i - 3) * (i - 3) / 4.0);
-			sum += t[i];
-		}
-		float kf[7];
-		for (int i = 0; i < 7; ++i) kf[i] = static_cast<float>(t[i] / sum);
-		LCD_CUDA(e, cudaMemcpyToSymbolAsync(kOrbGauss7, kf, sizeof(kf), 0, cudaMemcpyHostToDevice, s));
-		LCD_CUDA(e, cudaStreamSynchronize(s));
-		e->gauss_sigma_loaded = 2.0f;
-	}
+	LCD_TRY(load_gauss7(e, s));
 	prof_mark(e, LCD_PROF_ORB, s);
 	LCD_CUDA(e, zero_fill_async(w_cand_count, slots * sizeof(int), s));
 	{
@@ -2603,36 +2804,7 @@ static int orb_run(lcd_engine * e, int n_frames, const uint8_t * d_images, int w
 			orb_describe_kernel<<<grd, 256, 0, s>>>(w_gray, w_blur, g, d_kp, d_n, cap, d_desc);
 		LCD_CHECK_LAUNCH(e);
 	}
-	if (d_xyz || d_uv)
-	{
-		if (d_xyz)
-		{
-			OrbXyzArgs a{};
-			a.depth = (depth_type != LCD_DEPTH_NONE && depth_type != LCD_DEPTH_MASK_U8) ? d_depth : nullptr;
-			a.depth_type = depth_type;
-			a.w = width;
-			a.h = height;
-			a.fx = p->fx;
-			a.fy = p->fy;
-			a.cx = p->cx;
-			a.cy = p->cy;
-			a.min_depth = p->min_depth;
-			a.max_depth = p->max_depth;
-			a.kps = d_kp;
-			a.n_kp = d_n;
-			a.cap = cap;
-			a.xyz = d_xyz;
-			dim3 grd((cap + 255) / 256, n_frames);
-			orb_xyz_kernel<<<grd, 256, 0, s>>>(a);
-			LCD_CHECK_LAUNCH(e);
-		}
-		if (d_uv)
-		{
-			dim3 grd((cap + 255) / 256, n_frames);
-			orb_uv_kernel<<<grd, 256, 0, s>>>(d_kp, d_n, cap, d_uv);
-			LCD_CHECK_LAUNCH(e);
-		}
-	}
+	LCD_TRY(orb_lift(e, n_frames, width, height, d_depth, depth_type, p, cap, d_kp, d_n, d_xyz, d_uv, s));
 	prof_mark(e, LCD_PROF_ORB, s);
 	return LCD_OK;
 }
@@ -2683,8 +2855,36 @@ int lcd_orb_detect_describe(lcd_engine * e, int n_frames, const uint8_t * images
 	int overflow = 0;
 	LCD_CUDA(e, cudaMemcpyAsync(&overflow, e->o_overflow.p, sizeof(int), cudaMemcpyDeviceToHost, s));
 	LCD_CUDA(e, cudaStreamSynchronize(s));
+	if (overflow && e->detector == LCD_DETECTOR_GFTT_ORB)
+		LCD_FAIL(e, LCD_ERR_CAPACITY, "more than %d GFTT candidates in a frame: raise GFTT/QualityLevel", kGfttCandCap);
 	if (overflow) LCD_FAIL(e, LCD_ERR_CAPACITY, "more than %d FAST corners in pyramid level 0 (half as many per further level): raise FAST/Threshold", kOrbCandCap);
 	return LCD_OK;
+}
+
+int lcd_detector_set(lcd_engine * e, int detector, const lcd_gftt_params * params)
+{
+	if (!e) return LCD_ERR_INVALID;
+	if (detector == LCD_DETECTOR_ORB)
+	{
+		e->detector = detector;
+		return LCD_OK;
+	}
+	if (detector != LCD_DETECTOR_GFTT_ORB) LCD_FAIL(e, LCD_ERR_INVALID, "unknown detector %d", detector);
+	const lcd_gftt_params q = params ? *params : lcd_gftt_params{0.001, 7.0, 3, 0, 0.04};
+	if (q.use_harris != 0) LCD_FAIL(e, LCD_ERR_INVALID, "GFTT/UseHarrisDetector is not implemented");
+	if (q.block_size != 3) LCD_FAIL(e, LCD_ERR_INVALID, "only GFTT/BlockSize=3 is implemented");
+	if (!(q.quality_level > 0.0) || !std::isfinite(q.quality_level)) LCD_FAIL(e, LCD_ERR_INVALID, "GFTT/QualityLevel must be positive");
+	if (!(q.min_distance >= 0.0) || !std::isfinite(q.min_distance)) LCD_FAIL(e, LCD_ERR_INVALID, "GFTT/MinDistance must not be negative");
+	e->gftt = q;
+	e->detector = detector;
+	return LCD_OK;
+}
+
+int lcd_detector_get(const lcd_engine * e, lcd_gftt_params * params)
+{
+	if (!e) return LCD_ERR_INVALID;
+	if (params) *params = e->gftt;
+	return e->detector;
 }
 
 int lcd_orb_overflow(lcd_engine * e)
