@@ -291,7 +291,7 @@ struct lcd_engine
 	// --- scratch
 	DevBuf<uint32_t> d_queries;
 	DevBuf<uint2> d_partial;
-	DevBuf<uint4> tc_words;             // cached +-1 byte image of the vocabulary rows [0, tc_rows) for the tensor-core 2-NN
+	DevBuf<uint4> tc_words;             // cached packed image of the vocabulary rows [0, tc_rows) for the tensor-core 2-NN (tc_pack_kernel)
 	int tc_rows = 0;
 	DevBuf<uint32_t> d_keys;
 	DevBuf<int> d_word_ids, d_n_new, d_in_ids;
@@ -803,7 +803,7 @@ int run_knn(lcd_engine * e, const uint32_t * d_q, int nq_total, int n_rows, int 
 	}
 	if (e->nn_tensor && e->nw == 8 && n_rows > 0 && nq_total > 0 && kTcSmemBytes <= static_cast<size_t>(e->smem_optin))
 	{
-		// tensor-core path: expand both operands to the int8 images, then one CTA per (query tile, word split)
+		// tensor-core path: the cached packed word image, then one CTA per (query tile, word split)
 		const int n_wtiles = (n_rows + kTcBN - 1) / kTcBN, n_qtiles = (nq_total + kTcBM - 1) / kTcBM;
 		int best_split = 1;
 		long best_cost = -1;
@@ -826,14 +826,16 @@ int run_knn(lcd_engine * e, const uint32_t * d_q, int nq_total, int n_rows, int 
 		if (tc_recache) e->tc_rows = 0;
 		if (e->tc_rows < n_rows)
 		{
-			// the +-1 byte image of the words is cached with the dictionary: only tiles that gained rows since the last search are written
+			// the packed word image (operand layout + per-word popcounts) is cached with the dictionary: only tiles that gained rows since
+			// the last search are written
 			const int t0 = e->tc_rows / kTcBN;
-			const size_t tile16 = static_cast<size_t>(kTcBN) * 16;
+			const size_t tile16 = kTcBBytes / 16;
 			const int old_tiles = static_cast<int>(e->tc_words.cap / tile16);
 			if (n_wtiles > old_tiles)
 				LCD_CUDA(e, e->tc_words.reserve(static_cast<size_t>(std::max(n_wtiles, old_tiles + old_tiles / 2 + 16)) * tile16, static_cast<size_t>(t0) * tile16, false, s));
 			const size_t todo = static_cast<size_t>(n_wtiles - t0) * tile16;
-			tc_expand_kernel<<<static_cast<unsigned>((todo + 255) / 256), 256, 0, s>>>(e->vocab.p, n_rows, kTcBN, t0, n_wtiles, e->tc_words.p);
+			tc_pack_kernel<<<static_cast<unsigned>((todo + 255) / 256), 256, 0, s>>>(reinterpret_cast<const uint4 *>(e->vocab.p), n_rows, t0, n_wtiles,
+			                                                                      e->tc_words.p);
 			LCD_CHECK_LAUNCH(e);
 			e->tc_rows = n_rows;
 		}
@@ -854,7 +856,7 @@ int run_knn(lcd_engine * e, const uint32_t * d_q, int nq_total, int n_rows, int 
 		else if (nn_persist)
 			grid = std::min(n_items, e->sm_count);
 		knn2_tensor_kernel<<<grid, kTcThreads, kTcSmemBytes, s>>>(e->tc_words.p, n_rows, e->row_offset, d_q, nq_total, e->d_partial.p, tps,
-		                                                        static_cast<uint32_t>(-32), n_qtiles, best_split);
+		                                                        static_cast<uint32_t>(-128), n_qtiles, best_split);
 		prof_mark(e, LCD_PROF_NN, s);
 		LCD_CHECK_LAUNCH(e);
 		e->nn_last_tensor = 1;

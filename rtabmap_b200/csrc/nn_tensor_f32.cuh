@@ -171,7 +171,7 @@ __global__ void tf_query_init_kernel(const float * __restrict__ q, int nq, float
 	tau[i] = 0xFF800000u; // f2ord(+inf): no bound yet
 }
 
-// D[regs] (+)= A[smem] * B[smem]^T, f16 x f16 -> f32, M64 x N256 x K16 over one warpgroup (same fragment layout as wg_mma_i8)
+// D[regs] (+)= A[smem] * B[smem]^T, f16 x f16 -> f32, M64 x N256 x K16 over one warpgroup (same fragment layout as wg_mma_b1)
 __device__ __forceinline__ void wg_mma_f16(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
 {
 	asm volatile(
@@ -207,17 +207,6 @@ __device__ __forceinline__ void wg_mma_f16(float (&d)[128], uint64_t adesc, uint
 		  "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
 		: "l"(adesc), "l"(bdesc), "r"(accumulate)
 		: "memory");
-}
-
-// shared-memory matrix descriptor (GMMA) of an UN-swizzled K-major operand slab of one K-step (16 halves): 8 x 16-byte core matrices,
-// the two k-chunks of a row group 128 B apart (leading byte offset), row groups 256 B apart (stride byte offset)
-__device__ __forceinline__ uint64_t wg_smem_desc_noswz(uint32_t saddr)
-{
-	uint64_t d = 0;
-	d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);        // start address  [0,14)
-	d |= static_cast<uint64_t>(128 >> 4) << 16;                  // leading byte offset [16,30): next core matrix along K
-	d |= static_cast<uint64_t>(256 >> 4) << 32;                  // stride byte offset [32,46): next 8-row group
-	return d;                                                    // layout type 0: no swizzle
 }
 
 struct TfArgs
