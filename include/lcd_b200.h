@@ -612,6 +612,39 @@ int lcd_process_decide_batch_dev(lcd_engine * e, const void * d_queries, const f
                                  const lcd_verify_params * vp, const int * clients, const int * frame_flags, const lcd_decide_params * dp,
                                  int * d_word_ids_out, float * d_likelihood_out, float * d_posterior_out, void * stream);
 
+/* ---- the GPS filter of the place list (Rtabmap/LoopGPS, on by default) -------------------------------------------------------
+ * replaces: the construction of signaturesToCompare in Rtabmap::process (Rtabmap.cpp:2046-2115) in localisation mode.  A frame with a
+ * GPS fix compares only the places whose GPS position lies within RGBD/LocalRadius of its own (altitude differences under the frame's
+ * GPS error ignored) and every place without a fix; adjustLikelihood, the prediction and the posterior then run over those places only,
+ * as the reference's do over the shorter likelihood map.  Mapping mode (the nearest node's fix for a frame without one, a non-identity
+ * originOffsetENU, Rtabmap.cpp:2014-2038) is not covered. */
+typedef struct lcd_gps { /* the fields of rtabmap::GPS (GPS.h:68-72) the filter reads */
+	double stamp;            /* > 0: a fix; otherwise none */
+	double longitude, latitude, altitude, error; /* degrees, degrees, metres, metres */
+} lcd_gps;
+
+/* The GPS of every real place of the current map: ids[n] ascending exactly as lcd_clients_set_map received them after the virtual place,
+ * gps[n] each place's sensorData().gps() (or what Memory::getGPS found for it, Memory.cpp:4507-4553), offset_enu[n][3] the x, y, z of
+ * getGPS's offsetENU (NULL = zeros).  A place whose stamp is not > 0 is always compared (Rtabmap.cpp:2077: no cache entry -> accept).
+ * Each place's geocentric point (GeodeticCoords::toGeocentric_WGS84, GeodeticCoords.cpp:75-102) is computed here, once per map, with
+ * the host's libm.  LCD_ERR_STATE without a map; LCD_ERR_INVALID for other ids or a value that is not finite (nothing changes then).
+ * lcd_clients_set_map drops the table. */
+int lcd_clients_set_map_gps(lcd_engine * e, const int * ids, int n, const lcd_gps * gps, const float * offset_enu);
+
+/* lcd_decide_batch_dev where a frame that computes a posterior and has frame_gps[f].stamp > 0 compares only the places of
+ * Rtabmap.cpp:2046-2115 with radius local_radius (RGBD/LocalRadius, 10 by default; >= 0).  Frames without a fix, skipped and held frames
+ * (which ignore their fix, as the reference does), and every frame when frame_gps is NULL are decided exactly as lcd_decide_batch_dev
+ * decides them.  A gated frame's posterior row, and its client's state, hold 0 for the places it did not compare; the single-hypothesis
+ * check counts its compared places.  d_compared_out[n_frames][ns] (device, may be NULL): 1 where the frame compared the place (every
+ * place of a frame without a fix, none of a skipped or held frame).  lcd_decide_fetch, lcd_process_fetch, lcd_decide_epipolar_dev,
+ * lcd_decide_proximity_dev and lcd_verify_decided_dev take this decision as they take lcd_decide_batch_dev's.  LCD_ERR_INVALID (nothing
+ * changes) for a negative or non-finite radius, a frame GPS value that is not finite and lcd_decide_batch_dev's cases; LCD_ERR_STATE when
+ * a frame that computes has a fix and the current map has no GPS table.  Device scratch: n_frames x (ns + 1) bytes for the compared
+ * places and 12 bytes per (place, frame that computes) for the gated frames' prediction columns. */
+int lcd_decide_gps_batch_dev(lcd_engine * e, const float * d_likelihood, int n_frames, int ns, const int * clients, const int * frame_flags,
+                             const lcd_gps * frame_gps, float local_radius, const lcd_decide_params * dp, float * d_posterior_out,
+                             unsigned char * d_compared_out, void * stream);
+
 /* ---- word-range sharding across GPUs (SURVEY.md §8(e)) ---------------------------
  * Each rank owns the words whose row (in ascending id order) falls in its range; rows
  * are numbered globally: set the global row offset of this shard so that packed top-2

@@ -152,6 +152,19 @@ class ProximityResult(C.Structure):
     ]
 
 
+# lcd_gps: rtabmap::GPS's stamp (> 0: a fix), longitude, latitude (degrees), altitude and error (metres), as a structured array
+GPS_DTYPE = np.dtype([("stamp", np.float64), ("longitude", np.float64), ("latitude", np.float64), ("altitude", np.float64), ("error", np.float64)])
+
+
+def gps_array(gps) -> np.ndarray:
+    """lcd_gps records from a GPS_DTYPE array or rows of (stamp, longitude, latitude, altitude, error)."""
+    a = np.asarray(gps)
+    if a.dtype != GPS_DTYPE:
+        a = np.ascontiguousarray(a, np.float64).reshape(-1, 5)
+        a = np.ascontiguousarray(a).view(GPS_DTYPE).reshape(-1)
+    return np.ascontiguousarray(a)
+
+
 # frame flags and decision statuses of lcd_decide_batch_dev (lcd_b200.h)
 FRAME_SKIP, FRAME_HOLD, FRAME_AGGRESSIVE = 1, 2, 4
 DECIDE_STATUS = ("skipped", "held", "no hypothesis", "under threshold", "under ratio", "single hypothesis", "ratio", "last null", "accepted",
@@ -271,6 +284,8 @@ SIGNATURES = {
     "lcd_decide_epipolar_dev": (_I, [_P, _P, _P, _P, _I, _I, _P, _P]),
     "lcd_epipolar_fetch": (_I, [_P, _I, _P]),
     "lcd_clients_set_map_poses": (_I, [_P, _P, _I, _P, _P, _P]),
+    "lcd_clients_set_map_gps": (_I, [_P, _P, _I, _P, _P]),
+    "lcd_decide_gps_batch_dev": (_I, [_P, _P, _I, _I, _P, _P, _P, _F, _P, _P, _P, _P]),
     "lcd_decide_proximity_dev": (_I, [_P, _P, _P, _I, _I, _P, _P, _P, _P]),
     "lcd_proximity_fetch": (_I, [_P, _I, _P]),
     "lcd_profile_enable": (_I, [_P, _I]),
@@ -999,6 +1014,31 @@ class Engine:
             raise LcdError(-1, f"clients and frame_flags need {n_frames} entries")
         self._check(self._lib.lcd_decide_batch_dev(self._h, C.c_void_p(d_likelihood), int(n_frames), int(ns), _ptr(c), _ptr(f), C.byref(dp),
                                                     C.c_void_p(d_posterior_out or None), C.c_void_p(stream or None)))
+
+    def clients_set_map_gps(self, ids, gps, offset_enu=None):
+        """The GPS of every real place of the current map (ids ascending as set_map's; gps as gps_array takes it; offset_enu [n, 3] float32,
+        the x, y, z of Memory::getGPS's offsetENU, or None for zeros).  Dropped by the next clients_set_map."""
+        i = _i32(ids)
+        g = gps_array(gps)
+        o = None if offset_enu is None else np.ascontiguousarray(offset_enu, np.float32).reshape(-1, 3)
+        if len(g) != len(i) or (o is not None and len(o) != len(i)):
+            raise LcdError(-1, f"{len(i)} places need {len(i)} GPS records and offsets")
+        self._check(self._lib.lcd_clients_set_map_gps(self._h, _ptr(i), len(i), _ptr(g), None if o is None else _ptr(o)))
+
+    def decide_gps_batch_dev(self, d_likelihood: int, n_frames: int, ns: int, clients, frame_flags, frame_gps, local_radius: float,
+                             dp: DecideParams, d_posterior_out: int = 0, d_compared_out: int = 0, stream: int = 0):
+        """decide_batch_dev with Rtabmap/LoopGPS: a frame that computes and carries a fix (frame_gps as gps_array takes it, one per frame,
+        or None for no fixes) compares only the places within local_radius (RGBD/LocalRadius) of it.  d_compared_out: uint8 [n_frames][ns]
+        on the device, 1 where the place was compared, or 0."""
+        c = _i32(clients)
+        f = _i32(frame_flags)
+        g = None if frame_gps is None else gps_array(frame_gps)
+        if len(c) != n_frames or len(f) != n_frames or (g is not None and len(g) != n_frames):
+            raise LcdError(-1, f"clients, frame_flags and frame_gps need {n_frames} entries")
+        self._check(self._lib.lcd_decide_gps_batch_dev(self._h, C.c_void_p(d_likelihood), int(n_frames), int(ns), _ptr(c), _ptr(f),
+                                                        None if g is None else _ptr(g), float(local_radius), C.byref(dp),
+                                                        C.c_void_p(d_posterior_out or None), C.c_void_p(d_compared_out or None),
+                                                        C.c_void_p(stream or None)))
 
     def sig_words_add_batch(self, sig_ids, word_ids, uv, n):
         """The stored places' words and keypoints for the epipolar check: word_ids [k, cap] int32, uv [k, cap, 2] float32, n [k]."""

@@ -101,7 +101,9 @@ struct BayesColumn
 	float u, scale, delta;
 };
 
-__device__ inline BayesColumn bayes_column(const BayesArgs & a, int c)
+// listed (nullptr: every row): the rows of the places in this call's matrix; a.n then counts those places (the prediction of a frame
+// whose place list was cut, Rtabmap.cpp:2046-2115: generatePrediction only sees the listed neighbours, BayesFilter.cpp:352-372)
+__device__ inline BayesColumn bayes_column(const BayesArgs & a, int c, const unsigned char * listed = nullptr)
 {
 	if (a.ids[c] < 0) return BayesColumn{0.f, 1.f, 0.f};
 	const int first = a.vp_used ? 1 : 0;
@@ -110,6 +112,7 @@ __device__ inline BayesColumn bayes_column(const BayesArgs & a, int c)
 	bool diag_zero = false;
 	for (int e = a.col_ptr[c]; e < a.col_ptr[c + 1]; ++e)
 	{
+		if (listed && !listed[a.nbr_row[e]]) continue;
 		const float v = static_cast<float>(a.lc[a.nbr_level[e] + 1]);
 		s = __fadd_rn(s, v);
 		if (a.nbr_row[e] < first) continue;
@@ -146,20 +149,24 @@ __device__ inline BayesColumn bayes_column(const BayesArgs & a, int c)
 	return BayesColumn{value, 1.f, delta};
 }
 
+// P[r][c] of a listed entry with LC value v (float) in column col (the diagonal gets the column's delta)
+__device__ inline float bayes_entry_pv(float v, bool diag, const BayesColumn & col, float eps)
+{
+	if (diag) v = __fadd_rn(v, col.delta);
+	float pv = v;
+	if (v == 0.f) pv = col.u; // a listed neighbour with a zero LC value is filled like any other zero row (already scaled)
+	else if (col.scale < 0.f)
+	{
+		pv = __fmul_rn(v, -col.scale);
+		if (pv < eps) pv = 0.f;
+	}
+	return pv;
+}
+
 // P[r][c] of listed entry e (row r of column c), the columns' values already in col_u / col_scale / col_delta
 __device__ inline float bayes_entry_value(const BayesArgs & a, int e, int c, int r)
 {
-	float v = static_cast<float>(a.lc[a.nbr_level[e] + 1]);
-	if (r == c) v = __fadd_rn(v, a.col_delta[c]);
-	const float sc = a.col_scale[c];
-	float pv = v;
-	if (v == 0.f) pv = a.col_u[c]; // a listed neighbour with a zero LC value is filled like any other zero row (already scaled)
-	else if (sc < 0.f)
-	{
-		pv = __fmul_rn(v, -sc);
-		if (pv < a.eps) pv = 0.f;
-	}
-	return pv;
+	return bayes_entry_pv(static_cast<float>(a.lc[a.nbr_level[e] + 1]), r == c, BayesColumn{a.col_u[c], a.col_scale[c], a.col_delta[c]}, a.eps);
 }
 
 // the virtual-place row and column (:375-411, :482-487): P[0][0], and P[r][0] of every real place r

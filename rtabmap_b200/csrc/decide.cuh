@@ -10,6 +10,11 @@
 // last posteriors stored [place][frame], so an entry reads B contiguous values.  Every sum over places (U, the real places' last
 // posterior, the posterior sum) runs in a fixed order that depends on the number of places only: a frame's posterior is the same
 // bits whatever the batch size, its position in the batch and the other clients in it.
+//
+// A frame with a GPS fix (lcd_decide_gps_batch_dev) compares only the places within RGBD/LocalRadius of it (Rtabmap.cpp:2046-2115).
+// Such a "gated" frame keeps the map's layout: its places that are not compared get a last posterior and an adjusted likelihood of
+// exactly 0, so they add exact zeros to every fixed-order sum, and its prediction columns are recomputed over the compared rows only
+// (decide_gps_columns_kernel).  A gate that keeps every place therefore gives the ungated bits.
 #pragma once
 #include "bayes.cuh"
 
@@ -43,6 +48,26 @@ struct DecideMap
 	const double * t_val;   // [nt] P[r][c] - u_c
 	double lc0;             // Bayes/PredictionLC[0] (P[0][c] of every real place, as a float)
 	float vpp;              // Bayes/VirtualPlacePriorThr
+	const float * t_lv;     // [nt] LC value of each listed entry, as a float (for the columns of gated frames)
+	float eps;              // _predictionEpsilon
+};
+
+// the GPS filter of the place list (Rtabmap/LoopGPS, Rtabmap.cpp:2046-2115).  A place's geocentric point (GeodeticCoords::toGeocentric_WGS84, computed on the host) and the x, y, z of its offsetENU (Memory::getGPS).
+struct GpsPlace
+{
+	double x, y, z;
+	float ox, oy, oz;
+	int fix; // stamp > 0: otherwise the place has no cache entry and is always compared (:2077)
+};
+
+// a frame's place list: kGpsNone computes nothing (skipped / held), kGpsAll compares every place, kGpsGated runs the filter with the
+// frame's geocentric origin and the sines and cosines of its latitude and longitude (computed on the host)
+constexpr int kGpsNone = 0, kGpsAll = 1, kGpsGated = 2;
+struct GpsFrame
+{
+	double x, y, z, slat, clat, slon, clon, error;
+	int mode;
+	int pad;
 };
 
 // set_map: the listed entries in row order, k -> (entry e of column c, row r); t_val[k] = P[r][c] - u_c in double
@@ -86,7 +111,16 @@ struct DecideBatch
 	double * u;                 // [B] U
 	double * s1;                // [B] sum of the real places' last posterior
 	double * psum;              // [B] posterior sum (normalised by it as a float, as the reference does)
+	// gated frames (nullptr in lcd_decide_batch_dev: no frame is gated)
+	const GpsFrame * gps;       // [n_frames] kGpsGated: the frame compares only the places of listed
+	const int * count;          // [n_frames] real places a gated frame compares
+	const unsigned char * listed; // [n_frames][n] 1 = compared
+	float * fu;                 // [n][B] columns of the gated frames: uniform value, scale, delta
+	float * fscale;
+	float * fdelta;
 };
+
+__device__ __forceinline__ bool decide_gated(const DecideBatch & d, int f) { return d.gps && d.gps[f].mode == kGpsGated; }
 
 __global__ void decide_last_kernel(const DecideMap m, const DecideBatch d)
 {
@@ -95,7 +129,31 @@ __global__ void decide_last_kernel(const DecideMap m, const DecideBatch d)
 	const int r = static_cast<int>(i / d.B), b = static_cast<int>(i % d.B);
 	const int * prev_ids = reinterpret_cast<const int *>(d.prev_ids[b]);
 	const float * prev = d.cl_post + d.client[b] * d.stride;
-	d.last_t[i] = bayes_rekey(prev_ids, prev, static_cast<int>(d.prev_n[b]), m.ids[r]);
+	const int f = static_cast<int>(d.frame[b]);
+	float v = bayes_rekey(prev_ids, prev, static_cast<int>(d.prev_n[b]), m.ids[r]);
+	if (decide_gated(d, f) && !d.listed[static_cast<size_t>(f) * m.n + r]) v = 0.f; // updatePosterior over the compared ids only
+	d.last_t[i] = v;
+}
+
+// the prediction's columns of every gated frame over its compared places (generatePrediction + normalize with cols = compared + 1);
+// a column that is not compared gets (0, 1, 0), which its zero last posterior makes inert.  a: the map's columns (set_map's BayesArgs).
+__global__ void decide_gps_columns_kernel(BayesArgs a, const DecideBatch d)
+{
+	const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+	if (i >= static_cast<long long>(a.n) * d.B) return;
+	const int c = static_cast<int>(i / d.B), b = static_cast<int>(i % d.B);
+	const int f = static_cast<int>(d.frame[b]);
+	if (d.gps[f].mode != kGpsGated) return;
+	const unsigned char * listed = d.listed + static_cast<size_t>(f) * a.n;
+	BayesColumn col{0.f, 1.f, 0.f};
+	if (listed[c])
+	{
+		a.n = d.count[f] + 1;
+		col = bayes_column(a, c, listed);
+	}
+	d.fu[i] = col.u;
+	d.fscale[i] = col.scale;
+	d.fdelta[i] = col.delta;
 }
 
 // partial U and last-posterior sums over a chunk of columns, each frame's columns added in ascending order
@@ -104,12 +162,14 @@ __global__ void __launch_bounds__(kDcThreads) decide_columns_kernel(const Decide
 	const int c0 = blockIdx.x * kDcColChunk, c1 = min(m.n, c0 + kDcColChunk);
 	for (int b = threadIdx.x; b < d.B; b += blockDim.x)
 	{
+		const float * col_u = decide_gated(d, static_cast<int>(d.frame[b])) ? d.fu : nullptr;
 		double u = 0.0, s1 = 0.0;
 		for (int c = c0; c < c1; ++c)
 		{
 			if (m.ids[c] < 0) continue;
 			const float last = d.last_t[static_cast<size_t>(c) * d.B + b];
-			const double up = static_cast<double>(m.col_u[c]) * static_cast<double>(last);
+			const float cu = col_u ? col_u[static_cast<size_t>(c) * d.B + b] : m.col_u[c];
+			const double up = static_cast<double>(cu) * static_cast<double>(last);
 			if (up != 0.0) u += up;
 			s1 += static_cast<double>(last);
 		}
@@ -132,11 +192,13 @@ __global__ void decide_sum_chunks_kernel(const double * __restrict__ part, int n
 __global__ void __launch_bounds__(kDcThreads) decide_rows_kernel(const DecideMap m, const DecideBatch d)
 {
 	const int r0 = blockIdx.x * kDcRowChunk, r1 = min(m.n, r0 + kDcRowChunk);
-	const float p00 = bayes_vp_p00(m.vpp, m.n);
-	const float pr0 = m.n > 1 ? bayes_vp_pr0(m.vpp, m.n) : 0.f;
 	const double lc0f = static_cast<double>(static_cast<float>(m.lc0));
 	for (int b = threadIdx.x; b < d.B; b += blockDim.x)
 	{
+		const bool gated = decide_gated(d, static_cast<int>(d.frame[b]));
+		const int n = gated ? d.count[d.frame[b]] + 1 : m.n; // places of the frame's matrix
+		const float p00 = bayes_vp_p00(m.vpp, n);
+		const float pr0 = n > 1 ? bayes_vp_pr0(m.vpp, n) : 0.f;
 		const double last0 = static_cast<double>(d.last_t[b]);
 		const double u = d.u[b];
 		const float * like = d.adj + d.frame[b] * m.n;
@@ -148,8 +210,19 @@ __global__ void __launch_bounds__(kDcThreads) decide_rows_kernel(const DecideMap
 			else
 			{
 				double acc = 0.0;
-				for (int k = m.t_ptr[r]; k < m.t_ptr[r + 1]; ++k)
-					acc += m.t_val[k] * static_cast<double>(d.last_t[static_cast<size_t>(m.t_col[k]) * d.B + b]);
+				if (!gated)
+					for (int k = m.t_ptr[r]; k < m.t_ptr[r + 1]; ++k)
+						acc += m.t_val[k] * static_cast<double>(d.last_t[static_cast<size_t>(m.t_col[k]) * d.B + b]);
+				else
+					for (int k = m.t_ptr[r]; k < m.t_ptr[r + 1]; ++k)
+					{
+						// decide_entry_values_kernel's P[r][c] - u_c, from the frame's own column c
+						const int c = m.t_col[k];
+						const size_t ci = static_cast<size_t>(c) * d.B + b;
+						const BayesColumn col{d.fu[ci], d.fscale[ci], d.fdelta[ci]};
+						const double tv = static_cast<double>(bayes_entry_pv(m.t_lv[k], r == c, col, m.eps)) - static_cast<double>(col.u);
+						acc += tv * static_cast<double>(d.last_t[ci]);
+					}
 				prior = acc + u;
 				prior += static_cast<double>(pr0) * last0;
 			}
@@ -205,6 +278,8 @@ struct DecideSelect
 	Decision * dec;            // [n_frames]
 	int * hyp_id;              // [n_frames] accepted id or 0
 	int * hyp_slot;            // [n_frames] its store row or -1
+	const GpsFrame * gps;      // [n_frames] or nullptr (DecideBatch::gps)
+	const int * count;         // [n_frames] real places a gated frame compares
 };
 
 // Rtabmap.cpp:2143-2233 for one frame per CTA: the highest real-place posterior (scanned in descending id order with a strict '>', so
@@ -276,7 +351,8 @@ __global__ void decide_select_kernel(const DecideMap m, const DecideSelect a)
 			if ((flags & kDcFlagAggressive) && thr > a.aggressive_loop_thr) thr = a.aggressive_loop_thr;
 			if (d.highest_value >= thr)
 			{
-				if (m.n <= 2 && thr > 0.f) d.status = kDcSingle;
+				const int n = a.gps && a.gps[f].mode == kGpsGated ? a.count[f] + 1 : m.n; // entries of the posterior map
+				if (n <= 2 && thr > 0.f) d.status = kDcSingle;
 				else if (a.loop_ratio > 0.f && last_val != 0.f && d.highest_value < __fmul_rn(a.loop_ratio, last_val)) d.status = kDcRatio;
 				else if (a.loop_ratio > 0.f && last_val == 0.f) d.status = kDcLastNull;
 				else
@@ -320,6 +396,39 @@ __global__ void decide_verified_kernel(int n_frames, const int * __restrict__ ok
 		dec[f].status = status;
 		dec[f].loop_id = 0;
 		hyp_id[f] = 0;
+	}
+}
+
+// listed[f][r] for every frame f and place r (r = 0 the virtual place, always listed by a frame that computes), and count[f] += the real
+// places a gated frame compares.  Geocentric_WGS84ToENU_WGS84 (GeodeticCoords.cpp:119-149), the offset, the altitude tolerance of
+// :2087-2099 and uNormSquared(...) < r2, in the reference's double statements, each operation rounded on its own (no FMA).
+__global__ void decide_gps_gate_kernel(int n, const GpsPlace * __restrict__ places, const GpsFrame * __restrict__ frames, double r2,
+                                       unsigned char * __restrict__ listed, int * __restrict__ count)
+{
+	const int r = blockIdx.x * blockDim.x + threadIdx.x, f = blockIdx.y;
+	const int mode = frames[f].mode;
+	bool keep = mode != kGpsNone;
+	if (mode == kGpsGated && r > 0 && r < n && places[r - 1].fix)
+	{
+		const GpsFrame g = frames[f];
+		const GpsPlace p = places[r - 1];
+		const double rx = __dsub_rn(p.x, g.x), ry = __dsub_rn(p.y, g.y), rz = __dsub_rn(p.z, g.z);
+		double x = __dadd_rn(__dmul_rn(-g.slon, rx), __dmul_rn(g.clon, ry));
+		double y = __dadd_rn(__dsub_rn(__dmul_rn(__dmul_rn(-g.clon, g.slat), rx), __dmul_rn(__dmul_rn(g.slon, g.slat), ry)), __dmul_rn(g.clat, rz));
+		double z = __dadd_rn(__dadd_rn(__dmul_rn(__dmul_rn(g.clon, g.clat), rx), __dmul_rn(__dmul_rn(g.slon, g.clat), ry)), __dmul_rn(g.slat, rz));
+		x = __dadd_rn(x, static_cast<double>(p.ox)); // offsetENU.x() - originOffsetENU.x() (identity in localisation mode), a float
+		y = __dadd_rn(y, static_cast<double>(p.oy));
+		z = __dadd_rn(z, static_cast<double>(p.oz));
+		if (z > g.error) z = __dsub_rn(z, g.error);
+		else if (z < -g.error) z = __dadd_rn(z, g.error);
+		else z = 0.0;
+		keep = __dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dmul_rn(z, z)) < r2;
+	}
+	if (r < n) listed[static_cast<size_t>(f) * n + r] = keep ? 1 : 0;
+	if (mode == kGpsGated)
+	{
+		const unsigned m = __ballot_sync(0xFFFFFFFFu, keep && r > 0 && r < n);
+		if ((threadIdx.x & 31) == 0 && m) atomicAdd(&count[f], __popc(m));
 	}
 }
 

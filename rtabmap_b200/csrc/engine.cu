@@ -326,8 +326,19 @@ struct lcd_engine
 		DevBuf<int> tptr;     // [n+1] listed entries by row
 		DevBuf<int> tcol;     // [nt] their columns
 		DevBuf<double> tval;  // [nt] P[r][c] - u_c
+		// what the columns of a frame with a cut place list are computed from (lcd_decide_gps_batch_dev)
+		DevBuf<float> tlv;    // [nt] LC value of each listed entry as a float
+		DevBuf<int> cptr;     // [n+1] neighbour lists by column, as lcd_clients_set_map received them
+		DevBuf<int> crow, clev;
+		DevBuf<double> lc;    // [n_lc] Bayes/PredictionLC
+		int n_lc = 0;
+		float total = 0.f, eps = 0.f;
 	};
 	std::unique_ptr<MapTables> dc_tables; // the current map's; replaced as a whole by lcd_clients_set_map
+	std::unique_ptr<DevBuf<GpsPlace>> gps_places; // the current map's GPS table (lcd_clients_set_map_gps); dropped by lcd_clients_set_map
+	DevBuf<unsigned char> gps_listed;     // [n_frames][n] the places each frame of the last GPS call compared
+	DevBuf<int> gps_count;                // [n_frames]
+	DevBuf<float> gps_fu, gps_fscale, gps_fdelta; // [n][B] the gated frames' columns
 	double dc_lc0 = 0.0;
 	float dc_vpp = 0.f;
 	int dc_clients = 0;
@@ -4285,43 +4296,49 @@ int lcd_clients_set_map(lcd_engine * e, const int * ids, int n, const int64_t * 
 	auto ver = std::make_unique<lcd_engine::MapVersion>();
 	auto tab = std::make_unique<lcd_engine::MapTables>();
 	ver->n = n;
-	DevBuf<double> d_lc;
 	DevBuf<int> d_tentry;
 	const size_t nz = static_cast<size_t>(std::max<int64_t>(nnz, 1)), ntz = static_cast<size_t>(std::max(nt, 1));
+	std::vector<float> tlv(ntz, 0.f);
+	for (int k = 0; k < nt; ++k) tlv[k] = static_cast<float>(prediction_lc[nbr_level[tentry[k]] + 1]);
 	// the scratch buffers below may be in use by queued work of the single-client path
 	LCD_CUDA(e, cudaStreamSynchronize(s));
-	if (ver->ids.reserve(n, 0, false, s) != cudaSuccess || e->by_colptr.reserve(n + 1, 0, false, s) != cudaSuccess ||
-	    e->by_row.reserve(nz, 0, false, s) != cudaSuccess || e->by_level.reserve(nz, 0, false, s) != cudaSuccess ||
+	if (ver->ids.reserve(n, 0, false, s) != cudaSuccess || tab->cptr.reserve(n + 1, 0, false, s) != cudaSuccess ||
+	    tab->crow.reserve(nz, 0, false, s) != cudaSuccess || tab->clev.reserve(nz, 0, false, s) != cudaSuccess ||
 	    e->by_scale.reserve(n, 0, false, s) != cudaSuccess || e->by_delta.reserve(n, 0, false, s) != cudaSuccess ||
-	    d_lc.reserve(n_lc, 0, false, s) != cudaSuccess || d_tentry.reserve(ntz, 0, false, s) != cudaSuccess ||
+	    tab->lc.reserve(n_lc, 0, false, s) != cudaSuccess || d_tentry.reserve(ntz, 0, false, s) != cudaSuccess ||
 	    tab->u.reserve(n, 0, false, s) != cudaSuccess || tab->tptr.reserve(n + 1, 0, false, s) != cudaSuccess ||
-	    tab->tcol.reserve(ntz, 0, false, s) != cudaSuccess || tab->tval.reserve(ntz, 0, false, s) != cudaSuccess)
+	    tab->tcol.reserve(ntz, 0, false, s) != cudaSuccess || tab->tval.reserve(ntz, 0, false, s) != cudaSuccess ||
+	    tab->tlv.reserve(ntz, 0, false, s) != cudaSuccess)
 	{
 		cudaGetLastError();
 		LCD_FAIL(e, LCD_ERR_CAPACITY, "no device memory for a map of %d places and %d listed entries", n, nt);
 	}
 	LCD_CUDA(e, cudaMemcpyAsync(ver->ids.p, ids, n * sizeof(int), cudaMemcpyHostToDevice, s));
-	LCD_CUDA(e, cudaMemcpyAsync(e->by_colptr.p, cp.data(), (n + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, cudaMemcpyAsync(tab->cptr.p, cp.data(), (n + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
 	if (nnz)
 	{
-		LCD_CUDA(e, cudaMemcpyAsync(e->by_row.p, nbr_row, nnz * sizeof(int), cudaMemcpyHostToDevice, s));
-		LCD_CUDA(e, cudaMemcpyAsync(e->by_level.p, nbr_level, nnz * sizeof(int), cudaMemcpyHostToDevice, s));
+		LCD_CUDA(e, cudaMemcpyAsync(tab->crow.p, nbr_row, nnz * sizeof(int), cudaMemcpyHostToDevice, s));
+		LCD_CUDA(e, cudaMemcpyAsync(tab->clev.p, nbr_level, nnz * sizeof(int), cudaMemcpyHostToDevice, s));
 	}
-	LCD_CUDA(e, cudaMemcpyAsync(d_lc.p, prediction_lc, n_lc * sizeof(double), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, cudaMemcpyAsync(tab->lc.p, prediction_lc, n_lc * sizeof(double), cudaMemcpyHostToDevice, s));
 	LCD_CUDA(e, cudaMemcpyAsync(tab->tptr.p, tptr.data(), (n + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
 	if (nt)
 	{
 		LCD_CUDA(e, cudaMemcpyAsync(d_tentry.p, tentry.data(), nt * sizeof(int), cudaMemcpyHostToDevice, s));
 		LCD_CUDA(e, cudaMemcpyAsync(tab->tcol.p, tcol.data(), nt * sizeof(int), cudaMemcpyHostToDevice, s));
+		LCD_CUDA(e, cudaMemcpyAsync(tab->tlv.p, tlv.data(), nt * sizeof(float), cudaMemcpyHostToDevice, s));
 	}
+	tab->n_lc = n_lc;
+	tab->total = total;
+	tab->eps = static_cast<float>(eps);
 	BayesArgs a{};
 	a.n = n;
 	a.vp_used = 1;
 	a.ids = ver->ids.p;
-	a.col_ptr = e->by_colptr.p;
-	a.nbr_row = e->by_row.p;
-	a.nbr_level = e->by_level.p;
-	a.lc = d_lc.p;
+	a.col_ptr = tab->cptr.p;
+	a.nbr_row = tab->crow.p;
+	a.nbr_level = tab->clev.p;
+	a.lc = tab->lc.p;
 	a.n_lc = n_lc;
 	a.total = total;
 	a.eps = static_cast<float>(eps);
@@ -4363,6 +4380,7 @@ int lcd_clients_set_map(lcd_engine * e, const int * ids, int n, const int64_t * 
 	}
 	e->dc_stride = stride;
 	e->dc_tables = std::move(tab);
+	e->gps_places.reset();
 	e->dc_map_ver = e->dc_next_ver++;
 	e->dc_versions[e->dc_map_ver] = std::move(ver);
 	e->dc_n = n;
@@ -4385,9 +4403,10 @@ static int check_decide_params(lcd_engine * e, const lcd_decide_params * dp)
 	return LCD_OK;
 }
 
-// checks of one decision call and the upload of its frame tables (before any kernel of the call is queued)
+// checks of one decision call and the upload of its frame tables (before any kernel of the call is queued); gps[n_frames] (may be null)
+// is uploaded behind them
 static int decide_prepare(lcd_engine * e, int n_frames, int ns, const int * clients, const int * frame_flags, const lcd_decide_params * dp,
-                          cudaStream_t s)
+                          cudaStream_t s, const GpsFrame * gps = nullptr)
 {
 	if (e->dc_clients <= 0) LCD_FAIL(e, LCD_ERR_STATE, "no clients: call lcd_clients_create first");
 	if (e->dc_map_ver < 0) LCD_FAIL(e, LCD_ERR_STATE, "no map: call lcd_clients_set_map first");
@@ -4405,7 +4424,9 @@ static int decide_prepare(lcd_engine * e, int n_frames, int ns, const int * clie
 		if (!(frame_flags[f] & (kDcFlagSkip | kDcFlagHold))) e->dc_active.push_back(f);
 	}
 	const int B = static_cast<int>(e->dc_active.size());
-	const size_t words = 2 * static_cast<size_t>(n_frames) + 4 * static_cast<size_t>(B);
+	static_assert(sizeof(GpsFrame) % sizeof(long long) == 0, "GPS frame table layout");
+	const size_t gps_words = gps ? n_frames * (sizeof(GpsFrame) / sizeof(long long)) : 0;
+	const size_t words = 2 * static_cast<size_t>(n_frames) + 4 * static_cast<size_t>(B) + gps_words;
 	if (!e->dc_h_ev) LCD_CUDA(e, cudaEventCreateWithFlags(&e->dc_h_ev, cudaEventDisableTiming));
 	else LCD_CUDA(e, cudaEventSynchronize(e->dc_h_ev)); // the staging buffer of the last call has been copied
 	LCD_CUDA(e, e->dc_h_tab.reserve(words));
@@ -4426,21 +4447,36 @@ static int decide_prepare(lcd_engine * e, int n_frames, int ns, const int * clie
 		hb[3 * B + b] = static_cast<long long>(reinterpret_cast<uintptr_t>(mv ? mv->ids.p : nullptr));
 		e->dc_active[b] = c;
 	}
+	if (gps) std::memcpy(hb + 4 * B, gps, n_frames * sizeof(GpsFrame));
 	LCD_CUDA(e, e->dc_tab.reserve(words, 0, false, s));
 	LCD_CUDA(e, cudaMemcpyAsync(e->dc_tab.p, h, words * sizeof(long long), cudaMemcpyHostToDevice, s));
 	LCD_CUDA(e, cudaEventRecord(e->dc_h_ev, s));
 	return LCD_OK;
 }
 
-// adjustLikelihood, the posterior of every frame that computes one, the hypothesis selection and checks
-static int decide_launch(lcd_engine * e, const float * d_like, int n_frames, int ns, const lcd_decide_params * dp, float * d_post_out, cudaStream_t s)
+// adjustLikelihood, the posterior of every frame that computes one, the hypothesis selection and checks.  r2 >= 0 (a call with a GPS
+// table uploaded by decide_prepare): the GPS filter of each frame's place list first, with RGBD/LocalRadius squared
+static int decide_launch(lcd_engine * e, const float * d_like, int n_frames, int ns, const lcd_decide_params * dp, float * d_post_out, cudaStream_t s,
+                         double r2 = -1.0)
 {
 	const int n = e->dc_n, B = static_cast<int>(e->dc_active.size());
 	const lcd_engine::MapTables & t = *e->dc_tables;
-	DecideMap m{n, e->dc_versions.at(e->dc_map_ver)->ids.p, t.u.p, t.tptr.p, t.tcol.p, t.tval.p, e->dc_lc0, e->dc_vpp};
+	DecideMap m{n, e->dc_versions.at(e->dc_map_ver)->ids.p, t.u.p, t.tptr.p, t.tcol.p, t.tval.p, e->dc_lc0, e->dc_vpp, t.tlv.p, t.eps};
 	const long long * tab = e->dc_tab.p;
+	const GpsFrame * gps = r2 >= 0.0 ? reinterpret_cast<const GpsFrame *>(tab + 2 * n_frames + 4 * B) : nullptr;
 	LCD_CUDA(e, e->dc_adj.reserve(static_cast<size_t>(n_frames) * n, 0, false, s));
-	adjust_likelihood_kernel<<<n_frames, kAdjustThreads, 0, s>>>(d_like, ns, dp->virtual_place_ratio, e->dc_adj.p);
+	if (gps)
+	{
+		LCD_CUDA(e, e->gps_listed.reserve(static_cast<size_t>(n_frames) * n, 0, false, s));
+		LCD_CUDA(e, e->gps_count.reserve(n_frames, 0, false, s));
+		LCD_CUDA(e, cudaMemsetAsync(e->gps_count.p, 0, n_frames * sizeof(int), s));
+		// without a table no frame is gated (lcd_decide_gps_batch_dev refuses fixes then), and the kernel reads no place
+		decide_gps_gate_kernel<<<dim3((n + 255) / 256, n_frames), 256, 0, s>>>(n, e->gps_places ? e->gps_places->p : nullptr, gps, r2, e->gps_listed.p,
+		                                                                         e->gps_count.p);
+		LCD_CHECK_LAUNCH(e);
+		adjust_likelihood_listed_kernel<<<n_frames, kAdjustThreads, 0, s>>>(d_like, ns, dp->virtual_place_ratio, e->dc_adj.p, e->gps_listed.p);
+	}
+	else adjust_likelihood_kernel<<<n_frames, kAdjustThreads, 0, s>>>(d_like, ns, dp->virtual_place_ratio, e->dc_adj.p);
 	LCD_CHECK_LAUNCH(e);
 	if (B > 0)
 	{
@@ -4469,6 +4505,32 @@ static int decide_launch(lcd_engine * e, const float * d_like, int n_frames, int
 		d.u = e->dc_sums.p;
 		d.s1 = e->dc_sums.p + B;
 		d.psum = e->dc_sums.p + 2 * B;
+		if (gps)
+		{
+			LCD_CUDA(e, e->gps_fu.reserve(nb, 0, false, s));
+			LCD_CUDA(e, e->gps_fscale.reserve(nb, 0, false, s));
+			LCD_CUDA(e, e->gps_fdelta.reserve(nb, 0, false, s));
+			d.gps = gps;
+			d.count = e->gps_count.p;
+			d.listed = e->gps_listed.p;
+			d.fu = e->gps_fu.p;
+			d.fscale = e->gps_fscale.p;
+			d.fdelta = e->gps_fdelta.p;
+			BayesArgs a{};
+			a.n = n;
+			a.vp_used = 1;
+			a.ids = m.ids;
+			a.col_ptr = t.cptr.p;
+			a.nbr_row = t.crow.p;
+			a.nbr_level = t.clev.p;
+			a.lc = t.lc.p;
+			a.n_lc = t.n_lc;
+			a.total = t.total;
+			a.eps = t.eps;
+			a.vpp = e->dc_vpp;
+			decide_gps_columns_kernel<<<static_cast<unsigned>((nb + 255) / 256), 256, 0, s>>>(a, d);
+			LCD_CHECK_LAUNCH(e);
+		}
 		const int threads = std::min(kDcThreads, (B + 31) / 32 * 32);
 		decide_last_kernel<<<static_cast<unsigned>((nb + 255) / 256), 256, 0, s>>>(m, d);
 		LCD_CHECK_LAUNCH(e);
@@ -4504,6 +4566,8 @@ static int decide_launch(lcd_engine * e, const float * d_like, int n_frames, int
 	a.dec = e->dc_dec.p;
 	a.hyp_id = e->d_hyp_id.p;
 	a.hyp_slot = e->d_hyp_slot.p;
+	a.gps = gps;
+	a.count = gps ? e->gps_count.p : nullptr;
 	decide_select_kernel<<<n_frames, 256, 0, s>>>(m, a);
 	LCD_CHECK_LAUNCH(e);
 	// the clients that computed now hold posteriors keyed to the current map
@@ -4526,6 +4590,115 @@ int lcd_decide_batch_dev(lcd_engine * e, const float * d_likelihood, int n_frame
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
 	LCD_TRY(decide_prepare(e, n_frames, ns, clients, frame_flags, dp, s));
 	return decide_launch(e, d_likelihood, n_frames, ns, dp, d_posterior_out, s);
+}
+
+// ---- the GPS filter of the place list (Rtabmap/LoopGPS) ----------------------------------------------------------------
+static_assert(sizeof(GpsFrame) == 72 && sizeof(GpsPlace) == 40, "GPS table layout");
+
+// GeodeticCoords::toGeocentric_WGS84 (GeodeticCoords.cpp:75-102): the same double statements, glibc's trigonometry
+static void geocentric_wgs84(const lcd_gps & g, double & x, double & y, double & z)
+{
+	static const double a = 6378137;
+	static const double b = 6356752.3142;
+	static const double ae = std::acos(b / a);
+	static const double cos2_ae_earth = std::cos(ae) * std::cos(ae);
+	static const double sin2_ae_earth = std::sin(ae) * std::sin(ae);
+	const double lon = g.longitude * M_PI / 180.0;
+	const double lat = g.latitude * M_PI / 180.0;
+	const double sin_lat = std::sin(lat);
+	const double N = a / std::sqrt(1.0 - sin2_ae_earth * (sin_lat * sin_lat));
+	x = (N + g.altitude) * std::cos(lat) * std::cos(lon);
+	y = (N + g.altitude) * std::cos(lat) * std::sin(lon);
+	z = (cos2_ae_earth * N + g.altitude) * sin_lat;
+}
+
+static bool gps_finite(const lcd_gps & g)
+{
+	return std::isfinite(g.stamp) && std::isfinite(g.longitude) && std::isfinite(g.latitude) && std::isfinite(g.altitude) && std::isfinite(g.error);
+}
+
+int lcd_clients_set_map_gps(lcd_engine * e, const int * ids, int n, const lcd_gps * gps, const float * offset_enu)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (e->dc_map_ver < 0) LCD_FAIL(e, LCD_ERR_STATE, "no map: call lcd_clients_set_map first");
+	if (!ids || !gps || n != e->dc_n - 1) LCD_FAIL(e, LCD_ERR_INVALID, "n = %d, but the map holds %d real places", n, e->dc_n - 1);
+	for (int i = 0; i < n; ++i)
+	{
+		if (ids[i] != e->dc_h_ids[i + 1]) LCD_FAIL(e, LCD_ERR_INVALID, "ids[%d] = %d differs from the map's %d", i, ids[i], e->dc_h_ids[i + 1]);
+		if (!gps_finite(gps[i])) LCD_FAIL(e, LCD_ERR_INVALID, "the GPS of place %d is not finite", ids[i]);
+		if (offset_enu && !(std::isfinite(offset_enu[3 * i]) && std::isfinite(offset_enu[3 * i + 1]) && std::isfinite(offset_enu[3 * i + 2])))
+			LCD_FAIL(e, LCD_ERR_INVALID, "the ENU offset of place %d is not finite", ids[i]);
+	}
+	std::vector<GpsPlace> h(std::max(n, 1));
+	for (int i = 0; i < n; ++i)
+	{
+		GpsPlace & p = h[i];
+		p = GpsPlace{};
+		p.fix = gps[i].stamp > 0.0;
+		if (p.fix) geocentric_wgs84(gps[i], p.x, p.y, p.z);
+		if (offset_enu)
+		{
+			p.ox = offset_enu[3 * i];
+			p.oy = offset_enu[3 * i + 1];
+			p.oz = offset_enu[3 * i + 2];
+		}
+	}
+	cudaStream_t s = e->stream;
+	auto buf = std::make_unique<DevBuf<GpsPlace>>();
+	if (buf->reserve(h.size(), 0, false, s) != cudaSuccess)
+	{
+		cudaGetLastError();
+		LCD_FAIL(e, LCD_ERR_CAPACITY, "no device memory for the GPS of %d places", n);
+	}
+	LCD_CUDA(e, cudaMemcpyAsync(buf->p, h.data(), h.size() * sizeof(GpsPlace), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, cudaStreamSynchronize(s));
+	// kernels of the last GPS decision may still read the table this call replaces
+	LCD_CUDA(e, cudaDeviceSynchronize());
+	e->gps_places = std::move(buf);
+	return LCD_OK;
+}
+
+int lcd_decide_gps_batch_dev(lcd_engine * e, const float * d_likelihood, int n_frames, int ns, const int * clients, const int * frame_flags,
+                             const lcd_gps * frame_gps, float local_radius, const lcd_decide_params * dp, float * d_posterior_out,
+                             unsigned char * d_compared_out, void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (!d_likelihood) LCD_FAIL(e, LCD_ERR_INVALID, "likelihood is empty");
+	if (n_frames <= 0 || !clients || !frame_flags) LCD_FAIL(e, LCD_ERR_INVALID, "no frames");
+	if (!(local_radius >= 0.f) || !std::isfinite(local_radius)) LCD_FAIL(e, LCD_ERR_INVALID, "RGBD/LocalRadius must be >= 0");
+	// the frames that compute a posterior and carry a fix (the block of Rtabmap.cpp:1994 does not run for the others)
+	std::vector<GpsFrame> g(n_frames);
+	bool any_fix = false;
+	for (int f = 0; f < n_frames; ++f)
+	{
+		g[f] = GpsFrame{};
+		const bool compute = !(frame_flags[f] & (kDcFlagSkip | kDcFlagHold));
+		g[f].mode = compute ? kGpsAll : kGpsNone;
+		if (!frame_gps) continue;
+		if (!gps_finite(frame_gps[f])) LCD_FAIL(e, LCD_ERR_INVALID, "the GPS of frame %d is not finite", f);
+		if (!compute || !(frame_gps[f].stamp > 0.0)) continue;
+		any_fix = true;
+		const lcd_gps & o = frame_gps[f];
+		geocentric_wgs84(o, g[f].x, g[f].y, g[f].z);
+		// Geocentric_WGS84ToENU_WGS84's rotation (GeodeticCoords.cpp:134-135)
+		g[f].clat = std::cos(o.latitude * M_PI / 180.0);
+		g[f].slat = std::sin(o.latitude * M_PI / 180.0);
+		g[f].clon = std::cos(o.longitude * M_PI / 180.0);
+		g[f].slon = std::sin(o.longitude * M_PI / 180.0);
+		g[f].error = o.error;
+		g[f].mode = kGpsGated;
+	}
+	if (any_fix && (e->dc_map_ver < 0 || !e->gps_places))
+		LCD_FAIL(e, LCD_ERR_STATE, "frames carry a GPS fix but the map has no GPS table: call lcd_clients_set_map_gps");
+	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	LCD_TRY(decide_prepare(e, n_frames, ns, clients, frame_flags, dp, s, g.data()));
+	const float r2 = local_radius * local_radius; // _localRadius*_localRadius: a float, compared in double
+	LCD_TRY(decide_launch(e, d_likelihood, n_frames, ns, dp, d_posterior_out, s, static_cast<double>(r2)));
+	if (d_compared_out)
+		LCD_CUDA(e, cudaMemcpy2DAsync(d_compared_out, ns, e->gps_listed.p + 1, e->dc_n, ns, n_frames, cudaMemcpyDeviceToDevice, s));
+	return LCD_OK;
 }
 
 int lcd_decide_fetch(lcd_engine * e, int n_frames, lcd_decision * out)

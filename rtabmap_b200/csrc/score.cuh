@@ -243,9 +243,10 @@ __global__ void gather_rows_kernel(const uint32_t * __restrict__ src, const int 
 constexpr int kAdjustThreads = 256;
 constexpr int kAdjustChunk = 2048;
 
-__device__ inline int adjust_compact_chunk(const float * __restrict__ row, int c0, int n, float * s_val, int * s_cnt)
+__device__ inline int adjust_compact_chunk(const float * __restrict__ row, int c0, int n, float * s_val, int * s_cnt,
+                                           const unsigned char * __restrict__ listed = nullptr)
 {
-	// stable compaction of row[c0 .. c0+n) > 0 into s_val; returns the count (valid in all threads)
+	// stable compaction of row[c0 .. c0+n) > 0 (and listed, when a list is given) into s_val; returns the count (valid in all threads)
 	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 	__shared__ int s_warp[kAdjustThreads / 32];
 	int base = 0;
@@ -253,7 +254,7 @@ __device__ inline int adjust_compact_chunk(const float * __restrict__ row, int c
 	{
 		const int i = i0 + tid;
 		const float v = i < n ? row[c0 + i] : 0.f;
-		const bool keep = i < n && v > 0.f;
+		const bool keep = i < n && v > 0.f && (!listed || listed[c0 + i]);
 		const unsigned m = __ballot_sync(0xFFFFFFFFu, keep);
 		if (lane == 0) s_warp[warp] = __popc(m);
 		__syncthreads();
@@ -270,16 +271,16 @@ __device__ inline int adjust_compact_chunk(const float * __restrict__ row, int c
 	return *s_cnt;
 }
 
-__global__ void __launch_bounds__(kAdjustThreads)
-adjust_likelihood_kernel(const float * __restrict__ like, int ns, int virtual_place_ratio, float * __restrict__ adj)
+// listed[ns] (nullptr: every place): the places the frame compares; the others are left out of the mean, the deviation and the
+// maximum, as if absent from the likelihood map, and their adjusted value is 0 (they add exact zeros to the posterior after it)
+__device__ __forceinline__ void adjust_likelihood_row(const float * __restrict__ row, int ns, int virtual_place_ratio, float * __restrict__ out,
+                                                      const unsigned char * __restrict__ listed)
 {
 	__shared__ float s_val[kAdjustChunk];
 	__shared__ int s_cnt;
 	__shared__ float s_acc, s_mean, s_std, s_max[kAdjustThreads / 32];
 	__shared__ long long s_n;
 	const int tid = threadIdx.x;
-	const float * row = like + static_cast<size_t>(blockIdx.x) * ns;
-	float * out = adj + static_cast<size_t>(blockIdx.x) * (ns + 1);
 	if (tid == 0)
 	{
 		s_acc = 0.f;
@@ -289,7 +290,7 @@ adjust_likelihood_kernel(const float * __restrict__ like, int ns, int virtual_pl
 	// pass 1: mean of the values > 0
 	for (int c0 = 0; c0 < ns; c0 += kAdjustChunk)
 	{
-		const int cnt = adjust_compact_chunk(row, c0, min(kAdjustChunk, ns - c0), s_val, &s_cnt);
+		const int cnt = adjust_compact_chunk(row, c0, min(kAdjustChunk, ns - c0), s_val, &s_cnt, listed);
 		if (tid == 0)
 		{
 			float m = s_acc;
@@ -312,7 +313,7 @@ adjust_likelihood_kernel(const float * __restrict__ like, int ns, int virtual_pl
 	{
 		for (int c0 = 0; c0 < ns; c0 += kAdjustChunk)
 		{
-			const int cnt = adjust_compact_chunk(row, c0, min(kAdjustChunk, ns - c0), s_val, &s_cnt);
+			const int cnt = adjust_compact_chunk(row, c0, min(kAdjustChunk, ns - c0), s_val, &s_cnt, listed);
 			if (tid == 0)
 			{
 				float sum = s_acc;
@@ -338,6 +339,11 @@ adjust_likelihood_kernel(const float * __restrict__ like, int ns, int virtual_pl
 	float mx = 0.f;
 	for (int i = tid; i < ns; i += kAdjustThreads)
 	{
+		if (listed && !listed[i])
+		{
+			out[1 + i] = 0.f;
+			continue;
+		}
 		const float value = row[i];
 		float r = 1.0f;
 		if (value > thr)
@@ -360,6 +366,22 @@ adjust_likelihood_kernel(const float * __restrict__ like, int ns, int virtual_pl
 		else if (virtual_place_ratio != 0 && m > mean) vp = __fadd_rn(__fdiv_rn(sd, __fsub_rn(m, mean)), 1.0f);
 		out[0] = vp;
 	}
+}
+
+__global__ void __launch_bounds__(kAdjustThreads)
+adjust_likelihood_kernel(const float * __restrict__ like, int ns, int virtual_place_ratio, float * __restrict__ adj)
+{
+	adjust_likelihood_row(like + static_cast<size_t>(blockIdx.x) * ns, ns, virtual_place_ratio, adj + static_cast<size_t>(blockIdx.x) * (ns + 1),
+	                      nullptr);
+}
+
+// the same over the places of listed[frame][ns + 1] (element 0 the virtual place); a row that lists every place gives the bits above
+__global__ void __launch_bounds__(kAdjustThreads)
+adjust_likelihood_listed_kernel(const float * __restrict__ like, int ns, int virtual_place_ratio, float * __restrict__ adj,
+                                const unsigned char * __restrict__ listed)
+{
+	const size_t f = blockIdx.x;
+	adjust_likelihood_row(like + f * ns, ns, virtual_place_ratio, adj + f * (ns + 1), listed + f * (ns + 1) + 1);
 }
 
 } // namespace lcd

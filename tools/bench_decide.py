@@ -1,6 +1,6 @@
 """Time the batched loop-closure decision of many localisation clients.
 
-    python tools/bench_decide.py [--clients 128 --steps 20 --warmup 5 --places 1000,10000,50000] [--no-fused]
+    python tools/bench_decide.py [--clients 128 --steps 20 --warmup 5 --places 1000,10000,50000] [--no-fused] [--gps 10000]
 
 1. lcd_decide_batch_dev (adjustLikelihood + the posterior of every client + the hypothesis selection) at `clients` clients over a map of
    `places` places (a chain graph with the default Bayes/PredictionLC), against `clients` sequential lcd_bayes_compute_posterior calls
@@ -9,6 +9,9 @@
    descriptors revisiting them): lcd_process_decide_batch_dev against lcd_process_batch_dev (quantise + score + verification of the
    raw-likelihood arg-max).  Rtabmap/LoopThr is 0 here, so that every frame's hypothesis is accepted and verified, as
    lcd_process_batch_dev verifies every frame; with the default 0.11 the decision may verify fewer frames and cost less.
+3. With --gps N: at `clients` clients over N places with a GPS fix each (4 m apart on a straight line), lcd_decide_batch_dev against
+   lcd_decide_gps_batch_dev with frames that carry no fix and with every frame carrying a fix, at radii (Rtabmap/LoopGPS with
+   RGBD/LocalRadius) that keep about 1 %, 30 % and 100 % of the places; the calls alternate, twice each.
 Device time with CUDA events after warm-up, over `steps` back-to-back calls; the sequential single-client calls are timed with the host
 clock (they synchronise).  One JSON line on stdout, with the card's name and power limit read in this run."""
 import argparse
@@ -98,6 +101,55 @@ def bench_posterior(B, n, steps, warmup, st):
     return {"places": n, "decide_batch_ms": ms, "sequential_bayes_ms": seq_ms, "state_mb": state_mb, "speedup": seq_ms / ms}
 
 
+def bench_gps(B, n, steps, warmup):
+    eng = Engine()
+    lc = [float(np.float32(v)) for v in DEFAULT_PREDICTION_LC]
+    ids = np.concatenate([[-1], np.arange(1, n + 1)]).astype(np.int32)
+    cp, rows, lv = chain_tables(n, len(lc) - 2)
+    eng.clients_create(B)
+    eng.clients_set_map(ids, cp, rows, lv, lc, 0.9)
+    lat0, lon0, spacing = 46.78, -71.27, 4.0
+    deg_e = 1.0 / (111320.0 * np.cos(np.radians(lat0)))
+    gps = np.zeros((n, 5))
+    gps[:, 0] = 1.0
+    gps[:, 1] = lon0 + spacing * np.arange(n) * deg_e
+    gps[:, 2] = lat0
+    eng.clients_set_map_gps(ids[1:], gps)
+    rng = np.random.default_rng(n)
+    raw = (0.05 * rng.random((B, n))).astype(np.float32)
+    raw[np.arange(B), rng.integers(0, n, B)] = 2.0
+    fix = np.zeros((B, 5))
+    fix[:, 0] = 2.0
+    fix[:, 1] = lon0 + spacing * (n / 2 + rng.uniform(-0.1, 0.1, B) * n) * deg_e   # frames near the middle of the line
+    fix[:, 2] = lat0
+    fix[:, 4] = 2.0
+    d_like = torch.from_numpy(raw.reshape(-1)).cuda()
+    d_post = torch.zeros(B * (n + 1), dtype=torch.float32, device="cuda")
+    d_cmp = torch.zeros(B * n, dtype=torch.uint8, device="cuda")
+    clients = np.arange(B, dtype=np.int32)
+    flags = np.zeros(B, np.int32)
+    dp = Engine.decide_params()
+    st = eng.stream
+    length = spacing * n
+    calls = {"decide_batch_ms": lambda: eng.decide_batch_dev(d_like.data_ptr(), B, n, clients, flags, dp, d_post.data_ptr(), stream=st),
+             "gps_no_fix_ms": lambda: eng.decide_gps_batch_dev(d_like.data_ptr(), B, n, clients, flags, None, 10.0, dp, d_post.data_ptr(),
+                                                               d_cmp.data_ptr(), stream=st)}
+    for share in (0.01, 0.3, 1.0):
+        r = share * length / 2 if share < 1 else 2 * length
+        calls[f"gps_{int(share * 100)}pct_ms"] = (lambda r=r: eng.decide_gps_batch_dev(d_like.data_ptr(), B, n, clients, flags, fix, r, dp,
+                                                                                          d_post.data_ptr(), d_cmp.data_ptr(), stream=st))
+    res = {"places": n}
+    ext = torch.cuda.ExternalStream(st)
+    with torch.cuda.stream(ext):
+        for _ in range(2):
+            for k, fn in calls.items():
+                res.setdefault(k, []).append(time_ms(fn, steps, warmup))
+                if k.startswith("gps_") and k != "gps_no_fix_ms":
+                    torch.cuda.synchronize()
+                    res.setdefault(k.replace("_ms", "_kept"), float(d_cmp.float().mean()))
+    return res
+
+
 def bench_fused(B, steps, warmup):
     vocab = synth.make_binary_vocabulary(W, 32, 1)
     ids = np.arange(1, W + 1, dtype=np.int32)
@@ -155,11 +207,14 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--places", default="1000,10000,50000")
     ap.add_argument("--no-fused", action="store_true")
+    ap.add_argument("--gps", type=int, default=0, help="places of the GPS-filter comparison (0: not run)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_decide needs a CUDA device")
     res = {"clients": args.clients, "steps": args.steps, "warmup": args.warmup}
     res["posterior"] = [bench_posterior(args.clients, int(n), args.steps, args.warmup, lambda e: e.stream) for n in args.places.split(",")]
+    if args.gps:
+        res["gps"] = bench_gps(args.clients, args.gps, args.steps, args.warmup)
     if not args.no_fused:
         res["c2"] = bench_fused(args.clients, args.steps, args.warmup)
     res.update(card())
