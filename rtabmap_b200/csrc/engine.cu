@@ -66,6 +66,11 @@ struct DevBuf
 		p = nullptr;
 		cap = 0;
 	}
+	void swap(DevBuf & o)
+	{
+		std::swap(p, o.p);
+		std::swap(cap, o.cap);
+	}
 	// grow to at least n elements; keep the first `keep` elements; zero the rest if asked.
 	// A re-growth replaces a buffer that kernels on ANY stream of the engine (caller streams of the _dev entry points, the ORB side
 	// streams) may still be reading or writing: the device is drained first, so the copy sees final data and the free is safe.
@@ -91,6 +96,80 @@ struct DevBuf
 		return cudaSuccess;
 	}
 };
+
+// Signature id -> row ("slot") of a per-signature store in HBM, on the host and as the device copy the kernels read through
+// (d.p, n_ids).  Freed slots are reused first, the last freed first: the WM -> LTM transfer adds and removes one signature per
+// frame, and the store must not grow.
+struct SlotMap
+{
+	std::vector<int> h;     // by id, -1: none
+	std::vector<int> freed;
+	int slots = 0;          // handed out, freed ones included
+	DevBuf<int> d;
+	int n_ids = 0;          // ids the device copy holds
+
+	int count() const { return slots - static_cast<int>(freed.size()); }
+	// the slot of each id: the one it has, else a freed one, else a new one.  false: an id is not > 0, and nothing changed.
+	bool assign(const int * ids, int n, std::vector<int> & slot)
+	{
+		int max_id = 0;
+		for (int i = 0; i < n; ++i)
+		{
+			if (ids[i] <= 0) return false;
+			max_id = std::max(max_id, ids[i]);
+		}
+		if (static_cast<size_t>(max_id) >= h.size()) h.resize(std::max<size_t>(max_id + 1, h.size() + h.size() / 2 + 1024), -1);
+		slot.resize(n);
+		for (int i = 0; i < n; ++i)
+		{
+			int & s = h[ids[i]];
+			if (s < 0 && !freed.empty())
+			{
+				s = freed.back();
+				freed.pop_back();
+			}
+			else if (s < 0)
+				s = slots++;
+			slot[i] = s;
+		}
+		return true;
+	}
+	// the slot id held, now free; -1: it held none
+	int release(int id)
+	{
+		if (id <= 0 || id >= static_cast<int>(h.size()) || h[id] < 0) return -1;
+		const int s = h[id];
+		h[id] = -1;
+		freed.push_back(s);
+		return s;
+	}
+	cudaError_t upload(cudaStream_t s)
+	{
+		cudaError_t err = d.reserve(h.size(), 0, false, s);
+		if (err == cudaSuccess) err = cudaMemcpyAsync(d.p, h.data(), h.size() * sizeof(int), cudaMemcpyHostToDevice, s);
+		if (err == cudaSuccess) n_ids = static_cast<int>(h.size());
+		return err;
+	}
+	// the entry of one id
+	cudaError_t upload(int id, cudaStream_t s)
+	{
+		return id < n_ids ? cudaMemcpyAsync(d.p + id, &h[id], sizeof(int), cudaMemcpyHostToDevice, s) : cudaSuccess;
+	}
+};
+
+// Rows i of a batch to rows slot[i] of a store: put(slot, i, k) writes k rows from row i on; one call when the slots are
+// consecutive, else one per row.
+template <typename Put>
+cudaError_t write_rows(const std::vector<int> & slot, Put put)
+{
+	const size_t n = slot.size();
+	size_t i = 1;
+	while (i < n && slot[i] == slot[0] + static_cast<int>(i)) ++i;
+	if (i == n) return put(static_cast<size_t>(slot[0]), 0, n);
+	for (i = 0; i < n; ++i)
+		if (cudaError_t err = put(static_cast<size_t>(slot[i]), i, 1)) return err;
+	return cudaSuccess;
+}
 
 template <typename T>
 struct PinBuf
@@ -386,11 +465,10 @@ struct lcd_engine
 	DevBuf<int> ep_slot, ep_skip;
 	int ep_last_frames = 0; // frames of the last lcd_decide_epipolar_dev (0: none)
 	// word store of the stored places for the epipolar check: Signature::getWords() / getWordsKpts() by row
-	DevBuf<int> ws_ids, ws_n, ws_slot_of_sig;
+	DevBuf<int> ws_ids, ws_n;
 	DevBuf<float> ws_uv;
-	int ws_cap = 0, ws_rows = 0;
-	std::vector<int> h_ws_slot_of_sig, ws_free;
-	int ws_count = 0;
+	int ws_cap = 0;
+	SlotMap ws_map;
 	DevBuf<double> v_cov6;
 	DevBuf<ulonglong2> bf_keys_a, bf_keys_b;
 	DevBuf<unsigned long long> bf_best;
@@ -400,7 +478,7 @@ struct lcd_engine
 	// signature store (Signature::getWordsDescriptors / getWords3 of the nodes in working memory)
 	DevBuf<uint32_t> st_desc;
 	DevBuf<float> st_xyz;
-	DevBuf<int> st_n, st_slot_of_sig;
+	DevBuf<int> st_n;
 	// each row's temporary FROM dictionary of the matching kernel (verify.cuh, from_dict_build_kernel), built on first use for the
 	// (nf, Vis/CorNNDR) of the call: word of each descriptor, creator of each word [slot][st_cap], and what it was built for [slot]
 	DevBuf<uint16_t> st_kof, st_creator;
@@ -409,13 +487,12 @@ struct lcd_engine
 	DevBuf<uint16_t> v_kof, v_creator;
 	DevBuf<FromDictTag> v_ftag;
 	DevBuf<ulonglong2> v_keys64;
-	std::vector<int> h_slot_of_sig, free_slots;
-	int st_cap = 0, st_slots = 0;
-	// global descriptors (SensorData::globalDescriptors(), type 1, one per signature): rows [slot][gd_dim], the signature store's slot scheme
+	int st_cap = 0;
+	SlotMap st_map;
+	// global descriptors (SensorData::globalDescriptors(), type 1, one per signature): rows [slot][gd_dim]
 	DevBuf<float> gd_rows, gd_query, gd_dot;
-	DevBuf<int> gd_slot_of_sig;
-	std::vector<int> h_gd_slot_of_sig, gd_free;
-	int gd_dim = 0, gd_slots = 0;
+	int gd_dim = 0;
+	SlotMap gd_map;
 	DevBuf<int> d_hyp_id, d_hyp_slot;
 	// ORB workspace
 	DevBuf<uint8_t> o_img, o_gray, o_mask, o_blur, o_desc;
@@ -1148,19 +1225,18 @@ int check_queries(lcd_engine * e, const void * q, int nq)
 int launch_similarity(lcd_engine * e, int n_frames, int nq, const float * d_gdesc, const int * d_sig_ids, int ns, float * d_like, cudaStream_t s)
 {
 	LCD_TRY(launch_score(e, n_frames, nq, s, true));
-	const bool gd = d_gdesc && e->gd_slots > static_cast<int>(e->gd_free.size());
+	const bool gd = d_gdesc && e->gd_map.count() > 0;
 	if (gd)
 	{
 		LCD_CUDA(e, e->gd_dot.reserve(static_cast<size_t>(n_frames) * ns, 0, false, s));
-		GdescArgs g{d_gdesc, n_frames, e->gd_rows.p, e->gd_dim, e->gd_slot_of_sig.p, static_cast<int>(e->h_gd_slot_of_sig.size()), d_sig_ids, ns,
-		            e->gd_dot.p};
+		GdescArgs g{d_gdesc, n_frames, e->gd_rows.p, e->gd_dim, e->gd_map.d.p, e->gd_map.n_ids, d_sig_ids, ns, e->gd_dot.p};
 		prof_mark(e, LCD_PROF_SCORE, s);
 		gdesc_dot_kernel<<<dim3((ns + kGdBN - 1) / kGdBN, (n_frames + kGdBM - 1) / kGdBM), kGdThreads, 0, s>>>(g);
 		prof_mark(e, LCD_PROF_SCORE, s);
 		LCD_CHECK_LAUNCH(e);
 	}
 	SimilarityArgs f{e->acc.p, e->acc_stride, e->nvalid.p, static_cast<int>(e->h_nvalid.size()), e->q_valid.p, gd ? e->gd_dot.p : nullptr,
-	                 e->gd_slot_of_sig.p, static_cast<int>(e->h_gd_slot_of_sig.size()), d_sig_ids, ns, d_like};
+	                 e->gd_map.d.p, e->gd_map.n_ids, d_sig_ids, ns, d_like};
 	similarity_finalize_kernel<<<dim3((ns + 255) / 256, n_frames), 256, 0, s>>>(f);
 	LCD_CHECK_LAUNCH(e);
 	return LCD_OK;
@@ -1563,10 +1639,8 @@ int lcd_dict_update(lcd_engine * e)
 			LCD_CUDA(e, cudaMemcpyAsync(e->row_ids_alt.p, kid.data(), nk * sizeof(int), cudaMemcpyHostToDevice, e->stream));
 		}
 		LCD_CUDA(e, cudaStreamSynchronize(e->stream));
-		std::swap(e->vocab.p, e->vocab_alt.p);
-		std::swap(e->vocab.cap, e->vocab_alt.cap);
-		std::swap(e->row_ids.p, e->row_ids_alt.p);
-		std::swap(e->row_ids.cap, e->row_ids_alt.cap);
+		e->vocab.swap(e->vocab_alt);
+		e->row_ids.swap(e->row_ids_alt);
 		e->h_row_ids.swap(kid);
 		e->id2row.clear();
 		for (int i = 0; i < nk; ++i) e->id2row[e->h_row_ids[i]] = i;
@@ -2190,7 +2264,7 @@ int lcd_localize_batch(lcd_engine * e, const void * queries, int n_frames, int n
 }
 
 // ---- similarity likelihood: Memory::computeLikelihood with Kp/TfIdfLikelihoodUsed=false ----------------------------------------
-int lcd_gdesc_count(const lcd_engine * e) { return e ? e->gd_slots - static_cast<int>(e->gd_free.size()) : 0; }
+int lcd_gdesc_count(const lcd_engine * e) { return e ? e->gd_map.count() : 0; }
 int lcd_gdesc_dim(const lcd_engine * e) { return e ? e->gd_dim : 0; }
 
 int lcd_gdesc_add(lcd_engine * e, const int * sig_ids, int n, int dim, const float * data)
@@ -2201,50 +2275,19 @@ int lcd_gdesc_add(lcd_engine * e, const int * sig_ids, int n, int dim, const flo
 	if (!sig_ids || !data) LCD_FAIL(e, LCD_ERR_INVALID, "null global descriptors");
 	if (dim <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "global descriptors need at least one dimension, got %d", dim);
 	if (e->gd_dim != 0 && dim != e->gd_dim) LCD_FAIL(e, LCD_ERR_INVALID, "global descriptors of this engine have %d dimensions, got %d", e->gd_dim, dim);
-	int max_id = 0;
-	for (int i = 0; i < n; ++i)
-	{
-		if (sig_ids[i] <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "signature id must be positive");
-		max_id = std::max(max_id, sig_ids[i]);
-	}
 	LCD_TRY(set_device(e));
 	cudaStream_t s = e->stream;
+	// a signature that has a descriptor keeps its slot (replace)
+	const size_t prev_slots = static_cast<size_t>(e->gd_map.slots);
+	std::vector<int> slots;
+	if (!e->gd_map.assign(sig_ids, n, slots)) LCD_FAIL(e, LCD_ERR_INVALID, "signature id must be positive");
 	e->gd_dim = dim;
-	if (static_cast<size_t>(max_id) + 1 > e->h_gd_slot_of_sig.size())
-	{
-		const size_t old = e->h_gd_slot_of_sig.size();
-		e->h_gd_slot_of_sig.resize(std::max<size_t>(max_id + 1, old + old / 2 + 1024), -1);
-	}
-	// a signature that has a descriptor keeps its slot (replace); freed slots are reused before the store grows
-	const size_t prev_slots = static_cast<size_t>(e->gd_slots);
-	std::vector<int> slots(n);
-	bool contiguous = true;
-	for (int i = 0; i < n; ++i)
-	{
-		int slot = e->h_gd_slot_of_sig[sig_ids[i]];
-		if (slot < 0)
-		{
-			if (!e->gd_free.empty())
-			{
-				slot = e->gd_free.back();
-				e->gd_free.pop_back();
-			}
-			else slot = e->gd_slots++;
-		}
-		slots[i] = slot;
-		if (i > 0 && slots[i] != slots[i - 1] + 1) contiguous = false;
-		e->h_gd_slot_of_sig[sig_ids[i]] = slot;
-	}
 	const size_t row = static_cast<size_t>(dim);
-	LCD_CUDA(e, e->gd_rows.reserve(static_cast<size_t>(e->gd_slots) * row, prev_slots * row, false, s));
-	if (contiguous)
-		LCD_CUDA(e, cudaMemcpyAsync(e->gd_rows.p + static_cast<size_t>(slots[0]) * row, data, row * n * sizeof(float), cudaMemcpyHostToDevice, s));
-	else
-		for (int i = 0; i < n; ++i)
-			LCD_CUDA(e, cudaMemcpyAsync(e->gd_rows.p + static_cast<size_t>(slots[i]) * row, data + static_cast<size_t>(i) * row, row * sizeof(float),
-			                            cudaMemcpyHostToDevice, s));
-	LCD_CUDA(e, e->gd_slot_of_sig.reserve(e->h_gd_slot_of_sig.size(), 0, false, s));
-	LCD_CUDA(e, cudaMemcpyAsync(e->gd_slot_of_sig.p, e->h_gd_slot_of_sig.data(), e->h_gd_slot_of_sig.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, e->gd_rows.reserve(static_cast<size_t>(e->gd_map.slots) * row, prev_slots * row, false, s));
+	LCD_CUDA(e, write_rows(slots, [&](size_t slot, size_t i, size_t k) {
+		return cudaMemcpyAsync(e->gd_rows.p + slot * row, data + i * row, k * row * sizeof(float), cudaMemcpyHostToDevice, s);
+	}));
+	LCD_CUDA(e, e->gd_map.upload(s));
 	LCD_CUDA(e, cudaStreamSynchronize(s));
 	return LCD_OK;
 }
@@ -2257,16 +2300,9 @@ int lcd_gdesc_remove(lcd_engine * e, const int * sig_ids, int n)
 	if (!sig_ids) LCD_FAIL(e, LCD_ERR_INVALID, "null signature ids");
 	LCD_TRY(set_device(e));
 	bool changed = false;
-	for (int i = 0; i < n; ++i)
-	{
-		const int id = sig_ids[i];
-		if (id <= 0 || id >= static_cast<int>(e->h_gd_slot_of_sig.size()) || e->h_gd_slot_of_sig[id] < 0) continue;
-		e->gd_free.push_back(e->h_gd_slot_of_sig[id]);
-		e->h_gd_slot_of_sig[id] = -1;
-		changed = true;
-	}
+	for (int i = 0; i < n; ++i) changed |= e->gd_map.release(sig_ids[i]) >= 0;
 	if (!changed) return LCD_OK;
-	LCD_CUDA(e, cudaMemcpyAsync(e->gd_slot_of_sig.p, e->h_gd_slot_of_sig.data(), e->h_gd_slot_of_sig.size() * sizeof(int), cudaMemcpyHostToDevice, e->stream));
+	LCD_CUDA(e, e->gd_map.upload(e->stream));
 	LCD_CUDA(e, cudaStreamSynchronize(e->stream));
 	return LCD_OK;
 }
@@ -3521,56 +3557,34 @@ int lcd_sig_words_add_batch(lcd_engine * e, const int * sig_ids, int n_sigs, int
 	LCD_TRY(set_device(e));
 	if (n_sigs <= 0 || cap <= 0 || !sig_ids || !word_ids || !uv || !n) LCD_FAIL(e, LCD_ERR_INVALID, "null or empty word store input");
 	if (cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "at most %d words per signature", kMaxFrameQueries);
-	int max_id = 0;
 	for (int i = 0; i < n_sigs; ++i)
-	{
-		if (sig_ids[i] <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "signature id %d is not > 0", sig_ids[i]);
 		if (n[i] < 0 || n[i] > cap) LCD_FAIL(e, LCD_ERR_INVALID, "signature %d has %d words (cap %d)", sig_ids[i], n[i], cap);
-		max_id = std::max(max_id, sig_ids[i]);
-	}
 	cudaStream_t s = e->stream;
-	if (cap > e->ws_cap && e->ws_rows > 0)
+	const size_t prev_rows = static_cast<size_t>(e->ws_map.slots);
+	std::vector<int> slots;
+	if (!e->ws_map.assign(sig_ids, n_sigs, slots)) LCD_FAIL(e, LCD_ERR_INVALID, "signature ids must be > 0");
+	const size_t rows = static_cast<size_t>(e->ws_map.slots), wc = std::max(e->ws_cap, cap);
+	if (cap > e->ws_cap && prev_rows > 0)
 	{
 		// wider rows: re-lay the stored rows out at the new stride
 		DevBuf<int> ids2;
 		DevBuf<float> uv2;
-		LCD_CUDA(e, ids2.reserve(static_cast<size_t>(e->ws_rows) * cap, 0, false, s));
-		LCD_CUDA(e, uv2.reserve(static_cast<size_t>(e->ws_rows) * cap * 2, 0, false, s));
-		LCD_CUDA(e, cudaMemcpy2DAsync(ids2.p, cap * sizeof(int), e->ws_ids.p, e->ws_cap * sizeof(int), e->ws_cap * sizeof(int), e->ws_rows,
+		LCD_CUDA(e, ids2.reserve(rows * wc, 0, false, s));
+		LCD_CUDA(e, uv2.reserve(rows * wc * 2, 0, false, s));
+		// kernels on any stream may still read the rows being copied and freed
+		LCD_CUDA(e, cudaDeviceSynchronize());
+		LCD_CUDA(e, cudaMemcpy2DAsync(ids2.p, wc * sizeof(int), e->ws_ids.p, e->ws_cap * sizeof(int), e->ws_cap * sizeof(int), prev_rows,
 		                              cudaMemcpyDeviceToDevice, s));
-		LCD_CUDA(e, cudaMemcpy2DAsync(uv2.p, cap * 2 * sizeof(float), e->ws_uv.p, e->ws_cap * 2 * sizeof(float), e->ws_cap * 2 * sizeof(float),
-		                              e->ws_rows, cudaMemcpyDeviceToDevice, s));
+		LCD_CUDA(e, cudaMemcpy2DAsync(uv2.p, wc * 2 * sizeof(float), e->ws_uv.p, e->ws_cap * 2 * sizeof(float), e->ws_cap * 2 * sizeof(float),
+		                              prev_rows, cudaMemcpyDeviceToDevice, s));
 		LCD_CUDA(e, cudaStreamSynchronize(s));
-		std::swap(e->ws_ids.p, ids2.p);
-		std::swap(e->ws_ids.cap, ids2.cap);
-		std::swap(e->ws_uv.p, uv2.p);
-		std::swap(e->ws_uv.cap, uv2.cap);
+		e->ws_ids.swap(ids2);
+		e->ws_uv.swap(uv2);
 	}
-	e->ws_cap = std::max(e->ws_cap, cap);
-	if (static_cast<size_t>(max_id) + 1 > e->h_ws_slot_of_sig.size())
-		e->h_ws_slot_of_sig.resize(std::max<size_t>(max_id + 1, e->h_ws_slot_of_sig.size() * 3 / 2 + 1024), -1);
-	std::vector<int> slots(n_sigs);
-	for (int i = 0; i < n_sigs; ++i)
-	{
-		int slot = e->h_ws_slot_of_sig[sig_ids[i]];
-		if (slot < 0)
-		{
-			if (!e->ws_free.empty())
-			{
-				slot = e->ws_free.back();
-				e->ws_free.pop_back();
-			}
-			else
-				slot = e->ws_rows++;
-			e->h_ws_slot_of_sig[sig_ids[i]] = slot;
-			++e->ws_count;
-		}
-		slots[i] = slot;
-	}
-	const size_t wc = e->ws_cap;
-	LCD_CUDA(e, e->ws_ids.reserve(static_cast<size_t>(e->ws_rows) * wc, e->ws_ids.cap, false, s));
-	LCD_CUDA(e, e->ws_uv.reserve(static_cast<size_t>(e->ws_rows) * wc * 2, e->ws_uv.cap, false, s));
-	LCD_CUDA(e, e->ws_n.reserve(e->ws_rows, e->ws_n.cap, false, s));
+	e->ws_cap = static_cast<int>(wc);
+	LCD_CUDA(e, e->ws_ids.reserve(rows * wc, e->ws_ids.cap, false, s));
+	LCD_CUDA(e, e->ws_uv.reserve(rows * wc * 2, e->ws_uv.cap, false, s));
+	LCD_CUDA(e, e->ws_n.reserve(rows, e->ws_n.cap, false, s));
 	for (int i = 0; i < n_sigs; ++i)
 	{
 		const size_t r = slots[i];
@@ -3578,8 +3592,7 @@ int lcd_sig_words_add_batch(lcd_engine * e, const int * sig_ids, int n_sigs, int
 		LCD_CUDA(e, cudaMemcpyAsync(e->ws_uv.p + r * wc * 2, uv + static_cast<size_t>(i) * cap * 2, n[i] * 2 * sizeof(float), cudaMemcpyHostToDevice, s));
 		LCD_CUDA(e, cudaMemcpyAsync(e->ws_n.p + r, n + i, sizeof(int), cudaMemcpyHostToDevice, s));
 	}
-	LCD_CUDA(e, e->ws_slot_of_sig.reserve(e->h_ws_slot_of_sig.size(), 0, false, s));
-	LCD_CUDA(e, cudaMemcpyAsync(e->ws_slot_of_sig.p, e->h_ws_slot_of_sig.data(), e->h_ws_slot_of_sig.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+	LCD_CUDA(e, e->ws_map.upload(s));
 	LCD_CUDA(e, cudaStreamSynchronize(s));
 	return LCD_OK;
 }
@@ -3588,16 +3601,13 @@ int lcd_sig_words_remove(lcd_engine * e, int sig_id)
 {
 	if (!e) return LCD_ERR_INVALID;
 	LCD_TRY(set_device(e));
-	if (sig_id <= 0 || sig_id >= static_cast<int>(e->h_ws_slot_of_sig.size()) || e->h_ws_slot_of_sig[sig_id] < 0) return LCD_OK;
-	e->ws_free.push_back(e->h_ws_slot_of_sig[sig_id]);
-	e->h_ws_slot_of_sig[sig_id] = -1;
-	--e->ws_count;
-	const int minus1 = -1;
-	LCD_CUDA(e, cudaMemcpy(e->ws_slot_of_sig.p + sig_id, &minus1, sizeof(int), cudaMemcpyHostToDevice));
+	if (e->ws_map.release(sig_id) < 0) return LCD_OK;
+	LCD_CUDA(e, e->ws_map.upload(sig_id, e->stream));
+	LCD_CUDA(e, cudaStreamSynchronize(e->stream));
 	return LCD_OK;
 }
 
-int lcd_sig_words_count(const lcd_engine * e) { return e ? e->ws_count : 0; }
+int lcd_sig_words_count(const lcd_engine * e) { return e ? e->ws_map.count() : 0; }
 
 int lcd_decide_epipolar_dev(lcd_engine * e, const int * d_word_ids, const float * d_uv, const int * d_n_per_frame, int n_frames, int nq_per_frame,
                             const lcd_epipolar_params * p, void * stream)
@@ -3615,8 +3625,8 @@ int lcd_decide_epipolar_dev(lcd_engine * e, const int * d_word_ids, const float 
 	LCD_CUDA(e, e->ws_n.reserve(1, 0, true, s)); // an empty store: every hypothesis is a signature without words
 	LCD_CUDA(e, e->ws_ids.reserve(1, 0, false, s));
 	LCD_CUDA(e, e->ws_uv.reserve(2, 0, false, s));
-	epi_decide_prep_kernel<<<(n_frames + 127) / 128, 128, 0, s>>>(n_frames, e->dc_dec.p, e->ws_slot_of_sig.p,
-	                                                                 static_cast<int>(e->h_ws_slot_of_sig.size()), e->ep_slot.p, e->ep_skip.p);
+	epi_decide_prep_kernel<<<(n_frames + 127) / 128, 128, 0, s>>>(n_frames, e->dc_dec.p, e->ws_map.d.p, e->ws_map.n_ids, e->ep_slot.p,
+	                                                                 e->ep_skip.p);
 	LCD_CHECK_LAUNCH(e);
 	EpiArgs a{};
 	a.ids_a = d_word_ids;
@@ -3750,8 +3760,8 @@ int lcd_match_bf(lcd_engine * e, int n_pairs, int cap, const void * desc_query, 
 }
 
 // ---- signature store + fused query -------------------------------------------------------------
-int lcd_sig_count(const lcd_engine * e) { return e ? e->st_slots - static_cast<int>(e->free_slots.size()) : 0; }
-int lcd_sig_slots(const lcd_engine * e) { return e ? e->st_slots : 0; }
+int lcd_sig_count(const lcd_engine * e) { return e ? e->st_map.count() : 0; }
+int lcd_sig_slots(const lcd_engine * e) { return e ? e->st_map.slots : 0; }
 
 int lcd_sig_add_batch(lcd_engine * e, const int * sig_ids, int n_sigs, int cap, const void * desc, const float * xyz, const int * n)
 {
@@ -3759,70 +3769,31 @@ int lcd_sig_add_batch(lcd_engine * e, const int * sig_ids, int n_sigs, int cap, 
 	if (n_sigs <= 0) return LCD_OK;
 	if (!sig_ids || !desc || !xyz || !n || cap <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null signature data");
 	if (cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "at most %d features per signature", kMaxFrameQueries);
+	if (e->st_cap != 0 && cap != e->st_cap) LCD_FAIL(e, LCD_ERR_INVALID, "signature store was created with %d rows per signature, got %d", e->st_cap, cap);
 	LCD_TRY(set_device(e));
 	cudaStream_t s = e->stream;
-	if (e->st_cap == 0) e->st_cap = cap;
-	if (cap != e->st_cap) LCD_FAIL(e, LCD_ERR_INVALID, "signature store was created with %d rows per signature, got %d", e->st_cap, cap);
-	int max_id = 0;
-	for (int i = 0; i < n_sigs; ++i)
-	{
-		if (sig_ids[i] <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "signature id must be positive");
-		max_id = std::max(max_id, sig_ids[i]);
-	}
-	if (static_cast<size_t>(max_id) + 1 > e->h_slot_of_sig.size())
-	{
-		const size_t old = e->h_slot_of_sig.size();
-		const size_t ncap = std::max<size_t>(max_id + 1, old + old / 2 + 1024);
-		e->h_slot_of_sig.resize(ncap, -1);
-	}
-	// slots: freed slots are reused first (one add + one remove per frame is what the WM -> LTM transfer produces: the store must
-	// not grow); the bulk copy is used when the slots happen to be consecutive
-	const size_t prev_slots = static_cast<size_t>(e->st_slots);
-	std::vector<int> slots(n_sigs);
-	bool contiguous = true;
-	for (int i = 0; i < n_sigs; ++i)
-	{
-		int slot = e->h_slot_of_sig[sig_ids[i]];
-		if (slot < 0)
-		{
-			if (!e->free_slots.empty())
-			{
-				slot = e->free_slots.back();
-				e->free_slots.pop_back();
-			}
-			else slot = e->st_slots++;
-		}
-		slots[i] = slot;
-		if (i > 0 && slots[i] != slots[i - 1] + 1) contiguous = false;
-		e->h_slot_of_sig[sig_ids[i]] = slot;
-	}
-	LCD_CUDA(e, e->st_desc.reserve(static_cast<size_t>(e->st_slots) * cap * e->nw, prev_slots * cap * e->nw, false, s));
-	LCD_CUDA(e, e->st_xyz.reserve(static_cast<size_t>(e->st_slots) * cap * 3, prev_slots * cap * 3, false, s));
-	LCD_CUDA(e, e->st_n.reserve(static_cast<size_t>(e->st_slots), prev_slots, true, s));
-	LCD_CUDA(e, e->st_kof.reserve(static_cast<size_t>(e->st_slots) * cap, prev_slots * cap, false, s));
-	LCD_CUDA(e, e->st_creator.reserve(static_cast<size_t>(e->st_slots) * cap, prev_slots * cap, false, s));
-	LCD_CUDA(e, e->st_ftag.reserve(static_cast<size_t>(e->st_slots), prev_slots, false, s));
-	const size_t drow = static_cast<size_t>(cap) * e->nw * 4, xrow = static_cast<size_t>(cap) * 3 * sizeof(float);
+	const size_t prev_slots = static_cast<size_t>(e->st_map.slots);
+	std::vector<int> slots;
+	if (!e->st_map.assign(sig_ids, n_sigs, slots)) LCD_FAIL(e, LCD_ERR_INVALID, "signature id must be positive");
+	e->st_cap = cap;
+	const size_t nst = static_cast<size_t>(e->st_map.slots), drow = static_cast<size_t>(cap) * e->nw, xrow = static_cast<size_t>(cap) * 3;
+	LCD_CUDA(e, e->st_desc.reserve(nst * drow, prev_slots * drow, false, s));
+	LCD_CUDA(e, e->st_xyz.reserve(nst * xrow, prev_slots * xrow, false, s));
+	LCD_CUDA(e, e->st_n.reserve(nst, prev_slots, true, s));
+	LCD_CUDA(e, e->st_kof.reserve(nst * cap, prev_slots * cap, false, s));
+	LCD_CUDA(e, e->st_creator.reserve(nst * cap, prev_slots * cap, false, s));
+	LCD_CUDA(e, e->st_ftag.reserve(nst, prev_slots, false, s));
 	// a written row's cached FROM dictionary is stale (0xFF..: nf = -1 matches no call)
-	if (contiguous)
-	{
-		LCD_CUDA(e, cudaMemcpyAsync(e->st_desc.p + static_cast<size_t>(slots[0]) * cap * e->nw, desc, drow * n_sigs, cudaMemcpyHostToDevice, s));
-		LCD_CUDA(e, cudaMemcpyAsync(e->st_xyz.p + static_cast<size_t>(slots[0]) * cap * 3, xyz, xrow * n_sigs, cudaMemcpyHostToDevice, s));
-		LCD_CUDA(e, cudaMemcpyAsync(e->st_n.p + slots[0], n, n_sigs * sizeof(int), cudaMemcpyHostToDevice, s));
-		LCD_CUDA(e, cudaMemsetAsync(e->st_ftag.p + slots[0], 0xFF, n_sigs * sizeof(FromDictTag), s));
-	}
-	else
-	{
-		for (int i = 0; i < n_sigs; ++i)
-		{
-			LCD_CUDA(e, cudaMemcpyAsync(e->st_desc.p + static_cast<size_t>(slots[i]) * cap * e->nw, static_cast<const char *>(desc) + drow * i, drow, cudaMemcpyHostToDevice, s));
-			LCD_CUDA(e, cudaMemcpyAsync(e->st_xyz.p + static_cast<size_t>(slots[i]) * cap * 3, xyz + static_cast<size_t>(i) * cap * 3, xrow, cudaMemcpyHostToDevice, s));
-			LCD_CUDA(e, cudaMemcpyAsync(e->st_n.p + slots[i], n + i, sizeof(int), cudaMemcpyHostToDevice, s));
-			LCD_CUDA(e, cudaMemsetAsync(e->st_ftag.p + slots[i], 0xFF, sizeof(FromDictTag), s));
-		}
-	}
-	LCD_CUDA(e, e->st_slot_of_sig.reserve(e->h_slot_of_sig.size(), 0, false, s));
-	LCD_CUDA(e, cudaMemcpyAsync(e->st_slot_of_sig.p, e->h_slot_of_sig.data(), e->h_slot_of_sig.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+	const auto put = [&](size_t slot, size_t i, size_t k) {
+		const uint32_t * src = static_cast<const uint32_t *>(desc) + i * drow;
+		cudaError_t err = cudaMemcpyAsync(e->st_desc.p + slot * drow, src, k * drow * sizeof(uint32_t), cudaMemcpyHostToDevice, s);
+		if (err == cudaSuccess) err = cudaMemcpyAsync(e->st_xyz.p + slot * xrow, xyz + i * xrow, k * xrow * sizeof(float), cudaMemcpyHostToDevice, s);
+		if (err == cudaSuccess) err = cudaMemcpyAsync(e->st_n.p + slot, n + i, k * sizeof(int), cudaMemcpyHostToDevice, s);
+		if (err == cudaSuccess) err = cudaMemsetAsync(e->st_ftag.p + slot, 0xFF, k * sizeof(FromDictTag), s);
+		return err;
+	};
+	LCD_CUDA(e, write_rows(slots, put));
+	LCD_CUDA(e, e->st_map.upload(s));
 	LCD_CUDA(e, cudaStreamSynchronize(s));
 	return LCD_OK;
 }
@@ -3831,12 +3802,9 @@ int lcd_sig_remove(lcd_engine * e, int sig_id)
 {
 	if (!e) return LCD_ERR_INVALID;
 	LCD_TRY(set_device(e));
-	if (sig_id <= 0 || sig_id >= static_cast<int>(e->h_slot_of_sig.size()) || e->h_slot_of_sig[sig_id] < 0) return LCD_OK;
-	const int slot = e->h_slot_of_sig[sig_id];
-	e->h_slot_of_sig[sig_id] = -1;
-	e->free_slots.push_back(slot);
-	const int minus1 = -1;
-	LCD_CUDA(e, cudaMemcpyAsync(e->st_slot_of_sig.p + sig_id, &minus1, sizeof(int), cudaMemcpyHostToDevice, e->stream));
+	const int slot = e->st_map.release(sig_id);
+	if (slot < 0) return LCD_OK;
+	LCD_CUDA(e, e->st_map.upload(sig_id, e->stream));
 	LCD_CUDA(e, cudaMemsetAsync(e->st_n.p + slot, 0, sizeof(int), e->stream));
 	LCD_CUDA(e, cudaMemsetAsync(e->st_ftag.p + slot, 0xFF, sizeof(FromDictTag), e->stream));
 	LCD_CUDA(e, cudaStreamSynchronize(e->stream));
@@ -3851,8 +3819,7 @@ static int verify_top_dev(lcd_engine * e, const uint32_t * d_q, const float * d_
 	LCD_CUDA(e, e->d_hyp_id.reserve(n_frames, 0, false, s));
 	LCD_CUDA(e, e->d_hyp_slot.reserve(n_frames, 0, false, s));
 	e->dc_hyp_valid = false; // the arg-max replaces the hypotheses of the last decision
-	argmax_hypothesis_kernel<<<n_frames, 256, 0, s>>>(d_like, ns, d_sig_ids, e->st_slot_of_sig.p, static_cast<int>(e->h_slot_of_sig.size()),
-	                                                  e->d_hyp_id.p, e->d_hyp_slot.p);
+	argmax_hypothesis_kernel<<<n_frames, 256, 0, s>>>(d_like, ns, d_sig_ids, e->st_map.d.p, e->st_map.n_ids, e->d_hyp_id.p, e->d_hyp_slot.p);
 	LCD_CHECK_LAUNCH(e);
 	const PairSource src{{e->st_desc.p, e->st_xyz.p, e->st_n.p, e->d_hyp_slot.p, e->st_cap}, {d_q, d_uv, d_xyz_to, d_nq_frame, nq, nq, nullptr}};
 	return register_pairs(e, src, n_frames, std::max(e->st_cap, nq), vp, s);
@@ -4373,11 +4340,7 @@ int lcd_clients_set_map(lcd_engine * e, const int * ids, int n, const int64_t * 
 	// kernels of the last decision may still read the tables this call replaces
 	LCD_CUDA(e, cudaDeviceSynchronize());
 	// commit: nothing below can fail
-	if (grown.p)
-	{
-		std::swap(grown.p, e->dc_post.p);
-		std::swap(grown.cap, e->dc_post.cap);
-	}
+	if (grown.p) e->dc_post.swap(grown);
 	e->dc_stride = stride;
 	e->dc_tables = std::move(tab);
 	e->gps_places.reset();
@@ -4561,8 +4524,8 @@ static int decide_launch(lcd_engine * e, const float * d_like, int n_frames, int
 	a.loop_thr = dp->loop_thr;
 	a.aggressive_loop_thr = dp->aggressive_loop_thr;
 	a.loop_ratio = dp->loop_ratio;
-	a.sig_slot = e->st_slot_of_sig.p;
-	a.slot_cap = e->st_slot_of_sig.p ? static_cast<int>(e->h_slot_of_sig.size()) : 0;
+	a.sig_slot = e->st_map.d.p;
+	a.slot_cap = e->st_map.n_ids;
 	a.dec = e->dc_dec.p;
 	a.hyp_id = e->d_hyp_id.p;
 	a.hyp_slot = e->d_hyp_slot.p;
@@ -4867,8 +4830,8 @@ int lcd_decide_proximity_dev(lcd_engine * e, const void * d_queries, const float
 	a.flags = e->dc_tab.p + n_frames;
 	a.adj = e->dc_adj.p;
 	a.dec = e->dc_dec.p;
-	a.sig_slot = e->st_slot_of_sig.p;
-	a.slot_cap = e->st_slot_of_sig.p ? static_cast<int>(e->h_slot_of_sig.size()) : 0;
+	a.sig_slot = e->st_map.d.p;
+	a.slot_cap = e->st_map.n_ids;
 	a.radius = pp->local_radius;
 	// _proximityAngle *= M_PI/180.0f, a float (Rtabmap.cpp:609-612)
 	a.angle = static_cast<float>(static_cast<double>(pp->angle) * (M_PI / 180.0));

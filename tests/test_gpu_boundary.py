@@ -219,6 +219,11 @@ def test_signature_store_reuses_freed_rows():
     cap = 50
     d = rng.integers(0, 256, (8, cap, 32), dtype=np.uint8)
     x = rng.normal(0, 1, (8, cap, 3)).astype(np.float32)
+    # a refused first add (id 0) stores nothing, so it does not fix the rows per signature either
+    with pytest.raises(LcdError) as ex:
+        eng.sig_add_batch([0], d[:1, :8], x[:1, :8])
+    assert ex.value.code == -1
+    assert eng.sig_count() == 0
     eng.sig_add_batch(np.arange(1, 9), d, x)
     assert eng.sig_slots() == 8 and eng.sig_count() == 8
     for k in range(40):

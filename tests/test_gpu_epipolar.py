@@ -151,8 +151,12 @@ def test_decision_epipolar():
             for i, p in enumerate(batch):
                 w[i, :300], u[i, :300] = words[p], views[p][0]
             e.sig_words_add_batch(batch, w, u, [300] * len(batch))
-        e.sig_words_add_batch([99], np.zeros((1, 8), np.int32), np.zeros((1, 8, 2), np.float32), [8])
-        e.sig_words_remove(99)
+            if cap == 320:
+                # a place added and removed between the batches: the first place of the wider batch takes its freed row while the
+                # store widens its rows
+                e.sig_words_add_batch([99], np.zeros((1, 8), np.int32), np.zeros((1, 8, 2), np.float32), [8])
+                e.sig_words_remove(99)
+                assert e.sig_words_count == len(batch)
         assert e.sig_words_count == len(places)
         dp = Engine.decide_params(loop_thr=0.11, loop_ratio=0.9)
         seen = set()
