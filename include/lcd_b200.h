@@ -300,7 +300,8 @@ int lcd_localize_batch_dev(lcd_engine * e, const void * d_queries, int n_frames,
  * The dot product is one fp32 fused multiply-add chain in ascending dimension order: the same bits for a (query, signature)
  * whatever the batch, the frame's position, ns or the entry point, within gamma_D * sum |q_i s_i| of the exact value
  * (gamma_D = D u / (1 - D u), u = 2^-24).  OpenCV's cv::Mat::dot is dispatched per CPU, so no single reference bit pattern exists.
- * Sharded engines (lcd_shard_set_row_offset != 0) get LCD_ERR_STATE from every call of this group.
+ * Sharded engines (lcd_shard_set_row_offset != 0) get LCD_ERR_STATE from every call of this group: they use
+ * lcd_shard_localize_similarity_batch_dev and its stages (word-range sharding, below).
  *
  * Global descriptors: Signature::sensorData().globalDescriptors(), type 1, one per signature, fp32 [n][dim] row-major.  The
  * dimension is fixed by the first add; a later add with another dimension is LCD_ERR_INVALID.  Adding an id that has a
@@ -683,6 +684,26 @@ int lcd_shard_resolve_score_dev(lcd_engine * e, const void * d_queries, int n_fr
                                 int * d_word_ids_out, long long * d_scores_out, void * stream);
 int lcd_shard_finalize_dev(lcd_engine * e, const long long * d_scores, int n, float * d_likelihood_out,
                            void * stream);
+/* The similarity likelihood (Kp/TfIdfLikelihoodUsed=false, see lcd_localize_similarity_batch_dev) in the same stages.  A word's
+ * postings live on one rank, so the pair count of (frame, place) and valid(s) are exact sums of per-rank parts, and the result equals
+ * the unsharded engine's bit for bit.
+ * lcd_shard_similarity_ids_dev: from the word ids of ALL frames d_word_ids_all[n_frames*nq_per_frame] (the all-gathered output of
+ * lcd_shard_resolve_frames_dev), this rank's pair counts over its word range d_pairs_out[n_frames*ns] int32, by position in
+ * d_sig_ids, and this rank's valid(s) of the listed places d_valid_out[ns] int32.  All-reduce(sum) both across ranks (exact: a pair
+ * count is at most nq_per_frame), then call lcd_shard_similarity_finalize_dev on every rank for its own frames.
+ * lcd_shard_similarity_finalize_dev: compareTo of n_frames frames from the summed counts d_pairs[n_frames*ns], the summed valid(s)
+ * d_valid[ns] and the frames' own word ids d_word_ids[n_frames*nq_per_frame] (valid(q) = their ids > 0, new words included) into
+ * d_likelihood_out[n_frames*ns].  Global descriptors (all may be NULL): d_frame_gdesc[n_frames][dim] the frames' own, and the map's
+ * as a table d_map_gdesc[n_map_rows][dim] with d_map_gdesc_row[ns] the row of each listed place or -1 for none (the descriptor store
+ * of lcd_gdesc_add refuses sharded engines).  A (frame, place) pair takes the descriptor value when both sides carry one.  Returns
+ * LCD_ERR_INVALID when dim <= 0 while descriptors are given, or when a row index lies outside [-1, n_map_rows): the row indices are
+ * read back to check them, which synchronises `stream` once. */
+int lcd_shard_similarity_ids_dev(lcd_engine * e, const int * d_word_ids_all, int n_frames, int nq_per_frame, const int * d_sig_ids,
+                                 int ns, int * d_pairs_out, int * d_valid_out, void * stream);
+int lcd_shard_similarity_finalize_dev(lcd_engine * e, const int * d_pairs, const int * d_valid, const int * d_word_ids, int n_frames,
+                                      int nq_per_frame, const float * d_frame_gdesc, const float * d_map_gdesc,
+                                      const int * d_map_gdesc_row, int n_map_rows, int dim, const int * d_sig_ids, int ns,
+                                      float * d_likelihood_out, void * stream);
 
 /* ---- the exchanges behind the C ABI: one engine = one rank of a word-range-sharded job ----------------------------------
  * NCCL is loaded at run time (dlopen of libnccl.so.2: the host's own copy when it has one).  Bootstrap as any NCCL program: rank 0 calls
@@ -718,6 +739,18 @@ int lcd_shard_localize_batch_dev(lcd_engine * e, const void * d_queries, int n_f
                                  int incremental, float nndr, int new_words_compared_together,
                                  const int * d_sig_ids, int ns, int n_total, const int * d_row_ids_global, int last_word_id,
                                  int * d_word_ids_out, float * d_likelihood_out, void * stream);
+/* lcd_shard_localize_batch_dev with the similarity likelihood: equal bit for bit to lcd_localize_similarity_batch_dev on one unsharded
+ * engine.  The exchanges of the descriptors, keys and word ids are those of lcd_shard_localize_batch_dev; then every rank counts the
+ * word pairs of all frames over its word range and a reduce-scatter of int32 counts returns each rank the sums of its own frames, with
+ * the ranks' valid(s) of the listed places summed in the same collective.  The dot products of the local frames' global descriptors
+ * need no exchange.  Global descriptors as lcd_shard_similarity_finalize_dev (d_frame_gdesc of the LOCAL frames; the checks of the
+ * row indices synchronise `stream` once per call when d_map_gdesc is given).  n_total has no role in the similarity likelihood and
+ * is not taken. */
+int lcd_shard_localize_similarity_batch_dev(lcd_engine * e, const void * d_queries, int n_frames, int nq_per_frame, int incremental,
+                                            float nndr, int new_words_compared_together, const float * d_frame_gdesc,
+                                            const float * d_map_gdesc, const int * d_map_gdesc_row, int n_map_rows, int dim,
+                                            const int * d_sig_ids, int ns, const int * d_row_ids_global, int last_word_id,
+                                            int * d_word_ids_out, float * d_likelihood_out, void * stream);
 
 /* ---- epipolar verification of loop-closure hypotheses (VhEp/Enabled) ---------------------------------------------------------
  * EpipolarGeometry::check(A, B) (corelib/src/EpipolarGeometry.cpp:65-102) of a new signature A and a hypothesis B, from word ids and

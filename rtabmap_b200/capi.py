@@ -271,12 +271,15 @@ SIGNATURES = {
     "lcd_shard_resolve_frames_dev": (_I, [_P, _P, _I, _I, _I, _I, _P, _I, _P, _I, _I, _F, _I, _P, _P, _P]),
     "lcd_shard_score_ids_dev": (_I, [_P, _P, _I, _I, _P, _I, _I, _P, _P]),
     "lcd_shard_finalize_dev": (_I, [_P, _P, _I, _P, _P]),
+    "lcd_shard_similarity_ids_dev": (_I, [_P, _P, _I, _I, _P, _I, _P, _P, _P]),
+    "lcd_shard_similarity_finalize_dev": (_I, [_P, _P, _P, _P, _I, _I, _P, _P, _P, _I, _I, _P, _I, _P, _P]),
     "lcd_shard_unique_id": (_I, [_P]),
     "lcd_shard_comm_init": (_I, [_P, _P, _I, _I]),
     "lcd_shard_comm_adopt": (_I, [_P, _P, _I, _I]),
     "lcd_shard_comm_destroy": (_I, [_P]),
     "lcd_shard_process_frames_dev": (_I, [_P, _I, _P, _I, _I, _I, _P, _I, _P, _I, _F, _I, _P, _I, _I, _P, _I, _P, _P, _P, _P]),
     "lcd_shard_localize_batch_dev": (_I, [_P, _P, _I, _I, _I, _F, _I, _P, _I, _I, _P, _I, _P, _P, _P]),
+    "lcd_shard_localize_similarity_batch_dev": (_I, [_P, _P, _I, _I, _I, _F, _I, _P, _P, _P, _I, _I, _P, _I, _P, _I, _P, _P, _P]),
     "lcd_epipolar_check_batch": (_I, [_P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "lcd_sig_words_add_batch": (_I, [_P, _P, _I, _I, _P, _P, _P]),
     "lcd_sig_words_remove": (_I, [_P, _I]),
@@ -1188,6 +1191,18 @@ class Engine:
                                                             C.c_void_p(d_sig_ids), ns, int(n_total), C.c_void_p(d_row_ids_global), int(last_word_id),
                                                             C.c_void_p(d_words_out or None), C.c_void_p(d_like_out), C.c_void_p(stream or None)))
 
+    def shard_localize_similarity_batch_dev(self, d_queries: int, n_frames: int, nq: int, d_sig_ids: int, ns: int, d_row_ids_global: int,
+                                            last_word_id: int, d_words_out: int, d_like_out: int, d_frame_gdesc: int = 0, d_map_gdesc: int = 0,
+                                            d_map_gdesc_row: int = 0, n_map_rows: int = 0, dim: int = 0, incremental: bool = True,
+                                            nndr: float = 0.8, cmp_new: bool = True, stream: int = 0):
+        """shard_localize_batch_dev with the similarity likelihood: equal to localize_similarity_batch_dev on one unsharded engine.
+        d_frame_gdesc [n_frames, dim] float32 (this rank's frames) or 0; the map's descriptors d_map_gdesc [n_map_rows, dim] float32 with
+        d_map_gdesc_row [ns] int32 (row of each listed place, -1 = none), or 0 and 0."""
+        self._check(self._lib.lcd_shard_localize_similarity_batch_dev(
+            self._h, C.c_void_p(d_queries), n_frames, nq, int(incremental), float(nndr), int(cmp_new), C.c_void_p(d_frame_gdesc or None),
+            C.c_void_p(d_map_gdesc or None), C.c_void_p(d_map_gdesc_row or None), int(n_map_rows), int(dim), C.c_void_p(d_sig_ids), ns,
+            C.c_void_p(d_row_ids_global), int(last_word_id), C.c_void_p(d_words_out or None), C.c_void_p(d_like_out), C.c_void_p(stream or None)))
+
     def shard_set_row_offset(self, off: int):
         self._check(self._lib.lcd_shard_set_row_offset(self._h, int(off)))
 
@@ -1222,3 +1237,20 @@ class Engine:
 
     def shard_finalize_dev(self, d_scores: int, n: int, d_like_out: int, stream: int = 0):
         self._check(self._lib.lcd_shard_finalize_dev(self._h, C.c_void_p(d_scores), n, C.c_void_p(d_like_out), C.c_void_p(stream or None)))
+
+    def shard_similarity_ids_dev(self, d_word_ids_all: int, n_frames: int, nq: int, d_sig_ids: int, ns: int, d_pairs_out: int, d_valid_out: int,
+                                 stream: int = 0):
+        """This rank's word pairs of every frame over its word range, d_pairs_out [n_frames, ns] int32, and its valid(s) of the listed
+        places, d_valid_out [ns] int32: sum both over the ranks, then shard_similarity_finalize_dev."""
+        self._check(self._lib.lcd_shard_similarity_ids_dev(self._h, C.c_void_p(d_word_ids_all), n_frames, nq, C.c_void_p(d_sig_ids), ns,
+                                                            C.c_void_p(d_pairs_out), C.c_void_p(d_valid_out), C.c_void_p(stream or None)))
+
+    def shard_similarity_finalize_dev(self, d_pairs: int, d_valid: int, d_word_ids: int, n_frames: int, nq: int, d_sig_ids: int, ns: int,
+                                      d_like_out: int, d_frame_gdesc: int = 0, d_map_gdesc: int = 0, d_map_gdesc_row: int = 0,
+                                      n_map_rows: int = 0, dim: int = 0, stream: int = 0):
+        """The similarity likelihood of n_frames frames (their word ids d_word_ids [n_frames, nq]) from the summed pair counts and
+        valid(s); global descriptors as shard_localize_similarity_batch_dev."""
+        self._check(self._lib.lcd_shard_similarity_finalize_dev(
+            self._h, C.c_void_p(d_pairs), C.c_void_p(d_valid), C.c_void_p(d_word_ids), n_frames, nq, C.c_void_p(d_frame_gdesc or None),
+            C.c_void_p(d_map_gdesc or None), C.c_void_p(d_map_gdesc_row or None), int(n_map_rows), int(dim), C.c_void_p(d_sig_ids), ns,
+            C.c_void_p(d_like_out), C.c_void_p(stream or None)))

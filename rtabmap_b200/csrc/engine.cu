@@ -567,6 +567,7 @@ struct lcd_engine
 	DevBuf<int> sh_n_all, sh_words_loc[2], sh_words_all[2];
 	DevBuf<uint32_t> sh_keys[2], sh_keys_mine[2];
 	DevBuf<long long> sh_scores[2], sh_scores_loc[2];
+	DevBuf<int> sh_pairs[2], sh_pairs_loc[2]; // similarity variant: [rank][frames + 1][ns] pair counts + valid(s), and the local sums
 };
 
 #define LCD_FAIL(e, code, ...)                          \
@@ -1229,15 +1230,15 @@ int launch_similarity(lcd_engine * e, int n_frames, int nq, const float * d_gdes
 	if (gd)
 	{
 		LCD_CUDA(e, e->gd_dot.reserve(static_cast<size_t>(n_frames) * ns, 0, false, s));
-		GdescArgs g{d_gdesc, n_frames, e->gd_rows.p, e->gd_dim, e->gd_map.d.p, e->gd_map.n_ids, d_sig_ids, ns, e->gd_dot.p};
+		GdescArgs g{d_gdesc, n_frames, e->gd_rows.p, e->gd_dim, e->gd_map.d.p, e->gd_map.n_ids, d_sig_ids, ns, e->gd_dot.p, nullptr};
 		prof_mark(e, LCD_PROF_SCORE, s);
 		gdesc_dot_kernel<<<dim3((ns + kGdBN - 1) / kGdBN, (n_frames + kGdBM - 1) / kGdBM), kGdThreads, 0, s>>>(g);
 		prof_mark(e, LCD_PROF_SCORE, s);
 		LCD_CHECK_LAUNCH(e);
 	}
-	SimilarityArgs f{e->acc.p, e->acc_stride, e->nvalid.p, static_cast<int>(e->h_nvalid.size()), e->q_valid.p, gd ? e->gd_dot.p : nullptr,
+	SimilarityArgs f{e->acc.p, e->acc_stride, nullptr, e->nvalid.p, static_cast<int>(e->h_nvalid.size()), e->q_valid.p, gd ? e->gd_dot.p : nullptr,
 	                 e->gd_map.d.p, e->gd_map.n_ids, d_sig_ids, ns, d_like};
-	similarity_finalize_kernel<<<dim3((ns + 255) / 256, n_frames), 256, 0, s>>>(f);
+	similarity_finalize_kernel<false><<<dim3((ns + 255) / 256, n_frames), 256, 0, s>>>(f);
 	LCD_CHECK_LAUNCH(e);
 	return LCD_OK;
 }
@@ -5036,6 +5037,114 @@ int lcd_shard_score_ids_dev(lcd_engine * e, const int * d_word_ids_all, int n_fr
 	return LCD_OK;
 }
 
+// ---- the similarity likelihood over word-range shards ----------------------------------------------------------------------
+// Global descriptors of the sharded similarity step: the local frames' own (frames [n_frames][dim] or nullptr), and the map's, given by
+// the caller because the descriptor store refuses sharded engines (rows [n_rows][dim], row_of_k [ns] the row of each listed place or -1).
+struct ShardGdesc
+{
+	const float * frames;
+	const float * rows;
+	const int * row_of_k;
+	int n_rows;
+	int dim;
+};
+
+// The row indices are read back (one synchronisation of `s`) so that an index outside the table is refused before any kernel reads it.
+static int shard_check_gdesc(lcd_engine * e, const ShardGdesc & g, int ns, cudaStream_t s)
+{
+	if (!g.frames && !g.rows && !g.row_of_k) return LCD_OK;
+	if (g.dim <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "global descriptors need dim > 0, got %d", g.dim);
+	if (!g.rows != !g.row_of_k) LCD_FAIL(e, LCD_ERR_INVALID, "the map's global descriptors need both the table and the row of each listed place");
+	if (!g.rows) return LCD_OK;
+	if (g.n_rows <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "the global-descriptor table needs at least one row, got %d", g.n_rows);
+	std::vector<int> h(ns);
+	LCD_CUDA(e, cudaMemcpyAsync(h.data(), g.row_of_k, static_cast<size_t>(ns) * sizeof(int), cudaMemcpyDeviceToHost, s));
+	LCD_CUDA(e, cudaStreamSynchronize(s));
+	for (int k = 0; k < ns; ++k)
+		if (h[k] < -1 || h[k] >= g.n_rows)
+			LCD_FAIL(e, LCD_ERR_INVALID, "global-descriptor row %d of listed place %d is outside the table of %d rows", h[k], k, g.n_rows);
+	return LCD_OK;
+}
+
+// valid(q) of n_frames local frames from their word ids [n_frames][nq] into e->q_valid, and their dot products with the listed places'
+// descriptors into e->gd_dot when both sides carry descriptors.  Returns whether the dot products exist through *gd.
+static int shard_similarity_prepare(lcd_engine * e, int n_frames, int nq, const int * d_word_ids, const ShardGdesc & g, const int * d_sig_ids, int ns,
+                                    bool * gd, cudaStream_t s)
+{
+	LCD_CUDA(e, e->q_valid.reserve(n_frames, 0, false, s));
+	valid_ids_kernel<<<n_frames, kValidThreads, 0, s>>>(d_word_ids, nq, e->q_valid.p);
+	LCD_CHECK_LAUNCH(e);
+	*gd = g.frames && g.rows;
+	if (*gd)
+	{
+		LCD_CUDA(e, e->gd_dot.reserve(static_cast<size_t>(n_frames) * ns, 0, false, s));
+		GdescArgs a{g.frames, n_frames, g.rows, g.dim, nullptr, 0, d_sig_ids, ns, e->gd_dot.p, g.row_of_k};
+		prof_mark(e, LCD_PROF_SCORE, s);
+		gdesc_dot_kernel<<<dim3((ns + kGdBN - 1) / kGdBN, (n_frames + kGdBM - 1) / kGdBM), kGdThreads, 0, s>>>(a);
+		prof_mark(e, LCD_PROF_SCORE, s);
+		LCD_CHECK_LAUNCH(e);
+	}
+	return LCD_OK;
+}
+
+// compareTo of the local frames [f0, f0 + n_frames) from the summed pair counts d_pairs [n_frames][ns] and valid(s) d_valid [ns], after
+// shard_similarity_prepare of all local frames
+static int shard_similarity_finalize(lcd_engine * e, int f0, int n_frames, const int * d_pairs, const int * d_valid, const ShardGdesc & g, bool gd,
+                                     const int * d_sig_ids, int ns, float * d_likelihood_out, cudaStream_t s)
+{
+	const size_t o = static_cast<size_t>(f0) * ns;
+	SimilarityArgs a{nullptr, 0, d_pairs, d_valid, 0, e->q_valid.p + f0, gd ? e->gd_dot.p + o : nullptr, g.row_of_k, 0, d_sig_ids, ns, d_likelihood_out + o};
+	similarity_finalize_kernel<true><<<dim3((ns + 255) / 256, n_frames), 256, 0, s>>>(a);
+	LCD_CHECK_LAUNCH(e);
+	return LCD_OK;
+}
+
+int lcd_shard_similarity_ids_dev(lcd_engine * e, const int * d_word_ids_all, int n_frames, int nq_per_frame, const int * d_sig_ids, int ns,
+                                 int * d_pairs_out, int * d_valid_out, void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (!d_word_ids_all || !d_sig_ids || !d_pairs_out || !d_valid_out || n_frames <= 0 || ns <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
+	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d words per signature", kMaxFrameQueries);
+	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	LCD_TRY(ensure_uq(e, n_frames, nq_per_frame, s, true));
+	LCD_TRY(ensure_acc(e, n_frames));
+	LCD_CUDA(e, zero_fill_async(e->acc.p, static_cast<size_t>(e->acc_stride) * n_frames * sizeof(long long), s));
+	ResolveArgs a{};
+	a.nq = nq_per_frame;
+	fill_prep(e, a, 0.0f, 1);
+	fill_pairs(e, a);
+	int nq_pad = 32;
+	while (nq_pad < nq_per_frame) nq_pad <<= 1;
+	prof_mark(e, LCD_PROF_RESOLVE, s);
+	prep_local_ids_kernel<<<n_frames, kResolveThreads, nq_pad * sizeof(uint32_t), s>>>(d_word_ids_all, a, n_frames, 0, n_frames);
+	prof_mark(e, LCD_PROF_RESOLVE, s);
+	LCD_CHECK_LAUNCH(e);
+	LCD_TRY(launch_score(e, n_frames, nq_per_frame, s, true));
+	gather_pairs_kernel<<<dim3((ns + 255) / 256, n_frames), 256, 0, s>>>(e->acc.p, e->acc_stride, static_cast<int>(e->h_ni.size()), d_sig_ids, ns, n_frames,
+	                                                                  d_pairs_out);
+	LCD_CHECK_LAUNCH(e);
+	gather_valid_kernel<<<(ns + 255) / 256, 256, 0, s>>>(e->nvalid.p, static_cast<int>(e->h_nvalid.size()), d_sig_ids, ns, d_valid_out, 0);
+	LCD_CHECK_LAUNCH(e);
+	return LCD_OK;
+}
+
+int lcd_shard_similarity_finalize_dev(lcd_engine * e, const int * d_pairs, const int * d_valid, const int * d_word_ids, int n_frames, int nq_per_frame,
+                                      const float * d_frame_gdesc, const float * d_map_gdesc, const int * d_map_gdesc_row, int n_map_rows, int dim,
+                                      const int * d_sig_ids, int ns, float * d_likelihood_out, void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (!d_pairs || !d_valid || !d_word_ids || !d_sig_ids || !d_likelihood_out || n_frames <= 0 || ns <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
+	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d words per signature", kMaxFrameQueries);
+	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	const ShardGdesc g{d_frame_gdesc, d_map_gdesc, d_map_gdesc_row, n_map_rows, dim};
+	LCD_TRY(shard_check_gdesc(e, g, ns, s));
+	bool gd = false;
+	LCD_TRY(shard_similarity_prepare(e, n_frames, nq_per_frame, d_word_ids, g, d_sig_ids, ns, &gd, s));
+	return shard_similarity_finalize(e, 0, n_frames, d_pairs, d_valid, g, gd, d_sig_ids, ns, d_likelihood_out, s);
+}
+
 // ---- mapping mode: Memory::update for a stream of frames ------------------------------------------------------------------
 int lcd_map_detect_async(lcd_engine * e, const uint8_t * image, int width, int height, int channels, const void * depth, int depth_type,
                          const lcd_orb_params * params)
@@ -5200,15 +5309,18 @@ int lcd_shard_comm_destroy(lcd_engine * e)
 	return LCD_OK;
 }
 
-// The exchange body of one sharded step, shared by lcd_shard_process_frames_dev and lcd_shard_localize_batch_dev.  desc: the n_frames
-// local frames of `cap` descriptor rows each (e->nw * 4 bytes per row); n_local: valid rows of each local frame, or nullptr (full frames).
-// `detect` runs first on the compute stream and produces desc / n_local (ORB); `finish` runs after the likelihood of the local frames
-// (verification).  Either may be empty.  Keys are exchanged as two u32 (binary) or two u64 (float) per query.
+// The exchange body of one sharded step, shared by lcd_shard_process_frames_dev, lcd_shard_localize_batch_dev and
+// lcd_shard_localize_similarity_batch_dev.  desc: the n_frames local frames of `cap` descriptor rows each (e->nw * 4 bytes per row); n_local:
+// valid rows of each local frame, or nullptr (full frames).  `detect` runs first on the compute stream and produces desc / n_local (ORB);
+// `finish` runs after the likelihood of the local frames (verification).  Either may be empty.  Keys are exchanged as two u32 (binary) or
+// two u64 (float) per query.  sim: nullptr = the TF-IDF likelihood; else the similarity likelihood, whose phase 4 counts word pairs instead
+// of TF-IDF terms and reduce-scatters int32 counts with this rank's valid(s) row folded into every rank's segment.
 using ShardHook = std::function<int(cudaStream_t)>;
 
 static int shard_step(lcd_engine * e, int n_frames, int cap, const uint8_t * desc, const int * n_local, const ShardHook & detect, const ShardHook & finish,
                       int incremental, float nndr, int new_words_compared_together, const int * d_sig_ids, int ns, int n_total,
-                      const int * d_row_ids_global, int last_word_id, int * d_word_ids_out, float * d_likelihood_out, cudaStream_t s)
+                      const int * d_row_ids_global, int last_word_id, int * d_word_ids_out, float * d_likelihood_out, cudaStream_t s,
+                      const ShardGdesc * sim = nullptr)
 {
 	const NcclApi & nc = nccl_api();
 	cudaStream_t c = e->comm_stream;
@@ -5245,6 +5357,12 @@ static int shard_step(lcd_engine * e, int n_frames, int cap, const uint8_t * des
 	LCD_CUDA(e, e->sh_words_all[0].reserve(rows * G, 0, false, s));
 	for (int h = 0; h < s_parts; ++h)
 	{
+		if (sim)
+		{
+			LCD_CUDA(e, e->sh_pairs[h].reserve(static_cast<size_t>(score_frames[h] + 1) * G * ns, 0, false, s));
+			LCD_CUDA(e, e->sh_pairs_loc[h].reserve(static_cast<size_t>(score_frames[h] + 1) * ns, 0, false, s));
+			continue;
+		}
 		LCD_CUDA(e, e->sh_scores[h].reserve(static_cast<size_t>(score_frames[h]) * G * ns, 0, false, s));
 		LCD_CUDA(e, e->sh_scores_loc[h].reserve(static_cast<size_t>(score_frames[h]) * ns, 0, false, s));
 	}
@@ -5335,37 +5453,66 @@ static int shard_step(lcd_engine * e, int n_frames, int cap, const uint8_t * des
 		LCD_TRY(shard_record(e, h, 5, c));
 	}
 	host_t[3] = std::chrono::steady_clock::now();
-	// phase 4: TF-IDF of every rank's frames over the local word range, reduce-scatter of the exact fixed-point sums
+	// phase 4: TF-IDF (or word pairs) of every rank's frames over the local word range, reduce-scatter of the exact integer sums
 	for (int h = 0; h < s_parts; ++h)
 	{
 		const int nf_all = score_frames[h] * G; // frames [score_f0, +score_frames) of every rank, rank-major
 		LCD_CUDA(e, cudaStreamWaitEvent(s, e->sh_ev[0][5], 0));
-		LCD_TRY(ensure_uq(e, nf_all, cap, s));
+		LCD_TRY(ensure_uq(e, nf_all, cap, s, sim != nullptr));
 		LCD_TRY(ensure_acc(e, nf_all));
 		LCD_CUDA(e, zero_fill_async(e->acc.p, static_cast<size_t>(e->acc_stride) * nf_all * sizeof(long long), s));
 		ResolveArgs a{};
 		a.nq = cap;
 		fill_prep(e, a, static_cast<float>(n_total), 1);
+		if (sim) fill_pairs(e, a);
 		int nq_pad = 32;
 		while (nq_pad < cap) nq_pad <<= 1;
 		prof_mark(e, LCD_PROF_RESOLVE, s);
 		prep_local_ids_kernel<<<nf_all, kResolveThreads, nq_pad * sizeof(uint32_t), s>>>(e->sh_words_all[0].p, a, n_frames, score_f0[h], score_frames[h]);
 		prof_mark(e, LCD_PROF_RESOLVE, s);
 		LCD_CHECK_LAUNCH(e);
-		LCD_TRY(launch_score(e, nf_all, cap, s));
-		gather_fixed_kernel<<<dim3((ns + 255) / 256, nf_all), 256, 0, s>>>(e->acc.p, e->acc_stride, static_cast<int>(e->h_ni.size()), d_sig_ids, ns, e->sh_scores[h].p);
-		LCD_CHECK_LAUNCH(e);
-		LCD_TRY(shard_record(e, h, 6, s));
-		LCD_CUDA(e, cudaStreamWaitEvent(c, e->sh_ev[h][6], 0));
-		LCD_NCCL(e, nc.ReduceScatter(e->sh_scores[h].p, e->sh_scores_loc[h].p, static_cast<size_t>(score_frames[h]) * ns, ncclInt64, ncclSum, e->comm, c));
+		LCD_TRY(launch_score(e, nf_all, cap, s, sim != nullptr));
+		if (sim)
+		{
+			// [rank][score_frames + 1][ns]: the pair counts of the rank's frames, then this rank's valid(s) in every segment, so that the
+			// reduce-scatter that sums the counts sums valid(s) across ranks too (no collective of its own)
+			const size_t seg = static_cast<size_t>(score_frames[h] + 1) * ns;
+			gather_pairs_kernel<<<dim3((ns + 255) / 256, nf_all), 256, 0, s>>>(e->acc.p, e->acc_stride, static_cast<int>(e->h_ni.size()), d_sig_ids, ns,
+			                                                                score_frames[h], e->sh_pairs[h].p);
+			LCD_CHECK_LAUNCH(e);
+			gather_valid_kernel<<<dim3((ns + 255) / 256, G), 256, 0, s>>>(e->nvalid.p, static_cast<int>(e->h_nvalid.size()), d_sig_ids, ns,
+			                                                           e->sh_pairs[h].p + static_cast<size_t>(score_frames[h]) * ns, seg);
+			LCD_CHECK_LAUNCH(e);
+			LCD_TRY(shard_record(e, h, 6, s));
+			LCD_CUDA(e, cudaStreamWaitEvent(c, e->sh_ev[h][6], 0));
+			LCD_NCCL(e, nc.ReduceScatter(e->sh_pairs[h].p, e->sh_pairs_loc[h].p, seg, ncclInt32, ncclSum, e->comm, c));
+		}
+		else
+		{
+			gather_fixed_kernel<<<dim3((ns + 255) / 256, nf_all), 256, 0, s>>>(e->acc.p, e->acc_stride, static_cast<int>(e->h_ni.size()), d_sig_ids, ns,
+			                                                                e->sh_scores[h].p);
+			LCD_CHECK_LAUNCH(e);
+			LCD_TRY(shard_record(e, h, 6, s));
+			LCD_CUDA(e, cudaStreamWaitEvent(c, e->sh_ev[h][6], 0));
+			LCD_NCCL(e, nc.ReduceScatter(e->sh_scores[h].p, e->sh_scores_loc[h].p, static_cast<size_t>(score_frames[h]) * ns, ncclInt64, ncclSum, e->comm, c));
+		}
 		LCD_TRY(shard_record(e, h, 7, c));
 	}
 	host_t[4] = std::chrono::steady_clock::now();
-	// phase 5: likelihood of the local frames (then `finish`: verification of their top hypothesis)
+	// phase 5: likelihood of the local frames (then `finish`: verification of their top hypothesis).  The similarity variant first
+	// counts valid(q) of the local frames and takes their dot products, under the last reduce-scatter.
+	bool gd = false;
+	if (sim) LCD_TRY(shard_similarity_prepare(e, n_frames, cap, e->sh_words_loc[0].p, *sim, d_sig_ids, ns, &gd, s));
 	for (int h = 0; h < s_parts; ++h)
 	{
 		const int n = score_frames[h] * ns;
 		LCD_CUDA(e, cudaStreamWaitEvent(s, e->sh_ev[h][7], 0));
+		if (sim)
+		{
+			LCD_TRY(shard_similarity_finalize(e, score_f0[h], score_frames[h], e->sh_pairs_loc[h].p, e->sh_pairs_loc[h].p + n, *sim, gd, d_sig_ids, ns,
+			                                  d_likelihood_out, s));
+			continue;
+		}
 		fixed_to_float_kernel<<<(n + 255) / 256, 256, 0, s>>>(e->sh_scores_loc[h].p, n, d_likelihood_out + static_cast<size_t>(score_f0[h]) * ns);
 		LCD_CHECK_LAUNCH(e);
 	}
@@ -5460,6 +5607,24 @@ int lcd_shard_localize_batch_dev(lcd_engine * e, const void * d_queries, int n_f
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
 	return shard_step(e, n_frames, nq_per_frame, static_cast<const uint8_t *>(d_queries), nullptr, ShardHook(), ShardHook(), incremental, nndr,
 	                  new_words_compared_together, d_sig_ids, ns, n_total, d_row_ids_global, last_word_id, d_word_ids_out, d_likelihood_out, s);
+}
+
+int lcd_shard_localize_similarity_batch_dev(lcd_engine * e, const void * d_queries, int n_frames, int nq_per_frame, int incremental, float nndr,
+                                            int new_words_compared_together, const float * d_frame_gdesc, const float * d_map_gdesc,
+                                            const int * d_map_gdesc_row, int n_map_rows, int dim, const int * d_sig_ids, int ns,
+                                            const int * d_row_ids_global, int last_word_id, int * d_word_ids_out, float * d_likelihood_out, void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (!e->comm) LCD_FAIL(e, LCD_ERR_STATE, "no communicator: call lcd_shard_comm_init first");
+	if (!d_queries || n_frames <= 0 || !d_sig_ids || ns <= 0 || !d_row_ids_global || !d_likelihood_out)
+		LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
+	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
+	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	const ShardGdesc g{d_frame_gdesc, d_map_gdesc, d_map_gdesc_row, n_map_rows, dim};
+	LCD_TRY(shard_check_gdesc(e, g, ns, s));
+	return shard_step(e, n_frames, nq_per_frame, static_cast<const uint8_t *>(d_queries), nullptr, ShardHook(), ShardHook(), incremental, nndr,
+	                  new_words_compared_together, d_sig_ids, ns, 0, d_row_ids_global, last_word_id, d_word_ids_out, d_likelihood_out, s, &g);
 }
 
 int lcd_shard_finalize_dev(lcd_engine * e, const long long * d_scores, int n, float * d_likelihood_out, void * stream)

@@ -9,6 +9,12 @@
 //     B x ns product of the frames' descriptors with the listed signatures' rows.
 // similarity_finalize_kernel applies the rules of compareTo per (frame, k).
 //
+// Word-range-sharded step (lcd_shard_*similarity*): a word's postings live on one rank, so the pair count of (frame, place) and
+// valid(s) are exact integer sums of per-rank parts.  Every rank counts the pairs of every rank's frames over its own words
+// (gather_pairs_kernel) and its own valid(s) of the listed places (gather_valid_kernel); the summed rows are read by list position
+// (similarity_finalize_kernel<true>), valid(q) comes from the frame's own word ids (valid_ids_kernel), and the dot products of a rank's
+// local frames need no exchange at all.
+//
 // Word ids <= 0 never pair here.  EpipolarGeometry::findPairs (EpipolarGeometry.h:119-151) tests id >= 0, so it would pair id 0;
 // the quantiser never puts id 0 into a signature (new and matched words are > 0, VWDictionary.cpp:1190-1216; unquantised features
 // get distinct negative ids, Memory.cpp:6029-6057), and the inverted index holds positive ids only.
@@ -41,6 +47,7 @@ struct GdescArgs
 	const int * sig_ids;       // [ns]
 	int ns;
 	float * dot;               // [n_frames][ns] (written where the signature has a descriptor)
+	const int * row_of_k;      // [ns] row of each listed place (-1 = none) in place of slot_of_sig, or nullptr
 };
 
 // grid = (ceil(ns / kGdBN), ceil(n_frames / kGdBM))
@@ -59,7 +66,8 @@ gdesc_dot_kernel(const GdescArgs a)
 		if (k < a.ns)
 		{
 			const int s = a.sig_ids[k];
-			if (s > 0 && s < a.gd_cap) slot = a.slot_of_sig[s];
+			if (a.row_of_k) slot = a.row_of_k[k];
+			else if (s > 0 && s < a.gd_cap) slot = a.slot_of_sig[s];
 		}
 		s_slot[tid] = slot;
 	}
@@ -146,20 +154,23 @@ gdesc_dot_kernel(const GdescArgs a)
 // ---- Signature::compareTo per (frame, k) ---------------------------------------------------------------------------------------
 struct SimilarityArgs
 {
-	const long long * acc;   // [n_frames][acc_stride] word pairs (score_kernel<true>)
+	const long long * acc;   // [n_frames][acc_stride] word pairs by signature id (score_kernel<true>)
 	int acc_stride;
-	const int * nvalid;      // valid(s) by signature id: sum of the signature's posting counts
-	int sig_cap;
+	const int * pairs;       // LISTED: [n_frames][ns] word pairs by list position (the sharded step's cross-rank sums)
+	const int * nvalid;      // valid(s) = sum of the signature's posting counts: by signature id, or by list position (LISTED)
+	int sig_cap;             // entries of nvalid by signature id
 	const int * q_valid;     // [n_frames] valid(q)
 	const float * dot;       // [n_frames][ns] or nullptr when the frames carry no global descriptor
-	const int * slot_of_sig; // global-descriptor slot by signature id (-1 = none)
-	int gd_cap;
+	const int * slot_of_sig; // global-descriptor slot (-1 = none): by signature id, or by list position (LISTED)
+	int gd_cap;              // entries of slot_of_sig by signature id
 	const int * sig_ids;     // [ns]
 	int ns;
 	float * out;             // [n_frames][ns]
 };
 
-// grid = (ceil(ns / 256), n_frames)
+// grid = (ceil(ns / 256), n_frames).  LISTED = false: one engine's arrays, indexed by signature id; true: the sharded step's rows,
+// indexed by list position.
+template <bool LISTED>
 __global__ void similarity_finalize_kernel(const SimilarityArgs a)
 {
 	const int k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -167,10 +178,11 @@ __global__ void similarity_finalize_kernel(const SimilarityArgs a)
 	if (k >= a.ns) return;
 	const int s = a.sig_ids[k];
 	const size_t o = static_cast<size_t>(frame) * a.ns + k;
+	const int key = LISTED ? k : s; // index of the per-place arrays
 	float v = 0.0f; // the virtual place (s <= 0) and bad signatures
 	if (s > 0)
 	{
-		if (a.dot && s < a.gd_cap && a.slot_of_sig[s] >= 0)
+		if (a.dot && (LISTED || s < a.gd_cap) && a.slot_of_sig[key] >= 0)
 		{
 			// (dot + 1.0f) / 2.0f on the double cv::Mat::dot returns, then the float of compareTo (Signature.cpp:263)
 			v = static_cast<float>((static_cast<double>(a.dot[o]) + 1.0) / 2.0);
@@ -178,15 +190,63 @@ __global__ void similarity_finalize_kernel(const SimilarityArgs a)
 		else
 		{
 			const int nq = a.q_valid[frame];
-			const int nsig = s < a.sig_cap ? a.nvalid[s] : 0;
+			const int nsig = LISTED || s < a.sig_cap ? a.nvalid[key] : 0;
 			if (nq > 0 && nsig > 0) // isBadSignature on either side (Signature.cpp:341-344) gives 0
 			{
-				const long long pairs = a.acc[static_cast<size_t>(frame) * a.acc_stride + s];
+				const long long pairs = LISTED ? a.pairs[o] : a.acc[static_cast<size_t>(frame) * a.acc_stride + s];
 				v = __fdiv_rn(static_cast<float>(pairs), static_cast<float>(max(nq, nsig))); // float(pairs) / float(totalWords)
 			}
 		}
 	}
 	a.out[o] = v;
+}
+
+// ---- the word-range-sharded step ---------------------------------------------------------------------------------------------
+// A pair count is at most valid(q) <= kMaxFrameQueries, and valid(s) a signature's reference count, so both are exchanged as int32.
+// Pair counts of `frame` by list position, from the accumulator rows score_kernel<true> filled: row frame + frame / rows_per_seg of
+// out[..][ns], i.e. one row is left free after every rows_per_seg frames (the reduce-scatter segment of a rank carries its valid(s)
+// there; rows_per_seg = n_frames leaves none).  grid = (ceil(ns / 256), n_frames)
+__global__ void gather_pairs_kernel(const long long * __restrict__ acc, int acc_stride, int sig_cap, const int * __restrict__ sig_ids, int ns,
+                                    int rows_per_seg, int * __restrict__ out)
+{
+	const int k = blockIdx.x * blockDim.x + threadIdx.x;
+	const int frame = blockIdx.y;
+	if (k >= ns) return;
+	const int s = sig_ids[k];
+	int v = 0;
+	if (s > 0 && s < sig_cap) v = static_cast<int>(acc[static_cast<size_t>(frame) * acc_stride + s]);
+	out[(static_cast<size_t>(frame) + frame / rows_per_seg) * ns + k] = v;
+}
+
+// this rank's valid(s) of the listed places, written to out + c * stride for c < gridDim.y.  grid = (ceil(ns / 256), copies)
+__global__ void gather_valid_kernel(const int * __restrict__ nvalid, int sig_cap, const int * __restrict__ sig_ids, int ns, int * __restrict__ out,
+                                    size_t stride)
+{
+	const int k = blockIdx.x * blockDim.x + threadIdx.x;
+	if (k >= ns) return;
+	const int s = sig_ids[k];
+	out[blockIdx.y * stride + k] = s > 0 && s < sig_cap ? nvalid[s] : 0;
+}
+
+// valid(q) of each frame from its word ids [n_frames][nq]: the ids > 0, new words included (the rule of the unsharded preparation).
+// grid = n_frames, block = kValidThreads
+constexpr int kValidThreads = 128;
+__global__ void __launch_bounds__(kValidThreads)
+valid_ids_kernel(const int * __restrict__ word_ids, int nq, int * __restrict__ out)
+{
+	__shared__ int s_warp[kValidThreads / 32];
+	const int * w = word_ids + static_cast<size_t>(blockIdx.x) * nq;
+	int n = 0;
+	for (int i = threadIdx.x; i < nq; i += kValidThreads) n += w[i] > 0;
+	n = __reduce_add_sync(0xFFFFFFFFu, n);
+	if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = n;
+	__syncthreads();
+	if (threadIdx.x == 0)
+	{
+		int t = 0;
+		for (int i = 0; i < kValidThreads / 32; ++i) t += s_warp[i];
+		out[blockIdx.x] = t;
+	}
 }
 
 } // namespace lcd
