@@ -155,6 +155,55 @@ int lcd_detector_set(lcd_engine * e, int detector, const lcd_gftt_params * param
 /* The selected detector; `params` (may be NULL) receives its GFTT parameters. */
 int lcd_detector_get(const lcd_engine * e, lcd_gftt_params * params);
 
+/* ---- detect: which keypoints of a frame are quantised (Memory::createSignature, Memory.cpp:5945-6100) ---------------------------
+ * With Mem/RawDescriptorsKept, an odometry pose and Kp/MaxFeatures < Vis/MaxFeatures, the reference detects Vis/MaxFeatures keypoints
+ * (Memory.cpp:5516-5538, :5725-5745) and keeps all of them in the signature (registration matches them all, Memory::getNi counts them,
+ * :4955-4968), but quantises only the Kp/MaxFeatures strongest:
+ *   gate   a frame with descriptors.rows < int(Kp/BadSignRatio * meanWordsPerLocation) (:5945-5947, :6051-6058) quantises nothing: a bad
+ *          signature, for which Rtabmap::process computes no likelihood;
+ *   limit  with more rows than Kp/MaxFeatures, Feature2D::limitKeypoints(keypoints, inliers, Kp/MaxFeatures, imageSize, ssc = false)
+ *          (Features2d.cpp:412-477) picks the rows: a std::multimap<fabs(response), index> walked in reverse, so the strongest first and,
+ *          among equal responses, the later index first (responses compared as bit patterns of their absolute value);
+ *   words  the picked rows go to addNewWords in ascending keypoint order (quantizedToRawIndices, :5954-6048); every other keypoint gets
+ *          a negative id, -1, -2, ... in keypoint order (:6070-6100).
+ * The limit is engine state, as lcd_detector_set.  Once set, every image-level call applies it to each frame: lcd_process_frames[_submit|
+ * _wait|_dev], lcd_map_detect_async + lcd_map_frame and lcd_shard_process_frames_dev.  lcd_orb_params.n_features stays the detection count
+ * (Vis/MaxFeatures when the caller's condition above holds).  word_ids_out keeps its [n_frames * n_features] shape: quantised rows carry
+ * their word ids, the other rows -1, -2, ..., padding rows 0.  The likelihood comes from the quantised words only; verification uses
+ * every detected row (descriptors, uv, xyz).  A bad frame gets a likelihood row of zeros, no hypothesis (0) and no registration (ok = 0,
+ * no matches).  In lcd_map_frame only quantised rows add references, ni(sig_id) grows by the keypoint count, and a bad frame creates
+ * no words and adds no references. */
+typedef struct lcd_quantize_limit {
+	int max_features;     /* Kp/MaxFeatures: quantise at most this many keypoints of a frame, the strongest (0 = all, the default) */
+	float bad_sign_ratio; /* Kp/BadSignRatio (0.5) */
+	int mean_words;       /* meanWordsPerLocation of Memory::update (Memory.cpp:5269-5278): Kp/MaxFeatures when > 0, the caller's
+	                         totalActiveReferences / treeSize otherwise, 0 with Mem/UseOdomFeatures.  0 = no bad-signature gate */
+} lcd_quantize_limit;
+/* Set the limit (NULL = {0, 0, 0}: every row quantised, no gate, every call as without this setting).  The gate's threshold is
+ * computed here once, as the reference does: (int)(bad_sign_ratio * (float)mean_words).  LCD_ERR_INVALID for a negative max_features or
+ * mean_words and for a bad_sign_ratio that is negative or not finite; the previous setting then stays.  A new engine holds {0, 0, 0}. */
+int lcd_quantize_limit_set(lcd_engine * e, const lcd_quantize_limit * p);
+int lcd_quantize_limit_get(const lcd_engine * e, lcd_quantize_limit * p);
+/* replaces: the gate and Feature2D::limitKeypoints(keypoints, inliers, ...) of Memory::createSignature (Memory.cpp:5945-6048,
+ * Features2d.cpp:412-477; tie rule above) for n_frames detected frames under the engine's limit: d_kp[n_frames][cap] (lcd_keypoint, as
+ * lcd_orb_detect_describe_dev writes them), d_n[n_frames], d_desc[n_frames][cap][row] (bytes of a binary engine, floats of a float
+ * engine).  Writes the quantised rows in ascending keypoint order, d_desc_out[n_frames][k][row] (zeros past a frame's count), their
+ * keypoint index d_index_out[n_frames][k] (quantizedToRawIndices; -1 past the count) and d_n_out[n_frames] (0 for a bad signature), with
+ * k = max_features > 0 ? min(max_features, cap) : cap.  lcd_localize_batch_dev has no per-frame counts: it quantises the zero rows of
+ * a frame with fewer than k quantised rows too, so a caller with such frames reads d_n_out (a bad signature is LCD_FRAME_SKIP for
+ * lcd_decide_batch_dev).  Asynchronous on `stream`.  LCD_ERR_INVALID for a null pointer or n_frames <= 0, LCD_ERR_CAPACITY for cap
+ * outside 1..4096. */
+int lcd_limit_keypoints_dev(lcd_engine * e, int n_frames, int cap, const lcd_keypoint * d_kp, const int * d_n, const void * d_desc,
+                            void * d_desc_out, int * d_index_out, int * d_n_out, void * stream);
+/* replaces: the word list assembly of Memory::createSignature (Memory.cpp:6070-6100).  Per-keypoint word ids d_words_out[n_frames][cap]
+ * from the k-strided ids of the quantised rows d_words_q[n_frames][k] (e.g. lcd_localize_batch_dev's output on d_desc_out): quantised
+ * rows take their id, the other rows of a frame -(1 + i - (quantised rows before i)), i.e. -1, -2, ... in keypoint order, padding rows
+ * (i >= d_n[f]) 0.  d_index / d_n_quantised as lcd_limit_keypoints_dev wrote them.  This is what lcd_decide_epipolar_dev needs beside
+ * the frame's full uv.  Asynchronous on `stream`.  LCD_ERR_INVALID for a null pointer, n_frames <= 0 or k outside 1..cap,
+ * LCD_ERR_CAPACITY for cap outside 1..4096. */
+int lcd_word_ids_expand_dev(lcd_engine * e, int n_frames, int cap, int k, const int * d_n, const int * d_index, const int * d_n_quantised,
+                            const int * d_words_q, int * d_words_out, void * stream);
+
 /* ---- dictionary: VWDictionary ------------------------------------------------ */
 /* replaces: VWDictionary::addWord (VWDictionary.cpp:1554-1580) for n words whose ids
  * the caller chose (DB load, LTM reactivation).  Words become "not indexed" until

@@ -59,6 +59,11 @@ class GfttParams(C.Structure):
     _fields_ = [("quality_level", C.c_double), ("min_distance", C.c_double), ("block_size", C.c_int), ("use_harris", C.c_int), ("k", C.c_double)]
 
 
+class QuantizeLimit(C.Structure):
+    """lcd_quantize_limit (Kp/MaxFeatures, Kp/BadSignRatio, Memory's meanWordsPerLocation)."""
+    _fields_ = [("max_features", C.c_int), ("bad_sign_ratio", C.c_float), ("mean_words", C.c_int)]
+
+
 # lcd_detector_set; depth type of a ready-made CV_8UC1 mask (lcd_b200.h)
 DETECTOR_ORB, DETECTOR_GFTT_ORB = 2, 8
 DEPTH_MASK_U8 = 3
@@ -199,6 +204,10 @@ SIGNATURES = {
     "lcd_orb_last_path": (_I, [_P]),
     "lcd_detector_set": (_I, [_P, _I, _P]),
     "lcd_detector_get": (_I, [_P, _P]),
+    "lcd_quantize_limit_set": (_I, [_P, _P]),
+    "lcd_quantize_limit_get": (_I, [_P, _P]),
+    "lcd_limit_keypoints_dev": (_I, [_P, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
+    "lcd_word_ids_expand_dev": (_I, [_P, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
     "lcd_dict_add_words": (_I, [_P, _P, _P, _I]),
     "lcd_dict_remove_words": (_I, [_P, _P, _I]),
     "lcd_dict_update": (_I, [_P]),
@@ -830,6 +839,32 @@ class Engine:
         """(detector, GfttParams) currently selected"""
         p = GfttParams()
         return self._lib.lcd_detector_get(self._h, C.byref(p)), p
+
+    def set_quantize_limit(self, max_features: int = 0, bad_sign_ratio: float = 0.0, mean_words: int = 0):
+        """Memory::createSignature's split for every image-level call: quantise at most max_features (Kp/MaxFeatures) keypoints of a
+        frame, the strongest, and none of a frame with fewer than int(bad_sign_ratio * mean_words) keypoints (0, 0, 0: all of them)"""
+        self._check(self._lib.lcd_quantize_limit_set(self._h, C.byref(QuantizeLimit(int(max_features), float(bad_sign_ratio), int(mean_words)))))
+
+    @property
+    def quantize_limit(self):
+        """(max_features, bad_sign_ratio, mean_words) currently set"""
+        p = QuantizeLimit()
+        self._check(self._lib.lcd_quantize_limit_get(self._h, C.byref(p)))
+        return p.max_features, p.bad_sign_ratio, p.mean_words
+
+    def limit_keypoints_dev(self, n_frames: int, cap: int, d_kp: int, d_n: int, d_desc: int, d_desc_out: int, d_index_out: int, d_n_out: int,
+                            stream: int = 0):
+        """lcd_limit_keypoints_dev: the quantised rows of n_frames detected frames [n_frames][cap] under the engine's limit, compacted to
+        [n_frames][k] rows with their keypoint indices and counts (device pointers)"""
+        self._check(self._lib.lcd_limit_keypoints_dev(self._h, n_frames, cap, C.c_void_p(d_kp), C.c_void_p(d_n), C.c_void_p(d_desc),
+                                                       C.c_void_p(d_desc_out), C.c_void_p(d_index_out), C.c_void_p(d_n_out),
+                                                       C.c_void_p(stream or None)))
+
+    def word_ids_expand_dev(self, n_frames: int, cap: int, k: int, d_n: int, d_index: int, d_n_quantised: int, d_words_q: int, d_words_out: int,
+                            stream: int = 0):
+        """lcd_word_ids_expand_dev: per-keypoint word ids [n_frames][cap] from the k-strided ids of the quantised rows (device pointers)"""
+        self._check(self._lib.lcd_word_ids_expand_dev(self._h, n_frames, cap, k, C.c_void_p(d_n), C.c_void_p(d_index), C.c_void_p(d_n_quantised),
+                                                       C.c_void_p(d_words_q), C.c_void_p(d_words_out), C.c_void_p(stream or None)))
 
     def orb_overflow(self) -> bool:
         r = self._lib.lcd_orb_overflow(self._h)

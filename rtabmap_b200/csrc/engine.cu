@@ -26,6 +26,7 @@
 #include "match_bf.cuh"
 #include "orb.cuh"
 #include "gftt.cuh"
+#include "limit.cuh"
 
 #include <cuda.h>
 #include <dlfcn.h>
@@ -506,6 +507,11 @@ struct lcd_engine
 	int orb_path = 0;     // lcd_orb_last_path flags of the last detection
 	int detector = LCD_DETECTOR_ORB; // lcd_detector_set: what orb_run detects
 	lcd_gftt_params gftt{0.001, 7.0, 3, 0, 0.04};
+	// lcd_quantize_limit_set: the split of Memory::createSignature for every image-level call (limit.cuh); ql_gate = int(ratio * mean_words)
+	lcd_quantize_limit ql{0, 0.0f, 0};
+	int ql_gate = 0;
+	DevBuf<uint32_t> ql_desc;          // [frame][k] the quantised rows
+	DevBuf<int> ql_index, ql_n, ql_words; // [frame][k] their keypoint index, [frame] their count, [frame][k] their word ids
 	DevBuf<float> g_eig;
 	DevBuf<unsigned> g_max_key;
 	DevBuf<unsigned long long> g_keys;
@@ -2937,6 +2943,85 @@ int lcd_detector_get(const lcd_engine * e, lcd_gftt_params * params)
 	return e->detector;
 }
 
+// ---- the quantisation limit of Memory::createSignature (limit.cuh) ----------------------------------------------------------------
+int lcd_quantize_limit_set(lcd_engine * e, const lcd_quantize_limit * p)
+{
+	if (!e) return LCD_ERR_INVALID;
+	const lcd_quantize_limit q = p ? *p : lcd_quantize_limit{0, 0.0f, 0};
+	if (q.max_features < 0) LCD_FAIL(e, LCD_ERR_INVALID, "Kp/MaxFeatures must not be negative");
+	if (q.mean_words < 0) LCD_FAIL(e, LCD_ERR_INVALID, "meanWordsPerLocation must not be negative");
+	if (!(q.bad_sign_ratio >= 0.0f) || !std::isfinite(q.bad_sign_ratio)) LCD_FAIL(e, LCD_ERR_INVALID, "Kp/BadSignRatio must be finite and not negative");
+	e->ql = q;
+	e->ql_gate = static_cast<int>(q.bad_sign_ratio * static_cast<float>(q.mean_words)); // Memory.cpp:5947
+	return LCD_OK;
+}
+
+int lcd_quantize_limit_get(const lcd_engine * e, lcd_quantize_limit * p)
+{
+	if (!e || !p) return LCD_ERR_INVALID;
+	*p = e->ql;
+	return LCD_OK;
+}
+
+// rows a frame of `cap` keypoints quantises at most under the engine's limit
+static int limit_rows(const lcd_engine * e, int cap) { return e->ql.max_features > 0 ? std::min(e->ql.max_features, cap) : cap; }
+// whether the image-level calls split their frames (the default {0, 0, 0} does not: today's path, bit for bit)
+static bool limit_active(const lcd_engine * e) { return e->ql.max_features > 0 || e->ql_gate > 0; }
+
+static int launch_limit(lcd_engine * e, int n_frames, int cap, const OrbKeypoint * d_kp, const int * d_n, const uint32_t * d_desc, uint32_t * d_desc_out,
+                        int * d_index_out, int * d_n_out, cudaStream_t s)
+{
+	int pad = 1;
+	while (pad < cap) pad <<= 1;
+	limit_keypoints_kernel<<<n_frames, kLimitThreads, pad * sizeof(unsigned long long), s>>>(d_kp, d_n, d_desc, cap, e->nw, e->ql.max_features,
+	                                                                                         limit_rows(e, cap), e->ql_gate, d_desc_out, d_index_out, d_n_out);
+	LCD_CHECK_LAUNCH(e);
+	return LCD_OK;
+}
+
+static int launch_expand(lcd_engine * e, int n_frames, int cap, int k, const int * d_n, const int * d_index, const int * d_nq, const int * d_words_q,
+                         int * d_words_out, cudaStream_t s)
+{
+	word_ids_expand_kernel<<<dim3((cap + 255) / 256, n_frames), 256, 0, s>>>(cap, k, d_n, d_index, d_nq, d_words_q, d_words_out);
+	LCD_CHECK_LAUNCH(e);
+	return LCD_OK;
+}
+
+// the quantised rows of n_frames detected frames in the engine's ql_* buffers
+static int limit_to_engine(lcd_engine * e, int n_frames, int cap, const OrbKeypoint * d_kp, const int * d_n, const uint32_t * d_desc, cudaStream_t s)
+{
+	const size_t rows = static_cast<size_t>(n_frames) * limit_rows(e, cap);
+	LCD_CUDA(e, e->ql_desc.reserve(rows * e->nw, 0, false, s));
+	LCD_CUDA(e, e->ql_index.reserve(rows, 0, false, s));
+	LCD_CUDA(e, e->ql_words.reserve(rows, 0, false, s));
+	LCD_CUDA(e, e->ql_n.reserve(n_frames, 0, false, s));
+	return launch_limit(e, n_frames, cap, d_kp, d_n, d_desc, e->ql_desc.p, e->ql_index.p, e->ql_n.p, s);
+}
+
+int lcd_limit_keypoints_dev(lcd_engine * e, int n_frames, int cap, const lcd_keypoint * d_kp, const int * d_n, const void * d_desc, void * d_desc_out,
+                            int * d_index_out, int * d_n_out, void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (n_frames <= 0 || !d_kp || !d_n || !d_desc || !d_desc_out || !d_index_out || !d_n_out) LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
+	if (cap <= 0 || cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "cap must be 1..%d", kMaxFrameQueries);
+	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	return launch_limit(e, n_frames, cap, reinterpret_cast<const OrbKeypoint *>(d_kp), d_n, static_cast<const uint32_t *>(d_desc),
+	                    static_cast<uint32_t *>(d_desc_out), d_index_out, d_n_out, s);
+}
+
+int lcd_word_ids_expand_dev(lcd_engine * e, int n_frames, int cap, int k, const int * d_n, const int * d_index, const int * d_n_quantised,
+                            const int * d_words_q, int * d_words_out, void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (n_frames <= 0 || !d_n || !d_index || !d_n_quantised || !d_words_q || !d_words_out) LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
+	if (cap <= 0 || cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "cap must be 1..%d", kMaxFrameQueries);
+	if (k <= 0 || k > cap) LCD_FAIL(e, LCD_ERR_INVALID, "k must be 1..cap");
+	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	return launch_expand(e, n_frames, cap, k, d_n, d_index, d_n_quantised, d_words_q, d_words_out, s);
+}
+
 int lcd_orb_overflow(lcd_engine * e)
 {
 	if (!e) return LCD_ERR_INVALID;
@@ -3924,7 +4009,17 @@ static int process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d_im
 		d_like = e->d_like.p;
 	}
 	const uint32_t * d_q = reinterpret_cast<const uint32_t *>(e->o_desc.p);
-	LCD_TRY(localize_dev(e, d_q, n_frames, cap, incremental, nndr, cmp_new, d_sig_ids, ns, n_total, d_words, d_like, s, e->o_n.p));
+	if (limit_active(e))
+	{
+		// Memory::createSignature's split: quantise the strongest rows only, verify with every detected row
+		const int k = limit_rows(e, cap);
+		LCD_TRY(limit_to_engine(e, n_frames, cap, e->o_kp.p, e->o_n.p, d_q, s));
+		LCD_TRY(localize_dev(e, e->ql_desc.p, n_frames, k, incremental, nndr, cmp_new, d_sig_ids, ns, n_total, d_words ? e->ql_words.p : nullptr, d_like,
+		                     s, e->ql_n.p));
+		if (d_words) LCD_TRY(launch_expand(e, n_frames, cap, k, e->o_n.p, e->ql_index.p, e->ql_n.p, e->ql_words.p, d_words, s));
+	}
+	else
+		LCD_TRY(localize_dev(e, d_q, n_frames, cap, incremental, nndr, cmp_new, d_sig_ids, ns, n_total, d_words, d_like, s, e->o_n.p));
 	if (vp) LCD_TRY(verify_top_dev(e, d_q, e->o_uv.p, n_frames, cap, d_like, d_sig_ids, ns, vp, s, e->o_n.p, e->o_xyz.p));
 	return LCD_OK;
 }
@@ -5201,9 +5296,41 @@ int lcd_map_frame(lcd_engine * e, int sig_id, int incremental, float nndr, int n
 	LCD_CUDA(e, cudaStreamWaitEvent(s, ms.done, 0));
 	const int cap = ms.cap;
 	int n_new = 0, n_kp = 0;
-	// Memory::createSignature: quantise the frame's descriptors (they never leave the device), references for sig_id
-	int rc = quantize_dev(e, reinterpret_cast<const uint32_t *>(ms.desc.p), cap, -1, ms.n.p, sig_id, incremental, nndr, new_words_compared_together,
-	                      word_ids_out, &n_new, &n_kp, s);
+	bool bad = false;
+	int rc = LCD_OK;
+	if (!limit_active(e))
+	{
+		// Memory::createSignature: quantise the frame's descriptors (they never leave the device), references for sig_id
+		rc = quantize_dev(e, reinterpret_cast<const uint32_t *>(ms.desc.p), cap, -1, ms.n.p, sig_id, incremental, nndr, new_words_compared_together,
+		                  word_ids_out, &n_new, &n_kp, s);
+	}
+	else
+	{
+		// the same with the split (limit.cuh): the strongest rows are quantised, the others get -1, -2, ...; the references are those of
+		// the quantised words, ni grows by the keypoint count (Memory::getNi counts every word of the signature)
+		auto split = [&]() -> int {
+			LCD_CUDA(e, cudaEventSynchronize(ms.done));
+			n_kp = std::min(std::max(*ms.h_n.p, 0), cap);
+			bad = n_kp < e->ql_gate;
+			if (bad)
+			{
+				for (int i = 0; i < cap; ++i) word_ids_out[i] = i < n_kp ? -(1 + i) : 0;
+			}
+			else
+			{
+				const int k = limit_rows(e, cap);
+				LCD_TRY(limit_to_engine(e, 1, cap, ms.kp.p, ms.n.p, reinterpret_cast<const uint32_t *>(ms.desc.p), s));
+				LCD_CUDA(e, e->ql_words.reserve(cap, 0, false, s));
+				std::vector<int> words_q(k);
+				LCD_TRY(quantize_dev(e, e->ql_desc.p, k, -1, e->ql_n.p, 0, incremental, nndr, new_words_compared_together, words_q.data(), &n_new, nullptr, s));
+				LCD_TRY(launch_expand(e, 1, cap, k, ms.n.p, e->ql_index.p, e->ql_n.p, e->d_word_ids.p, e->ql_words.p, s));
+				LCD_CUDA(e, cudaMemcpyAsync(word_ids_out, e->ql_words.p, cap * sizeof(int), cudaMemcpyDeviceToHost, s));
+				LCD_CUDA(e, cudaStreamSynchronize(s));
+			}
+			return sig_id > 0 ? add_refs_impl(e, sig_id, word_ids_out, n_kp) : LCD_OK;
+		};
+		rc = split();
+	}
 	e->map_head ^= 1;
 	--e->map_busy;
 	ms.busy = false;
@@ -5215,8 +5342,9 @@ int lcd_map_frame(lcd_engine * e, int sig_id, int incremental, float nndr, int n
 	if (kp_out) LCD_CUDA(e, cudaMemcpyAsync(kp_out, ms.kp.p, static_cast<size_t>(n_kp) * sizeof(OrbKeypoint), cudaMemcpyDeviceToHost, s));
 	if (desc_out) LCD_CUDA(e, cudaMemcpyAsync(desc_out, ms.desc.p, static_cast<size_t>(n_kp) * 32, cudaMemcpyDeviceToHost, s));
 	if (xyz_out) LCD_CUDA(e, cudaMemcpyAsync(xyz_out, ms.xyz.p, static_cast<size_t>(n_kp) * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
-	// Memory::computeLikelihood against the working memory
-	if (likelihood_out && wm_sig_ids && ns > 0 && n_kp > 0) return lcd_index_score(e, word_ids_out, n_kp, wm_sig_ids, ns, n_total, likelihood_out);
+	// Memory::computeLikelihood against the working memory (Rtabmap::process computes none for a bad signature: zeros)
+	if (bad && likelihood_out && wm_sig_ids && ns > 0) std::fill(likelihood_out, likelihood_out + ns, 0.0f);
+	else if (likelihood_out && wm_sig_ids && ns > 0 && n_kp > 0) return lcd_index_score(e, word_ids_out, n_kp, wm_sig_ids, ns, n_total, likelihood_out);
 	LCD_CUDA(e, cudaStreamSynchronize(s));
 	return LCD_OK;
 }
@@ -5590,8 +5718,28 @@ int lcd_shard_process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d
 		                           e->o_n.p, e->o_xyz.p)
 		          : LCD_OK;
 	};
-	return shard_step(e, n_frames, cap, e->o_desc.p, e->o_n.p, orb, verify, incremental, nndr, new_words_compared_together, d_sig_ids, ns, n_total,
-	                  d_row_ids_global, last_word_id, d_word_ids_out, d_likelihood_out, s);
+	if (!limit_active(e))
+		return shard_step(e, n_frames, cap, e->o_desc.p, e->o_n.p, orb, verify, incremental, nndr, new_words_compared_together, d_sig_ids, ns, n_total,
+		                  d_row_ids_global, last_word_id, d_word_ids_out, d_likelihood_out, s);
+	// Memory::createSignature's split (limit.cuh): the exchanges and the search carry the k quantised rows of every frame; the word ids
+	// are expanded to every detected row and the verification matches them all
+	const int k = limit_rows(e, cap);
+	// shard_step takes the buffers' addresses before the detect hook runs: they get their size here (the hook's reserve is then a no-op)
+	LCD_CUDA(e, e->ql_desc.reserve(static_cast<size_t>(n_frames) * k * e->nw, 0, false, s));
+	LCD_CUDA(e, e->ql_index.reserve(static_cast<size_t>(n_frames) * k, 0, false, s));
+	LCD_CUDA(e, e->ql_words.reserve(static_cast<size_t>(n_frames) * k, 0, false, s));
+	LCD_CUDA(e, e->ql_n.reserve(n_frames, 0, false, s));
+	const ShardHook orb_limit = [&](cudaStream_t st) {
+		LCD_TRY(orb(st));
+		return limit_to_engine(e, n_frames, cap, e->o_kp.p, e->o_n.p, reinterpret_cast<const uint32_t *>(e->o_desc.p), st);
+	};
+	const ShardHook expand_verify = [&](cudaStream_t st) {
+		if (d_word_ids_out) LCD_TRY(launch_expand(e, n_frames, cap, k, e->o_n.p, e->ql_index.p, e->ql_n.p, e->ql_words.p, d_word_ids_out, st));
+		return verify(st);
+	};
+	return shard_step(e, n_frames, k, reinterpret_cast<const uint8_t *>(e->ql_desc.p), e->ql_n.p, orb_limit, expand_verify, incremental, nndr,
+	                  new_words_compared_together, d_sig_ids, ns, n_total, d_row_ids_global, last_word_id, d_word_ids_out ? e->ql_words.p : nullptr,
+	                  d_likelihood_out, s);
 }
 
 int lcd_shard_localize_batch_dev(lcd_engine * e, const void * d_queries, int n_frames, int nq_per_frame, int incremental, float nndr,

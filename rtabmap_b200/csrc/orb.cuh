@@ -1059,6 +1059,39 @@ orb_select_kernel(const OrbSelectArgs a)
 	}
 }
 
+// Key of Feature2D::limitKeypoints' multimap<fabs(response), index>, walked in reverse (Features2d.cpp:412-477): a descending sort
+// of these keys puts the strongest first and, among equal responses, the later index first.  The absolute value is taken on the bit
+// pattern, so no flush-to-zero mode can change the order; 0 (padding) sorts after every keypoint.
+__device__ __forceinline__ unsigned long long limit_key(float response, int index)
+{
+	return (static_cast<unsigned long long>(__float_as_uint(response) & 0x7FFFFFFFu) << 32) | static_cast<unsigned>(index + 1);
+}
+__device__ __forceinline__ int limit_key_index(unsigned long long k) { return static_cast<int>(k & 0xFFFFFFFFull) - 1; }
+
+// Block-wide bitonic sort of skey[0, pad) in descending order (pad a power of two; every thread of the block calls it).
+__device__ __forceinline__ void block_sort_desc(unsigned long long * skey, int pad)
+{
+	__syncthreads();
+	for (int k = 2; k <= pad; k <<= 1)
+		for (int j = k >> 1; j > 0; j >>= 1)
+		{
+			for (int idx = threadIdx.x; idx < pad; idx += blockDim.x)
+			{
+				const int ixj = idx ^ j;
+				if (ixj > idx)
+				{
+					const unsigned long long x = skey[idx], y = skey[ixj];
+					if ((x < y) == ((idx & k) == 0)) // descending
+					{
+						skey[idx] = y;
+						skey[ixj] = x;
+					}
+				}
+			}
+			__syncthreads();
+		}
+}
+
 // ---- K4: concatenate the levels of a frame and apply Feature2D::limitKeypoints -----------------------
 __global__ void __launch_bounds__(1024)
 orb_merge_kernel(const OrbKeypoint * __restrict__ level_kp, const int * __restrict__ level_n, int n_levels, int level_cap, int max_features,
@@ -1090,37 +1123,10 @@ orb_merge_kernel(const OrbKeypoint * __restrict__ level_kp, const int * __restri
 	// multimap<fabs(response), index> walked in reverse: strongest first, later index first among equals
 	int pad = 1;
 	while (pad < total) pad <<= 1;
-	for (int i = tid; i < pad; i += blockDim.x)
-	{
-		unsigned long long k = 0ull; // sorts last in descending order
-		if (i < total)
-		{
-			const float r = fabsf(src(i).response);
-			k = (static_cast<unsigned long long>(__float_as_uint(r)) << 32) | static_cast<unsigned>(i + 1);
-		}
-		skey[i] = k;
-	}
-	__syncthreads();
-	for (int k = 2; k <= pad; k <<= 1)
-		for (int j = k >> 1; j > 0; j >>= 1)
-		{
-			for (int idx = tid; idx < pad; idx += blockDim.x)
-			{
-				const int ixj = idx ^ j;
-				if (ixj > idx)
-				{
-					const unsigned long long x = skey[idx], y = skey[ixj];
-					if ((x < y) == ((idx & k) == 0)) // descending
-					{
-						skey[idx] = y;
-						skey[ixj] = x;
-					}
-				}
-			}
-			__syncthreads();
-		}
+	for (int i = tid; i < pad; i += blockDim.x) skey[i] = i < total ? limit_key(src(i).response, i) : 0ull;
+	block_sort_desc(skey, pad);
 	const int n = min(max_features, out_cap);
-	for (int i = tid; i < n; i += blockDim.x) out[static_cast<size_t>(frame) * out_cap + i] = src(static_cast<int>(skey[i] & 0xFFFFFFFFull) - 1);
+	for (int i = tid; i < n; i += blockDim.x) out[static_cast<size_t>(frame) * out_cap + i] = src(limit_key_index(skey[i]));
 	if (tid == 0) out_n[frame] = n;
 }
 
