@@ -315,8 +315,7 @@ struct lcd_engine
 	mutable std::mutex err_mu;                // lcd_orb_* may fail on another thread than the dictionary calls
 	cudaStream_t stream = nullptr;
 	cudaStream_t orb_stream = nullptr;        // host-buffer lcd_orb_detect_describe: its own stream, so that it overlaps lcd_dict_update
-	cudaStream_t copy_stream = nullptr;       // host -> device image chunks of lcd_process_frames
-	std::vector<cudaEvent_t> copy_events;     // one per chunk
+	cudaStream_t copy_stream = nullptr;       // host -> device images of lcd_process_frames and lcd_process_frames_submit
 	cudaEvent_t copy_fence = nullptr;
 	cudaStream_t aux_stream[4] = {nullptr, nullptr, nullptr, nullptr}; // fork/join side streams (coarse pyramid levels of the ORB selection)
 	cudaEvent_t aux_fork = nullptr, aux_blur_done = nullptr, aux_join[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -327,7 +326,8 @@ struct lcd_engine
 		DevBuf<unsigned char> depth;
 		DevBuf<int> sig_ids;
 		PinBuf<PackedVerifyResult> res;
-		PinBuf<int> overflow;                  // ORB candidate overflow flag of the batch
+		PinBuf<int> overflow;                  // candidate overflow flag of the batch
+		int detector = LCD_DETECTOR_ORB;       // and the detector that set it
 		cudaEvent_t uploaded = nullptr, done = nullptr;
 		lcd_verify_result * user_results = nullptr;
 		int n_frames = 0;
@@ -552,6 +552,7 @@ struct lcd_engine
 		DevBuf<float> xyz;
 		DevBuf<int> n;
 		PinBuf<int> h_n, h_overflow;
+		int detector = LCD_DETECTOR_ORB;       // the detector that ran (h_overflow names its limit)
 		cudaEvent_t done = nullptr;
 		int cap = 0;
 		bool busy = false;
@@ -1431,7 +1432,6 @@ void lcd_destroy(lcd_engine * e)
 			cudaStreamDestroy(e->orb_stream);
 		}
 		if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
-		for (cudaEvent_t ev : e->copy_events) cudaEventDestroy(ev);
 		if (e->copy_fence) cudaEventDestroy(e->copy_fence);
 		if (e->dc_h_ev) cudaEventDestroy(e->dc_h_ev);
 		for (int i = 0; i < 4; ++i)
@@ -2474,7 +2474,7 @@ static int load_gauss7(lcd_engine * e, cudaStream_t s)
 	return LCD_OK;
 }
 
-// 3-D points and plain coordinates of the detected keypoints (pointers already at the first frame of the range)
+// 3-D points and plain coordinates of the detected keypoints
 static int orb_lift(lcd_engine * e, int n_frames, int width, int height, const void * d_depth, int depth_type, const lcd_orb_params * p, int cap,
                     const OrbKeypoint * d_kp, const int * d_n, float * d_xyz, float * d_uv, cudaStream_t s)
 {
@@ -2508,248 +2508,49 @@ static int orb_lift(lcd_engine * e, int n_frames, int width, int height, const v
 	return LCD_OK;
 }
 
-// GFTT/ORB (lcd_detector_set, Kp/DetectorStrategy=8): orb_run's inputs, outputs and frame ranges, one pyramid level.  Gray + mask
-// (orb_prepare*), corner map with the per-frame maximum, local maxima, per-frame sort, minDistance walk + ORB's border filter, then the
-// level-0 blur, the steered BRIEF descriptors and the 3-D points of the FAST path.
-static int gftt_run(lcd_engine * e, int n_frames, const uint8_t * d_images, int width, int height, int channels, const void * d_depth,
-                    int depth_type, const lcd_orb_params * p, int cap, OrbKeypoint * d_kp, uint8_t * d_desc, float * d_xyz, float * d_uv,
-                    int * d_n, cudaStream_t s, int frame0, int total_frames)
+// Gray + mask of every frame (orb_prepare*): the vectorised kernel where rows are whole 16-byte vectors and the height is even
+static int orb_prepare(lcd_engine * e, int n_frames, const OrbPrepArgs & a, cudaStream_t s)
 {
-	if (total_frames <= 0) total_frames = frame0 + n_frames;
-	if (!p) LCD_FAIL(e, LCD_ERR_INVALID, "null ORB parameters");
-	lcd_orb_params p1 = *p;
-	p1.n_levels = 1; // cv::ORB::compute builds the levels its keypoints use: GFTT corners are all octave 0
-	OrbGeom g{};
-	LCD_TRY(orb_geometry(e, width, height, &p1, g));
-	if (width % 2 || height % 2) LCD_FAIL(e, LCD_ERR_INVALID, "GFTT/ORB needs an even image width and height");
-	if (channels != 1 && channels != 3) LCD_FAIL(e, LCD_ERR_INVALID, "images must be 8UC1 or 8UC3 (BGR)");
-	if (cap <= 0 || cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "cap must be 1..%d", kMaxFrameQueries);
-	if (!d_depth) depth_type = LCD_DEPTH_NONE;
-	if (depth_type < LCD_DEPTH_NONE || depth_type > LCD_DEPTH_MASK_U8) LCD_FAIL(e, LCD_ERR_INVALID, "unknown depth type %d", depth_type);
-	const bool use_mask = depth_type == LCD_DEPTH_MASK_U8 || (depth_type != LCD_DEPTH_NONE && p->depth_as_mask);
-	const size_t px = static_cast<size_t>(width) * height;
-	const size_t pyr = static_cast<size_t>(total_frames) * g.frame_stride;
-	LCD_CUDA(e, e->o_gray.reserve(pyr, 0, false, s));
-	LCD_CUDA(e, e->o_blur.reserve(pyr, 0, false, s));
-	if (use_mask) LCD_CUDA(e, e->o_mask.reserve(pyr, 0, false, s));
-	LCD_CUDA(e, e->g_eig.reserve(static_cast<size_t>(total_frames) * px, 0, false, s));
-	LCD_CUDA(e, e->g_max_key.reserve(total_frames, 0, false, s));
-	LCD_CUDA(e, e->g_count.reserve(total_frames, 0, false, s));
-	LCD_CUDA(e, e->g_keys.reserve(static_cast<size_t>(total_frames) * kGfttCandCap, 0, false, s));
-	const int bitmap_words = (width + 31) / 32;
-	const size_t bitmap_bytes = static_cast<size_t>(bitmap_words) * height * sizeof(uint32_t);
-	const bool bitmap_smem = bitmap_bytes <= static_cast<size_t>(kGfttBitmapSmem);
-	if (!bitmap_smem) LCD_CUDA(e, e->g_bitmap.reserve(static_cast<size_t>(total_frames) * bitmap_words * height, 0, false, s));
-	if (frame0 == 0)
+	const int width = a.g.w[0], height = a.g.h[0];
+	const bool aligned = ((reinterpret_cast<uintptr_t>(a.images) | reinterpret_cast<uintptr_t>(a.depth) | reinterpret_cast<uintptr_t>(a.gray) |
+	                       reinterpret_cast<uintptr_t>(a.mask)) & 15u) == 0 && a.g.frame_stride % 16 == 0;
+	if (width % 8 == 0 && height % 2 == 0 && aligned && env_int("LCD_ORB_PREP_VEC", 1) != 0)
 	{
-		LCD_CUDA(e, e->o_overflow.reserve(1, 0, true, s));
-		LCD_CUDA(e, zero_fill_async(e->o_overflow.p, sizeof(int), s));
+		e->orb_path |= 4;
+		dim3 blk(16, 16), grd((width / 8 + 15) / 16, (height / 2 + 15) / 16, n_frames);
+		orb_prepare_vec_kernel<<<grd, blk, 0, s>>>(a);
 	}
-	if (!d_kp)
+	else
 	{
-		LCD_CUDA(e, e->o_kp.reserve(static_cast<size_t>(total_frames) * cap, 0, false, s));
-		d_kp = e->o_kp.p;
+		dim3 blk(32, 8), grd(((width + 1) / 2 + 31) / 32, ((height + 1) / 2 + 7) / 8, n_frames);
+		orb_prepare_kernel<<<grd, blk, 0, s>>>(a);
 	}
-	if (!d_n)
-	{
-		LCD_CUDA(e, e->o_n.reserve(total_frames, 0, false, s));
-		d_n = e->o_n.p;
-	}
-	d_images += static_cast<size_t>(frame0) * px * channels;
-	if (d_depth) d_depth = static_cast<const unsigned char *>(d_depth) + static_cast<size_t>(frame0) * px * (depth_elem_bytes(depth_type));
-	uint8_t * const w_gray = e->o_gray.p + static_cast<size_t>(frame0) * g.frame_stride;
-	uint8_t * const w_blur = e->o_blur.p + static_cast<size_t>(frame0) * g.frame_stride;
-	uint8_t * const w_mask = use_mask ? e->o_mask.p + static_cast<size_t>(frame0) * g.frame_stride : nullptr;
-	float * const w_eig = e->g_eig.p + static_cast<size_t>(frame0) * px;
-	unsigned * const w_max_key = e->g_max_key.p + frame0;
-	int * const w_count = e->g_count.p + frame0;
-	unsigned long long * const w_keys = e->g_keys.p + static_cast<size_t>(frame0) * kGfttCandCap;
-	uint32_t * const w_bitmap = bitmap_smem ? nullptr : e->g_bitmap.p + static_cast<size_t>(frame0) * bitmap_words * height;
-	d_kp += static_cast<size_t>(frame0) * cap;
-	d_n += frame0;
-	if (d_desc) d_desc += static_cast<size_t>(frame0) * cap * 32;
-	if (d_xyz) d_xyz += static_cast<size_t>(frame0) * cap * 3;
-	if (d_uv) d_uv += static_cast<size_t>(frame0) * cap * 2;
-	LCD_TRY(load_gauss7(e, s));
-	prof_mark(e, LCD_PROF_ORB, s);
-	LCD_CUDA(e, zero_fill_async(w_max_key, n_frames * sizeof(unsigned), s));
-	LCD_CUDA(e, zero_fill_async(w_count, n_frames * sizeof(int), s));
-	e->orb_path = 8;
-	{
-		OrbPrepArgs a{};
-		a.images = d_images;
-		a.channels = channels;
-		a.depth = use_mask ? d_depth : nullptr;
-		a.depth_type = depth_type;
-		a.min_depth = p->min_depth;
-		a.max_depth = p->max_depth;
-		a.gray = w_gray;
-		a.mask = w_mask;
-		a.g = g;
-		const bool aligned = ((reinterpret_cast<uintptr_t>(d_images) | reinterpret_cast<uintptr_t>(a.depth) | reinterpret_cast<uintptr_t>(w_gray) |
-		                       reinterpret_cast<uintptr_t>(w_mask)) & 15u) == 0 && g.frame_stride % 16 == 0;
-		if (width % 8 == 0 && aligned)
-		{
-			e->orb_path |= 4;
-			dim3 blk(16, 16), grd((width / 8 + 15) / 16, (height / 2 + 15) / 16, n_frames);
-			orb_prepare_vec_kernel<<<grd, blk, 0, s>>>(a);
-		}
-		else
-		{
-			dim3 blk(32, 8), grd(((width + 1) / 2 + 31) / 32, ((height + 1) / 2 + 7) / 8, n_frames);
-			orb_prepare_kernel<<<grd, blk, 0, s>>>(a);
-		}
-		LCD_CHECK_LAUNCH(e);
-	}
-	if (d_desc)
-	{
-		dim3 grd((width + kBlurTW - 1) / kBlurTW, (height + kBlurTH - 1) / kBlurTH, n_frames);
-		orb_blur_kernel<<<grd, 256, 0, s>>>(w_gray, w_blur, g, 0);
-		LCD_CHECK_LAUNCH(e);
-	}
-	{
-		GfttEigArgs a{w_gray, w_mask, width, height, g.frame_stride, w_eig, w_max_key};
-		gftt_eig_kernel<<<dim3((width + kGfttColTile - 1) / kGfttColTile, n_frames), 128, 0, s>>>(a);
-		LCD_CHECK_LAUNCH(e);
-	}
-	{
-		GfttCandArgs a{w_eig, w_mask, width, height, g.frame_stride, w_max_key, e->gftt.quality_level, w_keys, w_count, e->o_overflow.p};
-		gftt_cand_kernel<<<dim3((width + 31) / 32, (height + 7) / 8, n_frames), dim3(32, 8), 0, s>>>(a);
-		LCD_CHECK_LAUNCH(e);
-	}
-	{
-		const int smem = kGfttSortChunk * static_cast<int>(sizeof(unsigned long long));
-		LCD_CUDA(e, cudaFuncSetAttribute(gftt_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-		gftt_sort_kernel<<<n_frames, 1024, smem, s>>>(w_keys, w_count);
-		LCD_CHECK_LAUNCH(e);
-	}
-	{
-		GfttSelectArgs a{};
-		a.keys = w_keys;
-		a.count = w_count;
-		a.w = width;
-		a.h = height;
-		a.min_distance = e->gftt.min_distance;
-		a.max_corners = p->n_features;
-		a.edge = p->edge_threshold;
-		a.bitmap_words = bitmap_words;
-		a.bitmap = w_bitmap;
-		a.kps = d_kp;
-		a.n_kp = d_n;
-		a.cap = cap;
-		const int smem = (bitmap_smem && a.min_distance >= 1.0) ? static_cast<int>(bitmap_bytes) : 0;
-		LCD_CUDA(e, cudaFuncSetAttribute(gftt_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kGfttBitmapSmem));
-		gftt_select_kernel<<<n_frames, 256, smem, s>>>(a);
-		LCD_CHECK_LAUNCH(e);
-	}
-	if (d_desc)
-	{
-		dim3 grd((cap + kOrbDescribeKp - 1) / kOrbDescribeKp, n_frames);
-		if (g.edge >= kOrbPatchR && width % 4 == 0)
-		{
-			e->orb_path |= 2;
-			orb_describe_patch_kernel<<<grd, 256, 0, s>>>(w_blur, g, d_kp, d_n, cap, d_desc);
-		}
-		else
-			orb_describe_kernel<<<grd, 256, 0, s>>>(w_gray, w_blur, g, d_kp, d_n, cap, d_desc);
-		LCD_CHECK_LAUNCH(e);
-	}
-	LCD_TRY(orb_lift(e, n_frames, width, height, d_depth, depth_type, p, cap, d_kp, d_n, d_xyz, d_uv, s));
-	prof_mark(e, LCD_PROF_ORB, s);
+	LCD_CHECK_LAUNCH(e);
 	return LCD_OK;
 }
 
-// Detect + describe frames [frame0, frame0 + n_frames) of a batch of total_frames (total_frames = 0: the range is the whole
-// batch).  Every input, workspace and output pointer addresses frame 0 of the batch; ranges are independent, so the host
-// path runs them chunk by chunk while the next chunk's images are still on their way over PCIe.
-static int orb_run(lcd_engine * e, int n_frames, const uint8_t * d_images, int width, int height, int channels, const void * d_depth,
-                   int depth_type, const lcd_orb_params * p, int cap, OrbKeypoint * d_kp, uint8_t * d_desc, float * d_xyz, float * d_uv,
-                   int * d_n, cudaStream_t s, int frame0 = 0, int total_frames = 0)
+// ORB's keypoints: gray + mask, the coarser pyramid levels, FAST + selection per level, merged into n_features keypoints per frame.  With
+// `blur`, the blurred pyramid that feeds the descriptors runs on a side stream under them and s waits for it before returning.
+static int fast_pyramid(lcd_engine * e, int n_frames, const OrbPrepArgs & prep, int n_features, bool blur, OrbKeypoint * d_kp, int * d_n, int cap,
+                        cudaStream_t s)
 {
-	if (e->detector == LCD_DETECTOR_GFTT_ORB)
-		return gftt_run(e, n_frames, d_images, width, height, channels, d_depth, depth_type, p, cap, d_kp, d_desc, d_xyz, d_uv, d_n, s, frame0,
-		                total_frames);
-	if (total_frames <= 0) total_frames = frame0 + n_frames;
-	OrbGeom g{};
-	LCD_TRY(orb_geometry(e, width, height, p, g));
-	if (channels != 1 && channels != 3) LCD_FAIL(e, LCD_ERR_INVALID, "images must be 8UC1 or 8UC3 (BGR)");
-	if (cap <= 0 || cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "cap must be 1..%d", kMaxFrameQueries);
-	if (!d_depth) depth_type = LCD_DEPTH_NONE;
-	if (depth_type < LCD_DEPTH_NONE || depth_type > LCD_DEPTH_MASK_U8) LCD_FAIL(e, LCD_ERR_INVALID, "unknown depth type %d", depth_type);
-	const bool use_mask = depth_type == LCD_DEPTH_MASK_U8 || (depth_type != LCD_DEPTH_NONE && p->depth_as_mask);
-	const size_t pyr = static_cast<size_t>(total_frames) * g.frame_stride;
-	LCD_CUDA(e, e->o_gray.reserve(pyr, 0, false, s));
-	LCD_CUDA(e, e->o_blur.reserve(pyr, 0, false, s));
-	if (use_mask) LCD_CUDA(e, e->o_mask.reserve(pyr, 0, false, s));
-	const int slots = n_frames * g.n_levels, total_slots = total_frames * g.n_levels, slot0 = frame0 * g.n_levels;
+	const OrbGeom & g = prep.g;
+	const int slots = n_frames * g.n_levels;
 	int level_cap = 0;
 	for (int l = 0; l < g.n_levels; ++l) level_cap = std::max(level_cap, g.n_per_level[l] + 256);
-	LCD_CUDA(e, e->o_cand.reserve(static_cast<size_t>(total_slots) * kOrbCandCap, 0, false, s));
-	LCD_CUDA(e, e->o_cand_count.reserve(total_slots, 0, false, s));
-	LCD_CUDA(e, e->o_level_n.reserve(total_slots, 0, false, s));
-	LCD_CUDA(e, e->o_level_kp.reserve(static_cast<size_t>(total_slots) * level_cap, 0, false, s));
-	if (frame0 == 0)
-	{
-		// the "candidate list truncated" flag of this batch: cleared here, read back by the host entry points
-		LCD_CUDA(e, e->o_overflow.reserve(1, 0, true, s));
-		LCD_CUDA(e, zero_fill_async(e->o_overflow.p, sizeof(int), s));
-	}
-	if (!d_kp)
-	{
-		LCD_CUDA(e, e->o_kp.reserve(static_cast<size_t>(total_frames) * cap, 0, false, s));
-		d_kp = e->o_kp.p;
-	}
-	if (!d_n)
-	{
-		LCD_CUDA(e, e->o_n.reserve(total_frames, 0, false, s));
-		d_n = e->o_n.p;
-	}
-	// pointers of the range
-	const size_t px = static_cast<size_t>(width) * height;
-	d_images += static_cast<size_t>(frame0) * px * channels;
-	if (d_depth) d_depth = static_cast<const unsigned char *>(d_depth) + static_cast<size_t>(frame0) * px * (depth_elem_bytes(depth_type));
-	uint8_t * const w_gray = e->o_gray.p + static_cast<size_t>(frame0) * g.frame_stride;
-	uint8_t * const w_blur = e->o_blur.p + static_cast<size_t>(frame0) * g.frame_stride;
-	uint8_t * const w_mask = use_mask ? e->o_mask.p + static_cast<size_t>(frame0) * g.frame_stride : nullptr;
-	uint32_t * const w_cand = e->o_cand.p + static_cast<size_t>(slot0) * kOrbCandCap;
-	int * const w_cand_count = e->o_cand_count.p + slot0;
-	int * const w_level_n = e->o_level_n.p + slot0;
-	OrbKeypoint * const w_level_kp = e->o_level_kp.p + static_cast<size_t>(slot0) * level_cap;
-	d_kp += static_cast<size_t>(frame0) * cap;
-	d_n += frame0;
-	if (d_desc) d_desc += static_cast<size_t>(frame0) * cap * 32;
-	if (d_xyz) d_xyz += static_cast<size_t>(frame0) * cap * 3;
-	if (d_uv) d_uv += static_cast<size_t>(frame0) * cap * 2;
-	LCD_TRY(load_gauss7(e, s));
-	prof_mark(e, LCD_PROF_ORB, s);
+	LCD_CUDA(e, e->o_cand.reserve(static_cast<size_t>(slots) * kOrbCandCap, 0, false, s));
+	LCD_CUDA(e, e->o_cand_count.reserve(slots, 0, false, s));
+	LCD_CUDA(e, e->o_level_n.reserve(slots, 0, false, s));
+	LCD_CUDA(e, e->o_level_kp.reserve(static_cast<size_t>(slots) * level_cap, 0, false, s));
+	uint8_t * const w_gray = prep.gray;
+	uint8_t * const w_blur = e->o_blur.p;
+	uint8_t * const w_mask = prep.mask;
+	uint32_t * const w_cand = e->o_cand.p;
+	int * const w_cand_count = e->o_cand_count.p;
+	int * const w_level_n = e->o_level_n.p;
+	OrbKeypoint * const w_level_kp = e->o_level_kp.p;
 	LCD_CUDA(e, zero_fill_async(w_cand_count, slots * sizeof(int), s));
-	{
-		OrbPrepArgs a{};
-		a.images = d_images;
-		a.channels = channels;
-		a.depth = use_mask ? d_depth : nullptr;
-		a.depth_type = depth_type;
-		a.min_depth = p->min_depth;
-		a.max_depth = p->max_depth;
-		a.gray = w_gray;
-		a.mask = w_mask;
-		a.g = g;
-		const bool aligned = ((reinterpret_cast<uintptr_t>(d_images) | reinterpret_cast<uintptr_t>(a.depth) | reinterpret_cast<uintptr_t>(w_gray) |
-		                       reinterpret_cast<uintptr_t>(w_mask)) & 15u) == 0 && g.frame_stride % 16 == 0;
-		e->orb_path = 0;
-		if (width % 8 == 0 && height % 2 == 0 && aligned && env_int("LCD_ORB_PREP_VEC", 1) != 0)
-		{
-			e->orb_path |= 4;
-			dim3 blk(16, 16), grd((width / 8 + 15) / 16, (height / 2 + 15) / 16, n_frames);
-			orb_prepare_vec_kernel<<<grd, blk, 0, s>>>(a);
-		}
-		else
-		{
-			dim3 blk(32, 8), grd(((width + 1) / 2 + 31) / 32, ((height + 1) / 2 + 7) / 8, n_frames);
-			orb_prepare_kernel<<<grd, blk, 0, s>>>(a);
-		}
-		LCD_CHECK_LAUNCH(e);
-	}
+	LCD_TRY(orb_prepare(e, n_frames, prep, s));
 	for (int l = 2; l < g.n_levels; ++l)
 	{
 		dim3 blk(32, 8), grd((g.w[l] + 31) / 32, (g.h[l] + 7) / 8, n_frames);
@@ -2775,7 +2576,7 @@ static int orb_run(lcd_engine * e, int n_frames, const uint8_t * d_images, int w
 	e->orb_tma_used = tma_ok ? 1 : 0;
 	if (tma_ok) e->orb_path |= 1;
 	LCD_CUDA(e, cudaEventRecord(e->aux_fork, s));
-	if (d_desc)
+	if (blur)
 	{
 		// the blurred pyramid only feeds the descriptors: it runs on a side stream under FAST and the (latency-bound) selection
 		cudaStream_t bs = e->aux_stream[3];
@@ -2843,25 +2644,188 @@ static int orb_run(lcd_engine * e, int n_frames, const uint8_t * d_images, int w
 	{
 		int pad = 1;
 		while (pad < g.n_levels * level_cap) pad <<= 1;
-		orb_merge_kernel<<<n_frames, 1024, pad * sizeof(unsigned long long), s>>>(w_level_kp, w_level_n, g.n_levels, level_cap, p->n_features,
+		orb_merge_kernel<<<n_frames, 1024, pad * sizeof(unsigned long long), s>>>(w_level_kp, w_level_n, g.n_levels, level_cap, n_features,
 		                                                                          d_kp, d_n, cap);
 		LCD_CHECK_LAUNCH(e);
 	}
+	if (blur) LCD_CUDA(e, cudaStreamWaitEvent(s, e->aux_blur_done, 0));
+	return LCD_OK;
+}
+
+// GFTT/ORB's keypoints (lcd_detector_set, Kp/DetectorStrategy=8) on one pyramid level: gray + mask, the level-0 blur (with `blur`), the corner
+// map with the per-frame maximum, local maxima, per-frame sort, then the minDistance walk + ORB's border filter
+static int gftt_corners(lcd_engine * e, int n_frames, const OrbPrepArgs & prep, int n_features, bool blur, OrbKeypoint * d_kp, int * d_n, int cap,
+                        cudaStream_t s)
+{
+	const OrbGeom & g = prep.g;
+	const int width = g.w[0], height = g.h[0];
+	const int bitmap_words = (width + 31) / 32;
+	const size_t bitmap_bytes = static_cast<size_t>(bitmap_words) * height * sizeof(uint32_t);
+	const bool bitmap_smem = bitmap_bytes <= static_cast<size_t>(kGfttBitmapSmem);
+	LCD_CUDA(e, e->g_eig.reserve(static_cast<size_t>(n_frames) * width * height, 0, false, s));
+	LCD_CUDA(e, e->g_max_key.reserve(n_frames, 0, false, s));
+	LCD_CUDA(e, e->g_count.reserve(n_frames, 0, false, s));
+	LCD_CUDA(e, e->g_keys.reserve(static_cast<size_t>(n_frames) * kGfttCandCap, 0, false, s));
+	if (!bitmap_smem) LCD_CUDA(e, e->g_bitmap.reserve(static_cast<size_t>(n_frames) * bitmap_words * height, 0, false, s));
+	LCD_CUDA(e, zero_fill_async(e->g_max_key.p, n_frames * sizeof(unsigned), s));
+	LCD_CUDA(e, zero_fill_async(e->g_count.p, n_frames * sizeof(int), s));
+	LCD_TRY(orb_prepare(e, n_frames, prep, s));
+	if (blur)
+	{
+		dim3 grd((width + kBlurTW - 1) / kBlurTW, (height + kBlurTH - 1) / kBlurTH, n_frames);
+		orb_blur_kernel<<<grd, 256, 0, s>>>(prep.gray, e->o_blur.p, g, 0);
+		LCD_CHECK_LAUNCH(e);
+	}
+	{
+		GfttEigArgs a{prep.gray, prep.mask, width, height, g.frame_stride, e->g_eig.p, e->g_max_key.p};
+		gftt_eig_kernel<<<dim3((width + kGfttColTile - 1) / kGfttColTile, n_frames), 128, 0, s>>>(a);
+		LCD_CHECK_LAUNCH(e);
+	}
+	{
+		GfttCandArgs a{e->g_eig.p, prep.mask, width, height, g.frame_stride, e->g_max_key.p, e->gftt.quality_level, e->g_keys.p, e->g_count.p, e->o_overflow.p};
+		gftt_cand_kernel<<<dim3((width + 31) / 32, (height + 7) / 8, n_frames), dim3(32, 8), 0, s>>>(a);
+		LCD_CHECK_LAUNCH(e);
+	}
+	{
+		const int smem = kGfttSortChunk * static_cast<int>(sizeof(unsigned long long));
+		LCD_CUDA(e, cudaFuncSetAttribute(gftt_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+		gftt_sort_kernel<<<n_frames, 1024, smem, s>>>(e->g_keys.p, e->g_count.p);
+		LCD_CHECK_LAUNCH(e);
+	}
+	{
+		GfttSelectArgs a{};
+		a.keys = e->g_keys.p;
+		a.count = e->g_count.p;
+		a.w = width;
+		a.h = height;
+		a.min_distance = e->gftt.min_distance;
+		a.max_corners = n_features;
+		a.edge = g.edge;
+		a.bitmap_words = bitmap_words;
+		a.bitmap = bitmap_smem ? nullptr : e->g_bitmap.p;
+		a.kps = d_kp;
+		a.n_kp = d_n;
+		a.cap = cap;
+		const int smem = (bitmap_smem && a.min_distance >= 1.0) ? static_cast<int>(bitmap_bytes) : 0;
+		LCD_CUDA(e, cudaFuncSetAttribute(gftt_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kGfttBitmapSmem));
+		gftt_select_kernel<<<n_frames, 256, smem, s>>>(a);
+		LCD_CHECK_LAUNCH(e);
+	}
+	return LCD_OK;
+}
+
+// Detect + describe a batch of frames with the engine's detector (lcd_detector_set): the FAST pyramid or GFTT's corners between the
+// shared preparation and the steered BRIEF descriptors and 3-D points.  A null d_kp / d_n detects into the engine's own buffers.
+static int orb_run(lcd_engine * e, int n_frames, const uint8_t * d_images, int width, int height, int channels, const void * d_depth,
+                   int depth_type, const lcd_orb_params * p, int cap, OrbKeypoint * d_kp, uint8_t * d_desc, float * d_xyz, float * d_uv,
+                   int * d_n, cudaStream_t s)
+{
+	if (!p) LCD_FAIL(e, LCD_ERR_INVALID, "null ORB parameters");
+	const bool gftt = e->detector == LCD_DETECTOR_GFTT_ORB;
+	lcd_orb_params pl = *p;
+	if (gftt) pl.n_levels = 1; // cv::ORB::compute builds the levels its keypoints use: GFTT corners are all octave 0
+	OrbGeom g{};
+	LCD_TRY(orb_geometry(e, width, height, &pl, g));
+	if (gftt && (width % 2 || height % 2)) LCD_FAIL(e, LCD_ERR_INVALID, "GFTT/ORB needs an even image width and height");
+	if (channels != 1 && channels != 3) LCD_FAIL(e, LCD_ERR_INVALID, "images must be 8UC1 or 8UC3 (BGR)");
+	if (cap <= 0 || cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "cap must be 1..%d", kMaxFrameQueries);
+	if (!d_depth) depth_type = LCD_DEPTH_NONE;
+	if (depth_type < LCD_DEPTH_NONE || depth_type > LCD_DEPTH_MASK_U8) LCD_FAIL(e, LCD_ERR_INVALID, "unknown depth type %d", depth_type);
+	const bool use_mask = depth_type == LCD_DEPTH_MASK_U8 || (depth_type != LCD_DEPTH_NONE && p->depth_as_mask);
+	const size_t pyr = static_cast<size_t>(n_frames) * g.frame_stride;
+	LCD_CUDA(e, e->o_gray.reserve(pyr, 0, false, s));
+	LCD_CUDA(e, e->o_blur.reserve(pyr, 0, false, s));
+	if (use_mask) LCD_CUDA(e, e->o_mask.reserve(pyr, 0, false, s));
+	// the "candidate list truncated" flag of this batch: cleared here, read back by the host entry points
+	LCD_CUDA(e, e->o_overflow.reserve(1, 0, true, s));
+	LCD_CUDA(e, zero_fill_async(e->o_overflow.p, sizeof(int), s));
+	if (!d_kp)
+	{
+		LCD_CUDA(e, e->o_kp.reserve(static_cast<size_t>(n_frames) * cap, 0, false, s));
+		d_kp = e->o_kp.p;
+	}
+	if (!d_n)
+	{
+		LCD_CUDA(e, e->o_n.reserve(n_frames, 0, false, s));
+		d_n = e->o_n.p;
+	}
+	LCD_TRY(load_gauss7(e, s));
+	prof_mark(e, LCD_PROF_ORB, s);
+	OrbPrepArgs prep{};
+	prep.images = d_images;
+	prep.channels = channels;
+	prep.depth = use_mask ? d_depth : nullptr;
+	prep.depth_type = depth_type;
+	prep.min_depth = p->min_depth;
+	prep.max_depth = p->max_depth;
+	prep.gray = e->o_gray.p;
+	prep.mask = use_mask ? e->o_mask.p : nullptr;
+	prep.g = g;
+	e->orb_path = gftt ? 8 : 0;
+	if (gftt)
+		LCD_TRY(gftt_corners(e, n_frames, prep, p->n_features, d_desc != nullptr, d_kp, d_n, cap, s));
+	else
+		LCD_TRY(fast_pyramid(e, n_frames, prep, p->n_features, d_desc != nullptr, d_kp, d_n, cap, s));
 	if (d_desc)
 	{
-		LCD_CUDA(e, cudaStreamWaitEvent(s, e->aux_blur_done, 0));
 		dim3 grd((cap + kOrbDescribeKp - 1) / kOrbDescribeKp, n_frames);
 		bool patch_ok = g.edge >= kOrbPatchR && env_int("LCD_ORB_PATCH", 1) != 0;
 		for (int l = 0; l < g.n_levels; ++l) patch_ok = patch_ok && g.w[l] % 4 == 0;
-		if (patch_ok) e->orb_path |= 2;
 		if (patch_ok)
-			orb_describe_patch_kernel<<<grd, 256, 0, s>>>(w_blur, g, d_kp, d_n, cap, d_desc);
+		{
+			e->orb_path |= 2;
+			orb_describe_patch_kernel<<<grd, 256, 0, s>>>(e->o_blur.p, g, d_kp, d_n, cap, d_desc);
+		}
 		else
-			orb_describe_kernel<<<grd, 256, 0, s>>>(w_gray, w_blur, g, d_kp, d_n, cap, d_desc);
+			orb_describe_kernel<<<grd, 256, 0, s>>>(e->o_gray.p, e->o_blur.p, g, d_kp, d_n, cap, d_desc);
 		LCD_CHECK_LAUNCH(e);
 	}
 	LCD_TRY(orb_lift(e, n_frames, width, height, d_depth, depth_type, p, cap, d_kp, d_n, d_xyz, d_uv, s));
 	prof_mark(e, LCD_PROF_ORB, s);
+	return LCD_OK;
+}
+
+// LCD_ERR_CAPACITY when orb_run's overflow flag is set: a frame had more candidates than `detector` keeps, and the message names its limit
+static int overflow_report(lcd_engine * e, int overflow, int detector)
+{
+	if (overflow && detector == LCD_DETECTOR_GFTT_ORB)
+		LCD_FAIL(e, LCD_ERR_CAPACITY, "more than %d GFTT candidates in a frame: raise GFTT/QualityLevel", kGfttCandCap);
+	if (overflow) LCD_FAIL(e, LCD_ERR_CAPACITY, "more than %d FAST corners in pyramid level 0 (half as many per further level): raise FAST/Threshold", kOrbCandCap);
+	return LCD_OK;
+}
+
+// The detection outputs of the image-level calls whose descriptors feed the dictionary search: a 32-byte binary engine, Kp/MaxFeatures
+// (cap) in 1..kMaxFrameQueries, room for n_frames frames and zeroed descriptors, so that the padding rows of short frames hold defined
+// bytes for the NN kernel.  uv may be null.
+static int frame_front_end(lcd_engine * e, int n_frames, int cap, DevBuf<OrbKeypoint> & kp, DevBuf<uint8_t> & desc, DevBuf<float> & xyz,
+                           DevBuf<float> * uv, DevBuf<int> & n, cudaStream_t s)
+{
+	if (e->cfg.desc_type != LCD_DESC_U8 || e->cfg.desc_dim != 32) LCD_FAIL(e, LCD_ERR_INVALID, "ORB descriptors need an engine with 32-byte binary descriptors");
+	if (cap <= 0 || cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "Kp/MaxFeatures must be 1..%d", kMaxFrameQueries);
+	const size_t rows = static_cast<size_t>(n_frames) * cap;
+	LCD_CUDA(e, kp.reserve(rows, 0, false, s));
+	LCD_CUDA(e, desc.reserve(rows * 32, 0, false, s));
+	LCD_CUDA(e, xyz.reserve(rows * 3, 0, false, s));
+	if (uv) LCD_CUDA(e, uv->reserve(rows * 2, 0, false, s));
+	LCD_CUDA(e, n.reserve(n_frames, 0, false, s));
+	LCD_CUDA(e, zero_fill_async(desc.p, rows * 32, s));
+	return LCD_OK;
+}
+
+// n_frames host frames, and their depth when there is one (depth_type becomes LCD_DEPTH_NONE without), into device buffers on s
+static int upload_frames(lcd_engine * e, int n_frames, int width, int height, int channels, const uint8_t * images, const void * depth, int & depth_type,
+                         DevBuf<uint8_t> & d_images, DevBuf<unsigned char> & d_depth, cudaStream_t s)
+{
+	const size_t px = static_cast<size_t>(n_frames) * width * height;
+	if (!depth) depth_type = LCD_DEPTH_NONE;
+	LCD_CUDA(e, d_images.reserve(px * channels, 0, false, s));
+	LCD_CUDA(e, cudaMemcpyAsync(d_images.p, images, px * channels, cudaMemcpyHostToDevice, s));
+	if (depth_type != LCD_DEPTH_NONE)
+	{
+		const size_t bytes = px * depth_elem_bytes(depth_type);
+		LCD_CUDA(e, d_depth.reserve(bytes, 0, false, s));
+		LCD_CUDA(e, cudaMemcpyAsync(d_depth.p, depth, bytes, cudaMemcpyHostToDevice, s));
+	}
 	return LCD_OK;
 }
 
@@ -2887,16 +2851,7 @@ int lcd_orb_detect_describe(lcd_engine * e, int n_frames, const uint8_t * images
 	if (!images || n_frames <= 0 || width <= 0 || height <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null image");
 	if (cap <= 0 || cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "cap must be 1..%d", kMaxFrameQueries);
 	cudaStream_t s = e->orb_stream; // not the dictionary's stream: this call may overlap lcd_dict_update (Memory.cpp:5284)
-	const size_t px = static_cast<size_t>(n_frames) * width * height;
-	LCD_CUDA(e, e->o_img.reserve(px * channels, 0, false, s));
-	LCD_CUDA(e, cudaMemcpyAsync(e->o_img.p, images, px * channels, cudaMemcpyHostToDevice, s));
-	if (!depth) depth_type = LCD_DEPTH_NONE;
-	const size_t dbytes = depth_elem_bytes(depth_type);
-	if (depth_type != LCD_DEPTH_NONE)
-	{
-		LCD_CUDA(e, e->o_depth.reserve(px * dbytes, 0, false, s));
-		LCD_CUDA(e, cudaMemcpyAsync(e->o_depth.p, depth, px * dbytes, cudaMemcpyHostToDevice, s));
-	}
+	LCD_TRY(upload_frames(e, n_frames, width, height, channels, images, depth, depth_type, e->o_img, e->o_depth, s));
 	const size_t rows = static_cast<size_t>(n_frames) * cap;
 	LCD_CUDA(e, e->o_kp.reserve(rows, 0, false, s));
 	LCD_CUDA(e, e->o_desc.reserve(rows * 32, 0, false, s));
@@ -2911,10 +2866,7 @@ int lcd_orb_detect_describe(lcd_engine * e, int n_frames, const uint8_t * images
 	int overflow = 0;
 	LCD_CUDA(e, cudaMemcpyAsync(&overflow, e->o_overflow.p, sizeof(int), cudaMemcpyDeviceToHost, s));
 	LCD_CUDA(e, cudaStreamSynchronize(s));
-	if (overflow && e->detector == LCD_DETECTOR_GFTT_ORB)
-		LCD_FAIL(e, LCD_ERR_CAPACITY, "more than %d GFTT candidates in a frame: raise GFTT/QualityLevel", kGfttCandCap);
-	if (overflow) LCD_FAIL(e, LCD_ERR_CAPACITY, "more than %d FAST corners in pyramid level 0 (half as many per further level): raise FAST/Threshold", kOrbCandCap);
-	return LCD_OK;
+	return overflow_report(e, overflow, e->detector);
 }
 
 int lcd_detector_set(lcd_engine * e, int detector, const lcd_gftt_params * params)
@@ -3941,68 +3893,13 @@ int lcd_process_batch_dev(lcd_engine * e, const void * d_queries, const float * 
 // images -> detect -> quantise -> score -> verify, all on device buffers
 static int process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d_images, int width, int height, int channels, const void * d_depth,
                               int depth_type, const lcd_orb_params * op, int incremental, float nndr, int cmp_new, const int * d_sig_ids, int ns,
-                              int n_total, const lcd_verify_params * vp, int * d_words, float * d_like, cudaStream_t s,
-                              const uint8_t * h_images = nullptr, const void * h_depth = nullptr)
+                              int n_total, const lcd_verify_params * vp, int * d_words, float * d_like, cudaStream_t s)
 {
 	if (!op) LCD_FAIL(e, LCD_ERR_INVALID, "null ORB parameters");
-	if (e->cfg.desc_type != LCD_DESC_U8 || e->cfg.desc_dim != 32) LCD_FAIL(e, LCD_ERR_INVALID, "ORB descriptors need an engine with 32-byte binary descriptors");
 	const int cap = op->n_features;
-	if (cap <= 0 || cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "Kp/MaxFeatures must be 1..%d", kMaxFrameQueries);
-	const size_t rows = static_cast<size_t>(n_frames) * cap;
-	LCD_CUDA(e, e->o_kp.reserve(rows, 0, false, s));
-	LCD_CUDA(e, e->o_desc.reserve(rows * 32, 0, false, s));
-	LCD_CUDA(e, e->o_xyz.reserve(rows * 3, 0, false, s));
-	LCD_CUDA(e, e->o_uv.reserve(rows * 2, 0, false, s));
-	LCD_CUDA(e, e->o_n.reserve(n_frames, 0, false, s));
-	// padding rows of short frames must hold defined bytes for the NN kernel
-	LCD_CUDA(e, zero_fill_async(e->o_desc.p, rows * 32, s));
-	if (!h_images)
-	{
-		LCD_TRY(orb_run(e, n_frames, d_images, width, height, channels, d_depth, depth_type, op, cap, e->o_kp.p, e->o_desc.p, e->o_xyz.p, e->o_uv.p,
-		                e->o_n.p, s));
-	}
-	else
-	{
-		// host frames: upload in chunks on the copy stream and run detect + describe on each chunk as soon as it has
-		// landed, so that the PCIe transfer of chunk c+1 hides behind the ORB kernels of chunk c
-		if (!e->copy_stream)
-		{
-			LCD_CUDA(e, cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
-			LCD_CUDA(e, cudaEventCreateWithFlags(&e->copy_fence, cudaEventDisableTiming));
-		}
-		const int chunk_env = env_int("LCD_UPLOAD_CHUNK", 0); // 0: one chunk (per-chunk ORB launches are latency-bound, measured: chunking only pays for very large batches)
-		const int chunk = chunk_env > 0 ? chunk_env : n_frames;
-		const int n_chunks = (n_frames + chunk - 1) / chunk;
-		while (static_cast<int>(e->copy_events.size()) < n_chunks)
-		{
-			cudaEvent_t ev;
-			LCD_CUDA(e, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-			e->copy_events.push_back(ev);
-		}
-		const size_t px = static_cast<size_t>(width) * height;
-		const size_t dbytes = depth_elem_bytes(depth_type);
-		// the device staging buffers may still be read by work queued on s (a previous call): order the copies after it
-		LCD_CUDA(e, cudaEventRecord(e->copy_fence, s));
-		LCD_CUDA(e, cudaStreamWaitEvent(e->copy_stream, e->copy_fence, 0));
-		for (int c = 0; c < n_chunks; ++c)
-		{
-			const int f0 = c * chunk, nf = std::min(chunk, n_frames - f0);
-			LCD_CUDA(e, cudaMemcpyAsync(const_cast<uint8_t *>(d_images) + f0 * px * channels, h_images + f0 * px * channels, nf * px * channels,
-			                            cudaMemcpyHostToDevice, e->copy_stream));
-			if (h_depth && d_depth)
-				LCD_CUDA(e, cudaMemcpyAsync(static_cast<unsigned char *>(const_cast<void *>(d_depth)) + f0 * px * dbytes,
-				                            static_cast<const unsigned char *>(h_depth) + f0 * px * dbytes, nf * px * dbytes, cudaMemcpyHostToDevice,
-				                            e->copy_stream));
-			LCD_CUDA(e, cudaEventRecord(e->copy_events[c], e->copy_stream));
-		}
-		for (int c = 0; c < n_chunks; ++c)
-		{
-			const int f0 = c * chunk, nf = std::min(chunk, n_frames - f0);
-			LCD_CUDA(e, cudaStreamWaitEvent(s, e->copy_events[c], 0));
-			LCD_TRY(orb_run(e, nf, d_images, width, height, channels, d_depth, depth_type, op, cap, e->o_kp.p, e->o_desc.p, e->o_xyz.p, e->o_uv.p,
-			                e->o_n.p, s, f0, n_frames));
-		}
-	}
+	LCD_TRY(frame_front_end(e, n_frames, cap, e->o_kp, e->o_desc, e->o_xyz, &e->o_uv, e->o_n, s));
+	LCD_TRY(orb_run(e, n_frames, d_images, width, height, channels, d_depth, depth_type, op, cap, e->o_kp.p, e->o_desc.p, e->o_xyz.p, e->o_uv.p,
+	                e->o_n.p, s));
 	if (!d_like)
 	{
 		LCD_CUDA(e, e->d_like.reserve(static_cast<size_t>(n_frames) * ns, 0, false, s));
@@ -4038,6 +3935,28 @@ int lcd_process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d_image
 	                          d_sig_ids, ns, n_total, vp, d_word_ids_out, d_likelihood_out, s);
 }
 
+// the host -> device stream of lcd_process_frames and lcd_process_frames_submit, and the event that orders it against the engine stream
+static int copy_stream_ready(lcd_engine * e)
+{
+	if (e->copy_stream) return LCD_OK;
+	LCD_CUDA(e, cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
+	LCD_CUDA(e, cudaEventCreateWithFlags(&e->copy_fence, cudaEventDisableTiming));
+	return LCD_OK;
+}
+
+// the per-frame results of lcd_process_frames / _submit that the caller asked for, queued on s: keypoint counts, word ids ([frame][rows /
+// n_frames]), likelihoods and, with verification, the hypotheses
+static int download_frames(lcd_engine * e, int n_frames, size_t rows, int ns, const lcd_verify_params * vp, int * n_kp_out, int * word_ids_out,
+                           float * likelihood_out, int * hypothesis_out, cudaStream_t s)
+{
+	if (n_kp_out) LCD_CUDA(e, cudaMemcpyAsync(n_kp_out, e->o_n.p, n_frames * sizeof(int), cudaMemcpyDeviceToHost, s));
+	if (word_ids_out) LCD_CUDA(e, cudaMemcpyAsync(word_ids_out, e->d_word_ids.p, rows * sizeof(int), cudaMemcpyDeviceToHost, s));
+	if (likelihood_out)
+		LCD_CUDA(e, cudaMemcpyAsync(likelihood_out, e->d_like.p, static_cast<size_t>(n_frames) * ns * sizeof(float), cudaMemcpyDeviceToHost, s));
+	if (vp && hypothesis_out) LCD_CUDA(e, cudaMemcpyAsync(hypothesis_out, e->d_hyp_id.p, n_frames * sizeof(int), cudaMemcpyDeviceToHost, s));
+	return LCD_OK;
+}
+
 int lcd_process_frames(lcd_engine * e, int n_frames, const uint8_t * images, int width, int height, int channels, const void * depth, int depth_type,
                        const lcd_orb_params * op, int incremental, float nndr, int new_words_compared_together, const int * sig_ids, int ns,
                        int n_total, const lcd_verify_params * vp, int * n_kp_out, int * word_ids_out, float * likelihood_out, int * hypothesis_out,
@@ -4049,36 +3968,28 @@ int lcd_process_frames(lcd_engine * e, int n_frames, const uint8_t * images, int
 	if (!sig_ids || ns <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "ids list is empty");
 	if (!op) LCD_FAIL(e, LCD_ERR_INVALID, "null ORB parameters");
 	cudaStream_t s = e->stream;
-	const size_t px = static_cast<size_t>(n_frames) * width * height;
-	LCD_CUDA(e, e->o_img.reserve(px * channels, 0, false, s));
-	if (!depth) depth_type = LCD_DEPTH_NONE;
-	if (depth_type != LCD_DEPTH_NONE)
-	{
-		const size_t dbytes = depth_elem_bytes(depth_type);
-		LCD_CUDA(e, e->o_depth.reserve(px * dbytes, 0, false, s));
-	}
-	// the frames themselves are uploaded chunk by chunk inside process_frames_dev, overlapped with detect + describe
 	const int cap = op->n_features;
 	const size_t rows = static_cast<size_t>(n_frames) * std::max(cap, 1);
 	LCD_CUDA(e, e->d_sig_ids.reserve(ns, 0, false, s));
 	LCD_CUDA(e, e->d_like.reserve(static_cast<size_t>(n_frames) * ns, 0, false, s));
 	LCD_CUDA(e, e->d_word_ids.reserve(rows, 0, false, s));
 	LCD_CUDA(e, cudaMemcpyAsync(e->d_sig_ids.p, sig_ids, ns * sizeof(int), cudaMemcpyHostToDevice, s));
+	// the frames go up on the copy stream.  The device images may still be read by work queued on s (a previous call), so the copies
+	// wait for it; s waits for the copies.  Each wait binds to the fence's latest record, so one event serves both directions.
+	LCD_TRY(copy_stream_ready(e));
+	LCD_CUDA(e, cudaEventRecord(e->copy_fence, s));
+	LCD_CUDA(e, cudaStreamWaitEvent(e->copy_stream, e->copy_fence, 0));
+	LCD_TRY(upload_frames(e, n_frames, width, height, channels, images, depth, depth_type, e->o_img, e->o_depth, e->copy_stream));
+	LCD_CUDA(e, cudaEventRecord(e->copy_fence, e->copy_stream));
+	LCD_CUDA(e, cudaStreamWaitEvent(s, e->copy_fence, 0));
 	LCD_TRY(process_frames_dev(e, n_frames, e->o_img.p, width, height, channels, depth_type != LCD_DEPTH_NONE ? e->o_depth.p : nullptr, depth_type, op,
-	                           incremental, nndr, new_words_compared_together, e->d_sig_ids.p, ns, n_total, vp, e->d_word_ids.p, e->d_like.p, s, images,
-	                           depth_type != LCD_DEPTH_NONE ? depth : nullptr));
-	if (n_kp_out) LCD_CUDA(e, cudaMemcpyAsync(n_kp_out, e->o_n.p, n_frames * sizeof(int), cudaMemcpyDeviceToHost, s));
-	if (word_ids_out) LCD_CUDA(e, cudaMemcpyAsync(word_ids_out, e->d_word_ids.p, rows * sizeof(int), cudaMemcpyDeviceToHost, s));
-	if (likelihood_out)
-		LCD_CUDA(e, cudaMemcpyAsync(likelihood_out, e->d_like.p, static_cast<size_t>(n_frames) * ns * sizeof(float), cudaMemcpyDeviceToHost, s));
-	if (vp && hypothesis_out) LCD_CUDA(e, cudaMemcpyAsync(hypothesis_out, e->d_hyp_id.p, n_frames * sizeof(int), cudaMemcpyDeviceToHost, s));
+	                           incremental, nndr, new_words_compared_together, e->d_sig_ids.p, ns, n_total, vp, e->d_word_ids.p, e->d_like.p, s));
+	LCD_TRY(download_frames(e, n_frames, rows, ns, vp, n_kp_out, word_ids_out, likelihood_out, hypothesis_out, s));
 	LCD_CUDA(e, e->h_overflow.reserve(1));
 	LCD_CUDA(e, cudaMemcpyAsync(e->h_overflow.p, e->o_overflow.p, sizeof(int), cudaMemcpyDeviceToHost, s));
 	if (vp && results) LCD_TRY(verify_download(e, n_frames, 0, results, nullptr, nullptr, s));
 	LCD_CUDA(e, cudaStreamSynchronize(s));
-	if (*e->h_overflow.p)
-		LCD_FAIL(e, LCD_ERR_CAPACITY, "more than %d FAST corners in pyramid level 0 (half as many per further level): raise FAST/Threshold", kOrbCandCap);
-	return LCD_OK;
+	return overflow_report(e, *e->h_overflow.p, e->detector);
 }
 
 // ---- pipelined host path: two batches in flight ------------------------------------------------------------
@@ -4096,19 +4007,12 @@ int lcd_process_frames_submit(lcd_engine * e, int n_frames, const uint8_t * imag
 	cudaStream_t s = e->stream;
 	const int slot = (e->flight_head + e->flights_busy) & 1;
 	lcd_engine::Flight & f = e->flights[slot];
-	if (!e->copy_stream)
-	{
-		LCD_CUDA(e, cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
-		LCD_CUDA(e, cudaEventCreateWithFlags(&e->copy_fence, cudaEventDisableTiming));
-	}
+	LCD_TRY(copy_stream_ready(e));
 	if (!f.uploaded)
 	{
 		LCD_CUDA(e, cudaEventCreateWithFlags(&f.uploaded, cudaEventDisableTiming));
 		LCD_CUDA(e, cudaEventCreateWithFlags(&f.done, cudaEventDisableTiming));
 	}
-	const size_t px = static_cast<size_t>(n_frames) * width * height;
-	if (!depth) depth_type = LCD_DEPTH_NONE;
-	const size_t dbytes = depth_elem_bytes(depth_type);
 	// upload on the copy stream: the slot's previous batch was waited for, so its staging buffers are free
 	static const int dbg_tl = env_int("LCD_DEBUG_TIMELINE", 0); // diagnostics: print each batch's upload / compute window at _wait
 	if (dbg_tl && !f.t_h0)
@@ -4124,13 +4028,7 @@ int lcd_process_frames_submit(lcd_engine * e, int n_frames, const uint8_t * imag
 		}
 	}
 	if (dbg_tl) cudaEventRecord(f.t_h0, e->copy_stream);
-	LCD_CUDA(e, f.img.reserve(px * channels, 0, false, e->copy_stream));
-	LCD_CUDA(e, cudaMemcpyAsync(f.img.p, images, px * channels, cudaMemcpyHostToDevice, e->copy_stream));
-	if (depth_type != LCD_DEPTH_NONE)
-	{
-		LCD_CUDA(e, f.depth.reserve(px * dbytes, 0, false, e->copy_stream));
-		LCD_CUDA(e, cudaMemcpyAsync(f.depth.p, depth, px * dbytes, cudaMemcpyHostToDevice, e->copy_stream));
-	}
+	LCD_TRY(upload_frames(e, n_frames, width, height, channels, images, depth, depth_type, f.img, f.depth, e->copy_stream));
 	// the signature id list rides on the copy stream too: a host -> device copy queued on the compute stream would sit in the
 	// same copy-engine queue as the next batch's images and serialise the two batches (measured)
 	LCD_CUDA(e, f.sig_ids.reserve(ns, 0, false, e->copy_stream));
@@ -4146,11 +4044,7 @@ int lcd_process_frames_submit(lcd_engine * e, int n_frames, const uint8_t * imag
 	if (dbg_tl) cudaEventRecord(f.t_c0, s);
 	LCD_TRY(process_frames_dev(e, n_frames, f.img.p, width, height, channels, depth_type != LCD_DEPTH_NONE ? f.depth.p : nullptr, depth_type, op,
 	                           incremental, nndr, new_words_compared_together, f.sig_ids.p, ns, n_total, vp, e->d_word_ids.p, e->d_like.p, s));
-	if (n_kp_out) LCD_CUDA(e, cudaMemcpyAsync(n_kp_out, e->o_n.p, n_frames * sizeof(int), cudaMemcpyDeviceToHost, s));
-	if (word_ids_out) LCD_CUDA(e, cudaMemcpyAsync(word_ids_out, e->d_word_ids.p, rows * sizeof(int), cudaMemcpyDeviceToHost, s));
-	if (likelihood_out)
-		LCD_CUDA(e, cudaMemcpyAsync(likelihood_out, e->d_like.p, static_cast<size_t>(n_frames) * ns * sizeof(float), cudaMemcpyDeviceToHost, s));
-	if (vp && hypothesis_out) LCD_CUDA(e, cudaMemcpyAsync(hypothesis_out, e->d_hyp_id.p, n_frames * sizeof(int), cudaMemcpyDeviceToHost, s));
+	LCD_TRY(download_frames(e, n_frames, rows, ns, vp, n_kp_out, word_ids_out, likelihood_out, hypothesis_out, s));
 	f.user_results = nullptr;
 	if (vp && results)
 	{
@@ -4161,6 +4055,7 @@ int lcd_process_frames_submit(lcd_engine * e, int n_frames, const uint8_t * imag
 		f.user_results = results;
 	}
 	f.n_frames = n_frames;
+	f.detector = e->detector;
 	LCD_CUDA(e, f.overflow.reserve(1));
 	LCD_CUDA(e, cudaMemcpyAsync(f.overflow.p, e->o_overflow.p, sizeof(int), cudaMemcpyDeviceToHost, s));
 	if (dbg_tl) cudaEventRecord(f.t_c1, s);
@@ -4189,9 +4084,7 @@ int lcd_process_frames_wait(lcd_engine * e)
 	f.user_results = nullptr;
 	e->flight_head ^= 1;
 	--e->flights_busy;
-	if (f.overflow.p && *f.overflow.p)
-		LCD_FAIL(e, LCD_ERR_CAPACITY, "more than %d FAST corners in pyramid level 0 (half as many per further level): raise FAST/Threshold", kOrbCandCap);
-	return LCD_OK;
+	return overflow_report(e, f.overflow.p ? *f.overflow.p : 0, f.detector);
 }
 
 int lcd_verify_top_dev(lcd_engine * e, const void * d_queries, const float * d_uv, int n_frames, int nq_per_frame, const float * d_likelihood,
@@ -5247,35 +5140,22 @@ int lcd_map_detect_async(lcd_engine * e, const uint8_t * image, int width, int h
 	if (!e) return LCD_ERR_INVALID;
 	LCD_TRY(set_device(e));
 	if (!image || width <= 0 || height <= 0 || !params) LCD_FAIL(e, LCD_ERR_INVALID, "null image");
-	if (e->cfg.desc_type != LCD_DESC_U8 || e->cfg.desc_dim != 32) LCD_FAIL(e, LCD_ERR_INVALID, "ORB descriptors need an engine with 32-byte binary descriptors");
 	if (e->map_busy >= 2) LCD_FAIL(e, LCD_ERR_STATE, "two detections are already in flight: call lcd_map_frame first");
 	const int cap = params->n_features;
-	if (cap <= 0 || cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "Kp/MaxFeatures must be 1..%d", kMaxFrameQueries);
 	lcd_engine::MapSlot & ms = e->map_slots[(e->map_head + e->map_busy) & 1];
 	cudaStream_t s = e->orb_stream;
 	if (!ms.done) LCD_CUDA(e, cudaEventCreateWithFlags(&ms.done, cudaEventDisableTiming));
-	const size_t px = static_cast<size_t>(width) * height;
-	if (!depth) depth_type = LCD_DEPTH_NONE;
-	LCD_CUDA(e, ms.img.reserve(px * channels, 0, false, s));
-	LCD_CUDA(e, cudaMemcpyAsync(ms.img.p, image, px * channels, cudaMemcpyHostToDevice, s));
-	if (depth_type != LCD_DEPTH_NONE)
-	{
-		LCD_CUDA(e, ms.depth.reserve(px * depth_elem_bytes(depth_type), 0, false, s));
-		LCD_CUDA(e, cudaMemcpyAsync(ms.depth.p, depth, px * depth_elem_bytes(depth_type), cudaMemcpyHostToDevice, s));
-	}
-	LCD_CUDA(e, ms.kp.reserve(cap, 0, false, s));
-	LCD_CUDA(e, ms.desc.reserve(static_cast<size_t>(cap) * 32, 0, false, s));
-	LCD_CUDA(e, ms.xyz.reserve(static_cast<size_t>(cap) * 3, 0, false, s));
-	LCD_CUDA(e, ms.n.reserve(1, 0, false, s));
+	LCD_TRY(frame_front_end(e, 1, cap, ms.kp, ms.desc, ms.xyz, nullptr, ms.n, s));
+	LCD_TRY(upload_frames(e, 1, width, height, channels, image, depth, depth_type, ms.img, ms.depth, s));
 	LCD_CUDA(e, ms.h_n.reserve(1));
 	LCD_CUDA(e, ms.h_overflow.reserve(1));
-	LCD_CUDA(e, zero_fill_async(ms.desc.p, static_cast<size_t>(cap) * 32, s)); // padding rows feed the NN kernel: defined bytes
 	LCD_TRY(orb_run(e, 1, ms.img.p, width, height, channels, depth_type != LCD_DEPTH_NONE ? ms.depth.p : nullptr, depth_type, params, cap, ms.kp.p, ms.desc.p,
 	                ms.xyz.p, nullptr, ms.n.p, s));
 	LCD_CUDA(e, cudaMemcpyAsync(ms.h_n.p, ms.n.p, sizeof(int), cudaMemcpyDeviceToHost, s));
 	LCD_CUDA(e, cudaMemcpyAsync(ms.h_overflow.p, e->o_overflow.p, sizeof(int), cudaMemcpyDeviceToHost, s));
 	LCD_CUDA(e, cudaEventRecord(ms.done, s));
 	ms.cap = cap;
+	ms.detector = e->detector;
 	ms.busy = true;
 	++e->map_busy;
 	return LCD_OK;
@@ -5335,8 +5215,7 @@ int lcd_map_frame(lcd_engine * e, int sig_id, int incremental, float nndr, int n
 	--e->map_busy;
 	ms.busy = false;
 	if (rc != LCD_OK) return rc;
-	if (*ms.h_overflow.p)
-		LCD_FAIL(e, LCD_ERR_CAPACITY, "more than %d FAST corners in pyramid level 0 (half as many per further level): raise FAST/Threshold", kOrbCandCap);
+	LCD_TRY(overflow_report(e, *ms.h_overflow.p, ms.detector));
 	if (n_kp_out) *n_kp_out = n_kp;
 	if (n_new_out) *n_new_out = n_new;
 	if (kp_out) LCD_CUDA(e, cudaMemcpyAsync(kp_out, ms.kp.p, static_cast<size_t>(n_kp) * sizeof(OrbKeypoint), cudaMemcpyDeviceToHost, s));
@@ -5696,22 +5575,14 @@ int lcd_shard_process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d
 	if (!e->comm) LCD_FAIL(e, LCD_ERR_STATE, "no communicator: call lcd_shard_comm_init first");
 	if (!d_images || n_frames <= 0 || !op || !d_sig_ids || ns <= 0 || !d_row_ids_global || !d_likelihood_out)
 		LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
-	if (e->cfg.desc_dim != 32) LCD_FAIL(e, LCD_ERR_INVALID, "ORB descriptors need an engine with 32-byte binary descriptors");
 	const int cap = op->n_features;
-	if (cap <= 0 || cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "Kp/MaxFeatures must be 1..%d", kMaxFrameQueries);
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
-	const size_t rows = static_cast<size_t>(n_frames) * cap;
-	LCD_CUDA(e, e->o_kp.reserve(rows, 0, false, s));
-	LCD_CUDA(e, e->o_desc.reserve(rows * 32, 0, false, s));
-	LCD_CUDA(e, e->o_xyz.reserve(rows * 3, 0, false, s));
-	LCD_CUDA(e, e->o_uv.reserve(rows * 2, 0, false, s));
-	LCD_CUDA(e, e->o_n.reserve(n_frames, 0, false, s));
+	LCD_TRY(frame_front_end(e, n_frames, cap, e->o_kp, e->o_desc, e->o_xyz, &e->o_uv, e->o_n, s));
 	LCD_CUDA(e, e->d_like.reserve(static_cast<size_t>(n_frames) * ns, 0, false, s));
-	LCD_CUDA(e, zero_fill_async(e->o_desc.p, rows * 32, s)); // padding rows of short frames must hold defined bytes
 	// detect + describe the local frames, and after the likelihood verify their top hypothesis
 	const ShardHook orb = [&](cudaStream_t st) {
 		return orb_run(e, n_frames, d_images, width, height, channels, d_depth, depth_type, op, cap, e->o_kp.p, e->o_desc.p, e->o_xyz.p, e->o_uv.p, e->o_n.p,
-		               st, 0, n_frames);
+		               st);
 	};
 	const ShardHook verify = [&](cudaStream_t st) {
 		return vp ? verify_top_dev(e, reinterpret_cast<const uint32_t *>(e->o_desc.p), e->o_uv.p, n_frames, cap, d_likelihood_out, d_sig_ids, ns, vp, st,

@@ -15,6 +15,7 @@ from rtabmap_b200.capi import DEPTH_MASK_U8, DETECTOR_GFTT_ORB, DETECTOR_ORB
 pytestmark = pytest.mark.gpu
 K4 = synth.CAMERA_K4
 GOLDEN = Path(__file__).parent / "golden"
+LCD_ERR_CAPACITY = -3  # include/lcd_b200.h
 
 
 def gftt_engine(**kw):
@@ -121,16 +122,49 @@ def test_batch_position_does_not_matter():
         check_frame(a[i], gf.detect_describe_gftt(imgs[i], deps[i], K4, f2d.OrbParams()))
 
 
+def check_gftt_overflow(err):
+    assert err.value.code == LCD_ERR_CAPACITY
+    assert "65536 GFTT candidates" in str(err.value) and "GFTT/QualityLevel" in str(err.value) and "FAST" not in str(err.value), str(err.value)
+
+
 def test_candidate_overflow_is_reported():
+    """a frame with more local maxima than the candidate list holds: every image-level call fails with GFTT's limit, and the flag clears
+    on the next frame"""
     noise = np.random.default_rng(4).integers(0, 256, (1080, 1920), dtype=np.uint8)   # ~1 local maximum in 15 pixels: > 65 536
     eng = gftt_engine(min_distance=0.0)
-    with pytest.raises(LcdError):
+    with pytest.raises(LcdError) as err:
         eng.orb_detect_describe(noise[None], None, Engine.orb_params(K4))
+    check_gftt_overflow(err)
     assert eng.orb_overflow()
     img = synth.make_image(480, 640, 3)
     check_frame(eng.orb_detect_describe(img[None], None, Engine.orb_params(K4))[0],
                 gf.detect_describe_gftt(img, None, K4, f2d.OrbParams(), gf.GfttParams(min_distance=0.0)))
     assert not eng.orb_overflow()
+
+    # the calls that go on to the dictionary search, on a small dictionary and store
+    vocab = synth.make_binary_vocabulary(2048, 32, 1)
+    ids = np.arange(1, 2049, dtype=np.int32)
+    smap = synth.make_map(ids, 50, 200, seed=2)
+    eng = Engine(max_words=8192, max_signatures=400)
+    eng.add_words(ids, vocab)
+    eng.last_word_id = 2048
+    eng.update()
+    eng.load_csr(smap.word_ids, smap.row_ptr, smap.sig, smap.cnt)
+    eng.set_detector(DETECTOR_GFTT_ORB, Engine.gftt_params(min_distance=0.0))
+    op = Engine.orb_params(K4)
+    ns = len(smap.sig_ids)
+    with pytest.raises(LcdError) as err:
+        eng.process_frames(noise[None], None, op, smap.sig_ids, ns + 1)
+    check_gftt_overflow(err)
+    out = (np.zeros(1, np.int32), np.zeros((1, op.n_features), np.int32), np.zeros((1, ns), np.float32), np.zeros(1, np.int32), None)
+    eng.process_frames_submit(noise[None], None, op, smap.sig_ids, ns + 1, None, *out)
+    with pytest.raises(LcdError) as err:
+        eng.process_frames_wait()
+    check_gftt_overflow(err)
+    eng.map_detect_async(noise, None, op)
+    with pytest.raises(LcdError) as err:
+        eng.map_frame(ns + 1)
+    check_gftt_overflow(err)
 
 
 def test_switching_back_to_orb_and_parameters():

@@ -7,6 +7,7 @@ import pytest
 
 from oracle import feature2d_py as f2d
 from rtabmap_b200 import Engine, synth
+from rtabmap_b200.capi import DETECTOR_GFTT_ORB
 
 pytestmark = pytest.mark.gpu
 K4 = synth.CAMERA_K4
@@ -132,22 +133,32 @@ def test_orb_1280x720():
     check_frame(got, want)
 
 
-def test_orb_general_kernels_equal_the_fast_paths(monkeypatch):
-    """Every specialised kernel (TMA-staged FAST / blur, patch-staged descriptors, vectorised preparation) keeps its general predecessor
-    as the fallback for shapes it does not cover; with the specialisations switched off the output must not change by a bit."""
+def check_general_kernels_equal_the_fast_paths(monkeypatch, eng, fast_path, general_path):
     imgs = np.stack([synth.make_image(480, 640, 40 + i, bgr=True) for i in range(2)])
     depth = np.stack([synth.make_depth(480, 640, 50 + i) for i in range(2)])
-    eng = Engine()
     op = Engine.orb_params(K4)
     fast = eng.orb_detect_describe(imgs, depth, op)
-    assert eng.orb_last_path == 7
+    assert eng.orb_last_path == fast_path
     for name in ("LCD_ORB_TMA", "LCD_ORB_PATCH", "LCD_ORB_PREP_VEC"):
         monkeypatch.setenv(name, "0")
     general = eng.orb_detect_describe(imgs, depth, op)
-    assert eng.orb_last_path == 0
+    assert eng.orb_last_path == general_path
     for a, b in zip(fast, general):
         for x, y in zip(a, b):
             assert np.array_equal(np.nan_to_num(x).view(np.uint8), np.nan_to_num(y).view(np.uint8))
+
+
+def test_orb_general_kernels_equal_the_fast_paths(monkeypatch):
+    """Every specialised kernel (TMA-staged FAST / blur, patch-staged descriptors, vectorised preparation) keeps its general predecessor
+    as the fallback for shapes it does not cover; with the specialisations switched off the output must not change by a bit."""
+    check_general_kernels_equal_the_fast_paths(monkeypatch, Engine(), 7, 0)
+
+
+def test_gftt_general_kernels_equal_the_fast_paths(monkeypatch):
+    """GFTT/ORB (path bit 8) shares the preparation and the descriptors with ORB, and so their switches: the same bar"""
+    eng = Engine()
+    eng.set_detector(DETECTOR_GFTT_ORB)
+    check_general_kernels_equal_the_fast_paths(monkeypatch, eng, 14, 8)
 
 
 @pytest.mark.parametrize("hw", [(252, 332), (244, 324)])
