@@ -89,7 +89,7 @@ typedef struct lcd_orb_params {
 	int n_levels;         /* ORB/NLevels (1..4) */
 	float scale_factor;   /* ORB/ScaleFactor: 2.0 (the reference default) is the only value implemented */
 	int edge_threshold;   /* ORB/EdgeThreshold (19) */
-	int fast_threshold;   /* FAST/Threshold (20) */
+	int fast_threshold;   /* FAST/Threshold (20), 0..255 (cv::ORB wraps other values modulo 256; they are rejected here) */
 	int patch_size;       /* ORB/PatchSize: 31 (the learned rBRIEF pattern) */
 	float min_depth;      /* Kp/MinDepth */
 	float max_depth;      /* Kp/MaxDepth (0 = unlimited) */

@@ -2428,6 +2428,8 @@ static int orb_geometry(lcd_engine * e, int width, int height, const lcd_orb_par
 		LCD_FAIL(e, LCD_ERR_INVALID, "image size must be a multiple of 2^(levels-1)");
 	if (static_cast<long long>(width) * height >= (1 << 24)) LCD_FAIL(e, LCD_ERR_CAPACITY, "image too large");
 	if (p->n_features <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "Kp/MaxFeatures must be positive");
+	// FAST compares 8-bit differences; cv::ORB wraps other values modulo 256 rather than clamping them
+	if (p->fast_threshold < 0 || p->fast_threshold > 255) LCD_FAIL(e, LCD_ERR_INVALID, "FAST/Threshold must be 0..255");
 	g.n_levels = p->n_levels;
 	int off = 0;
 	for (int l = 0; l < p->n_levels; ++l)
@@ -2529,6 +2531,8 @@ static int orb_prepare(lcd_engine * e, int n_frames, const OrbPrepArgs & a, cuda
 	return LCD_OK;
 }
 
+static int fit_smem(lcd_engine * e, const void * kern, size_t dyn, int cap);
+
 // ORB's keypoints: gray + mask, the coarser pyramid levels, FAST + selection per level, merged into n_features keypoints per frame.  With
 // `blur`, the blurred pyramid that feeds the descriptors runs on a side stream under them and s waits for it before returning.
 static int fast_pyramid(lcd_engine * e, int n_frames, const OrbPrepArgs & prep, int n_features, bool blur, OrbKeypoint * d_kp, int * d_n, int cap,
@@ -2536,8 +2540,13 @@ static int fast_pyramid(lcd_engine * e, int n_frames, const OrbPrepArgs & prep, 
 {
 	const OrbGeom & g = prep.g;
 	const int slots = n_frames * g.n_levels;
-	int level_cap = 0;
-	for (int l = 0; l < g.n_levels; ++l) level_cap = std::max(level_cap, g.n_per_level[l] + 256);
+	// a level stores at most Kp/MaxFeatures keypoints (orb_select_kernel), and the merge sorts the stored keypoints of all levels of a
+	// frame in shared memory: 128 KB for 4 levels at the image-level calls' largest Kp/MaxFeatures; fit_smem checks any other size
+	static_assert(kOrbMaxLevels * kMaxFrameQueries * sizeof(unsigned long long) <= 128 * 1024, "merge keys of the largest frame");
+	const int level_cap = n_features;
+	int pad = 1;
+	while (pad < g.n_levels * level_cap) pad <<= 1;
+	LCD_TRY(fit_smem(e, reinterpret_cast<const void *>(orb_merge_kernel), pad * sizeof(unsigned long long), n_features));
 	LCD_CUDA(e, e->o_cand.reserve(static_cast<size_t>(slots) * kOrbCandCap, 0, false, s));
 	LCD_CUDA(e, e->o_cand_count.reserve(slots, 0, false, s));
 	LCD_CUDA(e, e->o_level_n.reserve(slots, 0, false, s));
@@ -2641,13 +2650,9 @@ static int fast_pyramid(lcd_engine * e, int n_frames, const OrbPrepArgs & prep, 
 		}
 		for (int l = 1; l < g.n_levels && l <= 3; ++l) LCD_CUDA(e, cudaStreamWaitEvent(s, e->aux_join[l - 1], 0));
 	}
-	{
-		int pad = 1;
-		while (pad < g.n_levels * level_cap) pad <<= 1;
-		orb_merge_kernel<<<n_frames, 1024, pad * sizeof(unsigned long long), s>>>(w_level_kp, w_level_n, g.n_levels, level_cap, n_features,
-		                                                                          d_kp, d_n, cap);
-		LCD_CHECK_LAUNCH(e);
-	}
+	orb_merge_kernel<<<n_frames, 1024, pad * sizeof(unsigned long long), s>>>(w_level_kp, w_level_n, g.n_levels, level_cap, n_features, d_kp, d_n,
+	                                                                          cap);
+	LCD_CHECK_LAUNCH(e);
 	if (blur) LCD_CUDA(e, cudaStreamWaitEvent(s, e->aux_blur_done, 0));
 	return LCD_OK;
 }

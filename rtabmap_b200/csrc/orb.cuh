@@ -774,6 +774,69 @@ __device__ inline int retain_best_replay(uint16_t * perm, const float * resp, in
 	return n_points + keep;
 }
 
+// The k strongest of perm[0, n) by Feature2D::limitKeypoints' key (|response| descending, the later position first among equals) moved to
+// perm[0, k) in their order: the k-th largest magnitude by a bitwise search over its 31 bits, then one stable compaction.  Segments of
+// <= 32 positions per thread as in partition_replay.  Called by all threads of the CTA; 0 < k < n.
+__device__ inline void keep_strongest_replay(uint16_t * perm, const float * resp, int n, int k, const SelectScratch & sc)
+{
+	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
+	const int seg = (n + static_cast<int>(blockDim.x) - 1) / static_cast<int>(blockDim.x);
+	const int b = tid * seg, e = min(b + seg, n);
+	auto mag = [&](int i) { return __float_as_uint(resp[perm[i]]) & 0x7FFFFFFFu; }; // limit_key's magnitude
+	uint32_t thr = 0u; // the largest t with #{mag >= t} >= k: the k-th largest magnitude
+	for (int bit = 30; bit >= 0; --bit)
+	{
+		const uint32_t t = thr | (1u << bit);
+		int c = 0;
+		for (int i = b; i < e; ++i) c += mag(i) >= t ? 1 : 0;
+		c = __reduce_add_sync(0xFFFFFFFFu, c);
+		if (lane == 0) sc.warp_tot[warp] = c;
+		__syncthreads();
+		int total = 0;
+		for (int w = 0; w < nwarps; ++w) total += sc.warp_tot[w];
+		__syncthreads();
+		if (total >= k) thr = t;
+	}
+	// every magnitude above thr is kept, and of those equal to it the last k - #{mag > thr}: block exclusive scan of (#gt | #eq << 16)
+	uint32_t mg = 0, me = 0;
+	for (int i = b; i < e; ++i)
+	{
+		const uint32_t m = mag(i);
+		mg |= (m > thr ? 1u : 0u) << (i - b);
+		me |= (m == thr ? 1u : 0u) << (i - b);
+	}
+	const int mine = __popc(mg) | (__popc(me) << 16);
+	int incl = mine;
+#pragma unroll
+	for (int o = 1; o < 32; o <<= 1)
+	{
+		const int t = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+		if (lane >= o) incl += t;
+	}
+	if (lane == 31) sc.warp_tot[warp] = incl;
+	__syncthreads();
+	int pre = 0, total = 0;
+	for (int w = 0; w < nwarps; ++w)
+	{
+		const int t = sc.warp_tot[w];
+		if (w < warp) pre += t;
+		total += t;
+	}
+	const int ex = pre + incl - mine;
+	const int skip = (total >> 16) - (k - (total & 0xFFFF)); // leading equal magnitudes that are dropped
+	int gt = ex & 0xFFFF, eq = ex >> 16;
+	for (int i = b; i < e; ++i)
+	{
+		const bool is_gt = (mg >> (i - b)) & 1u, is_eq = (me >> (i - b)) & 1u;
+		if (is_gt || (is_eq && eq >= skip)) sc.rpos[gt + max(eq - skip, 0)] = perm[i];
+		gt += is_gt;
+		eq += is_eq;
+	}
+	__syncthreads();
+	for (int i = tid; i < k; i += blockDim.x) perm[i] = sc.rpos[i];
+	__syncthreads();
+}
+
 __device__ __forceinline__ float fast_atan2_deg(float y, float x)
 {
 	const float K = static_cast<float>(180.0 / 3.141592653589793238462643383279502884197169399375);
@@ -806,8 +869,8 @@ struct OrbSelectArgs
 	const uint32_t * cand;
 	const int * cand_count;
 	OrbKeypoint * level_kp; // [n_frames][n_levels][level_cap]
-	int * level_n;          // [n_frames][n_levels]
-	int level_cap;
+	int * level_n;          // [n_frames][n_levels] keypoints the level keeps (level_kp holds at most level_cap of them)
+	int level_cap;          // Kp/MaxFeatures
 	int * overflow;         // set when a candidate list had to be truncated
 	int level;              // pyramid level this launch handles (one launch per level: shared memory is sized per level)
 	int cand_cap;           // candidates of this level kept in shared memory (<= kOrbCandCap)
@@ -987,12 +1050,16 @@ orb_select_kernel(const OrbSelectArgs a)
 	}
 	__syncthreads();
 	const int kept = retain_best_replay(perm, resp, m, n_level, sc);
-	m = min(kept, a.level_cap);
-	if (tid == 0)
+	// retainBest keeps every keypoint tied with its boundary response.  A level that keeps more than Kp/MaxFeatures makes the frame's
+	// total exceed it, so the merge cuts the frame to its Kp/MaxFeatures strongest, and only the level's own strongest by the same key can
+	// be among them: those are stored, in retainBest's order, and level_n holds the full count so that the merge still cuts.
+	m = kept;
+	if (kept > a.level_cap)
 	{
-		a.level_n[slot] = m;
-		if (kept > a.level_cap) atomicExch(a.overflow, 1);
+		keep_strongest_replay(perm, resp, kept, a.level_cap, sc);
+		m = a.level_cap;
 	}
+	if (tid == 0) a.level_n[slot] = kept;
 	// IC angle + output: one warp per keypoint, lane = column of the circular patch, so that a row of the patch is one coalesced load and
 	// the 31 rows are independent loads in flight (a thread per keypoint walked ~700 dependent byte loads).  The moments are integer sums:
 	// any summation order gives the reference's value.
@@ -1099,12 +1166,18 @@ orb_merge_kernel(const OrbKeypoint * __restrict__ level_kp, const int * __restri
 {
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	unsigned long long * skey = reinterpret_cast<unsigned long long *>(smem_raw); // [pad]
-	__shared__ int s_off[kOrbMaxLevels + 1];
+	__shared__ int s_off[kOrbMaxLevels + 1], s_kept;
 	const int frame = blockIdx.x, tid = threadIdx.x;
 	if (tid == 0)
 	{
+		// offsets of the stored keypoints; the cut below is decided on the levels' full counts (orb_select_kernel)
 		s_off[0] = 0;
-		for (int l = 0; l < n_levels; ++l) s_off[l + 1] = s_off[l] + level_n[frame * n_levels + l];
+		s_kept = 0;
+		for (int l = 0; l < n_levels; ++l)
+		{
+			s_off[l + 1] = s_off[l] + min(level_n[frame * n_levels + l], level_cap);
+			s_kept += level_n[frame * n_levels + l];
+		}
 	}
 	__syncthreads();
 	const int total = s_off[n_levels];
@@ -1113,7 +1186,7 @@ orb_merge_kernel(const OrbKeypoint * __restrict__ level_kp, const int * __restri
 		while (i >= s_off[l + 1]) ++l;
 		return level_kp[(static_cast<size_t>(frame) * n_levels + l) * level_cap + (i - s_off[l])];
 	};
-	if (max_features <= 0 || total <= max_features)
+	if (max_features <= 0 || s_kept <= max_features)
 	{
 		const int n = min(total, out_cap);
 		for (int i = tid; i < n; i += blockDim.x) out[static_cast<size_t>(frame) * out_cap + i] = src(i);
