@@ -289,7 +289,9 @@ int lcd_index_get_refs(lcd_engine * e, int word_id, int * sig, int * cnt, int ca
 /* replaces: the TF-IDF branch of Memory::computeLikelihood (Memory.cpp:2215-2291):
  * query_word_ids = the new signature's words (any order, duplicates and ids <= 0
  * allowed: uUniqueKeys + the *i>0 test are applied), sig_ids[ns] = the ids to score,
- * n_total = N = Memory::getSignatures().size().  likelihood_out[ns] float. */
+ * n_total = N = Memory::getSignatures().size().  likelihood_out[ns] float.
+ * Every call that takes n_total (this one, the localize, process, map and shard families) returns LCD_ERR_INVALID when
+ * n_total < 0; n_total = 0 gives 0 for every listed id, as the reference computes nothing when N is 0 (Memory.cpp:2250). */
 int lcd_index_score(lcd_engine * e, const int * query_word_ids, int nq,
                     const int * sig_ids, int ns, int n_total, float * likelihood_out);
 

@@ -1227,6 +1227,13 @@ int check_queries(lcd_engine * e, const void * q, int nq)
 	return LCD_OK;
 }
 
+// n_total is N = Memory::getSignatures().size(), a count: a negative one would give NaN idf terms, which the fixed-point sum turns into 0
+int check_n_total(lcd_engine * e, int n_total)
+{
+	if (n_total < 0) LCD_FAIL(e, LCD_ERR_INVALID, "n_total (the number of signatures, N) must be >= 0, got %d", n_total);
+	return LCD_OK;
+}
+
 // The similarity likelihood (Memory::computeLikelihood with Kp/TfIdfLikelihoodUsed=false) of n_frames frames whose word pairs the
 // resolve / prep kernel prepared (fill_pairs): word pairs, the global-descriptor dot products where the frames carry a descriptor
 // (d_gdesc [n_frames][gd_dim], or nullptr), then Signature::compareTo per (frame, k) into d_like [n_frames][ns].
@@ -2031,6 +2038,7 @@ int lcd_index_score(lcd_engine * e, const int * query_word_ids, int nq, const in
 	LCD_TRY(set_device(e));
 	if (!query_word_ids || nq <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "The signature is null");
 	if (!sig_ids || ns <= 0 || !likelihood_out) LCD_FAIL(e, LCD_ERR_INVALID, "ids list is empty");
+	LCD_TRY(check_n_total(e, n_total));
 	if (nq > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "at most %d words per signature", kMaxFrameQueries);
 	cudaStream_t s = e->stream;
 	LCD_CUDA(e, e->d_in_ids.reserve(nq, 0, false, s));
@@ -2235,6 +2243,7 @@ int lcd_localize_batch_dev(lcd_engine * e, const void * d_queries, int n_frames,
 	LCD_TRY(set_device(e));
 	if (!d_queries || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "Descriptors size is null!");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
+	LCD_TRY(check_n_total(e, n_total));
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
 	return localize_dev(e, static_cast<const uint32_t *>(d_queries), n_frames, nq_per_frame, incremental, nndr, new_words_compared_together,
 	                    d_sig_ids, ns, n_total, d_word_ids_out, d_likelihood_out, s);
@@ -2249,6 +2258,7 @@ int lcd_localize_batch(lcd_engine * e, const void * queries, int n_frames, int n
 	if (!queries || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "Descriptors size is null!");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
 	if (likelihood_out && (!sig_ids || ns <= 0)) LCD_FAIL(e, LCD_ERR_INVALID, "ids list is empty");
+	LCD_TRY(check_n_total(e, n_total));
 	cudaStream_t s = e->stream;
 	const size_t nq_total = static_cast<size_t>(n_frames) * nq_per_frame;
 	LCD_CUDA(e, e->d_queries.reserve(nq_total * e->nw, 0, false, s));
@@ -3890,6 +3900,7 @@ int lcd_process_batch_dev(lcd_engine * e, const void * d_queries, const float * 
 	LCD_TRY(set_device(e));
 	if (!d_queries || !d_uv || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "Descriptors size is null!");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
+	LCD_TRY(check_n_total(e, n_total));
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
 	return process_dev(e, static_cast<const uint32_t *>(d_queries), d_uv, n_frames, nq_per_frame, incremental, nndr, new_words_compared_together,
 	                   d_sig_ids, ns, n_total, vp, d_word_ids_out, d_likelihood_out, s);
@@ -3935,6 +3946,7 @@ int lcd_process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d_image
 	LCD_TRY(set_device(e));
 	if (!d_images || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null image");
 	if (!d_sig_ids || ns <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "ids list is empty");
+	LCD_TRY(check_n_total(e, n_total));
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
 	return process_frames_dev(e, n_frames, d_images, width, height, channels, d_depth, depth_type, op, incremental, nndr, new_words_compared_together,
 	                          d_sig_ids, ns, n_total, vp, d_word_ids_out, d_likelihood_out, s);
@@ -3972,6 +3984,7 @@ int lcd_process_frames(lcd_engine * e, int n_frames, const uint8_t * images, int
 	if (!images || n_frames <= 0 || width <= 0 || height <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null image");
 	if (!sig_ids || ns <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "ids list is empty");
 	if (!op) LCD_FAIL(e, LCD_ERR_INVALID, "null ORB parameters");
+	LCD_TRY(check_n_total(e, n_total));
 	cudaStream_t s = e->stream;
 	const int cap = op->n_features;
 	const size_t rows = static_cast<size_t>(n_frames) * std::max(cap, 1);
@@ -4009,6 +4022,7 @@ int lcd_process_frames_submit(lcd_engine * e, int n_frames, const uint8_t * imag
 	if (!sig_ids || ns <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "ids list is empty");
 	if (!op) LCD_FAIL(e, LCD_ERR_INVALID, "null ORB parameters");
 	if (e->flights_busy >= 2) LCD_FAIL(e, LCD_ERR_INVALID, "two batches are already in flight: call lcd_process_frames_wait first");
+	LCD_TRY(check_n_total(e, n_total));
 	cudaStream_t s = e->stream;
 	const int slot = (e->flight_head + e->flights_busy) & 1;
 	lcd_engine::Flight & f = e->flights[slot];
@@ -4142,6 +4156,7 @@ int lcd_process_batch(lcd_engine * e, const void * queries, const float * uv, in
 	if (!queries || !uv || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "Descriptors size is null!");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
 	if (!sig_ids || ns <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "ids list is empty");
+	LCD_TRY(check_n_total(e, n_total));
 	cudaStream_t s = e->stream;
 	const size_t nq_total = static_cast<size_t>(n_frames) * nq_per_frame;
 	LCD_CUDA(e, e->d_queries.reserve(nq_total * e->nw, 0, false, s));
@@ -4708,6 +4723,7 @@ int lcd_process_decide_batch_dev(lcd_engine * e, const void * d_queries, const f
 	LCD_TRY(set_device(e));
 	if (!d_queries || !d_uv || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "Descriptors size is null!");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
+	LCD_TRY(check_n_total(e, n_total));
 	LCD_TRY(check_verify_params(e, vp, true));
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
 	LCD_TRY(decide_prepare(e, n_frames, ns, clients, frame_flags, dp, s));
@@ -4943,6 +4959,7 @@ int lcd_shard_resolve_score_dev(lcd_engine * e, const void * d_queries, int n_fr
 	LCD_TRY(set_device(e));
 	if (!d_queries || !d_keys_gathered || !d_row_ids || n_frames <= 0 || n_ranks <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
+	LCD_TRY(check_n_total(e, n_total));
 	(void)total_rows_;
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
 	const bool score = d_scores_out != nullptr && ns > 0;
@@ -5010,6 +5027,7 @@ int lcd_shard_score_ids_dev(lcd_engine * e, const int * d_word_ids_all, int n_fr
 	LCD_TRY(set_device(e));
 	if (!d_word_ids_all || !d_sig_ids || !d_scores_out || n_frames <= 0 || ns <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d words per signature", kMaxFrameQueries);
+	LCD_TRY(check_n_total(e, n_total));
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
 	LCD_TRY(ensure_uq(e, n_frames, nq_per_frame, s));
 	LCD_TRY(ensure_acc(e, n_frames));
@@ -5174,6 +5192,7 @@ int lcd_map_frame(lcd_engine * e, int sig_id, int incremental, float nndr, int n
 	LCD_TRY(set_device(e));
 	if (e->map_busy <= 0) LCD_FAIL(e, LCD_ERR_STATE, "no detection in flight: call lcd_map_detect_async first");
 	if (!word_ids_out) LCD_FAIL(e, LCD_ERR_INVALID, "null output");
+	LCD_TRY(check_n_total(e, n_total)); // before the detection is taken: the call can be repeated with a valid N
 	lcd_engine::MapSlot & ms = e->map_slots[e->map_head];
 	cudaStream_t s = e->stream;
 	// Memory::preUpdate: the words of the previous frame join the index (VWDictionary::update)
@@ -5580,6 +5599,7 @@ int lcd_shard_process_frames_dev(lcd_engine * e, int n_frames, const uint8_t * d
 	if (!e->comm) LCD_FAIL(e, LCD_ERR_STATE, "no communicator: call lcd_shard_comm_init first");
 	if (!d_images || n_frames <= 0 || !op || !d_sig_ids || ns <= 0 || !d_row_ids_global || !d_likelihood_out)
 		LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
+	LCD_TRY(check_n_total(e, n_total));
 	const int cap = op->n_features;
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
 	LCD_TRY(frame_front_end(e, n_frames, cap, e->o_kp, e->o_desc, e->o_xyz, &e->o_uv, e->o_n, s));
@@ -5628,6 +5648,7 @@ int lcd_shard_localize_batch_dev(lcd_engine * e, const void * d_queries, int n_f
 	if (!d_queries || n_frames <= 0 || !d_sig_ids || ns <= 0 || !d_row_ids_global || !d_likelihood_out)
 		LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
+	LCD_TRY(check_n_total(e, n_total));
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
 	return shard_step(e, n_frames, nq_per_frame, static_cast<const uint8_t *>(d_queries), nullptr, ShardHook(), ShardHook(), incremental, nndr,
 	                  new_words_compared_together, d_sig_ids, ns, n_total, d_row_ids_global, last_word_id, d_word_ids_out, d_likelihood_out, s);

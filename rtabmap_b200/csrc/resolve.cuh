@@ -210,7 +210,8 @@ __device__ void score_prep(uint32_t * sbuf, int n_pad, int nq, const ResolveArgs
 				else
 				{
 					const float nw = static_cast<float>(plen + a.self_ref);
-					if (nw > 0.0f)
+					// the reference computes nothing when N is 0 (Memory.cpp:2250 `if(N)`): idf 0, the word adds nothing
+					if (nw > 0.0f && a.n_total != 0.0f)
 					{
 						// logNnw = log10(N/nw) on floats (Memory.cpp:2266)
 						idf = static_cast<float>(log10(static_cast<double>(__fdiv_rn(a.n_total, nw))));

@@ -12,8 +12,12 @@
 // reference's float term (nwi*logNnw)/ni, and accumulates it into a per-signature 2^-40
 // fixed-point int64 accumulator.  Integer accumulation is associative, so the result is
 // deterministic and independent of traversal order (and of how words are sharded across
-// GPUs); it differs from the reference's sequential float sum only by float rounding of the
-// running sum (<= ~1e-6 relative), inside the 1e-4 likelihood tolerance.
+// GPUs), and tests/tfidf_model.py reproduces it bit for bit.  It differs from the reference's
+// sequential float sum by the idf (log10f against the correctly rounded double log10: up to
+// 2 ulps with glibc), the float rounding of the reference's running sum and 2^-41 per term;
+// tests/tfidf_model.py derives that bound per signature (below the smallest single term in
+// nearly every signature at bench scale).  The int prefix of a frame's postings limits one
+// frame's query words to 2^31 postings in total; the arena itself holds up to 2^32.
 #pragma once
 #include "common.cuh"
 
