@@ -47,6 +47,7 @@
 #include <unordered_set>
 #include <utility>
 #include <chrono>
+#include <type_traits>
 #include <vector>
 
 using namespace lcd;
@@ -571,8 +572,8 @@ struct lcd_engine
 	bool sh_trace_armed = false;
 	std::vector<cudaEvent_t> sh_ring;  // [step][half][8 stage events + 1 begin/end]
 	DevBuf<uint8_t> sh_desc_all[2];
-	DevBuf<int> sh_n_all, sh_words_loc[2], sh_words_all[2];
-	DevBuf<uint32_t> sh_keys[2], sh_keys_mine[2];
+	DevBuf<int> sh_n_all, sh_words_loc, sh_words_all;
+	DevBuf<uint32_t> sh_keys[2], sh_keys_mine;
 	DevBuf<long long> sh_scores[2], sh_scores_loc[2];
 	DevBuf<int> sh_pairs[2], sh_pairs_loc[2]; // similarity variant: [rank][frames + 1][ns] pair counts + valid(s), and the local sums
 };
@@ -665,17 +666,6 @@ int ensure_sigs(lcd_engine * e, int max_sig)
 		LCD_CUDA(e, e->nvalid.reserve(e->ni.cap, old, true, e->stream));
 		e->h_ni.resize(e->ni.cap, 0);
 		e->h_nvalid.resize(e->ni.cap, 0);
-	}
-	return LCD_OK;
-}
-
-int ensure_acc(lcd_engine * e, int n_frames)
-{
-	const int stride = static_cast<int>(e->h_ni.size());
-	if (stride != e->acc_stride || e->acc.cap < static_cast<size_t>(stride) * n_frames)
-	{
-		LCD_CUDA(e, e->acc.reserve(static_cast<size_t>(std::max(stride, 1)) * n_frames, 0, false, e->stream));
-		e->acc_stride = stride;
 	}
 	return LCD_OK;
 }
@@ -1021,8 +1011,33 @@ int launch_resolve(lcd_engine * e, const ResolveArgs & a, int n_frames, cudaStre
 	return LCD_OK;
 }
 
-int ensure_uq(lcd_engine * e, int n_frames, int nq, cudaStream_t s, bool pairs = false)
+// The NNDR resolve of n_frames frames of nq descriptor rows (d_q) from the n_chunks top-2 key sets of nq_total queries each that run_knn
+// left in e->d_partial / e->d_partial64.  The sharded callers point the keys at the gathered sets (shard_set_keys).
+ResolveArgs resolve_args(const lcd_engine * e, const uint32_t * d_q, int nq, int nq_total, const int * d_nq_frame, int n_chunks, const int * row_ids,
+                         int incremental, float nndr, int cmp_new, int last_word_id, int * word_ids_out)
 {
+	ResolveArgs a{};
+	a.queries = d_q;
+	a.nq = nq;
+	a.nq_frame = d_nq_frame;
+	a.nq_total = nq_total;
+	a.partial = e->d_partial.p;
+	a.partial64 = e->d_partial64.p;
+	a.n_chunks = n_chunks;
+	a.row_ids = row_ids;
+	a.incremental = incremental;
+	a.nndr = nndr;
+	a.cmp_new = cmp_new;
+	a.last_word_id = last_word_id;
+	a.word_ids_out = word_ids_out;
+	return a;
+}
+
+// The set-up of the likelihood of n_frames frames of a.nq words each: the unique-word arrays (with `pairs`, the similarity likelihood's
+// word-pair arrays too) and the accumulator get their size, the accumulator is zeroed, and the preparation fields of `a` point at them.
+int score_begin(lcd_engine * e, ResolveArgs & a, int n_frames, int n_total, int self_ref, bool pairs, cudaStream_t s)
+{
+	const int nq = a.nq;
 	LCD_CUDA(e, e->uq_count.reserve(n_frames, 0, false, s));
 	LCD_CUDA(e, e->uq_word.reserve(static_cast<size_t>(n_frames) * nq, 0, false, s));
 	LCD_CUDA(e, e->uq_prefix.reserve(static_cast<size_t>(n_frames) * (nq + 1), 0, false, s));
@@ -1032,28 +1047,54 @@ int ensure_uq(lcd_engine * e, int n_frames, int nq, cudaStream_t s, bool pairs =
 		LCD_CUDA(e, e->uq_mult.reserve(static_cast<size_t>(n_frames) * nq, 0, false, s));
 		LCD_CUDA(e, e->q_valid.reserve(n_frames, 0, false, s));
 	}
-	return LCD_OK;
-}
-
-void fill_prep(lcd_engine * e, ResolveArgs & a, float n_total, int self_ref)
-{
+	const int stride = static_cast<int>(e->h_ni.size());
+	if (stride != e->acc_stride || e->acc.cap < static_cast<size_t>(stride) * n_frames)
+	{
+		LCD_CUDA(e, e->acc.reserve(static_cast<size_t>(std::max(stride, 1)) * n_frames, 0, false, e->stream));
+		e->acc_stride = stride;
+	}
+	LCD_CUDA(e, zero_fill_async(e->acc.p, static_cast<size_t>(e->acc_stride) * n_frames * sizeof(long long), s));
 	a.do_prep = 1;
 	a.post_len = e->post_len.p;
 	a.id_cap = static_cast<int>(e->h_len.size());
-	a.n_total = n_total;
+	a.n_total = static_cast<float>(n_total);
 	a.self_ref = self_ref;
 	a.uq_count = e->uq_count.p;
 	a.uq_word = e->uq_word.p;
 	a.uq_prefix = e->uq_prefix.p;
 	a.uq_idf = e->uq_idf.p;
+	if (pairs)
+	{
+		a.pairs = 1;
+		a.uq_mult = e->uq_mult.p;
+		a.q_valid = e->q_valid.p;
+	}
+	return LCD_OK;
 }
 
-// the preparation of the similarity likelihood's word pairs (after fill_prep; ensure_uq(..., pairs = true))
-void fill_pairs(lcd_engine * e, ResolveArgs & a)
+// The word-id layout of the sharded step, [rank][frames_per_rank][nq], of which frames [part_f0, part_f0 + part_frames) of every rank are
+// prepared
+struct ShardIds
 {
-	a.pairs = 1;
-	a.uq_mult = e->uq_mult.p;
-	a.q_valid = e->q_valid.p;
+	int frames_per_rank, part_f0, part_frames;
+};
+
+// The preparation of n_frames frames from their word ids d_ids [n_frames][nq], one CTA per frame after score_begin: prep_from_ids_kernel,
+// or with `local` (the sharded layout) prep_local_ids_kernel, which keeps only the ids with postings on this rank.
+int prep_ids(lcd_engine * e, const int * d_ids, int n_frames, int nq, int n_total, int self_ref, bool pairs, cudaStream_t s, const ShardIds * local = nullptr)
+{
+	ResolveArgs a{};
+	a.nq = nq;
+	LCD_TRY(score_begin(e, a, n_frames, n_total, self_ref, pairs, s));
+	int nq_pad = 32;
+	while (nq_pad < nq) nq_pad <<= 1;
+	const size_t smem = nq_pad * sizeof(uint32_t);
+	prof_mark(e, LCD_PROF_RESOLVE, s);
+	if (local) prep_local_ids_kernel<<<n_frames, kResolveThreads, smem, s>>>(d_ids, a, local->frames_per_rank, local->part_f0, local->part_frames);
+	else prep_from_ids_kernel<<<n_frames, kResolveThreads, smem, s>>>(d_ids, a);
+	prof_mark(e, LCD_PROF_RESOLVE, s);
+	LCD_CHECK_LAUNCH(e);
+	return LCD_OK;
 }
 
 int launch_score(lcd_engine * e, int n_frames, int nq, cudaStream_t s, bool pairs = false)
@@ -1076,6 +1117,35 @@ int launch_score(lcd_engine * e, int n_frames, int nq, cudaStream_t s, bool pair
 	if (pairs) score_kernel<true><<<grid, kScoreThreads, (nq + 1) * sizeof(int), s>>>(sa);
 	else score_kernel<false><<<grid, kScoreThreads, (nq + 1) * sizeof(int), s>>>(sa);
 	prof_mark(e, LCD_PROF_SCORE, s);
+	LCD_CHECK_LAUNCH(e);
+	return LCD_OK;
+}
+
+// The TF-IDF sums of n_frames prepared frames over the ns listed places, d_out [n_frames][ns]: the likelihood (float), or the exact
+// fixed-point sums (long long) that the sharded callers add up across ranks
+template <typename T>
+int score_tfidf(lcd_engine * e, int n_frames, int nq, const int * d_sig_ids, int ns, T * d_out, cudaStream_t s)
+{
+	LCD_TRY(launch_score(e, n_frames, nq, s));
+	const dim3 grid((ns + 255) / 256, n_frames);
+	const int sig_cap = static_cast<int>(e->h_ni.size());
+	if constexpr (std::is_same_v<T, float>) gather_likelihood_kernel<<<grid, 256, 0, s>>>(e->acc.p, e->acc_stride, sig_cap, d_sig_ids, ns, d_out);
+	else gather_fixed_kernel<<<grid, 256, 0, s>>>(e->acc.p, e->acc_stride, sig_cap, d_sig_ids, ns, d_out);
+	LCD_CHECK_LAUNCH(e);
+	return LCD_OK;
+}
+
+// The word pairs of n_frames prepared frames over the ns listed places: their counts into d_pairs (one free row after every rows_per_seg
+// frames, see gather_pairs_kernel), and this engine's valid(s) once per segment, at d_valid + segment * valid_stride
+int score_pairs(lcd_engine * e, int n_frames, int nq, const int * d_sig_ids, int ns, int rows_per_seg, int * d_pairs, int * d_valid, size_t valid_stride,
+                cudaStream_t s)
+{
+	LCD_TRY(launch_score(e, n_frames, nq, s, true));
+	gather_pairs_kernel<<<dim3((ns + 255) / 256, n_frames), 256, 0, s>>>(e->acc.p, e->acc_stride, static_cast<int>(e->h_ni.size()), d_sig_ids, ns,
+	                                                                  rows_per_seg, d_pairs);
+	LCD_CHECK_LAUNCH(e);
+	gather_valid_kernel<<<dim3((ns + 255) / 256, n_frames / rows_per_seg), 256, 0, s>>>(e->nvalid.p, static_cast<int>(e->h_nvalid.size()), d_sig_ids, ns,
+	                                                                                 d_valid, valid_stride);
 	LCD_CHECK_LAUNCH(e);
 	return LCD_OK;
 }
@@ -1235,7 +1305,7 @@ int check_n_total(lcd_engine * e, int n_total)
 }
 
 // The similarity likelihood (Memory::computeLikelihood with Kp/TfIdfLikelihoodUsed=false) of n_frames frames whose word pairs the
-// resolve / prep kernel prepared (fill_pairs): word pairs, the global-descriptor dot products where the frames carry a descriptor
+// resolve / prep kernel prepared (score_begin with pairs): word pairs, the global-descriptor dot products where the frames carry a descriptor
 // (d_gdesc [n_frames][gd_dim], or nullptr), then Signature::compareTo per (frame, k) into d_like [n_frames][ns].
 int launch_similarity(lcd_engine * e, int n_frames, int nq, const float * d_gdesc, const int * d_sig_ids, int ns, float * d_like, cudaStream_t s)
 {
@@ -1257,6 +1327,23 @@ int launch_similarity(lcd_engine * e, int n_frames, int nq, const float * d_gdes
 	return LCD_OK;
 }
 
+// The resolve of n_frames frames (a from resolve_args) and, when d_out and ns > 0 are given, the likelihood of the listed places from the
+// words it found: the TF-IDF sums (score_tfidf), or with `sim` (T = float) the similarity likelihood (launch_similarity, d_gdesc)
+template <typename T>
+int resolve_score(lcd_engine * e, ResolveArgs & a, int n_frames, int n_total, bool sim, const float * d_gdesc, const int * d_sig_ids, int ns, T * d_out,
+                  cudaStream_t s)
+{
+	const bool score = d_out != nullptr && ns > 0;
+	if (score) LCD_TRY(score_begin(e, a, n_frames, n_total, 1, sim, s));
+	LCD_TRY(launch_resolve(e, a, n_frames, s));
+	if (!score) return LCD_OK;
+	if constexpr (std::is_same_v<T, float>)
+	{
+		if (sim) return launch_similarity(e, n_frames, a.nq, d_gdesc, d_sig_ids, ns, d_out, s);
+	}
+	return score_tfidf(e, n_frames, a.nq, d_sig_ids, ns, d_out, s);
+}
+
 // which branch of Memory::computeLikelihood localize_dev scores with (Kp/TfIdfLikelihoodUsed)
 enum class LikelihoodKind
 {
@@ -1270,48 +1357,13 @@ int localize_dev(lcd_engine * e, const uint32_t * d_q, int n_frames, int nq, int
                  const int * d_sig_ids, int ns, int n_total, int * d_word_ids_out, float * d_like_out, cudaStream_t s,
                  const int * d_nq_frame = nullptr, LikelihoodKind kind = LikelihoodKind::TfIdf, const float * d_gdesc = nullptr)
 {
-	const bool sim = kind == LikelihoodKind::Similarity;
 	if (e->n_indexed == 0 && !incremental) LCD_FAIL(e, LCD_ERR_STATE, "Dictionary mode is set to fixed but no words are in it!");
 	LCD_TRY(require_unsharded(e, "localisation on one engine"));
 	const int nq_total = n_frames * nq;
 	int n_chunks = 0;
 	LCD_TRY(run_knn(e, d_q, nq_total, e->n_indexed, &n_chunks, s));
-	const bool score = d_like_out != nullptr && ns > 0;
-	ResolveArgs a{};
-	a.queries = d_q;
-	a.nq = nq;
-	a.nq_frame = d_nq_frame;
-	a.nq_total = nq_total;
-	a.partial = e->d_partial.p;
-	a.partial64 = e->d_partial64.p;
-	a.n_chunks = n_chunks;
-	a.row_ids = e->row_ids.p;
-	a.incremental = incremental;
-	a.nndr = nndr;
-	a.cmp_new = cmp_new;
-	a.last_word_id = e->last_word_id;
-	a.word_ids_out = d_word_ids_out;
-	a.n_new_out = nullptr;
-	a.pending_desc = nullptr;
-	a.pending_ids = nullptr;
-	if (score)
-	{
-		LCD_TRY(ensure_uq(e, n_frames, nq, s, sim));
-		LCD_TRY(ensure_acc(e, n_frames));
-		LCD_CUDA(e, zero_fill_async(e->acc.p, static_cast<size_t>(e->acc_stride) * n_frames * sizeof(long long), s));
-		fill_prep(e, a, static_cast<float>(n_total), 1);
-		if (sim) fill_pairs(e, a);
-	}
-	LCD_TRY(launch_resolve(e, a, n_frames, s));
-	if (score && sim) return launch_similarity(e, n_frames, nq, d_gdesc, d_sig_ids, ns, d_like_out, s);
-	if (score)
-	{
-		LCD_TRY(launch_score(e, n_frames, nq, s));
-		dim3 grid((ns + 255) / 256, n_frames);
-		gather_likelihood_kernel<<<grid, 256, 0, s>>>(e->acc.p, e->acc_stride, static_cast<int>(e->h_ni.size()), d_sig_ids, ns, d_like_out);
-		LCD_CHECK_LAUNCH(e);
-	}
-	return LCD_OK;
+	ResolveArgs a = resolve_args(e, d_q, nq, nq_total, d_nq_frame, n_chunks, e->row_ids.p, incremental, nndr, cmp_new, e->last_word_id, d_word_ids_out);
+	return resolve_score(e, a, n_frames, n_total, kind == LikelihoodKind::Similarity, d_gdesc, d_sig_ids, ns, d_like_out, s);
 }
 
 } // namespace
@@ -1781,24 +1833,11 @@ static int quantize_dev(lcd_engine * e, const uint32_t * d_q, int rows, int n_va
 	LCD_TRY(run_knn(e, d_q, rows, e->n_indexed, &n_chunks, s));
 	LCD_CUDA(e, e->d_word_ids.reserve(rows, 0, false, s));
 	LCD_CUDA(e, e->d_n_new.reserve(1, 0, false, s));
-	ResolveArgs a{};
-	a.queries = d_q;
-	a.nq = rows;
-	a.nq_total = rows;
-	a.nq_frame = n_valid < 0 ? d_n_valid : nullptr;
-	a.partial = e->d_partial.p;
-	a.partial64 = e->d_partial64.p;
-	a.n_chunks = n_chunks;
-	a.row_ids = e->row_ids.p;
-	a.incremental = incremental;
-	a.nndr = nndr;
-	a.cmp_new = cmp_new;
-	a.last_word_id = e->last_word_id;
-	a.word_ids_out = e->d_word_ids.p;
+	ResolveArgs a = resolve_args(e, d_q, rows, rows, n_valid < 0 ? d_n_valid : nullptr, n_chunks, e->row_ids.p, incremental, nndr, cmp_new, e->last_word_id,
+	                             e->d_word_ids.p);
 	a.n_new_out = e->d_n_new.p;
 	a.pending_desc = e->vocab.p + static_cast<size_t>(rows0) * e->nw;
 	a.pending_ids = e->row_ids.p + rows0;
-	a.do_prep = 0;
 	LCD_TRY(launch_resolve(e, a, 1, s));
 	int n_new = 0, nv = n_valid;
 	LCD_CUDA(e, cudaMemcpyAsync(word_ids_out, e->d_word_ids.p, rows * sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -1860,20 +1899,8 @@ int lcd_dict_find_nn(lcd_engine * e, const void * queries, int nq, int increment
 	LCD_TRY(run_knn(e, e->d_queries.p, nq, total_rows(e), &n_chunks, s));
 	LCD_CUDA(e, e->d_word_ids.reserve(nq, 0, false, s));
 	LCD_CUDA(e, e->d_n_new.reserve(1, 0, false, s));
-	ResolveArgs a{};
-	a.queries = e->d_queries.p;
-	a.nq = nq;
-	a.nq_total = nq;
-	a.partial = e->d_partial.p;
-	a.partial64 = e->d_partial64.p;
-	a.n_chunks = n_chunks;
-	a.row_ids = e->row_ids.p;
-	a.incremental = incremental;
-	a.nndr = nndr;
-	a.cmp_new = 0;
-	a.last_word_id = e->last_word_id;
+	ResolveArgs a = resolve_args(e, e->d_queries.p, nq, nq, nullptr, n_chunks, e->row_ids.p, incremental, nndr, 0, e->last_word_id, e->d_word_ids.p);
 	a.find_only = 1;
-	a.word_ids_out = e->d_word_ids.p;
 	a.n_new_out = e->d_n_new.p;
 	LCD_TRY(launch_resolve(e, a, 1, s));
 	LCD_CUDA(e, cudaMemcpyAsync(word_ids_out, e->d_word_ids.p, nq * sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -2046,19 +2073,8 @@ int lcd_index_score(lcd_engine * e, const int * query_word_ids, int nq, const in
 	LCD_CUDA(e, e->d_like.reserve(ns, 0, false, s));
 	LCD_CUDA(e, cudaMemcpyAsync(e->d_in_ids.p, query_word_ids, nq * sizeof(int), cudaMemcpyHostToDevice, s));
 	LCD_CUDA(e, cudaMemcpyAsync(e->d_sig_ids.p, sig_ids, ns * sizeof(int), cudaMemcpyHostToDevice, s));
-	LCD_TRY(ensure_uq(e, 1, nq, s));
-	LCD_TRY(ensure_acc(e, 1));
-	LCD_CUDA(e, cudaMemsetAsync(e->acc.p, 0, static_cast<size_t>(e->acc_stride) * sizeof(long long), s));
-	ResolveArgs a{};
-	a.nq = nq;
-	fill_prep(e, a, static_cast<float>(n_total), 0);
-	int nq_pad = 32;
-	while (nq_pad < nq) nq_pad <<= 1;
-	prep_from_ids_kernel<<<1, kResolveThreads, nq_pad * sizeof(uint32_t), s>>>(e->d_in_ids.p, a);
-	LCD_CHECK_LAUNCH(e);
-	LCD_TRY(launch_score(e, 1, nq, s));
-	gather_likelihood_kernel<<<dim3((ns + 255) / 256, 1), 256, 0, s>>>(e->acc.p, e->acc_stride, static_cast<int>(e->h_ni.size()), e->d_sig_ids.p, ns, e->d_like.p);
-	LCD_CHECK_LAUNCH(e);
+	LCD_TRY(prep_ids(e, e->d_in_ids.p, 1, nq, n_total, 0, false, s));
+	LCD_TRY(score_tfidf(e, 1, nq, e->d_sig_ids.p, ns, e->d_like.p, s));
 	LCD_CUDA(e, cudaMemcpyAsync(likelihood_out, e->d_like.p, ns * sizeof(float), cudaMemcpyDeviceToHost, s));
 	LCD_CUDA(e, cudaStreamSynchronize(s));
 	return LCD_OK;
@@ -2356,17 +2372,7 @@ int lcd_index_similarity(lcd_engine * e, const int * query_word_ids, int nq, con
 		LCD_CUDA(e, cudaMemcpyAsync(e->gd_query.p, query_gdesc, e->gd_dim * sizeof(float), cudaMemcpyHostToDevice, s));
 		d_g = e->gd_query.p;
 	}
-	LCD_TRY(ensure_uq(e, 1, nq1, s, true));
-	LCD_TRY(ensure_acc(e, 1));
-	LCD_CUDA(e, cudaMemsetAsync(e->acc.p, 0, static_cast<size_t>(e->acc_stride) * sizeof(long long), s));
-	ResolveArgs a{};
-	a.nq = nq1;
-	fill_prep(e, a, 0.0f, 0);
-	fill_pairs(e, a);
-	int nq_pad = 32;
-	while (nq_pad < nq1) nq_pad <<= 1;
-	prep_from_ids_kernel<<<1, kResolveThreads, nq_pad * sizeof(uint32_t), s>>>(e->d_in_ids.p, a);
-	LCD_CHECK_LAUNCH(e);
+	LCD_TRY(prep_ids(e, e->d_in_ids.p, 1, nq1, 0, 0, true, s));
 	LCD_TRY(launch_similarity(e, 1, nq1, d_g, e->d_sig_ids.p, ns, e->d_like.p, s));
 	LCD_CUDA(e, cudaMemcpyAsync(likelihood_out, e->d_like.p, ns * sizeof(float), cudaMemcpyDeviceToHost, s));
 	LCD_CUDA(e, cudaStreamSynchronize(s));
@@ -4962,35 +4968,10 @@ int lcd_shard_resolve_score_dev(lcd_engine * e, const void * d_queries, int n_fr
 	LCD_TRY(check_n_total(e, n_total));
 	(void)total_rows_;
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
-	const bool score = d_scores_out != nullptr && ns > 0;
-	ResolveArgs a{};
-	a.queries = static_cast<const uint32_t *>(d_queries);
-	a.nq = nq_per_frame;
-	a.nq_total = n_frames * nq_per_frame;
+	ResolveArgs a = resolve_args(e, static_cast<const uint32_t *>(d_queries), nq_per_frame, n_frames * nq_per_frame, nullptr, n_ranks, d_row_ids, incremental,
+	                             nndr, new_words_compared_together, last_word_id, d_word_ids_out);
 	shard_set_keys(e, a, d_keys_gathered, 0);
-	a.n_chunks = n_ranks;
-	a.row_ids = d_row_ids;
-	a.incremental = incremental;
-	a.nndr = nndr;
-	a.cmp_new = new_words_compared_together;
-	a.last_word_id = last_word_id;
-	a.word_ids_out = d_word_ids_out;
-	if (score)
-	{
-		LCD_TRY(ensure_uq(e, n_frames, nq_per_frame, s));
-		LCD_TRY(ensure_acc(e, n_frames));
-		LCD_CUDA(e, zero_fill_async(e->acc.p, static_cast<size_t>(e->acc_stride) * n_frames * sizeof(long long), s));
-		fill_prep(e, a, static_cast<float>(n_total), 1);
-	}
-	LCD_TRY(launch_resolve(e, a, n_frames, s));
-	if (score)
-	{
-		LCD_TRY(launch_score(e, n_frames, nq_per_frame, s));
-		dim3 grid((ns + 255) / 256, n_frames);
-		gather_fixed_kernel<<<grid, 256, 0, s>>>(e->acc.p, e->acc_stride, static_cast<int>(e->h_ni.size()), d_sig_ids, ns, d_scores_out);
-		LCD_CHECK_LAUNCH(e);
-	}
-	return LCD_OK;
+	return resolve_score(e, a, n_frames, n_total, false, nullptr, d_sig_ids, ns, d_scores_out, s);
 }
 
 int lcd_shard_resolve_frames_dev(lcd_engine * e, const void * d_queries_all, int frame0, int n_frames, int n_frames_total, int nq_per_frame,
@@ -5004,19 +4985,11 @@ int lcd_shard_resolve_frames_dev(lcd_engine * e, const void * d_queries_all, int
 		LCD_FAIL(e, LCD_ERR_INVALID, "null argument or frame range outside the job");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
-	ResolveArgs a{};
-	a.queries = static_cast<const uint32_t *>(d_queries_all) + static_cast<size_t>(frame0) * nq_per_frame * e->nw;
-	a.nq = nq_per_frame;
-	a.nq_total = n_frames_total * nq_per_frame;                                     // stride between the gathered key sets
+	// nq_total = n_frames_total * nq_per_frame: the stride between the gathered key sets
+	ResolveArgs a = resolve_args(e, static_cast<const uint32_t *>(d_queries_all) + static_cast<size_t>(frame0) * nq_per_frame * e->nw, nq_per_frame,
+	                             n_frames_total * nq_per_frame, d_n_per_frame ? d_n_per_frame + frame0 : nullptr, n_ranks, d_row_ids, incremental, nndr,
+	                             new_words_compared_together, last_word_id, d_word_ids_out);
 	shard_set_keys(e, a, d_keys_gathered, static_cast<size_t>(frame0) * nq_per_frame);
-	a.n_chunks = n_ranks;
-	a.row_ids = d_row_ids;
-	a.incremental = incremental;
-	a.nndr = nndr;
-	a.cmp_new = new_words_compared_together;
-	a.last_word_id = last_word_id;
-	a.word_ids_out = d_word_ids_out;
-	a.nq_frame = d_n_per_frame ? d_n_per_frame + frame0 : nullptr;
 	return launch_resolve(e, a, n_frames, s);
 }
 
@@ -5029,23 +5002,8 @@ int lcd_shard_score_ids_dev(lcd_engine * e, const int * d_word_ids_all, int n_fr
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d words per signature", kMaxFrameQueries);
 	LCD_TRY(check_n_total(e, n_total));
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
-	LCD_TRY(ensure_uq(e, n_frames, nq_per_frame, s));
-	LCD_TRY(ensure_acc(e, n_frames));
-	LCD_CUDA(e, zero_fill_async(e->acc.p, static_cast<size_t>(e->acc_stride) * n_frames * sizeof(long long), s));
-	ResolveArgs a{};
-	a.nq = nq_per_frame;
-	fill_prep(e, a, static_cast<float>(n_total), 1);
-	int nq_pad = 32;
-	while (nq_pad < nq_per_frame) nq_pad <<= 1;
-	prof_mark(e, LCD_PROF_RESOLVE, s);
-	prep_from_ids_kernel<<<n_frames, kResolveThreads, nq_pad * sizeof(uint32_t), s>>>(d_word_ids_all, a);
-	prof_mark(e, LCD_PROF_RESOLVE, s);
-	LCD_CHECK_LAUNCH(e);
-	LCD_TRY(launch_score(e, n_frames, nq_per_frame, s));
-	dim3 grid((ns + 255) / 256, n_frames);
-	gather_fixed_kernel<<<grid, 256, 0, s>>>(e->acc.p, e->acc_stride, static_cast<int>(e->h_ni.size()), d_sig_ids, ns, d_scores_out);
-	LCD_CHECK_LAUNCH(e);
-	return LCD_OK;
+	LCD_TRY(prep_ids(e, d_word_ids_all, n_frames, nq_per_frame, n_total, 1, false, s));
+	return score_tfidf(e, n_frames, nq_per_frame, d_sig_ids, ns, d_scores_out, s);
 }
 
 // ---- the similarity likelihood over word-range shards ----------------------------------------------------------------------
@@ -5118,26 +5076,9 @@ int lcd_shard_similarity_ids_dev(lcd_engine * e, const int * d_word_ids_all, int
 	if (!d_word_ids_all || !d_sig_ids || !d_pairs_out || !d_valid_out || n_frames <= 0 || ns <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null argument");
 	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d words per signature", kMaxFrameQueries);
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
-	LCD_TRY(ensure_uq(e, n_frames, nq_per_frame, s, true));
-	LCD_TRY(ensure_acc(e, n_frames));
-	LCD_CUDA(e, zero_fill_async(e->acc.p, static_cast<size_t>(e->acc_stride) * n_frames * sizeof(long long), s));
-	ResolveArgs a{};
-	a.nq = nq_per_frame;
-	fill_prep(e, a, 0.0f, 1);
-	fill_pairs(e, a);
-	int nq_pad = 32;
-	while (nq_pad < nq_per_frame) nq_pad <<= 1;
-	prof_mark(e, LCD_PROF_RESOLVE, s);
-	prep_local_ids_kernel<<<n_frames, kResolveThreads, nq_pad * sizeof(uint32_t), s>>>(d_word_ids_all, a, n_frames, 0, n_frames);
-	prof_mark(e, LCD_PROF_RESOLVE, s);
-	LCD_CHECK_LAUNCH(e);
-	LCD_TRY(launch_score(e, n_frames, nq_per_frame, s, true));
-	gather_pairs_kernel<<<dim3((ns + 255) / 256, n_frames), 256, 0, s>>>(e->acc.p, e->acc_stride, static_cast<int>(e->h_ni.size()), d_sig_ids, ns, n_frames,
-	                                                                  d_pairs_out);
-	LCD_CHECK_LAUNCH(e);
-	gather_valid_kernel<<<(ns + 255) / 256, 256, 0, s>>>(e->nvalid.p, static_cast<int>(e->h_nvalid.size()), d_sig_ids, ns, d_valid_out, 0);
-	LCD_CHECK_LAUNCH(e);
-	return LCD_OK;
+	const ShardIds local{n_frames, 0, n_frames};
+	LCD_TRY(prep_ids(e, d_word_ids_all, n_frames, nq_per_frame, 0, 1, true, s, &local));
+	return score_pairs(e, n_frames, nq_per_frame, d_sig_ids, ns, n_frames, d_pairs_out, d_valid_out, 0, s);
 }
 
 int lcd_shard_similarity_finalize_dev(lcd_engine * e, const int * d_pairs, const int * d_valid, const int * d_word_ids, int n_frames, int nq_per_frame,
@@ -5368,9 +5309,6 @@ static int shard_step(lcd_engine * e, int n_frames, int cap, const uint8_t * des
 	// merge + NNDR always runs on the whole batch; the TF-IDF stage scores G x n_frames frames, so from 4 ranks on it is no longer a
 	// single-wave kernel and is split in two halves of every rank's frames: the reduce-scatter of the first half runs under the scoring of
 	// the second (LCD_SHARD_SCORE_PARTS=1|2 overrides)
-	const int t_parts = 1;
-	const int tail_frames[2] = {n_frames, 0};
-	const int tail_f0[2] = {0, n_frames};
 	const int s_parts_env = env_int("LCD_SHARD_SCORE_PARTS", 0);
 	const int s_parts = n_frames >= 2 && (s_parts_env ? s_parts_env >= 2 : G >= 4) ? 2 : 1;
 	const int score_frames[2] = {s_parts == 2 ? (n_frames + 1) / 2 : n_frames, s_parts == 2 ? n_frames / 2 : 0};
@@ -5383,9 +5321,9 @@ static int shard_step(lcd_engine * e, int n_frames, int cap, const uint8_t * des
 		LCD_CUDA(e, e->sh_desc_all[h].reserve(pr * row_bytes * G, 0, false, s));
 		LCD_CUDA(e, e->sh_keys[h].reserve(pr * kw * G, 0, false, s));
 	}
-	LCD_CUDA(e, e->sh_keys_mine[0].reserve(rows * kw * G, 0, false, s)); // [rank][local frame][feature]: both halves land in one array
-	LCD_CUDA(e, e->sh_words_loc[0].reserve(rows, 0, false, s));
-	LCD_CUDA(e, e->sh_words_all[0].reserve(rows * G, 0, false, s));
+	LCD_CUDA(e, e->sh_keys_mine.reserve(rows * kw * G, 0, false, s)); // [rank][local frame][feature]: both halves land in one array
+	LCD_CUDA(e, e->sh_words_loc.reserve(rows, 0, false, s));
+	LCD_CUDA(e, e->sh_words_all.reserve(rows * G, 0, false, s));
 	for (int h = 0; h < s_parts; ++h)
 	{
 		if (sim)
@@ -5409,7 +5347,7 @@ static int shard_step(lcd_engine * e, int n_frames, int cap, const uint8_t * des
 		fprintf(stderr, "[lcd shard trace rank %d]", R);
 		for (int h = 0; h < n_parts; ++h)
 			for (int k = 0; k < 8; ++k)
-				if ((k < 4 || (k < 6 ? h < t_parts : h < s_parts)) && cudaEventElapsedTime(&ms, e->sh_tr[0], e->sh_ev[h][k]) == cudaSuccess) fprintf(stderr, " %s%d=%.3f", names[k], h, ms);
+				if ((k < 4 || (k < 6 ? h == 0 : h < s_parts)) && cudaEventElapsedTime(&ms, e->sh_tr[0], e->sh_ev[h][k]) == cudaSuccess) fprintf(stderr, " %s%d=%.3f", names[k], h, ms);
 		if (cudaEventElapsedTime(&ms, e->sh_tr[0], e->sh_tr[1]) == cudaSuccess) fprintf(stderr, " end=%.3f", ms);
 		fprintf(stderr, "\n");
 	}
@@ -5451,78 +5389,46 @@ static int shard_step(lcd_engine * e, int n_frames, int cap, const uint8_t * des
 		for (int p = 0; p < G; ++p)
 		{
 			LCD_NCCL(e, nc.Send(e->sh_keys[h].p + static_cast<size_t>(p) * pr * kw, pr * 2, key_type, p, e->comm, c));
-			LCD_NCCL(e, nc.Recv(e->sh_keys_mine[0].p + (static_cast<size_t>(p) * rows + static_cast<size_t>(part_f0[h]) * cap) * kw, pr * 2, key_type, p, e->comm, c));
+			LCD_NCCL(e, nc.Recv(e->sh_keys_mine.p + (static_cast<size_t>(p) * rows + static_cast<size_t>(part_f0[h]) * cap) * kw, pr * 2, key_type, p, e->comm, c));
 		}
 		LCD_NCCL(e, nc.GroupEnd());
 		LCD_TRY(shard_record(e, h, 3, c));
 	}
 	host_t[2] = std::chrono::steady_clock::now();
 	// phase 3: merge + NNDR / new-word pass of the local frames, all-gather of their word ids
-	for (int h = 0; h < t_parts; ++h)
-	{
-		const size_t pr = static_cast<size_t>(tail_frames[h]) * cap;
-		LCD_CUDA(e, cudaStreamWaitEvent(s, e->sh_ev[t_parts == 2 ? h : n_parts - 1][3], 0));
-		ResolveArgs a{};
-		a.queries = reinterpret_cast<const uint32_t *>(desc) + static_cast<size_t>(tail_f0[h]) * cap * e->nw;
-		a.nq = cap;
-		a.nq_total = static_cast<int>(rows);                       // stride between the G key sets
-		shard_set_keys(e, a, e->sh_keys_mine[0].p, static_cast<size_t>(tail_f0[h]) * cap);
-		a.n_chunks = G;
-		a.row_ids = d_row_ids_global;
-		a.incremental = incremental;
-		a.nndr = nndr;
-		a.cmp_new = new_words_compared_together;
-		a.last_word_id = last_word_id;
-		a.word_ids_out = e->sh_words_loc[h].p;
-		a.nq_frame = n_local ? n_local + tail_f0[h] : nullptr;
-		LCD_TRY(launch_resolve(e, a, tail_frames[h], s));
-		if (d_word_ids_out)
-			LCD_CUDA(e, cudaMemcpyAsync(d_word_ids_out + static_cast<size_t>(tail_f0[h]) * cap, e->sh_words_loc[h].p, pr * sizeof(int), cudaMemcpyDeviceToDevice, s));
-		LCD_TRY(shard_record(e, h, 4, s));
-		LCD_CUDA(e, cudaStreamWaitEvent(c, e->sh_ev[h][4], 0));
-		LCD_NCCL(e, nc.AllGather(e->sh_words_loc[h].p, e->sh_words_all[h].p, pr, ncclInt32, e->comm, c));
-		LCD_TRY(shard_record(e, h, 5, c));
-	}
+	LCD_CUDA(e, cudaStreamWaitEvent(s, e->sh_ev[n_parts - 1][3], 0));
+	// nq_total = rows: the stride between the G key sets
+	ResolveArgs a = resolve_args(e, reinterpret_cast<const uint32_t *>(desc), cap, static_cast<int>(rows), n_local, G, d_row_ids_global, incremental, nndr,
+	                             new_words_compared_together, last_word_id, e->sh_words_loc.p);
+	shard_set_keys(e, a, e->sh_keys_mine.p, 0);
+	LCD_TRY(launch_resolve(e, a, n_frames, s));
+	if (d_word_ids_out) LCD_CUDA(e, cudaMemcpyAsync(d_word_ids_out, e->sh_words_loc.p, rows * sizeof(int), cudaMemcpyDeviceToDevice, s));
+	LCD_TRY(shard_record(e, 0, 4, s));
+	LCD_CUDA(e, cudaStreamWaitEvent(c, e->sh_ev[0][4], 0));
+	LCD_NCCL(e, nc.AllGather(e->sh_words_loc.p, e->sh_words_all.p, rows, ncclInt32, e->comm, c));
+	LCD_TRY(shard_record(e, 0, 5, c));
 	host_t[3] = std::chrono::steady_clock::now();
 	// phase 4: TF-IDF (or word pairs) of every rank's frames over the local word range, reduce-scatter of the exact integer sums
 	for (int h = 0; h < s_parts; ++h)
 	{
 		const int nf_all = score_frames[h] * G; // frames [score_f0, +score_frames) of every rank, rank-major
 		LCD_CUDA(e, cudaStreamWaitEvent(s, e->sh_ev[0][5], 0));
-		LCD_TRY(ensure_uq(e, nf_all, cap, s, sim != nullptr));
-		LCD_TRY(ensure_acc(e, nf_all));
-		LCD_CUDA(e, zero_fill_async(e->acc.p, static_cast<size_t>(e->acc_stride) * nf_all * sizeof(long long), s));
-		ResolveArgs a{};
-		a.nq = cap;
-		fill_prep(e, a, static_cast<float>(n_total), 1);
-		if (sim) fill_pairs(e, a);
-		int nq_pad = 32;
-		while (nq_pad < cap) nq_pad <<= 1;
-		prof_mark(e, LCD_PROF_RESOLVE, s);
-		prep_local_ids_kernel<<<nf_all, kResolveThreads, nq_pad * sizeof(uint32_t), s>>>(e->sh_words_all[0].p, a, n_frames, score_f0[h], score_frames[h]);
-		prof_mark(e, LCD_PROF_RESOLVE, s);
-		LCD_CHECK_LAUNCH(e);
-		LCD_TRY(launch_score(e, nf_all, cap, s, sim != nullptr));
+		const ShardIds local{n_frames, score_f0[h], score_frames[h]};
+		LCD_TRY(prep_ids(e, e->sh_words_all.p, nf_all, cap, n_total, 1, sim != nullptr, s, &local));
 		if (sim)
 		{
 			// [rank][score_frames + 1][ns]: the pair counts of the rank's frames, then this rank's valid(s) in every segment, so that the
 			// reduce-scatter that sums the counts sums valid(s) across ranks too (no collective of its own)
 			const size_t seg = static_cast<size_t>(score_frames[h] + 1) * ns;
-			gather_pairs_kernel<<<dim3((ns + 255) / 256, nf_all), 256, 0, s>>>(e->acc.p, e->acc_stride, static_cast<int>(e->h_ni.size()), d_sig_ids, ns,
-			                                                                score_frames[h], e->sh_pairs[h].p);
-			LCD_CHECK_LAUNCH(e);
-			gather_valid_kernel<<<dim3((ns + 255) / 256, G), 256, 0, s>>>(e->nvalid.p, static_cast<int>(e->h_nvalid.size()), d_sig_ids, ns,
-			                                                           e->sh_pairs[h].p + static_cast<size_t>(score_frames[h]) * ns, seg);
-			LCD_CHECK_LAUNCH(e);
+			LCD_TRY(score_pairs(e, nf_all, cap, d_sig_ids, ns, score_frames[h], e->sh_pairs[h].p, e->sh_pairs[h].p + static_cast<size_t>(score_frames[h]) * ns, seg,
+			                    s));
 			LCD_TRY(shard_record(e, h, 6, s));
 			LCD_CUDA(e, cudaStreamWaitEvent(c, e->sh_ev[h][6], 0));
 			LCD_NCCL(e, nc.ReduceScatter(e->sh_pairs[h].p, e->sh_pairs_loc[h].p, seg, ncclInt32, ncclSum, e->comm, c));
 		}
 		else
 		{
-			gather_fixed_kernel<<<dim3((ns + 255) / 256, nf_all), 256, 0, s>>>(e->acc.p, e->acc_stride, static_cast<int>(e->h_ni.size()), d_sig_ids, ns,
-			                                                                e->sh_scores[h].p);
-			LCD_CHECK_LAUNCH(e);
+			LCD_TRY(score_tfidf(e, nf_all, cap, d_sig_ids, ns, e->sh_scores[h].p, s));
 			LCD_TRY(shard_record(e, h, 6, s));
 			LCD_CUDA(e, cudaStreamWaitEvent(c, e->sh_ev[h][6], 0));
 			LCD_NCCL(e, nc.ReduceScatter(e->sh_scores[h].p, e->sh_scores_loc[h].p, static_cast<size_t>(score_frames[h]) * ns, ncclInt64, ncclSum, e->comm, c));
@@ -5533,7 +5439,7 @@ static int shard_step(lcd_engine * e, int n_frames, int cap, const uint8_t * des
 	// phase 5: likelihood of the local frames (then `finish`: verification of their top hypothesis).  The similarity variant first
 	// counts valid(q) of the local frames and takes their dot products, under the last reduce-scatter.
 	bool gd = false;
-	if (sim) LCD_TRY(shard_similarity_prepare(e, n_frames, cap, e->sh_words_loc[0].p, *sim, d_sig_ids, ns, &gd, s));
+	if (sim) LCD_TRY(shard_similarity_prepare(e, n_frames, cap, e->sh_words_loc.p, *sim, d_sig_ids, ns, &gd, s));
 	for (int h = 0; h < s_parts; ++h)
 	{
 		const int n = score_frames[h] * ns;
@@ -5579,7 +5485,7 @@ static int shard_step(lcd_engine * e, int n_frames, int cap, const uint8_t * des
 				if (cudaEventElapsedTime(&ms, origin, e->sh_ring[(st * 2 + 0) * 9 + 8]) == cudaSuccess) fprintf(stderr, " begin=%.3f", ms);
 				for (int h = 0; h < n_parts; ++h)
 					for (int k = 0; k < 8; ++k)
-						if ((k < 4 || (k < 6 ? h < t_parts : h < s_parts)) && cudaEventElapsedTime(&ms, origin, e->sh_ring[(st * 2 + h) * 9 + k]) == cudaSuccess) fprintf(stderr, " %s%d=%.3f", names[k], h, ms);
+						if ((k < 4 || (k < 6 ? h == 0 : h < s_parts)) && cudaEventElapsedTime(&ms, origin, e->sh_ring[(st * 2 + h) * 9 + k]) == cudaSuccess) fprintf(stderr, " %s%d=%.3f", names[k], h, ms);
 				if (cudaEventElapsedTime(&ms, origin, e->sh_ring[(st * 2 + 1) * 9 + 8]) == cudaSuccess) fprintf(stderr, " end=%.3f", ms);
 				fprintf(stderr, "\n");
 			}
