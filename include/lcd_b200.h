@@ -48,14 +48,14 @@ extern "C" {
 /* descriptor types: cv::Mat type()/cols of VisualWord::getDescriptor()
  * (VWDictionary.cpp:933-957 checks) */
 #define LCD_DESC_U8 0  /* CV_8U rows, desc_dim bytes (ORB/BRIEF: 32)  -> Hamming   */
-#define LCD_DESC_F32 1 /* CV_32F rows, desc_dim floats (SURF: 64/128) -> squared L2 */
+#define LCD_DESC_F32 1 /* CV_32F rows, desc_dim floats (SURF: 64/128, SIFT: 128, SuperPoint: 256) -> squared L2 */
 
 typedef struct lcd_engine lcd_engine;
 
 typedef struct lcd_config {
 	int device;         /* CUDA device ordinal                                          */
 	int desc_type;      /* LCD_DESC_U8 | LCD_DESC_F32                                   */
-	int desc_dim;       /* bytes (U8: 16/32/64) or floats (F32: 64/128)                 */
+	int desc_dim;       /* bytes (U8: 16/32/64) or floats (F32: 64/128/256)             */
 	int max_words;      /* initial capacity hint for vocabulary rows (grows)            */
 	int max_signatures; /* initial capacity hint for signature ids (grows)              */
 	int max_queries;    /* max descriptors per lcd_dict_* call / per frame (<= 4096)    */
@@ -431,18 +431,20 @@ int lcd_match_pairs(lcd_engine * e, int n_pairs, int cap, const void * desc_from
  * LCD_ERR_CAPACITY when its dynamic size (DESIGN.md §6) plus its static size exceeds the device's opt-in limit per block.  On an H100
  * (232 448 B per block) the largest cap is 3540 for 16-byte descriptors, 2248 for 32-byte and 1233 for 64-byte ones (2560 B static).
  * The refusal leaves the engine usable.
- * Float engines (LCD_DESC_F32, 64 or 128 floats; every registration call below, the store-backed ones included): the same temporary
+ * Float engines (LCD_DESC_F32, 64, 128 or 256 floats; every registration call below, the store-backed ones included): the same temporary
  * dictionary with squared L2 in place of Hamming (VWDictionary.cpp:1020-1028, NORM_L2SQR / rtflann L2), summed in rtflann's order
  * (dist.h:158-166) for the dictionary and for the Reg/RepeatOnce pass's cv::BFMatcher(NORM_L2SQR) ranking, whose OpenCV SIMD order can
  * differ in the last ulp (as lcd_match_bf).  Ties go to the first-created word.  Both sides are read from global memory and shared
- * memory holds per-row scalars only, so every cap up to 4096 is accepted at 64-D and 128-D (largest dynamic size 37 B per row). */
+ * memory holds per-row scalars only, so every cap up to 4096 is accepted at 64-D, 128-D and 256-D (largest dynamic size 37 B per row;
+ * at 256-D the new-word loop stages 32 descriptors in 32 896 B of static shared memory). */
 int lcd_verify_batch(lcd_engine * e, int n_pairs, int cap, const void * desc_from, const float * xyz_from, const int * n_from,
                      const void * desc_to, const float * uv_to, const float * xyz_to, const int * n_to,
                      const lcd_verify_params * params, lcd_verify_result * results, int * match_ids, int * inlier_ids);
 
 /* Static shared memory in bytes of a verification kernel at the engine's descriptor size: which = 0 pair matching, 1 matching with a
  * guess (Reg/RepeatOnce), 2 PnP RANSAC, 3 FROM-dictionary build; on a float engine 0 is the kernel that resolves the TO side and assembles the
- * correspondences (the TO x dictionary scan before it has only static shared memory).  < 0 on error. */
+ * correspondences (the TO x dictionary scan before it has only static shared memory).  Float engines have all four at 64, 128 and 256
+ * floats.  < 0 on error. */
 long long lcd_verify_static_smem(lcd_engine * e, int which);
 
 /* replaces: util3d::solvePnPRansac (util3d_motion_estimation.cpp:843-990; argument for argument: objectPoints, imagePoints,

@@ -842,7 +842,7 @@ int tf_search(lcd_engine * e, const float * d_q, int nq, int n_rows, cudaStream_
 	const int fb_slots = std::max(4 * nq, 1 << 18), fb_ctas = 2 * e->sm_count;
 	LCD_CUDA(e, e->tf_fb_scratch.reserve(static_cast<size_t>(fb_slots), 0, false, s));
 	LCD_CUDA(e, cudaFuncSetAttribute(knn2_l2_fallback_kernel<DIM>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(fallback_smem_bytes<DIM>())));
-	knn2_l2_fallback_kernel<DIM><<<fb_ctas, 256, fallback_smem_bytes<DIM>(), s>>>(vocab, n_rows, e->row_offset, d_q, e->tf_fb_list.p, e->tf_flags.p,
+	knn2_l2_fallback_kernel<DIM><<<fb_ctas, fallback_rows<DIM>(), fallback_smem_bytes<DIM>(), s>>>(vocab, n_rows, e->row_offset, d_q, e->tf_fb_list.p, e->tf_flags.p,
 	                                                                              e->tf_fb_scratch.p, fb_slots);
 	LCD_CHECK_LAUNCH(e);
 	knn2_l2_fallback_merge_kernel<<<64, 256, 0, s>>>(e->tf_fb_list.p, e->tf_flags.p, e->tf_fb_scratch.p, fb_slots, fb_ctas, e->d_partial64.p);
@@ -858,16 +858,16 @@ int run_knn(lcd_engine * e, const uint32_t * d_q, int nq_total, int n_rows, int 
 	e->nn_last_tensor = 0;
 	e->nn_last_f32_tensor = 0;
 	if (e->f32 && e->nn_f32_tensor && !e->tf_disabled && n_rows >= kTfMinRows && nq_total > 0 &&
-	    TfCfg<64>::smem <= static_cast<size_t>(e->smem_optin))
-		LCD_TRY(e->nw == 64 ? tf_prepare_words<64>(e, n_rows, s) : tf_prepare_words<128>(e, n_rows, s));
+	    tf_smem_bytes(e->nw) <= static_cast<size_t>(e->smem_optin))
+		LCD_TRY(e->nw == 64 ? tf_prepare_words<64>(e, n_rows, s) : e->nw == 128 ? tf_prepare_words<128>(e, n_rows, s) : tf_prepare_words<256>(e, n_rows, s));
 	if (e->f32 && e->nn_f32_tensor && !e->tf_disabled && n_rows >= kTfMinRows && nq_total > 0 &&
-	    TfCfg<64>::smem <= static_cast<size_t>(e->smem_optin))
+	    tf_smem_bytes(e->nw) <= static_cast<size_t>(e->smem_optin))
 	{
 		// float descriptors, large dictionary: distance matrix on the tensor cores as a filter + exact re-rank (nn_tensor_f32.cuh)
 		const float * q = reinterpret_cast<const float *>(d_q);
 		e->nn_last_f32_tensor = 1;
 		*n_chunks_out = 1;
-		return e->nw == 64 ? tf_search<64>(e, q, nq_total, n_rows, s) : tf_search<128>(e, q, nq_total, n_rows, s);
+		return e->nw == 64 ? tf_search<64>(e, q, nq_total, n_rows, s) : e->nw == 128 ? tf_search<128>(e, q, nq_total, n_rows, s) : tf_search<256>(e, q, nq_total, n_rows, s);
 	}
 	if (e->f32)
 	{
@@ -881,7 +881,8 @@ int run_knn(lcd_engine * e, const uint32_t * d_q, int nq_total, int n_rows, int 
 		const float * q = reinterpret_cast<const float *>(d_q);
 		prof_mark(e, LCD_PROF_NN, s);
 		if (e->nw == 64) knn2_l2_kernel<64><<<dim3(q_blocks, splits), kL2Threads, 0, s>>>(v, n_rows, e->row_offset, q, nq_total, e->d_partial64.p, rps);
-		else knn2_l2_kernel<128><<<dim3(q_blocks, splits), kL2Threads, 0, s>>>(v, n_rows, e->row_offset, q, nq_total, e->d_partial64.p, rps);
+		else if (e->nw == 128) knn2_l2_kernel<128><<<dim3(q_blocks, splits), kL2Threads, 0, s>>>(v, n_rows, e->row_offset, q, nq_total, e->d_partial64.p, rps);
+		else knn2_l2_kernel<256><<<dim3(q_blocks, splits), kL2Threads, 0, s>>>(v, n_rows, e->row_offset, q, nq_total, e->d_partial64.p, rps);
 		prof_mark(e, LCD_PROF_NN, s);
 		LCD_CHECK_LAUNCH(e);
 		*n_chunks_out = splits;
@@ -975,14 +976,17 @@ int launch_resolve(lcd_engine * e, const ResolveArgs & a, int n_frames, cudaStre
 	if (e->f32)
 	{
 		const size_t smem32 = resolve_l2_smem_bytes(a.nq);
-		if (smem32 > 48 * 1024)
+		// 256: resolve_rounds_l2 adds 32 staged descriptors (32 896 B) of static shared memory, so any dynamic size needs the opt-in
+		if (smem32 > 48 * 1024 || e->nw == 256)
 		{
 			if (e->nw == 64) LCD_CUDA(e, cudaFuncSetAttribute(resolve_l2_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem32)));
-			else LCD_CUDA(e, cudaFuncSetAttribute(resolve_l2_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem32)));
+			else if (e->nw == 128) LCD_CUDA(e, cudaFuncSetAttribute(resolve_l2_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem32)));
+			else LCD_CUDA(e, cudaFuncSetAttribute(resolve_l2_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem32)));
 		}
 		prof_mark(e, LCD_PROF_RESOLVE, s);
 		if (e->nw == 64) resolve_l2_kernel<64><<<n_frames, kL2ResolveThreads, smem32, s>>>(a, a.partial64);
-		else resolve_l2_kernel<128><<<n_frames, kL2ResolveThreads, smem32, s>>>(a, a.partial64);
+		else if (e->nw == 128) resolve_l2_kernel<128><<<n_frames, kL2ResolveThreads, smem32, s>>>(a, a.partial64);
+		else resolve_l2_kernel<256><<<n_frames, kL2ResolveThreads, smem32, s>>>(a, a.partial64);
 		prof_mark(e, LCD_PROF_RESOLVE, s);
 		LCD_CHECK_LAUNCH(e);
 		return LCD_OK;
@@ -1426,9 +1430,9 @@ lcd_engine * lcd_create(const lcd_config * cfg)
 		g_create_error = "binary descriptor size must be 16, 32 or 64 bytes";
 		return nullptr;
 	}
-	if (cfg->desc_type == LCD_DESC_F32 && cfg->desc_dim != 64 && cfg->desc_dim != 128)
+	if (cfg->desc_type == LCD_DESC_F32 && cfg->desc_dim != 64 && cfg->desc_dim != 128 && cfg->desc_dim != 256)
 	{
-		g_create_error = "float descriptors must have 64 or 128 dimensions (SURF-64, SURF-128 / SIFT)";
+		g_create_error = "float descriptors must have 64, 128 or 256 dimensions (SURF-64, SURF-128 / SIFT, SuperPoint)";
 		return nullptr;
 	}
 	int ndev = 0;
@@ -3113,10 +3117,10 @@ static int fit_smem(lcd_engine * e, const void * kern, size_t dyn, int cap)
 // loop and the correspondences (verify.cuh).  a: launch_match's arguments, with the store's FROM-dictionary cache when from_store.
 static int launch_match_l2(lcd_engine * e, const PairSource & src, int n_pairs, int cap, float nndr, bool from_store, MatchArgs a, cudaStream_t s)
 {
-	const bool d64 = e->nw == 64; // else 128
-	const auto kern_fd = d64 ? from_dict_l2_kernel<64> : from_dict_l2_kernel<128>;
-	const auto kern_scan = d64 ? to_dict_knn2_l2_kernel<64> : to_dict_knn2_l2_kernel<128>;
-	const auto kern = d64 ? pair_match_l2_kernel<64> : pair_match_l2_kernel<128>;
+	const int d = e->nw; // 64, 128 or 256
+	const auto kern_fd = d == 64 ? from_dict_l2_kernel<64> : d == 128 ? from_dict_l2_kernel<128> : from_dict_l2_kernel<256>;
+	const auto kern_scan = d == 64 ? to_dict_knn2_l2_kernel<64> : d == 128 ? to_dict_knn2_l2_kernel<128> : to_dict_knn2_l2_kernel<256>;
+	const auto kern = d == 64 ? pair_match_l2_kernel<64> : d == 128 ? pair_match_l2_kernel<128> : pair_match_l2_kernel<256>;
 	FromDictArgs fa{src.from.desc, src.from.n, src.from.slot, src.from.cap, std::min(cap, src.from.cap), nndr, e->st_ftag.p, e->st_kof.p, e->st_creator.p};
 	if (!from_store)
 	{
@@ -3296,13 +3300,14 @@ static int launch_second_pass(lcd_engine * e, const PairSource & src, int n_pair
 		prof_mark(e, LCD_PROF_MATCH, s);                                                                                 \
 		break;                                                                                                           \
 	}
-	switch (e->nw) // 32-bit words per row: 4, 8, 16 binary; 64, 128 float
+	switch (e->nw) // 32-bit words per row: 4, 8, 16 binary; 64, 128, 256 float
 	{
 		LCD_GUESS_CASE(4, HammingDesc<4>)
 		LCD_GUESS_CASE(8, HammingDesc<8>)
 		LCD_GUESS_CASE(16, HammingDesc<16>)
 		LCD_GUESS_CASE(64, L2Desc<64>)
 		LCD_GUESS_CASE(128, L2Desc<128>)
+		LCD_GUESS_CASE(256, L2Desc<256>)
 	default: LCD_FAIL(e, LCD_ERR_INVALID, "unsupported descriptor size");
 	}
 #undef LCD_GUESS_CASE
@@ -3405,7 +3410,7 @@ long long lcd_verify_static_smem(lcd_engine * e, int which)
 	if (!e) return LCD_ERR_INVALID;
 	LCD_TRY(set_device(e));
 	const void * kern = nullptr;
-	switch (which * 1000 + e->nw) // nw: 4, 8, 16 binary; 64, 128 float
+	switch (which * 1000 + e->nw) // nw: 4, 8, 16 binary; 64, 128, 256 float
 	{
 	case 4: kern = reinterpret_cast<const void *>(pair_match_kernel<4>); break;
 	case 8: kern = reinterpret_cast<const void *>(pair_match_kernel<8>); break;
@@ -3417,14 +3422,17 @@ long long lcd_verify_static_smem(lcd_engine * e, int which)
 	case 3004: kern = reinterpret_cast<const void *>(from_dict_build_kernel<4>); break;
 	case 3008: kern = reinterpret_cast<const void *>(from_dict_build_kernel<8>); break;
 	case 3016: kern = reinterpret_cast<const void *>(from_dict_build_kernel<16>); break;
-	// float engines (nw = 64, 128 floats)
+	// float engines (nw = 64, 128, 256 floats)
 	case 64: kern = reinterpret_cast<const void *>(pair_match_l2_kernel<64>); break;
 	case 128: kern = reinterpret_cast<const void *>(pair_match_l2_kernel<128>); break;
+	case 256: kern = reinterpret_cast<const void *>(pair_match_l2_kernel<256>); break;
 	case 1064: kern = reinterpret_cast<const void *>(guess_match_kernel<L2Desc<64>>); break;
 	case 1128: kern = reinterpret_cast<const void *>(guess_match_kernel<L2Desc<128>>); break;
-	case 2064: case 2128: kern = reinterpret_cast<const void *>(pnp_ransac_kernel); break;
+	case 1256: kern = reinterpret_cast<const void *>(guess_match_kernel<L2Desc<256>>); break;
+	case 2064: case 2128: case 2256: kern = reinterpret_cast<const void *>(pnp_ransac_kernel); break;
 	case 3064: kern = reinterpret_cast<const void *>(from_dict_l2_kernel<64>); break;
 	case 3128: kern = reinterpret_cast<const void *>(from_dict_l2_kernel<128>); break;
+	case 3256: kern = reinterpret_cast<const void *>(from_dict_l2_kernel<256>); break;
 	default: LCD_FAIL(e, LCD_ERR_INVALID, "no verification kernel %d", which);
 	}
 	cudaFuncAttributes fa{};
@@ -3730,7 +3738,8 @@ static int launch_bf(lcd_engine * e, int n_pairs, int cap, const uint32_t * A, c
 {
 	dim3 grid((cap + kBfThreads - 1) / kBfThreads, n_pairs);
 	prof_mark(e, LCD_PROF_MATCH, s);
-	bf_knn2_kernel<NW, F32><<<grid, kBfThreads, 0, s>>>(A, nA, B, nB, cap, keys);
+	if constexpr (F32 && NW == 256) bf_knn2_l2_chunked_kernel<NW><<<grid, kBfThreads, 0, s>>>(A, nA, B, nB, cap, keys);
+	else bf_knn2_kernel<NW, F32><<<grid, kBfThreads, 0, s>>>(A, nA, B, nB, cap, keys);
 	prof_mark(e, LCD_PROF_MATCH, s);
 	LCD_CHECK_LAUNCH(e);
 	return LCD_OK;
@@ -3739,7 +3748,10 @@ static int launch_bf(lcd_engine * e, int n_pairs, int cap, const uint32_t * A, c
 static int launch_bf_any(lcd_engine * e, int n_pairs, int cap, const uint32_t * A, const int * nA, const uint32_t * B, const int * nB,
                          ulonglong2 * keys, cudaStream_t s)
 {
-	if (e->f32) return e->nw == 64 ? launch_bf<64, true>(e, n_pairs, cap, A, nA, B, nB, keys, s) : launch_bf<128, true>(e, n_pairs, cap, A, nA, B, nB, keys, s);
+	if (e->f32)
+		return e->nw == 64    ? launch_bf<64, true>(e, n_pairs, cap, A, nA, B, nB, keys, s)
+		       : e->nw == 128 ? launch_bf<128, true>(e, n_pairs, cap, A, nA, B, nB, keys, s)
+		                      : launch_bf<256, true>(e, n_pairs, cap, A, nA, B, nB, keys, s);
 	switch (e->nw)
 	{
 	case 4: return launch_bf<4, false>(e, n_pairs, cap, A, nA, B, nB, keys, s);

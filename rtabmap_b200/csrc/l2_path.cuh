@@ -56,6 +56,48 @@ __device__ __forceinline__ float l2_rtflann(PA a, PB b)
 	return result;
 }
 
+// Descriptors too wide to keep in registers (256-D): thread tid's distances from its own vector q (global, 16-byte aligned) to the nr
+// rows staged in s_rows (DIM floats each), accumulated kL2Chunk dimensions at a time.  rtflann adds the groups of four to one running
+// total from left to right, so carrying each row's total across the chunks (in s_acc[r * kThreads + tid]) gives its bits exactly.
+constexpr int kL2Chunk = 64; // dimensions of q held in registers at a time
+template <int DIM, int kThreads>
+__device__ __forceinline__ void l2_chunked_rows(const float * __restrict__ q, const float * s_rows, int nr, float * s_acc, int tid)
+{
+	static_assert(DIM % kL2Chunk == 0, "whole chunks");
+#pragma unroll 1
+	for (int c = 0; c < DIM; c += kL2Chunk)
+	{
+		float qc[kL2Chunk];
+		const float4 * q4 = reinterpret_cast<const float4 *>(q + c);
+#pragma unroll
+		for (int v = 0; v < kL2Chunk / 4; ++v)
+		{
+			const float4 x = q4[v];
+			qc[4 * v] = x.x;
+			qc[4 * v + 1] = x.y;
+			qc[4 * v + 2] = x.z;
+			qc[4 * v + 3] = x.w;
+		}
+#pragma unroll 1
+		for (int r = 0; r < nr; ++r)
+		{
+			const float4 * b4 = reinterpret_cast<const float4 *>(s_rows + r * DIM + c);
+			float result = c == 0 ? 0.0f : s_acc[r * kThreads + tid];
+#pragma unroll
+			for (int i = 0; i < kL2Chunk; i += 4)
+			{
+				const float4 v = b4[i >> 2];
+				const float d0 = __fsub_rn(qc[i], v.x), d1 = __fsub_rn(qc[i + 1], v.y), d2 = __fsub_rn(qc[i + 2], v.z), d3 = __fsub_rn(qc[i + 3], v.w);
+				float g = __fadd_rn(__fmul_rn(d0, d0), __fmul_rn(d1, d1));
+				g = __fadd_rn(g, __fmul_rn(d2, d2));
+				g = __fadd_rn(g, __fmul_rn(d3, d3));
+				result = __fadd_rn(result, g);
+			}
+			s_acc[r * kThreads + tid] = result;
+		}
+	}
+}
+
 // partial[split * nq + query] = (best key, second key) over the rows [split * rows_per_split, ...) of the vocabulary
 template <int DIM>
 __global__ void __launch_bounds__(kL2Threads)
@@ -66,23 +108,47 @@ knn2_l2_kernel(const float * __restrict__ vocab, int n_rows, int row_offset, con
 	const int tid = threadIdx.x;
 	const int qi = blockIdx.x * kL2Threads + tid;
 	const int r_begin = blockIdx.y * rows_per_split, r_end = min(n_rows, r_begin + rows_per_split);
-	float q[DIM];
-#pragma unroll
-	for (int i = 0; i < DIM; ++i) q[i] = qi < nq ? queries[static_cast<size_t>(qi) * DIM + i] : 0.0f;
-	unsigned long long k1 = kKey64None, k2 = kKey64None;
-	for (int r0 = r_begin; r0 < r_end; r0 += kL2TileRows)
+	if constexpr (DIM > 128)
 	{
-		const int nr = min(kL2TileRows, r_end - r0);
-		__syncthreads();
-		for (int i = tid; i < nr * DIM; i += kL2Threads) s_rows[i] = vocab[static_cast<size_t>(r0) * DIM + i];
-		__syncthreads();
-		for (int r = 0; r < nr; ++r)
+		// the query stays in global memory (L1) and is read a chunk at a time; 32 KB of rows + 16 KB of running totals
+		__shared__ float s_acc[kL2TileRows * kL2Threads];
+		const float * q = queries + static_cast<size_t>(min(qi, max(nq - 1, 0))) * DIM;
+		unsigned long long k1 = kKey64None, k2 = kKey64None;
+		for (int r0 = r_begin; r0 < r_end; r0 += kL2TileRows)
 		{
-			const float d = l2_rtflann<DIM>(q, s_rows + r * DIM);
-			top2_insert64(k1, k2, pack64(d, static_cast<uint32_t>(row_offset + r0 + r)));
+			const int nr = min(kL2TileRows, r_end - r0);
+			__syncthreads();
+			for (int i = tid; i < nr * (DIM / 4); i += kL2Threads)
+				reinterpret_cast<float4 *>(s_rows)[i] = reinterpret_cast<const float4 *>(vocab + static_cast<size_t>(r0) * DIM)[i];
+			__syncthreads();
+			if (qi < nq)
+			{
+				l2_chunked_rows<DIM, kL2Threads>(q, s_rows, nr, s_acc, tid);
+				for (int r = 0; r < nr; ++r) top2_insert64(k1, k2, pack64(s_acc[r * kL2Threads + tid], static_cast<uint32_t>(row_offset + r0 + r)));
+			}
 		}
+		if (qi < nq) partial[static_cast<size_t>(blockIdx.y) * nq + qi] = make_ulonglong2(k1, k2);
 	}
-	if (qi < nq) partial[static_cast<size_t>(blockIdx.y) * nq + qi] = make_ulonglong2(k1, k2);
+	else
+	{
+		float q[DIM];
+#pragma unroll
+		for (int i = 0; i < DIM; ++i) q[i] = qi < nq ? queries[static_cast<size_t>(qi) * DIM + i] : 0.0f;
+		unsigned long long k1 = kKey64None, k2 = kKey64None;
+		for (int r0 = r_begin; r0 < r_end; r0 += kL2TileRows)
+		{
+			const int nr = min(kL2TileRows, r_end - r0);
+			__syncthreads();
+			for (int i = tid; i < nr * DIM; i += kL2Threads) s_rows[i] = vocab[static_cast<size_t>(r0) * DIM + i];
+			__syncthreads();
+			for (int r = 0; r < nr; ++r)
+			{
+				const float d = l2_rtflann<DIM>(q, s_rows + r * DIM);
+				top2_insert64(k1, k2, pack64(d, static_cast<uint32_t>(row_offset + r0 + r)));
+			}
+		}
+		if (qi < nq) partial[static_cast<size_t>(blockIdx.y) * nq + qi] = make_ulonglong2(k1, k2);
+	}
 }
 
 // lcd_dict_knn2 for float descriptors: merge the splits, decode to (word id, squared distance)
@@ -175,6 +241,25 @@ __device__ __forceinline__ float l2_reg_vs_stream(const float (&a)[DIM], const f
 	return result;
 }
 
+// the same with the descriptor in (shared) memory: a[i] is read per element
+template <int DIM>
+__device__ __forceinline__ float l2_ptr_vs_stream(const float * a, const float * __restrict__ b)
+{
+	const float4 * b4 = reinterpret_cast<const float4 *>(b);
+	float result = 0.0f;
+#pragma unroll 16
+	for (int i = 0; i < DIM; i += 4)
+	{
+		const float4 v = b4[i >> 2];
+		const float d0 = __fsub_rn(a[i], v.x), d1 = __fsub_rn(a[i + 1], v.y), d2 = __fsub_rn(a[i + 2], v.z), d3 = __fsub_rn(a[i + 3], v.w);
+		float g = __fadd_rn(__fmul_rn(d0, d0), __fmul_rn(d1, d1));
+		g = __fadd_rn(g, __fmul_rn(d2, d2));
+		g = __fadd_rn(g, __fmul_rn(d3, d3));
+		result = __fadd_rn(result, g);
+	}
+	return result;
+}
+
 template <int DIM>
 __device__ int resolve_rounds_l2(const float * __restrict__ fq, int nq, const unsigned long long * sa1, const unsigned long long * sa2, int * res,
                                  uint16_t * L, uint16_t * rank, uint8_t * flag, int * s_nL, float nndr, int cmp_new)
@@ -200,7 +285,30 @@ __device__ int resolve_rounds_l2(const float * __restrict__ fq, int nq, const un
 	{
 		const int nL = *s_nL;
 		// (A) lane j of EVERY warp holds descriptor c0 + j in registers; the warps share out the vectors it is compared with (the 32
-		// chunk-mates and the nL words created so far), each streamed once per warp with broadcast loads
+		// chunk-mates and the nL words created so far), each streamed once per warp with broadcast loads.  256-D: the descriptor does
+		// not fit in registers, so the chunk's 32 descriptors are staged in shared memory (row stride DIM + 1: lane j reads bank j + i)
+		if constexpr (DIM > 128)
+		{
+			__shared__ float s_cq[32 * (DIM + 1)]; // the previous chunk's readers passed the barrier at the end of the loop
+			for (int v = tid; v < 32 * DIM; v += blockDim.x)
+				s_cq[(v / DIM) * (DIM + 1) + v % DIM] = fq[static_cast<size_t>(min(c0 + v / DIM, nq - 1)) * DIM + v % DIM];
+			__syncthreads();
+			const float * q = s_cq + lane * (DIM + 1);
+			for (int e = warp; e < 32; e += kWarps)
+			{
+				const int m = c0 + e;
+				s_dl[e][lane] = m < nq ? l2_ptr_vs_stream<DIM>(q, fq + static_cast<size_t>(m) * DIM) : INFINITY;
+			}
+			unsigned long long k1 = kKey64None, k2 = kKey64None;
+			for (int k = warp; k < nL; k += kWarps)
+			{
+				const float d = l2_ptr_vs_stream<DIM>(q, fq + static_cast<size_t>(L[k]) * DIM);
+				top2_insert64(k1, k2, pack64(d, static_cast<uint32_t>(k)));
+			}
+			s_wk[warp][lane][0] = k1;
+			s_wk[warp][lane][1] = k2;
+		}
+		else
 		{
 			const int i = min(c0 + lane, nq - 1);
 			float q[DIM];

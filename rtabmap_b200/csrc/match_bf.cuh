@@ -74,6 +74,35 @@ bf_knn2_kernel(const uint32_t * __restrict__ A, const int * __restrict__ n_a, co
 	if (i < na) keys[static_cast<size_t>(pair) * cap + i] = make_ulonglong2(k1, k2);
 }
 
+// bf_knn2_kernel for 256-D float rows, whose query does not fit in registers: it is read a chunk at a time (l2_chunked_rows,
+// l2_path.cuh), with kBfTile / 2 rows per tile so that the rows (32 KB) and their running totals (16 KB) fit the static shared memory.
+template <int DIM>
+__global__ void __launch_bounds__(kBfThreads)
+bf_knn2_l2_chunked_kernel(const uint32_t * __restrict__ A, const int * __restrict__ n_a, const uint32_t * __restrict__ B, const int * __restrict__ n_b,
+                          int cap, ulonglong2 * __restrict__ keys /* [n_pairs][cap] */)
+{
+	constexpr int kTile = kBfTile / 2;
+	__shared__ __align__(16) float s_rows[kTile * DIM];
+	__shared__ float s_acc[kTile * kBfThreads];
+	const int pair = blockIdx.y, tid = threadIdx.x;
+	const int na = min(n_a[pair], cap), nb = min(n_b[pair], cap);
+	const int i = blockIdx.x * kBfThreads + tid;
+	if (blockIdx.x * kBfThreads >= na) return;
+	const float * q = reinterpret_cast<const float *>(A) + (static_cast<size_t>(pair) * cap + min(i, na - 1)) * DIM;
+	const float4 * b4 = reinterpret_cast<const float4 *>(B) + static_cast<size_t>(pair) * cap * (DIM / 4);
+	unsigned long long k1 = kKey64None, k2 = kKey64None;
+	for (int r0 = 0; r0 < nb; r0 += kTile)
+	{
+		const int nr = min(kTile, nb - r0);
+		__syncthreads();
+		for (int t = tid; t < nr * (DIM / 4); t += kBfThreads) reinterpret_cast<float4 *>(s_rows)[t] = b4[static_cast<size_t>(r0) * (DIM / 4) + t];
+		__syncthreads();
+		l2_chunked_rows<DIM, kBfThreads>(q, s_rows, nr, s_acc, tid);
+		for (int r = 0; r < nr; ++r) top2_insert64(k1, k2, pack64(s_acc[r * kBfThreads + tid], static_cast<uint32_t>(r0 + r)));
+	}
+	if (i < na) keys[static_cast<size_t>(pair) * cap + i] = make_ulonglong2(k1, k2);
+}
+
 // cross check: query q keeps its nearest train row t only if q is also the nearest query of t (ties -> lowest index on both sides).
 // query_keys[pair][q].x = (distance, t), train_keys[pair][t].x = (distance, q).
 __global__ void bf_cross_kernel(const ulonglong2 * __restrict__ query_keys, const ulonglong2 * __restrict__ train_keys, const int * __restrict__ n_query,

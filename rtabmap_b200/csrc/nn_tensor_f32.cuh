@@ -28,6 +28,26 @@
 // rounding, all far below 2^-15 (|q|^2 + |w|^2) + 4e-6:
 //     eps(q) = 1.02 * 2^-9 * |q| * Wmax + 2^-15 * (|q|^2 + Wmax^2) + 4e-6,      Wmax = largest |w| in the dictionary.
 // For unit-length descriptors eps ~ 2.1e-3 against nearest-neighbour distances of 1e-2 .. 1: the lists stay a few dozen rows long.
+//
+// D = 256 (SuperPoint).  Term (a) does not depend on D.  The terms of (b) grow with the length of the sums, and at 256 the lumped
+// 2^-15 is no longer shown to cover them, so 256 has its own constant (64 and 128 keep theirs: lcd_nn_f32_stats counts are observable).
+// Model: each of the K = 256 + 16 = 272 products of the tensor core's chain enters the fp32 accumulator with at most one rounding of
+// relative 2^-23 (truncation allowed) of a partial sum bounded by the sum of the terms' magnitudes, sum |2 q_i w_i| + |w|^2
+// <= 2 |q| Wmax + Wmax^2 (fp16 products are exact in fp32).  So the accumulation error is at most
+//     271 * 2^-23 * (2 |q| Wmax + Wmax^2) <= 6.5e-5 |q| Wmax + 3.3e-5 Wmax^2.
+// rtflann sums 4 squares per group and 64 groups: its distance d <= (|q| + Wmax)^2 carries at most 67 * 2^-24 * d <= 4.0e-6 (|q|^2 + Wmax^2)
+// + 8.0e-6 |q| Wmax.  The fp32 norm |w|^2 (67 * 2^-24 relative) and its hi + lo split (2^-22 relative) add 4.3e-6 Wmax^2.  In total
+// 7.3e-5 |q| Wmax + 4.2e-5 Wmax^2 + 4.0e-6 |q|^2, which the 256 constant covers with room for the subnormal terms:
+//     eps256(q) = (1.02 * 2^-9 + 2^-13) * |q| * Wmax + 2^-14 * (|q|^2 + Wmax^2) + 4e-6          (2^-13 = 1.2e-4, 2^-14 = 6.1e-5)
+// For unit-length rows eps256 ~ 2.24e-3 against 2.06e-3 with the 64 / 128 constant.
+//
+// Tiling at D = 256.  A 256-word tile is 128 KB of fp16, so two whole tiles per stage no longer fit: 64 KB query tile + 4 KB query slab
+// + 2 x (128 KB + 8 KB) = 340 KB against the H100's 227 KB per block.  The word tile is streamed in K slices instead: the image is
+// [tile][atom][rows][128 B], so one 128-byte swizzle atom (64 halves) of all 256 rows is one contiguous 32 KB bulk copy, and a ring of
+// 4 such stages holds one whole tile: 1 KB (alignment) + 64 KB + 4 KB + 4 x 32 KB + 8 KB word slab (with the last slice) + 512 B of
+// barriers = 205.5 KB.  The accumulators carry over the four slices of a tile; a stage is released as soon as the MMAs of the next
+// slice are issued and its own have completed, so the slices of the next tile stream in under the current tile's MMAs and epilogue.
+// The N = 256 epilogue is the one of 64 / 128.
 #pragma once
 #include "common.cuh"
 #include "l2_path.cuh"
@@ -54,9 +74,23 @@ struct TfCfg
 	static constexpr uint32_t b_bytes = kTfBN * DIM * 2;
 	static constexpr uint32_t a_aug_bytes = kTfBM * 32;    // one K-step (16 halves) per row, un-swizzled core-matrix layout
 	static constexpr uint32_t b_aug_bytes = kTfBN * 32;
-	static constexpr int stages = DIM == 64 ? 5 : 2;
-	static constexpr size_t smem = 1024 + a_bytes + a_aug_bytes + stages * (b_bytes + b_aug_bytes) + 512;
+	// 64 / 128: a stage holds a whole word tile and its augmentation slab.  256: a word tile is 128 KB, so a stage holds one K slice
+	// (one swizzle atom of all 256 rows, 32 KB, contiguous in the image) and the tile's slab sits beside the ring, written with the last
+	// slice; stages == slices, so slice k of every tile lands in stage k and the slab is covered by the last stage's barriers.
+	static constexpr int slices = DIM == 256 ? atoms : 1;
+	static constexpr uint32_t slice_bytes = b_bytes / slices;
+	static constexpr int stages = DIM == 64 ? 5 : DIM == 128 ? 2 : slices;
+	static constexpr uint32_t stage_bytes = slices == 1 ? b_bytes + b_aug_bytes : slice_bytes;
+	static constexpr uint32_t ring_bytes = stages * stage_bytes + (slices == 1 ? 0 : b_aug_bytes);
+	static constexpr size_t smem = 1024 + a_bytes + a_aug_bytes + ring_bytes + 512;
+	static_assert(slices == 1 || stages == slices, "the augmentation slab travels with the last stage");
 };
+
+// dynamic shared memory of the filter kernel at a descriptor width (0: the width has no filter)
+inline size_t tf_smem_bytes(int dim)
+{
+	return dim == 64 ? TfCfg<64>::smem : dim == 128 ? TfCfg<128>::smem : dim == 256 ? TfCfg<256>::smem : 0;
+}
 
 // order-preserving float <-> uint mapping (v can be negative), for atomicMin on the shared per-query bound
 __device__ __forceinline__ uint32_t f2ord(float f)
@@ -209,6 +243,10 @@ __device__ __forceinline__ void wg_mma_f16(float (&d)[128], uint64_t adesc, uint
 		: "memory");
 }
 
+// wait until at most N commit groups of this warpgroup's MMAs are pending
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
 struct TfArgs
 {
 	const uint4 * word_img;      // fp16 image of -2 w
@@ -236,12 +274,13 @@ knn2_tensor_f32_kernel(const TfArgs a)
 {
 	using Cfg = TfCfg<DIM>;
 	constexpr int kStages = Cfg::stages;
-	constexpr uint32_t kStageBytes = Cfg::b_bytes + Cfg::b_aug_bytes;
+	constexpr uint32_t kStageBytes = Cfg::stage_bytes;
 	extern __shared__ unsigned char smem_dyn[];
 	unsigned char * smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~static_cast<uintptr_t>(1023));
 	unsigned char * sA = smem;                                   // query tile, then its augmentation slab
 	unsigned char * sB = smem + Cfg::a_bytes + Cfg::a_aug_bytes; // stages of (word tile, augmentation slab)
-	uint64_t * bars = reinterpret_cast<uint64_t *>(sB + kStages * kStageBytes);
+	unsigned char * sBaug = sB + kStages * kStageBytes;          // 256: the word tile's augmentation slab
+	uint64_t * bars = reinterpret_cast<uint64_t *>(sB + Cfg::ring_bytes);
 	uint64_t * full = bars;                     // [kStages] word tile landed
 	uint64_t * empty = full + kStages;          // [kStages] word tile consumed by both consumer warpgroups
 	uint64_t * afull = empty + kStages;         // [1] query tile landed
@@ -272,17 +311,38 @@ knn2_tensor_f32_kernel(const TfArgs a)
 			bulk_g2s(sA, reinterpret_cast<const unsigned char *>(a.query_img) + static_cast<size_t>(qtile) * Cfg::a_bytes, Cfg::a_bytes, afull);
 			bulk_g2s(sA + Cfg::a_bytes, reinterpret_cast<const unsigned char *>(a.query_aug) + static_cast<size_t>(qtile) * Cfg::a_aug_bytes,
 			         Cfg::a_aug_bytes, afull);
-			for (int t = 0; t < n_tiles; ++t)
+			if constexpr (Cfg::slices == 1)
 			{
-				const int s = t % kStages;
-				if (t >= kStages) mbar_wait(&empty[s], ((t / kStages) - 1) & 1);
-				mbar_arrive_expect_tx(&full[s], kStageBytes);
-				const unsigned char * src = reinterpret_cast<const unsigned char *>(a.word_img) + static_cast<size_t>(tile_begin + t) * Cfg::b_bytes;
-				unsigned char * dst = sB + s * kStageBytes;
-				bulk_g2s(dst, src, Cfg::b_bytes / 2, &full[s]);
-				bulk_g2s(dst + Cfg::b_bytes / 2, src + Cfg::b_bytes / 2, Cfg::b_bytes / 2, &full[s]);
-				bulk_g2s(dst + Cfg::b_bytes, reinterpret_cast<const unsigned char *>(a.word_aug) + static_cast<size_t>(tile_begin + t) * Cfg::b_aug_bytes,
-				         Cfg::b_aug_bytes, &full[s]);
+				for (int t = 0; t < n_tiles; ++t)
+				{
+					const int s = t % kStages;
+					if (t >= kStages) mbar_wait(&empty[s], ((t / kStages) - 1) & 1);
+					mbar_arrive_expect_tx(&full[s], kStageBytes);
+					const unsigned char * src = reinterpret_cast<const unsigned char *>(a.word_img) + static_cast<size_t>(tile_begin + t) * Cfg::b_bytes;
+					unsigned char * dst = sB + s * kStageBytes;
+					bulk_g2s(dst, src, Cfg::b_bytes / 2, &full[s]);
+					bulk_g2s(dst + Cfg::b_bytes / 2, src + Cfg::b_bytes / 2, Cfg::b_bytes / 2, &full[s]);
+					bulk_g2s(dst + Cfg::b_bytes, reinterpret_cast<const unsigned char *>(a.word_aug) + static_cast<size_t>(tile_begin + t) * Cfg::b_aug_bytes,
+					         Cfg::b_aug_bytes, &full[s]);
+				}
+			}
+			else
+			{
+				// slice g of the launch = K slice g % slices of word tile g / slices; the image is [tile][atom][rows][128 B], so a slice
+				// is one contiguous copy
+				for (int g = 0; g < n_tiles * Cfg::slices; ++g)
+				{
+					const int s = g % kStages, t = g / Cfg::slices, k = g % Cfg::slices;
+					const bool last = k == Cfg::slices - 1;
+					if (g >= kStages) mbar_wait(&empty[s], ((g / kStages) - 1) & 1);
+					mbar_arrive_expect_tx(&full[s], Cfg::slice_bytes + (last ? Cfg::b_aug_bytes : 0u));
+					bulk_g2s(sB + s * kStageBytes,
+					         reinterpret_cast<const unsigned char *>(a.word_img) + static_cast<size_t>(tile_begin + t) * Cfg::b_bytes + static_cast<size_t>(k) * Cfg::slice_bytes,
+					         Cfg::slice_bytes, &full[s]);
+					if (last)
+						bulk_g2s(sBaug, reinterpret_cast<const unsigned char *>(a.word_aug) + static_cast<size_t>(tile_begin + t) * Cfg::b_aug_bytes, Cfg::b_aug_bytes,
+						         &full[s]);
+				}
 			}
 		}
 		return;
@@ -307,7 +367,11 @@ knn2_tensor_f32_kernel(const TfArgs a)
 		if (live[h])
 		{
 			const float q2 = a.qn[qi[h]], w2 = __uint_as_float(*a.wmax2_bits);
-			const float eps = 1.02f * 0.001953125f * sqrtf(q2) * sqrtf(w2) + 3.0517578125e-05f * (q2 + w2) + 4.0e-6f;
+			float eps;
+			if constexpr (DIM == 256)
+				eps = (1.02f * 0.001953125f + 1.220703125e-04f) * sqrtf(q2) * sqrtf(w2) + 6.103515625e-05f * (q2 + w2) + 4.0e-6f;
+			else
+				eps = 1.02f * 0.001953125f * sqrtf(q2) * sqrtf(w2) + 3.0517578125e-05f * (q2 + w2) + 4.0e-6f;
 			margin[h] = 2.0f * eps;
 			t2[h] = ord2f(a.tau[qi[h]]);
 		}
@@ -322,23 +386,52 @@ knn2_tensor_f32_kernel(const TfArgs a)
 	mbar_wait(afull, 0);
 	for (int t = 0; t < n_tiles; ++t)
 	{
-		const int s = t % kStages;
-		mbar_wait(&full[s], (t / kStages) & 1);
-		__syncwarp(); // wgmma is .aligned: the warp issues it converged
-		const uint32_t b_base = smem_u32(sB + s * kStageBytes);
-		wg_fence();
-#pragma unroll
-		for (int ks = 0; ks < DIM / 16; ++ks)
+		if constexpr (Cfg::slices == 1)
 		{
-			const uint32_t atom = ks >> 2, koff = (ks & 3) * 32; // 16 halves = 32 bytes per K step, 4 steps per 128-byte atom
-			wg_mma_f16(acc, wg_smem_desc(a_base + atom * (kTfBM * 128) + koff), wg_smem_desc(b_base + atom * (kTfBN * 128) + koff), ks > 0 ? 1u : 0u);
+			const int s = t % kStages;
+			mbar_wait(&full[s], (t / kStages) & 1);
+			__syncwarp(); // wgmma is .aligned: the warp issues it converged
+			const uint32_t b_base = smem_u32(sB + s * kStageBytes);
+			wg_fence();
+#pragma unroll
+			for (int ks = 0; ks < DIM / 16; ++ks)
+			{
+				const uint32_t atom = ks >> 2, koff = (ks & 3) * 32; // 16 halves = 32 bytes per K step, 4 steps per 128-byte atom
+				wg_mma_f16(acc, wg_smem_desc(a_base + atom * (kTfBM * 128) + koff), wg_smem_desc(b_base + atom * (kTfBN * 128) + koff), ks > 0 ? 1u : 0u);
+			}
+			// the augmentation K-step: + kTfAugScale * (hi + lo) = + |w|^2
+			wg_mma_f16(acc, a_aug, wg_smem_desc_noswz(b_base + Cfg::b_bytes), 1u);
+			wg_commit();
+			wg_wait_all();
+			// the stage is free as soon as the MMAs have completed: the accumulators are in registers
+			if (et == 0) mbar_arrive(&empty[s]);
 		}
-		// the augmentation K-step: + kTfAugScale * (hi + lo) = + |w|^2
-		wg_mma_f16(acc, a_aug, wg_smem_desc_noswz(b_base + Cfg::b_bytes), 1u);
-		wg_commit();
-		wg_wait_all();
-		// the stage is free as soon as the MMAs have completed: the accumulators are in registers
-		if (et == 0) mbar_arrive(&empty[s]);
+		else
+		{
+			// the accumulators carry over the K slices of the tile; a slice's stage is released as soon as the MMAs of the next slice
+			// are issued and its own have completed (one commit group per slice)
+#pragma unroll
+			for (int k = 0; k < Cfg::slices; ++k)
+			{
+				const int g = t * Cfg::slices + k, s = g % kStages;
+				mbar_wait(&full[s], (g / kStages) & 1);
+				__syncwarp();
+				const uint32_t b_base = smem_u32(sB + s * kStageBytes);
+				wg_fence();
+#pragma unroll
+				for (int ks = 0; ks < 4; ++ks)
+					wg_mma_f16(acc, wg_smem_desc(a_base + k * (kTfBM * 128) + ks * 32), wg_smem_desc(b_base + ks * 32), (k > 0 || ks > 0) ? 1u : 0u);
+				if (k == Cfg::slices - 1) wg_mma_f16(acc, a_aug, wg_smem_desc_noswz(smem_u32(sBaug)), 1u);
+				wg_commit();
+				if (k > 0)
+				{
+					wg_wait<1>();
+					if (et == 0) mbar_arrive(&empty[(g - 1) % kStages]);
+				}
+			}
+			wg_wait<0>();
+			if (et == 0) mbar_arrive(&empty[(t * Cfg::slices + Cfg::slices - 1) % kStages]);
+		}
 		const int row0 = (tile_begin + t) * kTfBN;
 #pragma unroll
 		for (int h = 0; h < 2; ++h)
@@ -401,7 +494,9 @@ __global__ void rerank_l2_kernel(const float * __restrict__ vocab, int row_offse
 	for (int c = lane; c < n; c += 32)
 	{
 		const uint32_t row = cand[static_cast<size_t>(qi) * kTfCandCap + c];
-		const float d = l2_rtflann<DIM>(q, vocab + static_cast<size_t>(row) * DIM);
+		float d;
+		if constexpr (DIM > 128) d = l2_ptr_vs_stream<DIM>(q, vocab + static_cast<size_t>(row) * DIM); // fully unrolled, 256-D spills
+		else d = l2_rtflann<DIM>(q, vocab + static_cast<size_t>(row) * DIM);
 		top2_insert64(k1, k2, pack64(d, static_cast<uint32_t>(row_offset) + row));
 	}
 #pragma unroll
@@ -419,21 +514,25 @@ __global__ void rerank_l2_kernel(const float * __restrict__ vocab, int row_offse
 // S row-splits x G query-group slots (S as large as the scratch allows: one overflowing query still uses every SM).  A CTA takes
 // kFbQueries queries at a time and streams its share of the vocabulary once for all of them: 256-row tiles are loaded coalesced
 // into (padded) shared memory, thread t then computes row t against every query in rtflann's summation order.  The per-split results
-// are merged by knn2_l2_fallback_merge_kernel.  Dynamic shared memory: 256 * (DIM + 1) + kFbQueries * DIM floats.
+// are merged by knn2_l2_fallback_merge_kernel.  Dynamic shared memory: R * (DIM + 1) + kFbQueries * DIM floats, R = fallback_rows<DIM>()
+// rows per tile and threads per CTA (256; 128 at 256-D, where 256 rows would need 267 KB).
 constexpr int kFbQueries = 4;
 template <int DIM>
-__host__ __device__ constexpr size_t fallback_smem_bytes() { return (256 * (DIM + 1) + kFbQueries * DIM) * sizeof(float); }
+__host__ __device__ constexpr int fallback_rows() { return DIM == 256 ? 128 : 256; }
+template <int DIM>
+__host__ __device__ constexpr size_t fallback_smem_bytes() { return (fallback_rows<DIM>() * (DIM + 1) + kFbQueries * DIM) * sizeof(float); }
 
 __device__ __forceinline__ int fallback_splits(int n_fb, int n_ctas, int slots) { return max(1, min(n_ctas, slots / max(n_fb, 1))); }
 
 template <int DIM>
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(fallback_rows<DIM>())
 knn2_l2_fallback_kernel(const float * __restrict__ vocab, int n_rows, int row_offset, const float * __restrict__ queries,
                         const int * __restrict__ fb_list, const int * __restrict__ fb_count, ulonglong2 * __restrict__ scratch, int slots)
 {
 	extern __shared__ __align__(16) float fb_smem[];
-	float * s_rows = fb_smem;                    // [256][DIM + 1]
-	float * s_q = fb_smem + 256 * (DIM + 1);     // [kFbQueries][DIM]
+	constexpr int kRows = fallback_rows<DIM>();
+	float * s_rows = fb_smem;                    // [kRows][DIM + 1]
+	float * s_q = fb_smem + kRows * (DIM + 1);   // [kFbQueries][DIM]
 	__shared__ unsigned long long s_k1[kFbQueries][8], s_k2[kFbQueries][8];
 	const int n_fb = *fb_count;
 	if (n_fb <= 0) return;
@@ -442,21 +541,21 @@ knn2_l2_fallback_kernel(const float * __restrict__ vocab, int n_rows, int row_of
 	const int split = blockIdx.x % S, gslot = blockIdx.x / S, n_gslots = gridDim.x / S;
 	if (gslot >= n_gslots) return;
 	const int n_groups = (n_fb + kFbQueries - 1) / kFbQueries;
-	const int n_tiles = (n_rows + 255) / 256;
+	const int n_tiles = (n_rows + kRows - 1) / kRows;
 	for (int g = gslot; g < n_groups; g += n_gslots)
 	{
 		const int nqg = min(kFbQueries, n_fb - g * kFbQueries);
 		__syncthreads();
-		for (int i = tid; i < nqg * DIM; i += 256) s_q[i] = queries[static_cast<size_t>(fb_list[g * kFbQueries + i / DIM]) * DIM + (i % DIM)];
+		for (int i = tid; i < nqg * DIM; i += kRows) s_q[i] = queries[static_cast<size_t>(fb_list[g * kFbQueries + i / DIM]) * DIM + (i % DIM)];
 		unsigned long long k1[kFbQueries], k2[kFbQueries];
 #pragma unroll
 		for (int j = 0; j < kFbQueries; ++j) k1[j] = k2[j] = kKey64None;
 		for (int t = split; t < n_tiles; t += S)
 		{
-			const int r0 = t * 256;
-			const int nr = min(256, n_rows - r0);
+			const int r0 = t * kRows;
+			const int nr = min(kRows, n_rows - r0);
 			__syncthreads();
-			for (int i = tid; i < nr * (DIM / 4); i += 256)
+			for (int i = tid; i < nr * (DIM / 4); i += kRows)
 			{
 				const int r = i / (DIM / 4), c = (i % (DIM / 4)) * 4;
 				const float4 v = *reinterpret_cast<const float4 *>(vocab + static_cast<size_t>(r0 + r) * DIM + c);
@@ -501,7 +600,7 @@ knn2_l2_fallback_kernel(const float * __restrict__ vocab, int n_rows, int row_of
 		if (tid < nqg)
 		{
 			unsigned long long a1 = kKey64None, a2 = kKey64None;
-			for (int w = 0; w < 8; ++w)
+			for (int w = 0; w < kRows / 32; ++w)
 			{
 				top2_insert64(a1, a2, s_k1[tid][w]);
 				top2_insert64(a1, a2, s_k2[tid][w]);

@@ -480,7 +480,7 @@ pair_match_kernel(const MatchArgs a)
 //   to_dict_knn2_l2_kernel   TO side, the 2-NN of every TO descriptor over the FROM words, exact, keys pack64(d, k) (ties -> lowest k)
 //   pair_match_l2_kernel     TO side, the NNDR decision and the new-word loop of addNewWords(descriptorsTo, 2), then the
 //                            correspondences into exactly the outputs pair_match_kernel writes
-constexpr int kL2ScanThreads = 128; // TO descriptors per CTA of the 2-NN scan, one per thread (DIM floats in registers)
+constexpr int kL2ScanThreads = 128; // TO descriptors per CTA of the 2-NN scan, one per thread (DIM floats in registers up to 128-D)
 constexpr int kL2ScanWords = 32;    // dictionary words staged per shared-memory tile of the scan
 
 __host__ __device__ inline size_t from_dict_l2_smem_bytes(int rows)
@@ -561,29 +561,48 @@ to_dict_knn2_l2_kernel(const MatchArgs a, ulonglong2 * __restrict__ keys)
 	const size_t fbase = static_cast<size_t>(frow >= 0 ? frow : 0) * a.src.from.cap;
 	const float4 * F4 = reinterpret_cast<const float4 *>(a.src.from.desc + fbase * DIM);
 	const uint16_t * creator = a.from_creator + fbase;
-	float q[DIM];
-	{
-		const float4 * t4 = reinterpret_cast<const float4 *>(a.src.to.desc + (a.src.to_base(pair) + min(j, nt - 1)) * DIM);
-#pragma unroll
-		for (int v = 0; v < DIM / 4; ++v)
-		{
-			const float4 x = t4[v];
-			q[4 * v] = x.x;
-			q[4 * v + 1] = x.y;
-			q[4 * v + 2] = x.z;
-			q[4 * v + 3] = x.w;
-		}
-	}
+	const float * tq = reinterpret_cast<const float *>(a.src.to.desc + (a.src.to_base(pair) + min(j, nt - 1)) * DIM);
 	unsigned long long k1 = kKey64None, k2 = kKey64None;
 	float4 * s_w4 = reinterpret_cast<float4 *>(s_w);
-	for (int w0 = 0; w0 < n_dict; w0 += kL2ScanWords)
+	if constexpr (DIM > 128)
 	{
-		const int nw = min(kL2ScanWords, n_dict - w0);
-		__syncthreads();
-		for (int i = tid; i < nw * (DIM / 4); i += kL2ScanThreads)
-			s_w4[i] = F4[static_cast<size_t>(creator[w0 + i / (DIM / 4)]) * (DIM / 4) + i % (DIM / 4)];
-		__syncthreads();
-		for (int r = 0; r < nw; ++r) top2_insert64(k1, k2, pack64(l2_reg_vs_stream<DIM>(q, s_w + r * DIM), static_cast<uint32_t>(w0 + r)));
+		// 256-D: the TO descriptor is read a chunk at a time (l2_chunked_rows); 32 KB of words + 16 KB of running totals
+		__shared__ float s_acc[kL2ScanWords * kL2ScanThreads];
+		for (int w0 = 0; w0 < n_dict; w0 += kL2ScanWords)
+		{
+			const int nw = min(kL2ScanWords, n_dict - w0);
+			__syncthreads();
+			for (int i = tid; i < nw * (DIM / 4); i += kL2ScanThreads)
+				s_w4[i] = F4[static_cast<size_t>(creator[w0 + i / (DIM / 4)]) * (DIM / 4) + i % (DIM / 4)];
+			__syncthreads();
+			l2_chunked_rows<DIM, kL2ScanThreads>(tq, s_w, nw, s_acc, tid);
+			for (int r = 0; r < nw; ++r) top2_insert64(k1, k2, pack64(s_acc[r * kL2ScanThreads + tid], static_cast<uint32_t>(w0 + r)));
+		}
+	}
+	else
+	{
+		float q[DIM];
+		{
+			const float4 * t4 = reinterpret_cast<const float4 *>(tq);
+#pragma unroll
+			for (int v = 0; v < DIM / 4; ++v)
+			{
+				const float4 x = t4[v];
+				q[4 * v] = x.x;
+				q[4 * v + 1] = x.y;
+				q[4 * v + 2] = x.z;
+				q[4 * v + 3] = x.w;
+			}
+		}
+		for (int w0 = 0; w0 < n_dict; w0 += kL2ScanWords)
+		{
+			const int nw = min(kL2ScanWords, n_dict - w0);
+			__syncthreads();
+			for (int i = tid; i < nw * (DIM / 4); i += kL2ScanThreads)
+				s_w4[i] = F4[static_cast<size_t>(creator[w0 + i / (DIM / 4)]) * (DIM / 4) + i % (DIM / 4)];
+			__syncthreads();
+			for (int r = 0; r < nw; ++r) top2_insert64(k1, k2, pack64(l2_reg_vs_stream<DIM>(q, s_w + r * DIM), static_cast<uint32_t>(w0 + r)));
+		}
 	}
 	if (j < nt) keys[static_cast<size_t>(pair) * a.cap + j] = make_ulonglong2(k1, k2);
 }
