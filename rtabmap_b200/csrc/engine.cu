@@ -900,7 +900,10 @@ int run_knn(lcd_engine * e, const uint32_t * d_q, int nq_total, int n_rows, int 
 			const int real_sp = (n_wtiles + tps - 1) / tps;
 			if (real_sp != sp) continue;
 			const long waves = (static_cast<long>(n_qtiles) * sp + e->sm_count - 1) / e->sm_count;
-			const long cost = waves * (tps + 3); // +3: prologue (barrier init, first loads) and drain, in tile times
+			// +2: prologue (barrier init, first loads) and drain, in tile times.  That fixed cost was 3 tiles of 128 queries; a tile of
+			// 256 queries takes 1.65 of those (1.09 ms per launch at the bench shape where 128-query tiles took 1.32 ms, H100 80GB HBM3
+			// at 700 W), so 3 / 1.65 = 1.8, rounded to 2.
+			const long cost = waves * (tps + 2);
 			if (best_cost < 0 || cost < best_cost)
 			{
 				best_cost = cost;
@@ -931,13 +934,14 @@ int run_knn(lcd_engine * e, const uint32_t * d_q, int nq_total, int n_rows, int 
 		// A CTA walks several (query tile, word split) items with one set of barriers and a running pipeline (LCD_NN_PERSIST=0: one CTA
 		// per item, as r01).  Unsharded: one CTA per SM takes them all.  Inside the sharded step the search runs beside NCCL kernels that
 		// need a few SMs now and then: a grid that holds every SM until the end starves them and then waits for them (measured at 4 ranks:
-		// 1.35 -> 1.48 ms), so there a CTA takes only enough items for ~96 word tiles and the grid stays several waves deep.
+		// 1.35 -> 1.48 ms), so there a CTA takes only enough items for ~48 word tiles of 256 queries (the time ~96 tiles of 128 queries
+		// took) and the grid stays several waves deep.
 		static const int nn_persist = env_int("LCD_NN_PERSIST", 1);
 		const int n_items = n_qtiles * best_split;
 		int grid = n_items;
 		if (nn_persist && e->comm)
 		{
-			const int per_cta = std::max(1, std::min(8, (96 + tps - 1) / std::max(tps, 1))); // items per CTA: 1 / 2 / 4 at 2 / 4 / 8 ranks of C2
+			const int per_cta = std::max(1, std::min(8, (48 + tps - 1) / std::max(tps, 1))); // items per CTA
 			grid = (n_items + per_cta - 1) / per_cta;
 		}
 		else if (nn_persist)
