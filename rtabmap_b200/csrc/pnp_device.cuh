@@ -185,24 +185,65 @@ __device__ inline void sym_eigen(double * a, double * z, int * ord, long long * 
 	// The QL sweeps are data dependent (iterations per eigenvalue, deflation point m).  Lanes of a warp that drift apart
 	// here would serialise, so every iteration starts from a warp vote: lanes that have converged on this l idle through
 	// the iteration instead of running ahead.  The arithmetic of each lane is untouched.
+	//
+	// d[] and e[] stay in registers: every access below has a compile-time index.  The rotation sweep i = m-1 .. l is unrolled over
+	// all N-1 positions, each guarded by l <= i < m, and the reads and writes at the run-time positions l and m go through
+	// select loops (sel / put).  Column i+1 of z that the previous rotation produced is carried in zc[] instead of being stored
+	// and loaded back (zc is stored once the sweep ends), and column i is loaded one rotation ahead, so z's local-memory traffic is
+	// off the rotation chain.
+	const auto sel = [](const double (&v)[N], int i) {
+		double r = v[0];
+#pragma unroll
+		for (int k = 1; k < N; ++k)
+			if (k == i) r = v[k];
+		return r;
+	};
+	const auto put = [](double (&v)[N], int i, double x) {
+#pragma unroll
+		for (int k = 0; k < N; ++k)
+			if (k == i) v[k] = x;
+	};
 	for (int l = 0; l < N; ++l)
 	{
 		for (int iter = 0; iter < 60; ++iter)
 		{
-			int m = l;
-			for (; m + 1 < N; ++m)
-				if (fabs(e[m]) <= 2.220446049250313e-16 * (fabs(d[m]) + fabs(d[m + 1]))) break;
+			int m = N - 1;
+			bool found = false;
+#pragma unroll
+			for (int k = 0; k + 1 < N; ++k)
+				if (!found && k >= l && fabs(e[k]) <= 2.220446049250313e-16 * (fabs(d[k]) + fabs(d[k + 1])))
+				{
+					m = k;
+					found = true;
+				}
 			const bool done = m == l;
 			if (__all_sync(mask, done)) break;
 			if (!done)
 			{
-				double g = (d[l + 1] - d[l]) / (2.0 * e[l]);
+				double g = (sel(d, l + 1) - sel(d, l)) / (2.0 * sel(e, l));
 				double r = sqrt(g * g + 1.0);
-				g = d[m] - d[l] + e[l] / (g + (g >= 0 ? r : -r));
+				g = sel(d, m) - sel(d, l) + sel(e, l) / (g + (g >= 0 ? r : -r));
 				double sn = 1.0, cs = 1.0, pp = 0.0;
 				bool underflow = false;
-				for (int i = m - 1; i >= l; --i)
+				double zc[N], zp[N];
+				int cz = m; // the column of z that zc holds
+#pragma unroll
+				for (int k = 0; k < N; ++k)
 				{
+					zc[k] = z[k * N + m];
+					zp[k] = z[k * N + m - 1];
+				}
+#pragma unroll
+				for (int i = N - 2; i >= 0; --i)
+				{
+					if (underflow || i >= m || i < l) continue;
+					double zi[N]; // column i of z, loaded one rotation ahead; column i-1 is loaded now for the next rotation
+#pragma unroll
+					for (int k = 0; k < N; ++k)
+					{
+						zi[k] = zp[k];
+						if (i > 0) zp[k] = z[k * N + i - 1];
+					}
 					double f = sn * e[i];
 					const double b = cs * e[i];
 					r = sqrt(f * f + g * g);
@@ -210,9 +251,9 @@ __device__ inline void sym_eigen(double * a, double * z, int * ord, long long * 
 					if (r == 0.0)
 					{
 						d[i + 1] -= pp;
-						e[m] = 0.0;
+						put(e, m, 0.0);
 						underflow = true;
-						break;
+						continue;
 					}
 					sn = f / r;
 					cs = g / r;
@@ -221,41 +262,57 @@ __device__ inline void sym_eigen(double * a, double * z, int * ord, long long * 
 					pp = sn * r;
 					d[i + 1] = g + pp;
 					g = cs * r - b;
-					// columns i, i+1 of z: loads first, then arithmetic and stores (off the critical chain)
-					double zi[N], zj[N];
+					// columns i, i+1 of z (off the critical chain): column i is loaded, column i+1 is the carried one
 #pragma unroll
 					for (int k = 0; k < N; ++k)
 					{
-						zi[k] = z[k * N + i];
-						zj[k] = z[k * N + i + 1];
+						z[k * N + i + 1] = sn * zi[k] + cs * zc[k];
+						zc[k] = cs * zi[k] - sn * zc[k];
 					}
-#pragma unroll
-					for (int k = 0; k < N; ++k)
-					{
-						z[k * N + i + 1] = sn * zi[k] + cs * zj[k];
-						z[k * N + i] = cs * zi[k] - sn * zj[k];
-					}
+					cz = i;
 				}
+#pragma unroll
+				for (int k = 0; k < N; ++k) z[k * N + cz] = zc[k];
 				if (!underflow)
 				{
-					d[l] -= pp;
-					e[l] = g;
-					e[m] = 0.0;
+					put(d, l, sel(d, l) - pp);
+					put(e, l, g);
+					put(e, m, 0.0);
 				}
 			}
 		}
 	}
+#pragma unroll
 	for (int i = 0; i < N; ++i) a[i * N + i] = d[i];
-	for (int i = 0; i < N; ++i) ord[i] = i;
+	int o[N];
+#pragma unroll
+	for (int i = 0; i < N; ++i) o[i] = i;
+#pragma unroll
 	for (int i = 0; i < N - 1; ++i) // selection sort, descending, stable
 	{
 		int j = i;
+		double dj = sel(d, o[i]);
+#pragma unroll
 		for (int k = i + 1; k < N; ++k)
-			if (d[ord[k]] > d[ord[j]]) j = k;
-		const int t = ord[j];
-		for (int k = j; k > i; --k) ord[k] = ord[k - 1];
-		ord[i] = t;
+		{
+			const double dk = sel(d, o[k]);
+			if (dk > dj)
+			{
+				j = k;
+				dj = dk;
+			}
+		}
+		int t = o[i];
+#pragma unroll
+		for (int k = i + 1; k < N; ++k)
+			if (k == j) t = o[k];
+#pragma unroll
+		for (int k = N - 1; k > i; --k)
+			if (k <= j) o[k] = o[k - 1];
+		o[i] = t;
 	}
+#pragma unroll
+	for (int i = 0; i < N; ++i) ord[i] = o[i];
 }
 
 // minimum-norm least squares of A x = b, A is M x N row-major (cvSolve(..., CV_SVD))
