@@ -126,7 +126,7 @@ int lcd_orb_overflow(lcd_engine * e);
 /* Which kernels the last detection used (bit flags; diagnostics for tests and benchmarks): 1 = FAST and blur tiles staged by TMA with a
  * tensor map (rows a multiple of 16 bytes), 2 = descriptors from shared-memory patches (rows a multiple of 4 bytes on every level, edge
  * threshold >= 19), 4 = vectorised gray / mask preparation (rows a multiple of 8 pixels, even height), 8 = the GFTT/ORB detector
- * (lcd_detector_set).  0 = the general kernels. */
+ * (lcd_detector_set), 16 = the ORB-OCTREE detector (lcd_detector_set_orb_octree; no other bit is set then).  0 = the general kernels. */
 int lcd_orb_last_path(const lcd_engine * e);
 
 /* ---- detect: the detector of every image-level call -----------------------------------------
@@ -154,6 +154,28 @@ typedef struct lcd_gftt_params {
 int lcd_detector_set(lcd_engine * e, int detector, const lcd_gftt_params * params);
 /* The selected detector; `params` (may be NULL) receives its GFTT parameters. */
 int lcd_detector_get(const lcd_engine * e, lcd_gftt_params * params);
+
+/* LCD_DETECTOR_ORB_OCTREE: Kp/DetectorStrategy=10, rtabmap::ORBOctree (Features2d.cpp:2479-2566) around RTAB-Map's ORB-SLAM2 extractor
+ * (corelib/src/opencv/ORBextractor.cc).  lcd_orb_params supplies n_features (nfeatures and Kp/MaxFeatures), n_levels (1..8), scale_factor
+ * (any finite value > 1), edge_threshold (>= 19), fast_threshold (the initial FAST threshold), patch_size (31) and the depth fields.
+ *   pyramid   level l = cv::resize(level l-1, cvRound(size / scale_factor^l), INTER_LINEAR)          ORBextractor.cc:1114-1139
+ *   keypoints FAST per 30-pixel cell with FAST/MinThreshold as fallback, spread by a quadtree      :772-855, :546-770
+ *             (DistributeOctTree) to the per-level counts of the constructor                      :416-477
+ *   describe  IC angle, GaussianBlur(7x7, 2) of each level, steered BRIEF                          :83-153, :1066-1111
+ *   wrapper   detection ignores the mask; keypoints whose level-0 mask byte at the truncated      Features2d.cpp:2527-2549
+ *             coordinates is 0 are dropped, then limitKeypoints(Kp/MaxFeatures)
+ * Phase 2 of DistributeOctTree orders nodes of equal size by their heap addresses, which the reference leaves undefined; the engine treats
+ * the node created later as the larger one (DESIGN.md §2).  LCD_ERR_INVALID, before any launch, for n_levels outside 1..8, a scale factor
+ * <= 1 or not finite, patch_size != 31, edge_threshold < 19, and a level whose span inside edge_threshold - 3 is under 30 pixels or more
+ * than twice as tall as wide (the reference divides by zero or indexes out of range there).  n_features <= 0 is refused as for the other
+ * detectors (the reference would run it with every level's count at 0 and no limit). */
+#define LCD_DETECTOR_ORB_OCTREE 10
+/* Select ORB-OCTREE with FAST/MinThreshold (7 in RTAB-Map, 0..255; LCD_ERR_INVALID otherwise, the previous selection then stays).
+ * lcd_detector_set(e, LCD_DETECTOR_ORB_OCTREE, ...) is refused: this call selects it.  lcd_detector_get then returns 10. */
+int lcd_detector_set_orb_octree(lcd_engine * e, int fast_min_threshold);
+/* Test hook: cosf and sinf as the ORB-OCTREE descriptor computes them on the device, for the `count` floats whose bit patterns start at
+ * `first` (d_cos, d_sin: device arrays of `count` floats).  Synchronous. */
+int lcd_debug_orb_sincos(lcd_engine * e, unsigned first, unsigned count, float * d_cos, float * d_sin);
 
 /* ---- detect: which keypoints of a frame are quantised (Memory::createSignature, Memory.cpp:5945-6100) ---------------------------
  * With Mem/RawDescriptorsKept, an odometry pose and Kp/MaxFeatures < Vis/MaxFeatures, the reference detects Vis/MaxFeatures keypoints

@@ -64,8 +64,8 @@ class QuantizeLimit(C.Structure):
     _fields_ = [("max_features", C.c_int), ("bad_sign_ratio", C.c_float), ("mean_words", C.c_int)]
 
 
-# lcd_detector_set; depth type of a ready-made CV_8UC1 mask (lcd_b200.h)
-DETECTOR_ORB, DETECTOR_GFTT_ORB = 2, 8
+# lcd_detector_set / lcd_detector_set_orb_octree; depth type of a ready-made CV_8UC1 mask (lcd_b200.h)
+DETECTOR_ORB, DETECTOR_GFTT_ORB, DETECTOR_ORB_OCTREE = 2, 8, 10
 DEPTH_MASK_U8 = 3
 
 
@@ -204,6 +204,8 @@ SIGNATURES = {
     "lcd_orb_last_path": (_I, [_P]),
     "lcd_detector_set": (_I, [_P, _I, _P]),
     "lcd_detector_get": (_I, [_P, _P]),
+    "lcd_detector_set_orb_octree": (_I, [_P, _I]),
+    "lcd_debug_orb_sincos": (_I, [_P, C.c_uint, C.c_uint, _P, _P]),
     "lcd_quantize_limit_set": (_I, [_P, _P]),
     "lcd_quantize_limit_get": (_I, [_P, _P]),
     "lcd_limit_keypoints_dev": (_I, [_P, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
@@ -834,6 +836,15 @@ class Engine:
     def set_detector(self, detector: int, params: "GfttParams" = None):
         """DETECTOR_ORB (Kp/DetectorStrategy=2, the default) or DETECTOR_GFTT_ORB (8) for every image-level call of this engine"""
         self._check(self._lib.lcd_detector_set(self._h, int(detector), C.byref(params) if params is not None else None))
+
+    def set_detector_orb_octree(self, fast_min_threshold: int = 7):
+        """DETECTOR_ORB_OCTREE (Kp/DetectorStrategy=10) with FAST/MinThreshold for every image-level call of this engine; lcd_orb_params
+        supplies the rest (ORB/NLevels up to 8, any ORB/ScaleFactor > 1, FAST/Threshold as the initial threshold)"""
+        self._check(self._lib.lcd_detector_set_orb_octree(self._h, int(fast_min_threshold)))
+
+    def debug_orb_sincos(self, first: int, count: int, d_cos, d_sin):
+        """the ORB-OCTREE descriptor's cosf / sinf of the `count` floats from bit pattern `first` into device arrays (torch tensors)"""
+        self._check(self._lib.lcd_debug_orb_sincos(self._h, int(first), int(count), C.c_void_p(d_cos.data_ptr()), C.c_void_p(d_sin.data_ptr())))
 
     def detector(self):
         """(detector, GfttParams) currently selected"""

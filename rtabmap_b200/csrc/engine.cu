@@ -26,6 +26,7 @@
 #include "match_bf.cuh"
 #include "orb.cuh"
 #include "gftt.cuh"
+#include "orb_octree.cuh"
 #include "limit.cuh"
 
 #include <cuda.h>
@@ -508,6 +509,17 @@ struct lcd_engine
 	int orb_path = 0;     // lcd_orb_last_path flags of the last detection
 	int detector = LCD_DETECTOR_ORB; // lcd_detector_set: what orb_run detects
 	lcd_gftt_params gftt{0.001, 7.0, 3, 0, 0.04};
+	int oct_min_threshold = 7; // lcd_detector_set_orb_octree: FAST/MinThreshold
+	// ORB-OCTREE workspace (orb_octree.cuh)
+	DevBuf<OctCell> oc_cells;
+	std::vector<OctCell> oc_cells_host; // what oc_cells holds (uploaded again only when the geometry changes)
+	const OctCell * oc_cells_at = nullptr;
+	DevBuf<uint32_t> oc_keys, oc_kk, oc_sel;
+	DevBuf<int> oc_cell_n, oc_perm, oc_scratch, oc_cand, oc_expand, oc_sel_n;
+	DevBuf<OctNode> oc_nodes;
+	DevBuf<int4> oc_cnt;
+	DevBuf<OrbKeypoint> oc_raw_kp;
+	DevBuf<uint8_t> oc_raw_desc, oc_desc;
 	// lcd_quantize_limit_set: the split of Memory::createSignature for every image-level call (limit.cuh); ql_gate = int(ratio * mean_words)
 	lcd_quantize_limit ql{0, 0.0f, 0};
 	int ql_gate = 0;
@@ -2743,6 +2755,260 @@ static int gftt_corners(lcd_engine * e, int n_frames, const OrbPrepArgs & prep, 
 	return LCD_OK;
 }
 
+// dynamic shared memory of orb_oct_tree_kernel (phase-2 sort keys of the largest level's nodes) and orb_oct_finish_kernel (a frame's keys)
+static size_t octree_tree_smem(const OctGeom & g)
+{
+	int max_nodes = 0;
+	for (int l = 0; l < g.n_levels; ++l) max_nodes = std::max(max_nodes, g.node0[l + 1] - g.node0[l]);
+	size_t pad = 1;
+	while (pad < static_cast<size_t>(max_nodes)) pad <<= 1;
+	return pad * sizeof(unsigned long long);
+}
+static size_t octree_finish_smem(const OctGeom & g)
+{
+	size_t pad = 1;
+	while (pad < static_cast<size_t>(g.raw_cap)) pad <<= 1;
+	return pad * sizeof(unsigned long long);
+}
+
+// ORB-OCTREE's pyramid, cells and quadtree workspaces (ORBextractor.cc:416-477, :772-855, :1114-1139) on the host, with the inputs on which
+// the reference divides by zero, indexes out of range or reads outside a level refused
+static int octree_geometry(lcd_engine * e, int width, int height, const lcd_orb_params * p, OctGeom & g, std::vector<OctCell> & cells)
+{
+	if (p->n_levels < 1 || p->n_levels > kOctMaxLevels) LCD_FAIL(e, LCD_ERR_INVALID, "ORB/NLevels must be 1..%d for ORB-OCTREE", kOctMaxLevels);
+	if (!std::isfinite(p->scale_factor) || !(p->scale_factor > 1.0f)) LCD_FAIL(e, LCD_ERR_INVALID, "ORB/ScaleFactor must be finite and > 1");
+	if (p->patch_size != 31) LCD_FAIL(e, LCD_ERR_INVALID, "only ORB/PatchSize=31 is implemented");
+	// keypoints lie ORB/EdgeThreshold pixels inside a level and the rotated pattern reaches 18: the blurred clone has no border
+	if (p->edge_threshold < 19) LCD_FAIL(e, LCD_ERR_INVALID, "ORB-OCTREE needs ORB/EdgeThreshold >= 19");
+	if (p->fast_threshold < 0 || p->fast_threshold > 255) LCD_FAIL(e, LCD_ERR_INVALID, "FAST/Threshold must be 0..255");
+	// the reference runs Kp/MaxFeatures = 0 (every level's N is 0, no limit); the engine refuses it as it does for the other detectors,
+	// whose outputs are sized by it
+	if (p->n_features <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "Kp/MaxFeatures must be positive");
+	if (width <= 0 || height <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null image");
+	if (static_cast<long long>(width) * height >= (1 << 24)) LCD_FAIL(e, LCD_ERR_CAPACITY, "image too large");
+	g = OctGeom{};
+	g.n_levels = p->n_levels;
+	g.edge = p->edge_threshold;
+	g.thr_ini = p->fast_threshold;
+	g.thr_min = e->oct_min_threshold;
+	// the constructor's tables: float scale chain, float per-level counts
+	float scale[kOctMaxLevels], inv[kOctMaxLevels];
+	scale[0] = 1.0f;
+	for (int l = 1; l < p->n_levels; ++l) scale[l] = scale[l - 1] * p->scale_factor;
+	for (int l = 0; l < p->n_levels; ++l) inv[l] = 1.0f / scale[l];
+	const float factor = 1.0f / p->scale_factor;
+	float nd = p->n_features * (1 - factor) / (1 - static_cast<float>(pow(static_cast<double>(factor), static_cast<double>(p->n_levels))));
+	int sum = 0;
+	for (int l = 0; l < p->n_levels - 1; ++l)
+	{
+		g.n_per_level[l] = static_cast<int>(nearbyintf(nd));
+		sum += g.n_per_level[l];
+		nd *= factor;
+	}
+	g.n_per_level[p->n_levels - 1] = std::max(p->n_features - sum, 0);
+	{
+		const int half = 15;
+		const int vmax = static_cast<int>(floorf(half * sqrtf(2.f) / 2 + 1)), vmin = static_cast<int>(ceilf(half * sqrtf(2.f) / 2));
+		for (int v = 0; v <= vmax; ++v) g.umax[v] = static_cast<int>(nearbyint(sqrt(static_cast<double>(half * half - v * v))));
+		for (int v = half, v0 = 0; v >= vmin; --v)
+		{
+			while (g.umax[v0] == g.umax[v0 + 1]) ++v0;
+			g.umax[v] = v0;
+			++v0;
+		}
+	}
+	const int min_b = p->edge_threshold - 3;
+	int off = 0, key = 0, node = 0;
+	cells.clear();
+	for (int l = 0; l < p->n_levels; ++l)
+	{
+		const int w = static_cast<int>(nearbyintf(static_cast<float>(width) * inv[l])), h = static_cast<int>(nearbyintf(static_cast<float>(height) * inv[l]));
+		const int max_bx = w - p->edge_threshold + 3, max_by = h - p->edge_threshold + 3;
+		const int sw = max_bx - min_b, sh = max_by - min_b;
+		// nCols = (maxX - minX) / 30 and nRows must not be 0 (the cell size divides by them)
+		if (sw < 30 || sh < 30)
+			LCD_FAIL(e, LCD_ERR_INVALID, "ORB-OCTREE level %d is %dx%d: under 30 pixels remain inside ORB/EdgeThreshold", l, w, h);
+		// DistributeOctTree's initial node count round(w / h) must not be 0 (a level more than twice as tall as wide)
+		const int n_ini = static_cast<int>(roundf(static_cast<float>(sw) / static_cast<float>(sh)));
+		if (n_ini == 0) LCD_FAIL(e, LCD_ERR_INVALID, "ORB-OCTREE level %d is %dx%d: more than twice as tall as wide", l, w, h);
+		g.w[l] = w;
+		g.h[l] = h;
+		g.off[l] = off;
+		off += w * h;
+		g.scale[l] = scale[l];
+		g.size[l] = static_cast<int>(31 * scale[l]);
+		g.span_w[l] = sw;
+		g.span_h[l] = sh;
+		g.n_ini[l] = n_ini;
+		g.hx[l] = static_cast<float>(sw) / n_ini;
+		// ComputeKeyPointsOctTree's cells, in float arithmetic as the reference
+		const float W = 30, width_f = static_cast<float>(sw), height_f = static_cast<float>(sh);
+		const int n_cols = static_cast<int>(width_f / W), n_rows = static_cast<int>(height_f / W);
+		const int w_cell = static_cast<int>(ceilf(width_f / n_cols)), h_cell = static_cast<int>(ceilf(height_f / n_rows));
+		g.cell0[l] = static_cast<int>(cells.size());
+		g.key0[l] = key;
+		for (int i = 0; i < n_rows; ++i)
+		{
+			const float ini_y = static_cast<float>(min_b + i * h_cell);
+			float max_y = ini_y + h_cell + 6;
+			if (ini_y >= max_by - 3) continue;
+			if (max_y > max_by) max_y = static_cast<float>(max_by);
+			for (int j = 0; j < n_cols; ++j)
+			{
+				const float ini_x = static_cast<float>(min_b + j * w_cell);
+				float max_x = ini_x + w_cell + 6;
+				if (ini_x >= max_bx - 6) continue;
+				if (max_x > max_bx) max_x = static_cast<float>(max_bx);
+				OctCell c{static_cast<int>(ini_x), static_cast<int>(ini_y), static_cast<int>(max_x), static_cast<int>(max_y), j * w_cell, i * h_cell, key, l};
+				// strict 3x3 maxima of the cell's [3, n-3) window are never 8-adjacent
+				const int iw = std::max(c.x1 - c.x0 - 6, 0), ih = std::max(c.y1 - c.y0 - 6, 0);
+				key += ((iw + 1) / 2) * ((ih + 1) / 2);
+				cells.push_back(c);
+			}
+		}
+		g.node0[l] = node;
+		node += std::max(g.n_per_level[l] + 3, 4 * n_ini) + 4;
+	}
+	g.cell0[p->n_levels] = static_cast<int>(cells.size());
+	g.key0[p->n_levels] = key;
+	g.node0[p->n_levels] = node;
+	g.raw_cap = node;
+	g.frame_stride = (off + 15) & ~15;
+	if (g.raw_cap >= 65536) LCD_FAIL(e, LCD_ERR_CAPACITY, "ORB-OCTREE keeps at most 65535 keypoints per frame before Kp/MaxFeatures");
+	// the shared memory of the quadtree's phase-2 sort and of the final limit, checked before anything is launched
+	LCD_TRY(fit_smem(e, reinterpret_cast<const void *>(orb_oct_tree_kernel), octree_tree_smem(g), p->n_features));
+	LCD_TRY(fit_smem(e, reinterpret_cast<const void *>(orb_oct_finish_kernel), octree_finish_smem(g), p->n_features));
+	return LCD_OK;
+}
+
+// ORB-OCTREE (lcd_detector_set_orb_octree, Kp/DetectorStrategy=10): gray + mask, pyramid, FAST per cell, quadtree per level, angle, blur,
+// descriptors, then the mask and Kp/MaxFeatures of rtabmap::ORBOctree, and the 3-D points
+static int octree_run(lcd_engine * e, int n_frames, const uint8_t * d_images, int width, int height, int channels, const void * d_depth, int depth_type,
+                      const lcd_orb_params * p, int cap, OrbKeypoint * d_kp, uint8_t * d_desc, float * d_xyz, float * d_uv, int * d_n, cudaStream_t s)
+{
+	OctGeom g{};
+	std::vector<OctCell> cells;
+	LCD_TRY(octree_geometry(e, width, height, p, g, cells));
+	if (channels != 1 && channels != 3) LCD_FAIL(e, LCD_ERR_INVALID, "images must be 8UC1 or 8UC3 (BGR)");
+	if (cap <= 0 || cap > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "cap must be 1..%d", kMaxFrameQueries);
+	if (!d_depth) depth_type = LCD_DEPTH_NONE;
+	if (depth_type < LCD_DEPTH_NONE || depth_type > LCD_DEPTH_MASK_U8) LCD_FAIL(e, LCD_ERR_INVALID, "unknown depth type %d", depth_type);
+	const bool use_mask = depth_type == LCD_DEPTH_MASK_U8 || (depth_type != LCD_DEPTH_NONE && p->depth_as_mask);
+	const int n_cells = static_cast<int>(cells.size());
+	const int key_stride = g.key0[g.n_levels], node_stride = g.node0[g.n_levels];
+	const size_t pyr = static_cast<size_t>(n_frames) * g.frame_stride;
+	LCD_CUDA(e, e->o_gray.reserve(pyr, 0, false, s));
+	LCD_CUDA(e, e->o_blur.reserve(pyr, 0, false, s));
+	if (use_mask) LCD_CUDA(e, e->o_mask.reserve(pyr, 0, false, s));
+	LCD_CUDA(e, e->o_overflow.reserve(1, 0, true, s));
+	LCD_CUDA(e, zero_fill_async(e->o_overflow.p, sizeof(int), s)); // no cell can overflow its slot: the flag stays clear
+	if (!d_kp)
+	{
+		LCD_CUDA(e, e->o_kp.reserve(static_cast<size_t>(n_frames) * cap, 0, false, s));
+		d_kp = e->o_kp.p;
+	}
+	if (!d_n)
+	{
+		LCD_CUDA(e, e->o_n.reserve(n_frames, 0, false, s));
+		d_n = e->o_n.p;
+	}
+	if (!d_desc)
+	{
+		LCD_CUDA(e, e->oc_desc.reserve(static_cast<size_t>(n_frames) * cap * 32, 0, false, s));
+		d_desc = e->oc_desc.p;
+	}
+	const size_t keys = static_cast<size_t>(n_frames) * key_stride, nodes = static_cast<size_t>(n_frames) * node_stride;
+	LCD_CUDA(e, e->oc_cells.reserve(n_cells, 0, false, s));
+	LCD_CUDA(e, e->oc_cell_n.reserve(static_cast<size_t>(n_frames) * n_cells, 0, false, s));
+	LCD_CUDA(e, e->oc_keys.reserve(keys, 0, false, s));
+	LCD_CUDA(e, e->oc_kk.reserve(keys, 0, false, s));
+	LCD_CUDA(e, e->oc_perm.reserve(keys, 0, false, s));
+	LCD_CUDA(e, e->oc_scratch.reserve(keys, 0, false, s));
+	LCD_CUDA(e, e->oc_nodes.reserve(2 * nodes, 0, false, s));
+	LCD_CUDA(e, e->oc_cand.reserve(nodes, 0, false, s));
+	LCD_CUDA(e, e->oc_cnt.reserve(nodes, 0, false, s));
+	LCD_CUDA(e, e->oc_expand.reserve(nodes, 0, false, s));
+	LCD_CUDA(e, e->oc_sel.reserve(nodes, 0, false, s));
+	LCD_CUDA(e, e->oc_sel_n.reserve(static_cast<size_t>(n_frames) * g.n_levels, 0, false, s));
+	LCD_CUDA(e, e->oc_raw_kp.reserve(static_cast<size_t>(n_frames) * g.raw_cap, 0, false, s));
+	LCD_CUDA(e, e->oc_raw_desc.reserve(static_cast<size_t>(n_frames) * g.raw_cap * 32, 0, false, s));
+	if (e->oc_cells_at != e->oc_cells.p || e->oc_cells_host.size() != cells.size() ||
+	    std::memcmp(e->oc_cells_host.data(), cells.data(), cells.size() * sizeof(OctCell)) != 0)
+	{
+		// a new geometry (or a regrown buffer): the table is a few KB, copied once from the engine's own host copy, which outlives the copy
+		e->oc_cells_host = cells;
+		e->oc_cells_at = e->oc_cells.p;
+		LCD_CUDA(e, cudaMemcpyAsync(e->oc_cells.p, e->oc_cells_host.data(), n_cells * sizeof(OctCell), cudaMemcpyHostToDevice, s));
+	}
+	prof_mark(e, LCD_PROF_ORB, s);
+	e->orb_path = 16;
+	{
+		OrbPrepArgs prep{};
+		prep.images = d_images;
+		prep.channels = channels;
+		prep.depth = use_mask ? d_depth : nullptr;
+		prep.depth_type = depth_type;
+		prep.min_depth = p->min_depth;
+		prep.max_depth = p->max_depth;
+		prep.gray = e->o_gray.p;
+		prep.mask = use_mask ? e->o_mask.p : nullptr;
+		prep.g.n_levels = 1;
+		prep.g.w[0] = width;
+		prep.g.h[0] = height;
+		prep.g.frame_stride = g.frame_stride;
+		orb_oct_prepare_kernel<<<dim3((width + 31) / 32, (height + 7) / 8, n_frames), dim3(32, 8), 0, s>>>(prep);
+		LCD_CHECK_LAUNCH(e);
+	}
+	for (int l = 1; l < g.n_levels; ++l)
+	{
+		orb_oct_resize_kernel<<<dim3((g.w[l] + 31) / 32, (g.h[l] + 7) / 8, n_frames), dim3(32, 8), 0, s>>>(e->o_gray.p, g, l);
+		LCD_CHECK_LAUNCH(e);
+	}
+	orb_oct_fast_kernel<<<dim3(n_cells, n_frames), 256, 0, s>>>(e->o_gray.p, g, e->oc_cells.p, n_cells, key_stride, e->oc_keys.p, e->oc_cell_n.p);
+	LCD_CHECK_LAUNCH(e);
+	{
+		OctTreeArgs a{};
+		a.g = g;
+		a.keys = e->oc_keys.p;
+		a.cell_n = e->oc_cell_n.p;
+		a.cells = e->oc_cells.p;
+		a.n_cells = n_cells;
+		a.key_stride = key_stride;
+		a.node_stride = node_stride;
+		a.kk = e->oc_kk.p;
+		a.perm = e->oc_perm.p;
+		a.scratch = e->oc_scratch.p;
+		a.nodes = e->oc_nodes.p;
+		a.cand = e->oc_cand.p;
+		a.cnt = e->oc_cnt.p;
+		a.expand = e->oc_expand.p;
+		a.sel = e->oc_sel.p;
+		a.sel_n = e->oc_sel_n.p;
+		orb_oct_tree_kernel<<<dim3(g.n_levels, n_frames), kOctTreeThreads, octree_tree_smem(g), s>>>(a);
+		LCD_CHECK_LAUNCH(e);
+	}
+	for (int l = 0; l < g.n_levels; ++l)
+	{
+		orb_oct_blur_kernel<<<dim3((g.w[l] + 31) / 32, (g.h[l] + 7) / 8, n_frames), dim3(32, 8), 0, s>>>(e->o_gray.p, e->o_blur.p, g, l);
+		LCD_CHECK_LAUNCH(e);
+	}
+	{
+		int max_nodes = 0;
+		for (int l = 0; l < g.n_levels; ++l) max_nodes = std::max(max_nodes, g.node0[l + 1] - g.node0[l]);
+		orb_oct_describe_kernel<<<dim3((max_nodes + 7) / 8, g.n_levels, n_frames), 256, 0, s>>>(e->o_gray.p, e->o_blur.p, g, e->oc_sel.p, e->oc_sel_n.p,
+		                                                                                      node_stride, e->oc_raw_kp.p, e->oc_raw_desc.p);
+		LCD_CHECK_LAUNCH(e);
+	}
+	{
+		orb_oct_finish_kernel<<<n_frames, 1024, octree_finish_smem(g), s>>>(e->oc_raw_kp.p, e->oc_raw_desc.p, e->oc_sel_n.p, g,
+		                                                                               use_mask ? e->o_mask.p : nullptr, p->n_features, d_kp, d_desc, d_n, cap);
+		LCD_CHECK_LAUNCH(e);
+	}
+	LCD_TRY(orb_lift(e, n_frames, width, height, d_depth, depth_type, p, cap, d_kp, d_n, d_xyz, d_uv, s));
+	prof_mark(e, LCD_PROF_ORB, s);
+	return LCD_OK;
+}
+
 // Detect + describe a batch of frames with the engine's detector (lcd_detector_set): the FAST pyramid or GFTT's corners between the
 // shared preparation and the steered BRIEF descriptors and 3-D points.  A null d_kp / d_n detects into the engine's own buffers.
 static int orb_run(lcd_engine * e, int n_frames, const uint8_t * d_images, int width, int height, int channels, const void * d_depth,
@@ -2750,6 +3016,8 @@ static int orb_run(lcd_engine * e, int n_frames, const uint8_t * d_images, int w
                    int * d_n, cudaStream_t s)
 {
 	if (!p) LCD_FAIL(e, LCD_ERR_INVALID, "null ORB parameters");
+	if (e->detector == LCD_DETECTOR_ORB_OCTREE)
+		return octree_run(e, n_frames, d_images, width, height, channels, d_depth, depth_type, p, cap, d_kp, d_desc, d_xyz, d_uv, d_n, s);
 	const bool gftt = e->detector == LCD_DETECTOR_GFTT_ORB;
 	lcd_orb_params pl = *p;
 	if (gftt) pl.n_levels = 1; // cv::ORB::compute builds the levels its keypoints use: GFTT corners are all octave 0
@@ -2906,6 +3174,7 @@ int lcd_detector_set(lcd_engine * e, int detector, const lcd_gftt_params * param
 		e->detector = detector;
 		return LCD_OK;
 	}
+	if (detector == LCD_DETECTOR_ORB_OCTREE) LCD_FAIL(e, LCD_ERR_INVALID, "ORB-OCTREE is selected with lcd_detector_set_orb_octree");
 	if (detector != LCD_DETECTOR_GFTT_ORB) LCD_FAIL(e, LCD_ERR_INVALID, "unknown detector %d", detector);
 	const lcd_gftt_params q = params ? *params : lcd_gftt_params{0.001, 7.0, 3, 0, 0.04};
 	if (q.use_harris != 0) LCD_FAIL(e, LCD_ERR_INVALID, "GFTT/UseHarrisDetector is not implemented");
@@ -2914,6 +3183,26 @@ int lcd_detector_set(lcd_engine * e, int detector, const lcd_gftt_params * param
 	if (!(q.min_distance >= 0.0) || !std::isfinite(q.min_distance)) LCD_FAIL(e, LCD_ERR_INVALID, "GFTT/MinDistance must not be negative");
 	e->gftt = q;
 	e->detector = detector;
+	return LCD_OK;
+}
+
+int lcd_detector_set_orb_octree(lcd_engine * e, int fast_min_threshold)
+{
+	if (!e) return LCD_ERR_INVALID;
+	if (fast_min_threshold < 0 || fast_min_threshold > 255) LCD_FAIL(e, LCD_ERR_INVALID, "FAST/MinThreshold must be 0..255");
+	e->oct_min_threshold = fast_min_threshold;
+	e->detector = LCD_DETECTOR_ORB_OCTREE;
+	return LCD_OK;
+}
+
+int lcd_debug_orb_sincos(lcd_engine * e, unsigned first, unsigned count, float * d_cos, float * d_sin)
+{
+	if (!e || !d_cos || !d_sin) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (count == 0) return LCD_OK;
+	orb_oct_sincos_kernel<<<(count + 255) / 256, 256, 0, e->stream>>>(first, count, d_cos, d_sin);
+	LCD_CHECK_LAUNCH(e);
+	LCD_CUDA(e, cudaStreamSynchronize(e->stream));
 	return LCD_OK;
 }
 
