@@ -22,8 +22,10 @@
 
 namespace lcd {
 
-constexpr int kPnpChunk = 128;      // RANSAC hypotheses evaluated per chunk (one thread each for EPnP)
-constexpr int kVerifyThreads = 256; // threads of the CTA: the second half helps with the inlier counts, LM sums and error passes
+constexpr int kPnpChunk = 128;      // sizes two areas of the PnP kernel's shared memory (pnp_smem_bytes)
+constexpr int kPnpWave = 16;        // RANSAC hypotheses of the first wave (one thread each for EPnP)
+constexpr int kPnpWaveMax = 256;    // hypotheses of every later wave
+constexpr int kVerifyThreads = 256; // threads of the CTA: RANSAC waves after the first, inlier counts, LM sums and error passes
 constexpr int kMaxRansacIters = 320;
 
 // What a signature-store row's cached FROM dictionary was built for.  The temporary dictionary of addNewWords(descriptorsFrom) is a
@@ -1119,15 +1121,15 @@ pnp_ransac_kernel(const PnpArgs a)
 {
 	extern __shared__ __align__(128) unsigned char smem_raw[];
 	const int cap = a.cap;
-	double * h_rt = reinterpret_cast<double *>(smem_raw);                    // [kPnpChunk][6] poses of the current chunk
+	double * h_rt = reinterpret_cast<double *>(smem_raw);                    // [kPnpChunk][6]
 	double * s_red = h_rt + kPnpChunk * 6;                              // [28*32]
 	double * s_out = s_red + 28 * 32;                                        // [32]
 	float * X = reinterpret_cast<float *>(s_out + 32);                       // [cap][3]
 	float * uv = X + static_cast<size_t>(cap) * 3;                           // [cap][2]
 	float * errs = uv + static_cast<size_t>(cap) * 2;                        // [cap]
 	float * cbuf = errs + cap;                                               // [cap] covariance pass: per-inlier error values
-	int * cnt = reinterpret_cast<int *>(cbuf + cap);                         // [kPnpChunk]
-	uint16_t * sidx = reinterpret_cast<uint16_t *>(cnt + kPnpChunk);    // [kMaxRansacIters][6]
+	// [kPnpChunk] ints after cbuf are not used since a wave's counts moved into h_rt + s_red; pnp_smem_bytes keeps its size unchanged
+	uint16_t * sidx = reinterpret_cast<uint16_t *>(reinterpret_cast<int *>(cbuf + cap) + kPnpChunk); // [kMaxRansacIters][6]
 	uint16_t * listA = sidx + kMaxRansacIters * 6;                           // [cap]
 	uint16_t * listB = listA + cap;                                          // [cap]
 	uint8_t * flag = reinterpret_cast<uint8_t *>(listB + cap);               // [cap]
@@ -1166,9 +1168,18 @@ pnp_ransac_kernel(const PnpArgs a)
 	__syncthreads();
 	PNP_PHASE(1);
 
-	// ---- hypotheses in parallel, a chunk of blockDim.x at a time: EPnP on the sample, then its inlier
-	//      count; thread 0 then replays the sequential bookkeeping of RANSACPointSetRegistrator::run
-	//      (solvepnp.cpp:358-399) over the chunk and decides whether another chunk is needed.
+	// ---- hypotheses in waves, one thread per hypothesis: EPnP on the sample, then the inlier counts; thread 0 then replays the
+	//      sequential bookkeeping of RANSACPointSetRegistrator::run (solvepnp.cpp:358-399) and decides whether the run goes on.
+	//      The adaptive iteration count of the reference usually ends the run within the first few hypotheses (a 90 % inlier ratio
+	//      needs 7 iterations at 0.99 confidence), so the first wave solves only kPnpWave hypotheses: 16 EPnP threads finish much
+	//      sooner than 128 (less stack-frame traffic, a shorter wait for the slowest hypothesis).  A run that goes past them (no good
+	//      model yet) takes the rest in waves of up to kPnpWaveMax, every thread of the CTA, so that a full 300-iteration run is
+	//      three waves (16, 256, 28), as many as the 128-hypothesis chunks it replaces.
+	//      A wave's poses and counts use the h_rt and s_red areas; s_red is the refinement's and is not in use yet.
+	double * w_rt = h_rt;                                                    // [kPnpWaveMax][6]
+	int * w_cnt = reinterpret_cast<int *>(w_rt + kPnpWaveMax * 6);            // [kPnpWaveMax]
+	static_assert(kPnpWaveMax * (6 * 8 + 4) <= (kPnpChunk * 6 + 28 * 32) * 8, "a wave's poses and counts must fit in h_rt + s_red");
+	static_assert(kPnpWaveMax <= kVerifyThreads, "one thread per hypothesis of a wave");
 	const float thr2 = static_cast<float>(static_cast<double>(a.reproj) * static_cast<double>(a.reproj));
 	__shared__ int s_niters, s_maxgood, s_it;
 	if (tid == 0)
@@ -1182,15 +1193,15 @@ pnp_ransac_kernel(const PnpArgs a)
 	__shared__ unsigned long long s_rng;
 	if (tid == 0) s_rng = 0xFFFFFFFFFFFFFFFFull;
 	__syncthreads();
-	for (int chunk0 = 0; chunk0 < s_niters; chunk0 += kPnpChunk)
+	for (int w0 = 0; w0 < s_niters;)
 	{
+		const int w1 = min(w0 + (w0 == 0 ? kPnpWave : kPnpWaveMax), s_niters);
 		if (tid == 0 && n != 6)
 		{
 			// RANSACPointSetRegistrator::getSubset with cv::RNG((uint64)-1): the draws depend only on n and are
-			// consumed in iteration order, so the samples of a chunk are generated when the chunk is reached
+			// consumed in iteration order, so the samples of a wave are generated when the wave is reached
 			unsigned long long state = s_rng;
-			const int it_end = min(chunk0 + kPnpChunk, s_niters);
-			for (int it = chunk0; it < it_end; ++it)
+			for (int it = w0; it < w1; ++it)
 			{
 				for (int i = 0; i < 6;)
 				{
@@ -1210,45 +1221,40 @@ pnp_ransac_kernel(const PnpArgs a)
 			s_rng = state;
 		}
 		__syncthreads();
-		// EPnP: one thread per hypothesis (threads [0, kPnpChunk))
-		if (tid < kPnpChunk)
+		// EPnP (the first wave runs on lanes 0..kPnpWave-1 of warp 0; spread over four warps it measured slower)
+		if (tid < w1 - w0)
 		{
-			const int it = chunk0 + tid;
+			const int it = w0 + tid;
+			int idx[6];
+			for (int k = 0; k < 6; ++k) idx[k] = (n == 6) ? k : sidx[it * 6 + k];
+			double rv[3], tv[3];
+			long long * clk = (a.phase_clk && it == 0) ? a.phase_clk + pair * 16 + 8 : nullptr;
 			int c = -1;
-			if (it < s_niters)
+			if (solve_pnp_epnp6(X, uv, idx, cam, rv, tv, clk))
 			{
-				int idx[6];
-				for (int k = 0; k < 6; ++k) idx[k] = (n == 6) ? k : sidx[it * 6 + k];
-				double rv[3], tv[3];
-				long long * clk = (a.phase_clk && tid == 0 && chunk0 == 0) ? a.phase_clk + pair * 16 + 8 : nullptr;
-				if (solve_pnp_epnp6(X, uv, idx, cam, rv, tv, clk))
+				if (clk) clk[4] = clock64();
+				c = 0;
+				for (int k = 0; k < 3; ++k)
 				{
-					if (clk) clk[4] = clock64();
-					c = 0;
-					for (int k = 0; k < 3; ++k)
-					{
-						h_rt[tid * 6 + k] = rv[k];
-						h_rt[tid * 6 + 3 + k] = tv[k];
-					}
+					w_rt[tid * 6 + k] = rv[k];
+					w_rt[tid * 6 + 3 + k] = tv[k];
 				}
 			}
-			cnt[tid] = c;
+			w_cnt[tid] = c;
 		}
 		__syncthreads();
-		// Inlier counts + the sequential bookkeeping, in two sub-chunks (16 hypotheses, then the other 112).  The adaptive iteration
-		// count of the reference usually ends the run within the first few hypotheses (a 90 % inlier ratio needs 7 iterations at 0.99
-		// confidence), so counting the inliers of all 128 poses first was mostly wasted fp64 work; the replay is the same sequential
-		// loop either way.  Every hypothesis of a sub-chunk is counted by blockDim.x / size threads, each over a slice of the points.
-		for (int sub0 = 0; sub0 < kPnpChunk;)
+		// Inlier counts + the bookkeeping in sub-chunks of kPnpWave hypotheses, so that the run can end inside a wave without counting
+		// the rest of it.  Every hypothesis of a sub-chunk is counted by blockDim.x / size threads, each over a slice of the points.
+		for (int s0 = w0; s0 < w1;)
 		{
-			const int sub1 = sub0 == 0 ? 16 : kPnpChunk;
-			const int nh = sub1 - sub0, parts = blockDim.x / nh;
-			const int h = sub0 + tid % nh, part = tid / nh;
-			if (part < parts && cnt[h] >= 0)
+			const int s1 = min(s0 + kPnpWave, w1);
+			const int nh = s1 - s0, parts = blockDim.x / nh;
+			const int h = s0 - w0 + tid % nh, part = tid / nh; // h: index in the wave
+			if (part < parts && w_cnt[h] >= 0)
 			{
 				double R[9];
-				rodrigues_v2m(h_rt + h * 6, R, nullptr);
-				const double tv[3] = {h_rt[h * 6 + 3], h_rt[h * 6 + 4], h_rt[h * 6 + 5]};
+				rodrigues_v2m(w_rt + h * 6, R, nullptr);
+				const double tv[3] = {w_rt[h * 6 + 3], w_rt[h * 6 + 4], w_rt[h * 6 + 5]};
 				const int i0 = static_cast<int>(static_cast<long long>(n) * part / parts), i1 = static_cast<int>(static_cast<long long>(n) * (part + 1) / parts);
 				int c = 0;
 				int i = i0;
@@ -1263,34 +1269,33 @@ pnp_ransac_kernel(const PnpArgs a)
 					c += (e0 <= thr2 ? 1 : 0) + (e1 <= thr2 ? 1 : 0) + (e2 <= thr2 ? 1 : 0) + (e3 <= thr2 ? 1 : 0);
 				}
 				for (; i < i1; ++i) c += reproj_err(R, tv, cam, X + 3 * i, uv + 2 * i) <= thr2 ? 1 : 0;
-				if (c) atomicAdd(&cnt[h], c);
+				if (c) atomicAdd(&w_cnt[h], c);
 			}
-			if (a.phase_clk && tid == 0 && chunk0 == 0 && sub0 == 0) a.phase_clk[pair * 16 + 8 + 5] = clock64();
+			if (a.phase_clk && tid == 0 && s0 == 0) a.phase_clk[pair * 16 + 8 + 5] = clock64();
 			__syncthreads();
 			if (tid == 0)
 			{
 				int it0 = s_it, niters = s_niters, maxGood = s_maxgood;
-				const int chunk_end = chunk0 + sub1;
 				if (n == 6)
 				{
-					if (cnt[0] >= 0)
+					if (w_cnt[0] >= 0)
 					{
 						s_best = 0;
-						for (int k = 0; k < 6; ++k) lm.param[k] = h_rt[k];
+						for (int k = 0; k < 6; ++k) lm.param[k] = w_rt[k];
 					}
 					it0 = 0;
 				}
 				else
 				{
-					for (; it0 < niters && it0 < chunk_end; ++it0)
+					for (; it0 < niters && it0 < s1; ++it0)
 					{
-						const int c = cnt[it0 - chunk0];
+						const int c = w_cnt[it0 - w0];
 						if (c < 0) continue;
 						if (c > max(maxGood, 5))
 						{
 							s_best = it0;
 							maxGood = c;
-							for (int k = 0; k < 6; ++k) lm.param[k] = h_rt[(it0 - chunk0) * 6 + k];
+							for (int k = 0; k < 6; ++k) lm.param[k] = w_rt[(it0 - w0) * 6 + k];
 							niters = ransac_update_num_iters(0.99, static_cast<double>(n - c) / n, 6, niters);
 						}
 					}
@@ -1300,11 +1305,12 @@ pnp_ransac_kernel(const PnpArgs a)
 				s_maxgood = maxGood;
 			}
 			__syncthreads();
-			if (s_niters <= chunk0 + sub1) break; // the run ended inside this sub-chunk (uniform: shared state read after the barrier)
-			sub0 = sub1;
+			if (s_niters <= s1) break; // the run ended inside this sub-chunk (uniform: shared state read after the barrier)
+			s0 = s1;
 		}
-		if (chunk0 == 0) PNP_PHASE(2);
-		__syncthreads();
+		if (w0 == 0) PNP_PHASE(5);
+		if (w0 == 0 ? s_niters <= w1 : w0 == kPnpWave) PNP_PHASE(2); // end of the first two waves
+		w0 = w1;
 	}
 	const int best = s_best;
 	PNP_PHASE(3);
