@@ -971,6 +971,65 @@ int lcd_decide_proximity_dev(lcd_engine * e, const void * d_queries, const float
 /* the per-frame results of the last lcd_decide_proximity_dev; synchronises */
 int lcd_proximity_fetch(lcd_engine * e, int n_frames, lcd_proximity_result * out);
 
+/* ---- the localisation step of Rtabmap::process from images, for many clients -------------------------------------------------
+ * The optional stages of the decision inside lcd_process_frames_decide_*; a NULL member turns its stage off.  Host arrays, read before
+ * the call returns. */
+typedef struct lcd_decide_stages {
+	const lcd_gps * frame_gps;              /* [n_frames]: Rtabmap/LoopGPS as lcd_decide_gps_batch_dev takes it (NULL: no GPS filter) */
+	float local_radius;                     /* RGBD/LocalRadius of the GPS filter (>= 0) */
+	const lcd_epipolar_params * epipolar;   /* VhEp/Enabled: lcd_decide_epipolar_dev (NULL: off) */
+	const lcd_proximity_params * proximity; /* RGBD/ProximityBySpace: lcd_decide_proximity_dev (NULL: off), with */
+	const float * frame_poses;              /*   [n_frames][12] each frame's optimised pose and */
+	const int * proximity_enabled;          /*   [n_frames] the caller's conditions of Rtabmap.cpp:2698-2723 */
+} lcd_decide_stages;
+
+/* replaces: the localisation step of Rtabmap::process (Mem/IncrementalMemory=false) for n_frames frames of distinct clients, from their
+ * device images (and depth), asynchronous on `stream`:
+ *  1. Memory::update's detection with the engine's detector (lcd_detector_*) and its quantisation limit (lcd_quantize_limit_set), then
+ *     Memory::computeLikelihood (Rtabmap.cpp:2117) against the map's real places (lcd_clients_set_map; ns must equal their number):
+ *     word ids and likelihood rows bit-identical to lcd_process_frames with those ids as sig_ids;
+ *  2. with stages->frame_gps, the GPS filter of the place list (:2046-2115), then adjustLikelihood, the client's Bayes posterior and the
+ *     hypothesis selection (:2119-2226) as lcd_decide_gps_batch_dev (lcd_decide_batch_dev without GPS) decides them;
+ *  3. with stages->epipolar, the epipolar check (:2193) on the frame's expanded word ids and keypoints, as lcd_decide_epipolar_dev;
+ *  4. with stages->proximity, proximity detection by space (:2698-2934), as lcd_decide_proximity_dev, with each frame's own rows;
+ *  5. Memory::computeTransform of the accepted hypotheses and its rejections (:3133-3191), as lcd_verify_decided_dev.
+ * Registrations (steps 4 and 5) take each frame's n_kp detected rows as TO, with their depth (words3) when there is depth: the rows a
+ * short frame pads with are never matched.  A frame without a quantised word is a bad signature (Signature::isBadSignature,
+ * Signature.cpp:341-344): it is decided as LCD_FRAME_SKIP decides it (Rtabmap.cpp:1994-1999), found on the device, so the caller needs no
+ * synchronisation to learn it: LCD_DECIDE_SKIPPED, highest (0, 0), its client's posterior untouched, no epipolar check, no proximity
+ * detection (status LCD_PROXIMITY_OFF) and no registration.  clients[n_frames] and frame_flags[n_frames] as lcd_decide_batch_dev takes
+ * them.  d_word_ids_out[n_frames][params->n_features] (expanded ids, negative for rows the limit did not quantise),
+ * d_likelihood_out[n_frames][ns] and d_posterior_out[n_frames][ns+1] (not written for skipped, held and bad-signature frames) may be NULL.
+ * This decision becomes the last decision: lcd_decide_fetch, lcd_process_fetch, lcd_epipolar_fetch and lcd_proximity_fetch read it.
+ * Binary 32-byte engines only: float engines get LCD_ERR_INVALID (no image detector builds float descriptors), sharded engines
+ * LCD_ERR_STATE.  LCD_ERR_STATE without clients or a map, with proximity but no poses for the current map, and for a GPS fix on a frame
+ * that computes while the map has no GPS table; LCD_ERR_INVALID for a client listed twice and for bad parameters or arrays; these
+ * refusals, and the epipolar check's shared-memory limit (LCD_ERR_CAPACITY), come before the decision changes any client state.  A
+ * detector refusal of the image geometry (as lcd_orb_detect_describe_dev's) comes before it too, once the frame tables are uploaded.  The
+ * registrations' own capacity limit (LCD_ERR_CAPACITY, as lcd_process_decide_batch_dev's) is met after the decision: the clients' state
+ * has then advanced, as it has after a refused lcd_verify_decided_dev.  Not covered: the similarity likelihood (Kp/TfIdfLikelihoodUsed=false), mapping
+ * mode, retrieval and intermediate nodes. */
+int lcd_process_frames_decide_dev(lcd_engine * e, int n_frames, const uint8_t * d_images, int width, int height, int channels,
+                                  const void * d_depth, int depth_type, const lcd_orb_params * params,
+                                  int incremental, float nndr, int new_words_compared_together, int ns, int n_total,
+                                  const lcd_verify_params * vp, const int * clients, const int * frame_flags, const lcd_decide_params * dp,
+                                  const lcd_decide_stages * stages, int * d_word_ids_out, float * d_likelihood_out, float * d_posterior_out,
+                                  void * stream);
+/* The same from host images for a relocalisation service: _submit queues the batch and returns, lcd_process_frames_wait completes it.
+ * It shares the two batches in flight of lcd_process_frames_submit (the two kinds may be interleaved; _wait always completes the oldest
+ * batch, LCD_ERR_INVALID for a third).  Host outputs, each may be NULL, filled when the matching _wait returns: n_kp_out, word_ids_out and
+ * likelihood_out shaped as lcd_process_frames' (word ids as lcd_process_frames_decide_dev's), decisions_out[n_frames],
+ * results_out[n_frames] (the verification of the accepted hypotheses, as lcd_process_fetch), epipolar_out[n_frames] and
+ * proximity_out[n_frames] (when those stages run, as lcd_epipolar_fetch / lcd_proximity_fetch).  Each batch stages its decision tables,
+ * poses and flags in pinned buffers of its own, so a submit never waits for the batch in flight. */
+int lcd_process_frames_decide_submit(lcd_engine * e, int n_frames, const uint8_t * images, int width, int height, int channels,
+                                     const void * depth, int depth_type, const lcd_orb_params * params,
+                                     int incremental, float nndr, int new_words_compared_together, int ns, int n_total,
+                                     const lcd_verify_params * vp, const int * clients, const int * frame_flags, const lcd_decide_params * dp,
+                                     const lcd_decide_stages * stages, int * n_kp_out, int * word_ids_out, float * likelihood_out,
+                                     lcd_decision * decisions_out, lcd_verify_result * results_out, lcd_epipolar_result * epipolar_out,
+                                     lcd_proximity_result * proximity_out);
+
 /* ---- measurement hooks ---------------------------------------------------------------
  * Optional per-kernel timing with CUDA events recorded on the launching stream around
  * every launch of kernel class `which` (0 = dictionary NN, 1 = resolve, 2 = score, 3 = pair

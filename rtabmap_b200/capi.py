@@ -157,6 +157,14 @@ class ProximityResult(C.Structure):
     ]
 
 
+class DecideStages(C.Structure):
+    """lcd_decide_stages: the optional stages of process_frames_decide_* (a NULL member turns its stage off)."""
+    _fields_ = [
+        ("frame_gps", C.c_void_p), ("local_radius", C.c_float), ("epipolar", C.POINTER(EpipolarParams)),
+        ("proximity", C.POINTER(ProximityParams)), ("frame_poses", C.c_void_p), ("proximity_enabled", C.c_void_p),
+    ]
+
+
 # lcd_gps: rtabmap::GPS's stamp (> 0: a fix), longitude, latitude (degrees), altitude and error (metres), as a structured array
 GPS_DTYPE = np.dtype([("stamp", np.float64), ("longitude", np.float64), ("latitude", np.float64), ("altitude", np.float64), ("error", np.float64)])
 
@@ -302,6 +310,9 @@ SIGNATURES = {
     "lcd_decide_gps_batch_dev": (_I, [_P, _P, _I, _I, _P, _P, _P, _F, _P, _P, _P, _P]),
     "lcd_decide_proximity_dev": (_I, [_P, _P, _P, _I, _I, _P, _P, _P, _P]),
     "lcd_proximity_fetch": (_I, [_P, _I, _P]),
+    "lcd_process_frames_decide_dev": (_I, [_P, _I, _P, _I, _I, _I, _P, _I, _P, _I, _F, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "lcd_process_frames_decide_submit": (_I, [_P, _I, _P, _I, _I, _I, _P, _I, _P, _I, _F, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
+                                              _P]),
     "lcd_profile_enable": (_I, [_P, _I]),
     "lcd_profile_read": (_I, [_P, _I, _P, _P]),
     "lcd_profile_reset": (_I, [_P]),
@@ -1117,7 +1128,7 @@ class Engine:
     def epipolar_fetch(self, n_frames: int):
         out = (EpipolarResult * n_frames)()
         self._check(self._lib.lcd_epipolar_fetch(self._h, int(n_frames), out))
-        return [_epi_dict(r) for r in out]
+        return self.epipolar_records(out)
 
     def epipolar_check_batch(self, ids_a, uv_a, n_a, ids_b, uv_b, n_b, match_count_min: int = 8, ransac_param1: float = 3.0,
                              ransac_param2: float = 0.99, with_status: bool = False):
@@ -1193,13 +1204,95 @@ class Engine:
         """The last proximity step's per-frame records: dicts with status, n_nearest, n_paths, suppressed_id and the attempted paths."""
         out = (ProximityResult * n_frames)()
         self._check(self._lib.lcd_proximity_fetch(self._h, int(n_frames), out))
+        return self.proximity_records(out)
+
+    # -- the localisation step of Rtabmap::process from images ------------------------------------------------------
+    @staticmethod
+    def decide_stages(n_frames: int, frame_gps=None, local_radius: float = 10.0, epipolar: "EpipolarParams" = None, proximity: "ProximityParams" = None,
+                      frame_poses=None, proximity_enabled=None):
+        """lcd_decide_stages for n_frames frames: frame_gps as gps_array takes it (None: no GPS filter), epipolar (EpipolarParams or None),
+        proximity (ProximityParams or None) with frame_poses [n_frames, 3, 4] and proximity_enabled [n_frames].  The returned structure
+        keeps its arrays alive."""
+        st = DecideStages()
+        keep = []
+        if frame_gps is not None:
+            g = gps_array(frame_gps)
+            if len(g) != n_frames:
+                raise LcdError(-1, f"frame_gps needs {n_frames} entries")
+            keep.append(g)
+            st.frame_gps = g.ctypes.data
+        st.local_radius = float(local_radius)
+        if epipolar is not None:
+            keep.append(epipolar)
+            st.epipolar = C.pointer(epipolar)
+        if proximity is not None:
+            p = np.ascontiguousarray(frame_poses, np.float32).reshape(-1)
+            en = _i32(proximity_enabled)
+            if len(p) != 12 * n_frames or len(en) != n_frames:
+                raise LcdError(-1, f"frame_poses and proximity_enabled need {n_frames} entries")
+            keep += [proximity, p, en]
+            st.proximity = C.pointer(proximity)
+            st.frame_poses = p.ctypes.data
+            st.proximity_enabled = en.ctypes.data
+        st._keep = keep
+        return st
+
+    @staticmethod
+    def _images(images, depth):
+        n, h, w = images.shape[:3]
+        ch = 1 if images.ndim == 3 else images.shape[3]
+        dtype = 0 if depth is None else (1 if depth.dtype == np.uint16 else 2)
+        return n, h, w, ch, dtype
+
+    def process_frames_decide_dev(self, d_images: int, n_frames: int, w: int, h: int, ch: int, d_depth: int, depth_type: int, op: "OrbParams", ns: int,
+                                  n_total: int, vp: "VerifyParams", clients, frame_flags, dp: DecideParams, stages: DecideStages = None,
+                                  d_words_out: int = 0, d_like_out: int = 0, d_posterior_out: int = 0, incremental: bool = True, nndr: float = 0.8,
+                                  cmp_new: bool = True, stream: int = 0):
+        """Rtabmap::process's localisation step for n_frames frames of distinct clients from device images: detect, quantise and score
+        against the map's real places, decide (with the optional stages), verify the accepted hypotheses.  Results stay on the device
+        (decide_fetch, process_fetch, epipolar_fetch, proximity_fetch)."""
+        c = _i32(clients)
+        f = _i32(frame_flags)
+        if len(c) != n_frames or len(f) != n_frames:
+            raise LcdError(-1, f"clients and frame_flags need {n_frames} entries")
+        self._check(self._lib.lcd_process_frames_decide_dev(self._h, int(n_frames), C.c_void_p(d_images), w, h, ch, C.c_void_p(d_depth or None),
+                                                             depth_type, C.byref(op), int(incremental), float(nndr), int(cmp_new), int(ns), int(n_total),
+                                                             C.byref(vp), _ptr(c), _ptr(f), C.byref(dp), C.byref(stages) if stages is not None else None,
+                                                             C.c_void_p(d_words_out or None), C.c_void_p(d_like_out or None),
+                                                             C.c_void_p(d_posterior_out or None), C.c_void_p(stream or None)))
+
+    def process_frames_decide_submit(self, images, depth, op: "OrbParams", ns: int, n_total: int, vp: "VerifyParams", clients, frame_flags,
+                                     dp: DecideParams, stages: DecideStages = None, out_nkp=None, out_words=None, out_like=None, out_dec=None,
+                                     out_res=None, out_epi=None, out_prox=None, incremental: bool = True, nndr: float = 0.8, cmp_new: bool = True):
+        """Pipelined process_frames_decide_dev from host images: queue one batch; process_frames_wait completes the oldest batch of either
+        kind.  images / depth as process_frames_submit takes them (alive until the wait); out_* (each may be None) must stay alive until the
+        wait: out_dec a DECISION_DTYPE array, out_res a (VerifyResult * n)(), out_epi a (EpipolarResult * n)(), out_prox a
+        (ProximityResult * n)().  clients, frame_flags and the stages' arrays are read before the call returns."""
+        n, h, w, ch, dtype = self._images(images, depth)
+        c = _i32(clients)
+        f = _i32(frame_flags)
+        if len(c) != n or len(f) != n:
+            raise LcdError(-1, f"clients and frame_flags need {n} entries")
+        self._check(self._lib.lcd_process_frames_decide_submit(self._h, n, _ptr(images), w, h, ch, _ptr(depth), dtype, C.byref(op), int(incremental),
+                                                                float(nndr), int(cmp_new), int(ns), int(n_total), C.byref(vp), _ptr(c), _ptr(f),
+                                                                C.byref(dp), C.byref(stages) if stages is not None else None, _ptr(out_nkp),
+                                                                _ptr(out_words), _ptr(out_like), _ptr(out_dec), out_res, out_epi, out_prox))
+
+    @staticmethod
+    def epipolar_records(out) -> list:
+        """the dicts epipolar_fetch returns, from an (EpipolarResult * n)() that a decision batch filled"""
+        return [_epi_dict(r) for r in out]
+
+    @staticmethod
+    def proximity_records(out) -> list:
+        """the dicts proximity_fetch returns, from a (ProximityResult * n)() that a decision batch filled"""
         recs = []
         for r in out:
             paths = []
             for j in range(r.n_attempts):
                 q = r.paths[j]
                 paths.append({"likelihood": np.float32(q.likelihood), "id": q.id, "distance": np.float32(q.distance), "candidate_id": q.candidate_id,
-                              "accepted": bool(q.accepted), "link_type": q.link_type, "result": self._results([q.result], 1)[0]})
+                              "accepted": bool(q.accepted), "link_type": q.link_type, "result": Engine._results([q.result], 1)[0]})
             recs.append({"status": r.status, "n_nearest": r.n_nearest, "n_paths": r.n_paths, "n_attempts": r.n_attempts,
                          "suppressed_id": r.suppressed_id, "paths": paths})
         return recs

@@ -98,8 +98,9 @@ struct DecideBatch
 	int B;
 	const long long * frame;    // [B] frame index in the call
 	const long long * client;   // [B]
-	const long long * prev_n;   // [B] places of the client's last posterior (0 = empty state)
-	const long long * prev_ids; // [B] device address of the ids the client's last posterior is keyed to
+	const int * key_n;          // [client] places of the client's last posterior (0 = empty state)
+	const long long * key_ids;  // [client] device address of the ids the client's last posterior is keyed to
+	const int * qn;             // [n_frames] quantised words of each frame, or nullptr: a frame with none is a bad signature
 	const float * cl_post;      // [client][stride] the clients' last posteriors
 	long long stride;
 	const float * adj;          // [n_frames][n] adjusted likelihood (element 0 = the virtual place)
@@ -127,10 +128,11 @@ __global__ void decide_last_kernel(const DecideMap m, const DecideBatch d)
 	const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
 	if (i >= static_cast<long long>(m.n) * d.B) return;
 	const int r = static_cast<int>(i / d.B), b = static_cast<int>(i % d.B);
-	const int * prev_ids = reinterpret_cast<const int *>(d.prev_ids[b]);
-	const float * prev = d.cl_post + d.client[b] * d.stride;
+	const long long c = d.client[b];
+	const int * prev_ids = reinterpret_cast<const int *>(d.key_ids[c]);
+	const float * prev = d.cl_post + c * d.stride;
 	const int f = static_cast<int>(d.frame[b]);
-	float v = bayes_rekey(prev_ids, prev, static_cast<int>(d.prev_n[b]), m.ids[r]);
+	float v = bayes_rekey(prev_ids, prev, d.key_n[c], m.ids[r]);
 	if (decide_gated(d, f) && !d.listed[static_cast<size_t>(f) * m.n + r]) v = 0.f; // updatePosterior over the compared ids only
 	d.last_t[i] = v;
 }
@@ -234,6 +236,10 @@ __global__ void __launch_bounds__(kDcThreads) decide_rows_kernel(const DecideMap
 	}
 }
 
+// a frame without quantised words (Signature::isBadSignature, Signature.cpp:341-344) is skipped as LCD_FRAME_SKIP skips it (Rtabmap.cpp:
+// 1994-1999), even when the host put it into the batch: its columns are computed but nothing of it is written
+__device__ __forceinline__ bool decide_bad(const int * qn, long long f) { return qn && qn[f] == 0; }
+
 // normalisation, transposed through shared memory: the client's new state [client][r] and the optional output [frame][r]
 __global__ void decide_normalize_kernel(const DecideMap m, const DecideBatch d, float * __restrict__ cl_post, float * __restrict__ out)
 {
@@ -254,7 +260,7 @@ __global__ void decide_normalize_kernel(const DecideMap m, const DecideBatch d, 
 	for (int j = threadIdx.y; j < 32; j += blockDim.y)
 	{
 		const int b = b0 + j, r = r0 + threadIdx.x;
-		if (r < m.n && b < d.B)
+		if (r < m.n && b < d.B && !decide_bad(d.qn, d.frame[b]))
 		{
 			const float v = tile[threadIdx.x][j];
 			cl_post[d.client[b] * d.stride + r] = v;
@@ -280,6 +286,9 @@ struct DecideSelect
 	int * hyp_slot;            // [n_frames] its store row or -1
 	const GpsFrame * gps;      // [n_frames] or nullptr (DecideBatch::gps)
 	const int * count;         // [n_frames] real places a gated frame compares
+	const int * qn;            // [n_frames] or nullptr (DecideBatch::qn)
+	int * key_n;               // [client] what each client's last posterior is keyed to (DecideBatch::key_n / key_ids)
+	long long * key_ids;
 };
 
 // Rtabmap.cpp:2143-2233 for one frame per CTA: the highest real-place posterior (scanned in descending id order with a strict '>', so
@@ -290,7 +299,7 @@ __global__ void decide_select_kernel(const DecideMap m, const DecideSelect a)
 	__shared__ int s_r[32];
 	const int f = blockIdx.x;
 	const int client = static_cast<int>(a.client[f]);
-	const int flags = static_cast<int>(a.flags[f]);
+	const int flags = static_cast<int>(a.flags[f]) | (decide_bad(a.qn, f) ? kDcFlagSkip : 0);
 	const bool compute = (flags & (kDcFlagSkip | kDcFlagHold)) == 0;
 	float bv = 0.f;
 	int br = -1;
@@ -367,6 +376,12 @@ __global__ void decide_select_kernel(const DecideMap m, const DecideSelect a)
 	}
 	a.hi_id[client] = d.highest_id;
 	a.hi_val[client] = d.highest_value;
+	if (compute)
+	{
+		// the posterior decide_normalize_kernel wrote is keyed to the current map
+		a.key_n[client] = m.n;
+		a.key_ids[client] = static_cast<long long>(reinterpret_cast<uintptr_t>(m.ids));
+	}
 	a.dec[f] = d;
 	int slot = -1;
 	if (d.loop_id > 0 && a.sig_slot && d.loop_id < a.slot_cap) slot = a.sig_slot[d.loop_id];
@@ -432,12 +447,15 @@ __global__ void decide_gps_gate_kernel(int n, const GpsPlace * __restrict__ plac
 	}
 }
 
-__global__ void decide_reset_clients_kernel(const int * __restrict__ clients, int n, int * __restrict__ hi_id, float * __restrict__ hi_val)
+__global__ void decide_reset_clients_kernel(const int * __restrict__ clients, int n, int * __restrict__ hi_id, float * __restrict__ hi_val,
+                                            int * __restrict__ key_n, long long * __restrict__ key_ids)
 {
 	const int i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= n) return;
 	hi_id[clients[i]] = 0;
 	hi_val[clients[i]] = 0.f;
+	key_n[clients[i]] = 0;
+	key_ids[clients[i]] = 0;
 }
 
 } // namespace lcd

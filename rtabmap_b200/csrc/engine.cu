@@ -333,6 +333,19 @@ struct lcd_engine
 		cudaEvent_t uploaded = nullptr, done = nullptr;
 		lcd_verify_result * user_results = nullptr;
 		int n_frames = 0;
+		// lcd_process_frames_decide_submit: the batch's own staging of the decision's host tables (decide_prepare), the proximity poses
+		// and flags, and the downloads of its decisions and epipolar and proximity records, so that no batch waits for another's copies
+		PinBuf<long long> h_tab;
+		PinBuf<float> h_pose;
+		PinBuf<int> h_enabled, h_ep_res;
+		PinBuf<double> h_ep_F;
+		PinBuf<Decision> h_dec;
+		PinBuf<ProxRecord> h_px_rec;
+		PinBuf<PackedVerifyResult> h_px_res;
+		lcd_decision * user_dec = nullptr;
+		lcd_epipolar_result * user_ep = nullptr;
+		lcd_proximity_result * user_px = nullptr;
+		int px_max_paths = 0;
 		cudaEvent_t t_h0 = nullptr, t_h1 = nullptr, t_c0 = nullptr, t_c1 = nullptr; // LCD_DEBUG_TIMELINE
 	};
 	cudaEvent_t t_base = nullptr;
@@ -424,7 +437,8 @@ struct lcd_engine
 	double dc_lc0 = 0.0;
 	float dc_vpp = 0.f;
 	int dc_clients = 0;
-	std::vector<int> dc_ver;              // per client: the map version its last posterior is keyed to (-1 = empty state)
+	DevBuf<int> dc_key_n;                 // [client] places of the ids its last posterior is keyed to (0 = empty state), and
+	DevBuf<long long> dc_key_ids;         // [client] their device address: kept on the device, where a bad signature is found
 	DevBuf<float> dc_post;                // [client][dc_stride] last posterior of every client
 	size_t dc_stride = 0;
 	DevBuf<int> dc_hi_id;                 // [client] last highest hypothesis
@@ -432,7 +446,7 @@ struct lcd_engine
 	PinBuf<long long> dc_h_tab;           // per-call frame tables, staged for the upload
 	cudaEvent_t dc_h_ev = nullptr;        // the last upload from dc_h_tab
 	DevBuf<long long> dc_tab;
-	std::vector<int> dc_active;           // clients whose posterior the call being launched computes
+	std::vector<int> dc_active;           // frames the call being launched computes a posterior for (unless they are bad signatures)
 	DevBuf<float> dc_adj, dc_last_t, dc_post_t;
 	DevBuf<double> dc_part_u, dc_part_s1, dc_part_p, dc_sums;
 	DevBuf<Decision> dc_dec;
@@ -3864,6 +3878,33 @@ static void epipolar_results(int n, const int * hr, const double * hF, lcd_epipo
 		for (int k = 0; k < 9; ++k) o.F[k] = hF[static_cast<size_t>(i) * 9 + k];
 	}
 }
+
+// lcd_proximity_result records of n frames from their device records and registrations [frame][mp]
+static void proximity_results(int n, int mp, const ProxRecord * rec, const PackedVerifyResult * res, lcd_proximity_result * out)
+{
+	for (int f = 0; f < n; ++f)
+	{
+		const ProxRecord & r = rec[f];
+		lcd_proximity_result & o = out[f];
+		memset(&o, 0, sizeof(o));
+		o.status = r.status;
+		o.n_nearest = r.n_nearest;
+		o.n_paths = r.n_paths;
+		o.n_attempts = r.n_attempts;
+		o.suppressed_id = r.suppressed;
+		for (int j = 0; j < r.n_attempts; ++j)
+		{
+			lcd_proximity_path & p = o.paths[j];
+			p.likelihood = r.path[j].likelihood;
+			p.id = r.path[j].id;
+			p.distance = r.path[j].distance;
+			p.candidate_id = r.path[j].candidate;
+			p.accepted = r.accepted[j];
+			p.link_type = r.link_type[j];
+			memcpy(&p.result, &res[static_cast<size_t>(f) * mp + j], sizeof(lcd_verify_result));
+		}
+	}
+}
 extern "C" {
 int lcd_epipolar_check_batch(lcd_engine * e, int n_pairs, int cap, const int * ids_a, const float * uv_a, const int * n_a, const int * ids_b,
                              const float * uv_b, const int * n_b, const lcd_epipolar_params * p, lcd_epipolar_result * out, uint8_t * status_out)
@@ -3969,17 +4010,11 @@ int lcd_sig_words_remove(lcd_engine * e, int sig_id)
 
 int lcd_sig_words_count(const lcd_engine * e) { return e ? e->ws_map.count() : 0; }
 
-int lcd_decide_epipolar_dev(lcd_engine * e, const int * d_word_ids, const float * d_uv, const int * d_n_per_frame, int n_frames, int nq_per_frame,
-                            const lcd_epipolar_params * p, void * stream)
+} // extern "C"
+// VhEp/Enabled on the last decision (checked by the callers): the frames' words d_word_ids[n_frames][nq] against the word store
+static int epipolar_decide(lcd_engine * e, const int * d_word_ids, const float * d_uv, const int * d_n_per_frame, int n_frames, int nq_per_frame,
+                           const lcd_epipolar_params * p, cudaStream_t s)
 {
-	if (!e) return LCD_ERR_INVALID;
-	LCD_TRY(set_device(e));
-	if (e->dc_last_frames == 0) LCD_FAIL(e, LCD_ERR_STATE, "no decision to check: run lcd_decide_batch_dev first");
-	if (!d_word_ids || !d_uv || !d_n_per_frame || !p) LCD_FAIL(e, LCD_ERR_INVALID, "null epipolar input");
-	if (n_frames != e->dc_last_frames) LCD_FAIL(e, LCD_ERR_INVALID, "the last decision has %d frames, not %d", e->dc_last_frames, n_frames);
-	if (nq_per_frame <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "nq_per_frame %d", nq_per_frame);
-	if (nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "at most %d words per frame", kMaxFrameQueries);
-	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
 	LCD_CUDA(e, e->ep_slot.reserve(n_frames, 0, false, s));
 	LCD_CUDA(e, e->ep_skip.reserve(n_frames, 0, false, s));
 	LCD_CUDA(e, e->ws_n.reserve(1, 0, true, s)); // an empty store: every hypothesis is a signature without words
@@ -4005,6 +4040,21 @@ int lcd_decide_epipolar_dev(lcd_engine * e, const int * d_word_ids, const float 
 	LCD_CHECK_LAUNCH(e);
 	e->ep_last_frames = n_frames;
 	return LCD_OK;
+}
+extern "C" {
+
+int lcd_decide_epipolar_dev(lcd_engine * e, const int * d_word_ids, const float * d_uv, const int * d_n_per_frame, int n_frames, int nq_per_frame,
+                            const lcd_epipolar_params * p, void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (e->dc_last_frames == 0) LCD_FAIL(e, LCD_ERR_STATE, "no decision to check: run lcd_decide_batch_dev first");
+	if (!d_word_ids || !d_uv || !d_n_per_frame || !p) LCD_FAIL(e, LCD_ERR_INVALID, "null epipolar input");
+	if (n_frames != e->dc_last_frames) LCD_FAIL(e, LCD_ERR_INVALID, "the last decision has %d frames, not %d", e->dc_last_frames, n_frames);
+	if (nq_per_frame <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "nq_per_frame %d", nq_per_frame);
+	if (nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "at most %d words per frame", kMaxFrameQueries);
+	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	return epipolar_decide(e, d_word_ids, d_uv, d_n_per_frame, n_frames, nq_per_frame, p, s);
 }
 
 int lcd_epipolar_fetch(lcd_engine * e, int n_frames, lcd_epipolar_result * out)
@@ -4411,7 +4461,13 @@ int lcd_process_frames_wait(lcd_engine * e)
 		fprintf(stderr, "[lcd timeline] upload %.2f..%.2f  compute %.2f..%.2f ms\n", a, b, c, d);
 	}
 	if (f.user_results) memcpy(f.user_results, f.res.p, f.n_frames * sizeof(lcd_verify_result));
+	if (f.user_dec) memcpy(f.user_dec, f.h_dec.p, f.n_frames * sizeof(lcd_decision));
+	if (f.user_ep) epipolar_results(f.n_frames, f.h_ep_res.p, f.h_ep_F.p, f.user_ep);
+	if (f.user_px) proximity_results(f.n_frames, f.px_max_paths, f.h_px_rec.p, f.h_px_res.p, f.user_px);
 	f.user_results = nullptr;
+	f.user_dec = nullptr;
+	f.user_ep = nullptr;
+	f.user_px = nullptr;
 	e->flight_head ^= 1;
 	--e->flights_busy;
 	return overflow_report(e, f.overflow.p ? *f.overflow.p : 0, f.detector);
@@ -4493,14 +4549,17 @@ int lcd_process_batch(lcd_engine * e, const void * queries, const float * uv, in
 static_assert(sizeof(Decision) == sizeof(lcd_decision), "decision layout");
 
 // drop the map versions that neither the current map nor any client's last posterior uses (the device must be idle)
-static void prune_map_versions(lcd_engine * e)
+static int prune_map_versions(lcd_engine * e)
 {
+	std::vector<long long> keys(e->dc_clients);
+	if (e->dc_clients > 0) LCD_CUDA(e, cudaMemcpy(keys.data(), e->dc_key_ids.p, keys.size() * sizeof(long long), cudaMemcpyDeviceToHost));
 	for (auto it = e->dc_versions.begin(); it != e->dc_versions.end();)
 	{
-		const int v = it->first;
-		const bool held = v == e->dc_map_ver || std::find(e->dc_ver.begin(), e->dc_ver.end(), v) != e->dc_ver.end();
+		const long long ids = static_cast<long long>(reinterpret_cast<uintptr_t>(it->second->ids.p));
+		const bool held = it->first == e->dc_map_ver || std::find(keys.begin(), keys.end(), ids) != keys.end();
 		it = held ? std::next(it) : e->dc_versions.erase(it);
 	}
+	return LCD_OK;
 }
 
 int lcd_clients_create(lcd_engine * e, int n_clients)
@@ -4512,22 +4571,22 @@ int lcd_clients_create(lcd_engine * e, int n_clients)
 	cudaStream_t s = e->stream;
 	const size_t n = static_cast<size_t>(n_clients);
 	if (e->dc_hi_id.reserve(n, 0, false, s) != cudaSuccess || e->dc_hi_val.reserve(n, 0, false, s) != cudaSuccess ||
+	    e->dc_key_n.reserve(n, 0, false, s) != cudaSuccess || e->dc_key_ids.reserve(n, 0, false, s) != cudaSuccess ||
 	    (e->dc_stride && e->dc_post.reserve(n * e->dc_stride, 0, false, s) != cudaSuccess))
 	{
 		cudaGetLastError();
 		e->dc_clients = 0;
-		e->dc_ver.clear();
 		LCD_FAIL(e, LCD_ERR_CAPACITY, "no device memory for the state of %d clients", n_clients);
 	}
 	LCD_CUDA(e, cudaMemsetAsync(e->dc_hi_id.p, 0, n * sizeof(int), s));
 	LCD_CUDA(e, cudaMemsetAsync(e->dc_hi_val.p, 0, n * sizeof(float), s));
+	LCD_CUDA(e, cudaMemsetAsync(e->dc_key_n.p, 0, n * sizeof(int), s));
+	LCD_CUDA(e, cudaMemsetAsync(e->dc_key_ids.p, 0, n * sizeof(long long), s));
 	LCD_CUDA(e, cudaStreamSynchronize(s));
 	e->dc_clients = n_clients;
-	e->dc_ver.assign(n, -1);
 	e->dc_last_frames = 0;
 	e->dc_hyp_valid = false;
-	prune_map_versions(e);
-	return LCD_OK;
+	return prune_map_versions(e);
 }
 
 int lcd_clients_reset(lcd_engine * e, const int * clients, int n)
@@ -4543,12 +4602,10 @@ int lcd_clients_reset(lcd_engine * e, const int * clients, int n)
 	cudaStream_t s = e->stream;
 	LCD_CUDA(e, e->d_i1.reserve(n, 0, false, s));
 	LCD_CUDA(e, cudaMemcpyAsync(e->d_i1.p, clients, n * sizeof(int), cudaMemcpyHostToDevice, s));
-	decide_reset_clients_kernel<<<(n + 255) / 256, 256, 0, s>>>(e->d_i1.p, n, e->dc_hi_id.p, e->dc_hi_val.p);
+	decide_reset_clients_kernel<<<(n + 255) / 256, 256, 0, s>>>(e->d_i1.p, n, e->dc_hi_id.p, e->dc_hi_val.p, e->dc_key_n.p, e->dc_key_ids.p);
 	LCD_CHECK_LAUNCH(e);
 	LCD_CUDA(e, cudaStreamSynchronize(s));
-	for (int i = 0; i < n; ++i) e->dc_ver[clients[i]] = -1;
-	prune_map_versions(e);
-	return LCD_OK;
+	return prune_map_versions(e);
 }
 
 int lcd_clients_set_map(lcd_engine * e, const int * ids, int n, const int64_t * col_ptr, const int * nbr_row, const int * nbr_level,
@@ -4670,8 +4727,7 @@ int lcd_clients_set_map(lcd_engine * e, const int * ids, int n, const int64_t * 
 	e->dc_h_ids.assign(ids, ids + n);
 	e->dc_lc0 = prediction_lc[0];
 	e->dc_vpp = virtual_place_prior;
-	prune_map_versions(e);
-	return LCD_OK;
+	return prune_map_versions(e);
 }
 
 static int check_decide_params(lcd_engine * e, const lcd_decide_params * dp)
@@ -4687,9 +4743,9 @@ static int check_decide_params(lcd_engine * e, const lcd_decide_params * dp)
 }
 
 // checks of one decision call and the upload of its frame tables (before any kernel of the call is queued); gps[n_frames] (may be null)
-// is uploaded behind them
+// is uploaded behind them.  stage: pinned staging the caller owns and knows to be free (null: the engine's, once its last upload is done)
 static int decide_prepare(lcd_engine * e, int n_frames, int ns, const int * clients, const int * frame_flags, const lcd_decide_params * dp,
-                          cudaStream_t s, const GpsFrame * gps = nullptr)
+                          cudaStream_t s, const GpsFrame * gps = nullptr, PinBuf<long long> * stage = nullptr)
 {
 	if (e->dc_clients <= 0) LCD_FAIL(e, LCD_ERR_STATE, "no clients: call lcd_clients_create first");
 	if (e->dc_map_ver < 0) LCD_FAIL(e, LCD_ERR_STATE, "no map: call lcd_clients_set_map first");
@@ -4709,11 +4765,15 @@ static int decide_prepare(lcd_engine * e, int n_frames, int ns, const int * clie
 	const int B = static_cast<int>(e->dc_active.size());
 	static_assert(sizeof(GpsFrame) % sizeof(long long) == 0, "GPS frame table layout");
 	const size_t gps_words = gps ? n_frames * (sizeof(GpsFrame) / sizeof(long long)) : 0;
-	const size_t words = 2 * static_cast<size_t>(n_frames) + 4 * static_cast<size_t>(B) + gps_words;
-	if (!e->dc_h_ev) LCD_CUDA(e, cudaEventCreateWithFlags(&e->dc_h_ev, cudaEventDisableTiming));
-	else LCD_CUDA(e, cudaEventSynchronize(e->dc_h_ev)); // the staging buffer of the last call has been copied
-	LCD_CUDA(e, e->dc_h_tab.reserve(words));
-	long long * h = e->dc_h_tab.p;
+	const size_t words = 2 * static_cast<size_t>(n_frames) + 2 * static_cast<size_t>(B) + gps_words;
+	if (!stage)
+	{
+		if (!e->dc_h_ev) LCD_CUDA(e, cudaEventCreateWithFlags(&e->dc_h_ev, cudaEventDisableTiming));
+		else LCD_CUDA(e, cudaEventSynchronize(e->dc_h_ev)); // the staging buffer of the last call has been copied
+		stage = &e->dc_h_tab;
+	}
+	LCD_CUDA(e, stage->reserve(words));
+	long long * h = stage->p;
 	for (int f = 0; f < n_frames; ++f)
 	{
 		h[f] = clients[f];
@@ -4722,31 +4782,28 @@ static int decide_prepare(lcd_engine * e, int n_frames, int ns, const int * clie
 	long long * hb = h + 2 * n_frames;
 	for (int b = 0; b < B; ++b)
 	{
-		const int f = e->dc_active[b], c = clients[f], v = e->dc_ver[c];
-		const lcd_engine::MapVersion * mv = v >= 0 ? e->dc_versions.at(v).get() : nullptr;
+		const int f = e->dc_active[b];
 		hb[b] = f;
-		hb[B + b] = c;
-		hb[2 * B + b] = mv ? mv->n : 0;
-		hb[3 * B + b] = static_cast<long long>(reinterpret_cast<uintptr_t>(mv ? mv->ids.p : nullptr));
-		e->dc_active[b] = c;
+		hb[B + b] = clients[f];
 	}
-	if (gps) std::memcpy(hb + 4 * B, gps, n_frames * sizeof(GpsFrame));
+	if (gps) std::memcpy(hb + 2 * B, gps, n_frames * sizeof(GpsFrame));
 	LCD_CUDA(e, e->dc_tab.reserve(words, 0, false, s));
 	LCD_CUDA(e, cudaMemcpyAsync(e->dc_tab.p, h, words * sizeof(long long), cudaMemcpyHostToDevice, s));
-	LCD_CUDA(e, cudaEventRecord(e->dc_h_ev, s));
+	if (stage == &e->dc_h_tab) LCD_CUDA(e, cudaEventRecord(e->dc_h_ev, s));
 	return LCD_OK;
 }
 
 // adjustLikelihood, the posterior of every frame that computes one, the hypothesis selection and checks.  r2 >= 0 (a call with a GPS
-// table uploaded by decide_prepare): the GPS filter of each frame's place list first, with RGBD/LocalRadius squared
+// table uploaded by decide_prepare): the GPS filter of each frame's place list first, with RGBD/LocalRadius squared.  d_qn[n_frames]
+// (may be null): each frame's quantised words; a frame with none is decided as LCD_FRAME_SKIP decides it (decide.cuh, decide_bad)
 static int decide_launch(lcd_engine * e, const float * d_like, int n_frames, int ns, const lcd_decide_params * dp, float * d_post_out, cudaStream_t s,
-                         double r2 = -1.0)
+                         double r2 = -1.0, const int * d_qn = nullptr)
 {
 	const int n = e->dc_n, B = static_cast<int>(e->dc_active.size());
 	const lcd_engine::MapTables & t = *e->dc_tables;
 	DecideMap m{n, e->dc_versions.at(e->dc_map_ver)->ids.p, t.u.p, t.tptr.p, t.tcol.p, t.tval.p, e->dc_lc0, e->dc_vpp, t.tlv.p, t.eps};
 	const long long * tab = e->dc_tab.p;
-	const GpsFrame * gps = r2 >= 0.0 ? reinterpret_cast<const GpsFrame *>(tab + 2 * n_frames + 4 * B) : nullptr;
+	const GpsFrame * gps = r2 >= 0.0 ? reinterpret_cast<const GpsFrame *>(tab + 2 * n_frames + 2 * B) : nullptr;
 	LCD_CUDA(e, e->dc_adj.reserve(static_cast<size_t>(n_frames) * n, 0, false, s));
 	if (gps)
 	{
@@ -4775,8 +4832,9 @@ static int decide_launch(lcd_engine * e, const float * d_like, int n_frames, int
 		d.B = B;
 		d.frame = tab + 2 * n_frames;
 		d.client = d.frame + B;
-		d.prev_n = d.client + B;
-		d.prev_ids = d.prev_n + B;
+		d.key_n = e->dc_key_n.p;
+		d.key_ids = e->dc_key_ids.p;
+		d.qn = d_qn;
 		d.cl_post = e->dc_post.p;
 		d.stride = static_cast<long long>(e->dc_stride);
 		d.adj = e->dc_adj.p;
@@ -4851,10 +4909,11 @@ static int decide_launch(lcd_engine * e, const float * d_like, int n_frames, int
 	a.hyp_slot = e->d_hyp_slot.p;
 	a.gps = gps;
 	a.count = gps ? e->gps_count.p : nullptr;
+	a.qn = d_qn;
+	a.key_n = e->dc_key_n.p;
+	a.key_ids = e->dc_key_ids.p;
 	decide_select_kernel<<<n_frames, 256, 0, s>>>(m, a);
 	LCD_CHECK_LAUNCH(e);
-	// the clients that computed now hold posteriors keyed to the current map
-	for (int c : e->dc_active) e->dc_ver[c] = e->dc_map_ver;
 	e->dc_last_frames = n_frames;
 	e->dc_hyp_valid = true;
 	e->px_valid = false;
@@ -4942,21 +5001,17 @@ int lcd_clients_set_map_gps(lcd_engine * e, const int * ids, int n, const lcd_gp
 	return LCD_OK;
 }
 
-int lcd_decide_gps_batch_dev(lcd_engine * e, const float * d_likelihood, int n_frames, int ns, const int * clients, const int * frame_flags,
-                             const lcd_gps * frame_gps, float local_radius, const lcd_decide_params * dp, float * d_posterior_out,
-                             unsigned char * d_compared_out, void * stream)
+} // extern "C"
+// the GPS frame table of a decision call (frame_gps may be null: no fixes): the frames that compute a posterior and carry a fix (the block
+// of Rtabmap.cpp:1994 does not run for the others) are gated
+static int gps_frames(lcd_engine * e, int n_frames, const int * frame_flags, const lcd_gps * frame_gps, float local_radius, std::vector<GpsFrame> & g)
 {
-	if (!e) return LCD_ERR_INVALID;
-	LCD_TRY(set_device(e));
-	if (!d_likelihood) LCD_FAIL(e, LCD_ERR_INVALID, "likelihood is empty");
-	if (n_frames <= 0 || !clients || !frame_flags) LCD_FAIL(e, LCD_ERR_INVALID, "no frames");
+	if (n_frames <= 0 || !frame_flags) LCD_FAIL(e, LCD_ERR_INVALID, "no frames");
 	if (!(local_radius >= 0.f) || !std::isfinite(local_radius)) LCD_FAIL(e, LCD_ERR_INVALID, "RGBD/LocalRadius must be >= 0");
-	// the frames that compute a posterior and carry a fix (the block of Rtabmap.cpp:1994 does not run for the others)
-	std::vector<GpsFrame> g(n_frames);
+	g.assign(n_frames, GpsFrame{});
 	bool any_fix = false;
 	for (int f = 0; f < n_frames; ++f)
 	{
-		g[f] = GpsFrame{};
 		const bool compute = !(frame_flags[f] & (kDcFlagSkip | kDcFlagHold));
 		g[f].mode = compute ? kGpsAll : kGpsNone;
 		if (!frame_gps) continue;
@@ -4975,6 +5030,20 @@ int lcd_decide_gps_batch_dev(lcd_engine * e, const float * d_likelihood, int n_f
 	}
 	if (any_fix && (e->dc_map_ver < 0 || !e->gps_places))
 		LCD_FAIL(e, LCD_ERR_STATE, "frames carry a GPS fix but the map has no GPS table: call lcd_clients_set_map_gps");
+	return LCD_OK;
+}
+extern "C" {
+
+int lcd_decide_gps_batch_dev(lcd_engine * e, const float * d_likelihood, int n_frames, int ns, const int * clients, const int * frame_flags,
+                             const lcd_gps * frame_gps, float local_radius, const lcd_decide_params * dp, float * d_posterior_out,
+                             unsigned char * d_compared_out, void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (!d_likelihood) LCD_FAIL(e, LCD_ERR_INVALID, "likelihood is empty");
+	if (!clients) LCD_FAIL(e, LCD_ERR_INVALID, "no frames");
+	std::vector<GpsFrame> g;
+	LCD_TRY(gps_frames(e, n_frames, frame_flags, frame_gps, local_radius, g));
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
 	LCD_TRY(decide_prepare(e, n_frames, ns, clients, frame_flags, dp, s, g.data()));
 	const float r2 = local_radius * local_radius; // _localRadius*_localRadius: a float, compared in double
@@ -4997,13 +5066,14 @@ int lcd_decide_fetch(lcd_engine * e, int n_frames, lcd_decision * out)
 }
 
 // Memory::computeTransform of every accepted hypothesis of the last decision (store slot -1: not verified), then the rejections of
-// Rtabmap.cpp:3156-3167
-static int verify_decided(lcd_engine * e, const uint32_t * d_q, const float * d_uv, int n_frames, int nq, const lcd_verify_params * vp, cudaStream_t s)
+// Rtabmap.cpp:3156-3167.  d_nq_frame / d_xyz_to as verify_top_dev takes them.
+static int verify_decided(lcd_engine * e, const uint32_t * d_q, const float * d_uv, int n_frames, int nq, const lcd_verify_params * vp, cudaStream_t s,
+                          const int * d_nq_frame = nullptr, const float * d_xyz_to = nullptr)
 {
 	LCD_TRY(check_verify_params(e, vp, true));
 	if (e->dc_last_frames == 0 || !e->dc_hyp_valid) LCD_FAIL(e, LCD_ERR_STATE, "no decision to verify: run lcd_decide_batch_dev first");
 	if (n_frames != e->dc_last_frames) LCD_FAIL(e, LCD_ERR_INVALID, "the last decision has %d frames, not %d", e->dc_last_frames, n_frames);
-	const PairSource src{{e->st_desc.p, e->st_xyz.p, e->st_n.p, e->d_hyp_slot.p, e->st_cap}, {d_q, d_uv, nullptr, nullptr, nq, nq, nullptr}};
+	const PairSource src{{e->st_desc.p, e->st_xyz.p, e->st_n.p, e->d_hyp_slot.p, e->st_cap}, {d_q, d_uv, d_xyz_to, d_nq_frame, nq, nq, nullptr}};
 	LCD_TRY(register_pairs(e, src, n_frames, std::max(e->st_cap, nq), vp, s));
 	decide_verified_kernel<<<(n_frames + 127) / 128, 128, 0, s>>>(n_frames, e->v_ok.p, e->v_T.p, e->dc_max_dist, e->dc_dec.p, e->d_hyp_id.p,
 	                                                             e->px_valid ? e->px_skip.p : nullptr);
@@ -5100,13 +5170,10 @@ int lcd_clients_set_map_poses(lcd_engine * e, const int * ids, int n, const floa
 	return LCD_OK;
 }
 
-int lcd_decide_proximity_dev(lcd_engine * e, const void * d_queries, const float * d_uv, int n_frames, int nq_per_frame, const float * frame_poses,
-                             const int * enabled, const lcd_proximity_params * pp, void * stream)
+} // extern "C"
+// the checks of a proximity step's parameters
+static int check_proximity_params(lcd_engine * e, const lcd_proximity_params * pp)
 {
-	if (!e) return LCD_ERR_INVALID;
-	LCD_TRY(set_device(e));
-	if (!d_queries || !d_uv || !frame_poses || !enabled || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null or empty frame input");
-	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
 	if (!pp || !pp->verify) LCD_FAIL(e, LCD_ERR_INVALID, "null proximity or verification parameters");
 	const lcd_verify_params * vp = pp->verify;
 	LCD_TRY(check_verify_params(e, vp, false));
@@ -5118,14 +5185,29 @@ int lcd_decide_proximity_dev(lcd_engine * e, const void * d_queries, const float
 	// <= 0 is "no limit" in the reference (Rtabmap.cpp:2829); at most kPxMaxPaths attempts per frame are supported
 	if (pp->max_paths <= 0 || pp->max_paths > kPxMaxPaths) LCD_FAIL(e, LCD_ERR_CAPACITY, "RGBD/ProximityMaxPaths must be 1..%d", kPxMaxPaths);
 	if (e->st_cap == 0) LCD_FAIL(e, LCD_ERR_STATE, "the signature store is empty: nothing to verify against");
-	if (e->dc_last_frames == 0 || !e->dc_hyp_valid) LCD_FAIL(e, LCD_ERR_STATE, "no decision: run lcd_decide_batch_dev first");
-	if (e->dc_verified) LCD_FAIL(e, LCD_ERR_STATE, "the decision was already verified: run proximity detection before lcd_verify_decided_dev");
-	if (n_frames != e->dc_last_frames) LCD_FAIL(e, LCD_ERR_INVALID, "the last decision has %d frames, not %d", e->dc_last_frames, n_frames);
+	return LCD_OK;
+}
+
+static int check_proximity_poses(lcd_engine * e)
+{
 	if (!e->px_map || e->px_ver != e->dc_map_ver) LCD_FAIL(e, LCD_ERR_STATE, "no poses for the current map: call lcd_clients_set_map_poses");
-	if (e->px_last_frames) LCD_FAIL(e, LCD_ERR_STATE, "proximity detection already ran on this decision");
+	return LCD_OK;
+}
+
+static int check_frame_poses(lcd_engine * e, int n_frames, const float * frame_poses)
+{
 	for (int k = 0; k < 12 * n_frames; ++k)
 		if (!std::isfinite(frame_poses[k])) LCD_FAIL(e, LCD_ERR_INVALID, "the pose of frame %d is not finite", k / 12);
-	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	return LCD_OK;
+}
+
+// proximity detection on the last decision (checked by the callers); frame_poses / enabled: host arrays.  d_n_frame[n_frames] (may be
+// null: nq_per_frame each) the frames' rows to register, with d_xyz_to their 3-D points (may be null); d_qn as decide_launch takes it.
+static int proximity_decide(lcd_engine * e, const uint32_t * d_q, const float * d_uv, int n_frames, int nq_per_frame, const float * frame_poses,
+                            const int * enabled, const lcd_proximity_params * pp, cudaStream_t s, const int * d_n_frame = nullptr,
+                            const float * d_xyz_to = nullptr, const int * d_qn = nullptr)
+{
+	const lcd_verify_params * vp = pp->verify;
 	const int mp = pp->max_paths, n_pairs = n_frames * mp;
 	LCD_CUDA(e, e->px_frame_pose.reserve(12 * static_cast<size_t>(n_frames), 0, false, s));
 	LCD_CUDA(e, e->px_enabled.reserve(n_frames, 0, false, s));
@@ -5164,6 +5246,8 @@ int lcd_decide_proximity_dev(lcd_engine * e, const void * d_queries, const float
 	a.pair_row = e->px_row.p;
 	a.pair_n_to = e->px_nto.p;
 	a.nq = nq_per_frame;
+	a.n_frame = d_n_frame;
+	a.qn = d_qn;
 	prof_mark(e, LCD_PROF_PROXIMITY, s);
 	proximity_paths_kernel<<<n_frames, kPxThreads, 0, s>>>(a);
 	prof_mark(e, LCD_PROF_PROXIMITY, s);
@@ -5171,8 +5255,7 @@ int lcd_decide_proximity_dev(lcd_engine * e, const void * d_queries, const float
 	// Memory::computeTransform(place, frame) of every attempted pair in one launch, with a null guess (RGBD/ProximityOdomGuess = false):
 	// FROM = the store row px_slot[i] (-1: none) with its cached dictionary, TO = row px_row[i] of the frames' descriptors, px_nto[i] of
 	// them (0: the pair is not registered)
-	const PairSource src{{e->st_desc.p, e->st_xyz.p, e->st_n.p, e->px_slot.p, e->st_cap},
-	                     {static_cast<const uint32_t *>(d_queries), d_uv, nullptr, e->px_nto.p, 0, nq_per_frame, e->px_row.p}};
+	const PairSource src{{e->st_desc.p, e->st_xyz.p, e->st_n.p, e->px_slot.p, e->st_cap}, {d_q, d_uv, d_xyz_to, e->px_nto.p, 0, nq_per_frame, e->px_row.p}};
 	LCD_TRY(register_pairs(e, src, n_pairs, std::max(e->st_cap, nq_per_frame), vp, s));
 	LCD_TRY(pack_verify_results(e, n_pairs, e->px_res.p, s));
 	proximity_apply_kernel<<<(n_frames + 127) / 128, 128, 0, s>>>(n_frames, mp, fr, e->v_ok.p, e->v_T.p, e->px_rec.p, e->dc_dec.p, e->d_hyp_id.p,
@@ -5182,6 +5265,26 @@ int lcd_decide_proximity_dev(lcd_engine * e, const void * d_queries, const float
 	e->px_max_paths = mp;
 	e->px_valid = true;
 	return LCD_OK;
+}
+
+extern "C" {
+
+int lcd_decide_proximity_dev(lcd_engine * e, const void * d_queries, const float * d_uv, int n_frames, int nq_per_frame, const float * frame_poses,
+                             const int * enabled, const lcd_proximity_params * pp, void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (!d_queries || !d_uv || !frame_poses || !enabled || n_frames <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null or empty frame input");
+	if (nq_per_frame <= 0 || nq_per_frame > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "1..%d descriptors per frame", kMaxFrameQueries);
+	LCD_TRY(check_proximity_params(e, pp));
+	if (e->dc_last_frames == 0 || !e->dc_hyp_valid) LCD_FAIL(e, LCD_ERR_STATE, "no decision: run lcd_decide_batch_dev first");
+	if (e->dc_verified) LCD_FAIL(e, LCD_ERR_STATE, "the decision was already verified: run proximity detection before lcd_verify_decided_dev");
+	if (n_frames != e->dc_last_frames) LCD_FAIL(e, LCD_ERR_INVALID, "the last decision has %d frames, not %d", e->dc_last_frames, n_frames);
+	LCD_TRY(check_proximity_poses(e));
+	if (e->px_last_frames) LCD_FAIL(e, LCD_ERR_STATE, "proximity detection already ran on this decision");
+	LCD_TRY(check_frame_poses(e, n_frames, frame_poses));
+	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	return proximity_decide(e, static_cast<const uint32_t *>(d_queries), d_uv, n_frames, nq_per_frame, frame_poses, enabled, pp, s);
 }
 
 int lcd_proximity_fetch(lcd_engine * e, int n_frames, lcd_proximity_result * out)
@@ -5197,28 +5300,199 @@ int lcd_proximity_fetch(lcd_engine * e, int n_frames, lcd_proximity_result * out
 	std::vector<PackedVerifyResult> res(static_cast<size_t>(n_frames) * mp);
 	LCD_CUDA(e, cudaMemcpy(rec.data(), e->px_rec.p, n_frames * sizeof(ProxRecord), cudaMemcpyDeviceToHost));
 	LCD_CUDA(e, cudaMemcpy(res.data(), e->px_res.p, res.size() * sizeof(PackedVerifyResult), cudaMemcpyDeviceToHost));
-	for (int f = 0; f < n_frames; ++f)
+	proximity_results(n_frames, mp, rec.data(), res.data(), out);
+	return LCD_OK;
+}
+
+// ---- the localisation step of Rtabmap::process from images (lcd_process_frames_decide_*) --------------------------------------------
+static_assert(sizeof(lcd_decide_stages) == 48 && offsetof(lcd_decide_stages, local_radius) == 8 && offsetof(lcd_decide_stages, epipolar) == 16 &&
+                  offsetof(lcd_decide_stages, proximity_enabled) == 40,
+              "lcd_decide_stages layout (rtabmap_b200/capi.py DecideStages)");
+} // extern "C"
+
+// the checks of lcd_process_frames_decide_*, before anything is queued (decide_prepare makes the decision's own); g: the GPS frame
+// table of the call, empty without the GPS filter
+static int frames_decide_check(lcd_engine * e, const char * what, int n_frames, const lcd_orb_params * op, int n_total, const lcd_verify_params * vp,
+                               const int * frame_flags, const lcd_decide_stages * st, std::vector<GpsFrame> & g)
+{
+	LCD_TRY(require_binary(e, what));
+	LCD_TRY(require_unsharded(e, what));
+	if (e->cfg.desc_type != LCD_DESC_U8 || e->cfg.desc_dim != 32) LCD_FAIL(e, LCD_ERR_INVALID, "ORB descriptors need an engine with 32-byte binary descriptors");
+	if (!op) LCD_FAIL(e, LCD_ERR_INVALID, "null ORB parameters");
+	if (op->n_features <= 0 || op->n_features > kMaxFrameQueries) LCD_FAIL(e, LCD_ERR_CAPACITY, "Kp/MaxFeatures must be 1..%d", kMaxFrameQueries);
+	if (n_frames <= 0 || !frame_flags) LCD_FAIL(e, LCD_ERR_INVALID, "no frames");
+	LCD_TRY(check_n_total(e, n_total));
+	LCD_TRY(check_verify_params(e, vp, true));
+	g.clear();
+	if (!st) return LCD_OK;
+	if (st->frame_gps) LCD_TRY(gps_frames(e, n_frames, frame_flags, st->frame_gps, st->local_radius, g));
+	if (st->epipolar)
 	{
-		const ProxRecord & r = rec[f];
-		lcd_proximity_result & o = out[f];
-		memset(&o, 0, sizeof(o));
-		o.status = r.status;
-		o.n_nearest = r.n_nearest;
-		o.n_paths = r.n_paths;
-		o.n_attempts = r.n_attempts;
-		o.suppressed_id = r.suppressed;
-		for (int j = 0; j < r.n_attempts; ++j)
-		{
-			lcd_proximity_path & p = o.paths[j];
-			p.likelihood = r.path[j].likelihood;
-			p.id = r.path[j].id;
-			p.distance = r.path[j].distance;
-			p.candidate_id = r.path[j].candidate;
-			p.accepted = r.accepted[j];
-			p.link_type = r.link_type[j];
-			memcpy(&p.result, &res[static_cast<size_t>(f) * mp + j], sizeof(lcd_verify_result));
-		}
+		// epipolar_decide's launch limit, checked before the decision changes any client state
+		const int cap = std::max(op->n_features, std::max(e->ws_cap, 1));
+		LCD_TRY(fit_smem(e, reinterpret_cast<const void *>(epipolar_check_kernel), epi_smem_bytes(cap), cap));
 	}
+	if (st->proximity)
+	{
+		if (!st->frame_poses || !st->proximity_enabled) LCD_FAIL(e, LCD_ERR_INVALID, "proximity detection needs the frames' poses and enabled flags");
+		LCD_TRY(check_proximity_params(e, st->proximity));
+		LCD_TRY(check_proximity_poses(e));
+		LCD_TRY(check_frame_poses(e, n_frames, st->frame_poses));
+	}
+	return LCD_OK;
+}
+
+// the device work of lcd_process_frames_decide_* on s, behind decide_prepare: detection, the likelihood against the map's real places,
+// the decision with its optional stages, and the verification of what it accepted.  poses / enabled: the proximity step's host arrays.
+static int frames_decide_dev(lcd_engine * e, int n_frames, const uint8_t * d_images, int width, int height, int channels, const void * d_depth,
+                             int depth_type, const lcd_orb_params * op, int incremental, float nndr, int cmp_new, int ns, int n_total,
+                             const lcd_verify_params * vp, const lcd_decide_params * dp, const lcd_decide_stages * st, const float * poses,
+                             const int * enabled, int * d_words, float * d_like, float * d_post, cudaStream_t s)
+{
+	const int cap = op->n_features;
+	LCD_TRY(frame_front_end(e, n_frames, cap, e->o_kp, e->o_desc, e->o_xyz, &e->o_uv, e->o_n, s));
+	LCD_TRY(orb_run(e, n_frames, d_images, width, height, channels, d_depth, depth_type, op, cap, e->o_kp.p, e->o_desc.p, e->o_xyz.p, e->o_uv.p,
+	                e->o_n.p, s));
+	const uint32_t * d_q = reinterpret_cast<const uint32_t *>(e->o_desc.p);
+	const int * d_sig_ids = e->dc_versions.at(e->dc_map_ver)->ids.p + 1; // the map's real places, ascending
+	const int * d_qn = e->o_n.p;                                         // quantised words of each frame: Signature::isBadSignature
+	if (limit_active(e))
+	{
+		const int k = limit_rows(e, cap);
+		LCD_TRY(limit_to_engine(e, n_frames, cap, e->o_kp.p, e->o_n.p, d_q, s));
+		LCD_TRY(localize_dev(e, e->ql_desc.p, n_frames, k, incremental, nndr, cmp_new, d_sig_ids, ns, n_total, e->ql_words.p, d_like, s, e->ql_n.p));
+		LCD_TRY(launch_expand(e, n_frames, cap, k, e->o_n.p, e->ql_index.p, e->ql_n.p, e->ql_words.p, d_words, s));
+		d_qn = e->ql_n.p;
+	}
+	else
+		LCD_TRY(localize_dev(e, d_q, n_frames, cap, incremental, nndr, cmp_new, d_sig_ids, ns, n_total, d_words, d_like, s, e->o_n.p));
+	const double r2 = st && st->frame_gps ? static_cast<double>(st->local_radius * st->local_radius) : -1.0;
+	LCD_TRY(decide_launch(e, d_like, n_frames, ns, dp, d_post, s, r2, d_qn));
+	if (st && st->epipolar) LCD_TRY(epipolar_decide(e, d_words, e->o_uv.p, e->o_n.p, n_frames, cap, st->epipolar, s));
+	if (st && st->proximity)
+		LCD_TRY(proximity_decide(e, d_q, e->o_uv.p, n_frames, cap, poses, enabled, st->proximity, s, e->o_n.p, e->o_xyz.p, d_qn));
+	return verify_decided(e, d_q, e->o_uv.p, n_frames, cap, vp, s, e->o_n.p, e->o_xyz.p);
+}
+extern "C" {
+
+int lcd_process_frames_decide_dev(lcd_engine * e, int n_frames, const uint8_t * d_images, int width, int height, int channels, const void * d_depth,
+                                  int depth_type, const lcd_orb_params * op, int incremental, float nndr, int new_words_compared_together, int ns,
+                                  int n_total, const lcd_verify_params * vp, const int * clients, const int * frame_flags, const lcd_decide_params * dp,
+                                  const lcd_decide_stages * stages, int * d_word_ids_out, float * d_likelihood_out, float * d_posterior_out,
+                                  void * stream)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (!d_images) LCD_FAIL(e, LCD_ERR_INVALID, "null image");
+	std::vector<GpsFrame> g;
+	LCD_TRY(frames_decide_check(e, "lcd_process_frames_decide_dev", n_frames, op, n_total, vp, frame_flags, stages, g));
+	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+	LCD_TRY(decide_prepare(e, n_frames, ns, clients, frame_flags, dp, s, g.empty() ? nullptr : g.data()));
+	int * d_words = d_word_ids_out;
+	if (!d_words)
+	{
+		LCD_CUDA(e, e->d_word_ids.reserve(static_cast<size_t>(n_frames) * op->n_features, 0, false, s));
+		d_words = e->d_word_ids.p;
+	}
+	float * d_like = d_likelihood_out;
+	if (!d_like)
+	{
+		LCD_CUDA(e, e->d_like.reserve(static_cast<size_t>(n_frames) * ns, 0, false, s));
+		d_like = e->d_like.p;
+	}
+	return frames_decide_dev(e, n_frames, d_images, width, height, channels, d_depth, depth_type, op, incremental, nndr, new_words_compared_together, ns,
+	                         n_total, vp, dp, stages, stages ? stages->frame_poses : nullptr, stages ? stages->proximity_enabled : nullptr, d_words,
+	                         d_like, d_posterior_out, s);
+}
+
+int lcd_process_frames_decide_submit(lcd_engine * e, int n_frames, const uint8_t * images, int width, int height, int channels, const void * depth,
+                                     int depth_type, const lcd_orb_params * op, int incremental, float nndr, int new_words_compared_together, int ns,
+                                     int n_total, const lcd_verify_params * vp, const int * clients, const int * frame_flags,
+                                     const lcd_decide_params * dp, const lcd_decide_stages * stages, int * n_kp_out, int * word_ids_out,
+                                     float * likelihood_out, lcd_decision * decisions_out, lcd_verify_result * results_out,
+                                     lcd_epipolar_result * epipolar_out, lcd_proximity_result * proximity_out)
+{
+	if (!e) return LCD_ERR_INVALID;
+	LCD_TRY(set_device(e));
+	if (!images || n_frames <= 0 || width <= 0 || height <= 0) LCD_FAIL(e, LCD_ERR_INVALID, "null image");
+	if (e->flights_busy >= 2) LCD_FAIL(e, LCD_ERR_INVALID, "two batches are already in flight: call lcd_process_frames_wait first");
+	std::vector<GpsFrame> g;
+	LCD_TRY(frames_decide_check(e, "lcd_process_frames_decide_submit", n_frames, op, n_total, vp, frame_flags, stages, g));
+	cudaStream_t s = e->stream;
+	const int slot = (e->flight_head + e->flights_busy) & 1;
+	lcd_engine::Flight & f = e->flights[slot];
+	LCD_TRY(copy_stream_ready(e));
+	if (!f.uploaded)
+	{
+		LCD_CUDA(e, cudaEventCreateWithFlags(&f.uploaded, cudaEventDisableTiming));
+		LCD_CUDA(e, cudaEventCreateWithFlags(&f.done, cudaEventDisableTiming));
+	}
+	// the slot's previous batch was waited for, so its staging buffers are free: nothing here waits for the batch in flight
+	LCD_TRY(decide_prepare(e, n_frames, ns, clients, frame_flags, dp, s, g.empty() ? nullptr : g.data(), &f.h_tab));
+	const float * poses = nullptr;
+	const int * enabled = nullptr;
+	if (stages && stages->proximity)
+	{
+		LCD_CUDA(e, f.h_pose.reserve(12 * static_cast<size_t>(n_frames)));
+		LCD_CUDA(e, f.h_enabled.reserve(n_frames));
+		std::memcpy(f.h_pose.p, stages->frame_poses, 12 * static_cast<size_t>(n_frames) * sizeof(float));
+		std::memcpy(f.h_enabled.p, stages->proximity_enabled, n_frames * sizeof(int));
+		poses = f.h_pose.p;
+		enabled = f.h_enabled.p;
+	}
+	LCD_TRY(upload_frames(e, n_frames, width, height, channels, images, depth, depth_type, f.img, f.depth, e->copy_stream));
+	LCD_CUDA(e, cudaEventRecord(f.uploaded, e->copy_stream));
+	const int cap = op->n_features;
+	const size_t rows = static_cast<size_t>(n_frames) * cap;
+	LCD_CUDA(e, e->d_like.reserve(static_cast<size_t>(n_frames) * ns, 0, false, s));
+	LCD_CUDA(e, e->d_word_ids.reserve(rows, 0, false, s));
+	LCD_CUDA(e, cudaStreamWaitEvent(s, f.uploaded, 0));
+	LCD_TRY(frames_decide_dev(e, n_frames, f.img.p, width, height, channels, depth_type != LCD_DEPTH_NONE ? f.depth.p : nullptr, depth_type, op,
+	                          incremental, nndr, new_words_compared_together, ns, n_total, vp, dp, stages, poses, enabled, e->d_word_ids.p, e->d_like.p,
+	                          nullptr, s));
+	LCD_TRY(download_frames(e, n_frames, rows, ns, nullptr, n_kp_out, word_ids_out, likelihood_out, nullptr, s));
+	f.user_results = nullptr;
+	f.user_dec = nullptr;
+	f.user_ep = nullptr;
+	f.user_px = nullptr;
+	if (results_out)
+	{
+		LCD_CUDA(e, e->v_packed.reserve(n_frames, 0, false, s));
+		LCD_CUDA(e, f.res.reserve(n_frames));
+		LCD_TRY(pack_verify_results(e, n_frames, e->v_packed.p, s));
+		LCD_CUDA(e, cudaMemcpyAsync(f.res.p, e->v_packed.p, n_frames * sizeof(PackedVerifyResult), cudaMemcpyDeviceToHost, s));
+		f.user_results = results_out;
+	}
+	if (decisions_out)
+	{
+		LCD_CUDA(e, f.h_dec.reserve(n_frames));
+		LCD_CUDA(e, cudaMemcpyAsync(f.h_dec.p, e->dc_dec.p, n_frames * sizeof(Decision), cudaMemcpyDeviceToHost, s));
+		f.user_dec = decisions_out;
+	}
+	if (epipolar_out && stages && stages->epipolar)
+	{
+		LCD_CUDA(e, f.h_ep_res.reserve(static_cast<size_t>(n_frames) * 8));
+		LCD_CUDA(e, f.h_ep_F.reserve(static_cast<size_t>(n_frames) * 9));
+		LCD_CUDA(e, cudaMemcpyAsync(f.h_ep_res.p, e->ep_res.p, static_cast<size_t>(n_frames) * 8 * sizeof(int), cudaMemcpyDeviceToHost, s));
+		LCD_CUDA(e, cudaMemcpyAsync(f.h_ep_F.p, e->ep_F.p, static_cast<size_t>(n_frames) * 9 * sizeof(double), cudaMemcpyDeviceToHost, s));
+		f.user_ep = epipolar_out;
+	}
+	if (proximity_out && stages && stages->proximity)
+	{
+		const size_t n_pairs = static_cast<size_t>(n_frames) * e->px_max_paths;
+		LCD_CUDA(e, f.h_px_rec.reserve(n_frames));
+		LCD_CUDA(e, f.h_px_res.reserve(n_pairs));
+		LCD_CUDA(e, cudaMemcpyAsync(f.h_px_rec.p, e->px_rec.p, n_frames * sizeof(ProxRecord), cudaMemcpyDeviceToHost, s));
+		LCD_CUDA(e, cudaMemcpyAsync(f.h_px_res.p, e->px_res.p, n_pairs * sizeof(PackedVerifyResult), cudaMemcpyDeviceToHost, s));
+		f.user_px = proximity_out;
+		f.px_max_paths = e->px_max_paths;
+	}
+	f.n_frames = n_frames;
+	f.detector = e->detector;
+	LCD_CUDA(e, f.overflow.reserve(1));
+	LCD_CUDA(e, cudaMemcpyAsync(f.overflow.p, e->o_overflow.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+	LCD_CUDA(e, cudaEventRecord(f.done, s));
+	++e->flights_busy;
 	return LCD_OK;
 }
 

@@ -52,6 +52,8 @@ struct ProxArgs
 	float radius, angle, filter_radius;
 	int max_paths, max_depth;
 	int nq;                     // descriptors per frame
+	const int * n_frame;        // [n_frames] descriptors of each frame (nullptr: nq each)
+	const int * qn;             // [n_frames] quantised words of each frame (nullptr: none is a bad signature), decide.cuh's decide_bad
 	ProxRecord * rec;           // [n_frames]
 	int * pair_slot;            // [n_frames][max_paths] store row of each attempted registration, -1 = none
 	int * pair_row;             // [n_frames][max_paths] its frame row
@@ -164,6 +166,7 @@ __global__ void __launch_bounds__(kPxThreads) proximity_paths_kernel(const ProxA
 	const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 	ProxRecord & rec = a.rec[f];
 	const float * P = a.frame_pose + 12 * static_cast<size_t>(f);
+	const bool enabled = a.enabled[f] && !decide_bad(a.qn, f); // a bad signature's frame is not a proximity candidate
 	for (int j = tid; j < a.max_paths; j += blockDim.x)
 	{
 		a.pair_slot[f * a.max_paths + j] = -1;
@@ -172,7 +175,7 @@ __global__ void __launch_bounds__(kPxThreads) proximity_paths_kernel(const ProxA
 	}
 	if (tid == 0)
 	{
-		rec.status = a.enabled[f] ? kPxRan : kPxOff;
+		rec.status = enabled ? kPxRan : kPxOff;
 		rec.n_nearest = rec.n_paths = rec.n_attempts = rec.loop_in_radius = rec.suppressed = 0;
 		for (int j = 0; j < kPxMaxPaths; ++j)
 		{
@@ -181,7 +184,7 @@ __global__ void __launch_bounds__(kPxThreads) proximity_paths_kernel(const ProxA
 		}
 		s_count = 0;
 	}
-	if (!a.enabled[f]) return;
+	if (!enabled) return;
 	__syncthreads();
 	// 1) graph::findNearestNodes(signature->id(), _optimizedPoses, radius): every place with d2 < radius^2, compacted in id order
 	const float r2 = __fmul_rn(a.radius, a.radius);
@@ -408,7 +411,7 @@ __global__ void __launch_bounds__(kPxThreads) proximity_paths_kernel(const ProxA
 				const int id = a.ids[s_row[k]];
 				rec.path[t] = ProxPath{s_kl[p], s_kid[p], s_kd[p], id};
 				a.pair_slot[f * a.max_paths + t] = (a.sig_slot && id < a.slot_cap) ? a.sig_slot[id] : -1;
-				a.pair_n_to[f * a.max_paths + t] = a.nq;
+				a.pair_n_to[f * a.max_paths + t] = a.n_frame ? a.n_frame[f] : a.nq;
 				s_attempts = t + 1;
 			}
 		}
