@@ -1049,8 +1049,9 @@ int lcd_profile_read(lcd_engine * e, int which, double * total_ms, long long * l
 int lcd_profile_reset(lcd_engine * e);
 
 /* copy an internal ORB buffer of the last lcd_orb_* call back to the host (diagnostics / tests):
- * which = 0 gray pyramid, 1 mask pyramid, 2 blurred pyramid, 3 FAST candidate keys, 4 candidate counts,
- * 5 keypoints per level counts, 6 FAST score pyramid.  Returns the number of bytes copied (<= cap_bytes) or <0. */
+ * which = 0 gray pyramid, 1 mask pyramid, 2 blurred pyramid, 3 FAST candidate keys (after the selection: the survivors of the
+ * first retainBest, in its order), 4 candidate counts, 5 keypoints per level counts, 6 survivors of the first retainBest per
+ * level.  Returns the number of bytes copied (<= cap_bytes) or <0. */
 long long lcd_debug_orb_buffer(lcd_engine * e, int which, void * out, long long cap_bytes);
 
 /* engine stream (cudaStream_t as void*) and a full device sync, for harnesses */

@@ -513,9 +513,9 @@ struct lcd_engine
 	DevBuf<int> d_hyp_id, d_hyp_slot;
 	// ORB workspace
 	DevBuf<uint8_t> o_img, o_gray, o_mask, o_blur, o_desc;
-	DevBuf<unsigned char> o_depth;
+	DevBuf<unsigned char> o_depth, o_rank_ws;
 	DevBuf<uint32_t> o_cand;
-	DevBuf<int> o_cand_count, o_level_n, o_n, o_overflow;
+	DevBuf<int> o_cand_count, o_surv_n, o_level_n, o_n, o_overflow;
 	DevBuf<OrbKeypoint> o_level_kp, o_kp;
 	DevBuf<float> o_xyz, o_uv;
 	float gauss_sigma_loaded = -1.f;
@@ -2590,7 +2590,7 @@ static int fast_pyramid(lcd_engine * e, int n_frames, const OrbPrepArgs & prep, 
 {
 	const OrbGeom & g = prep.g;
 	const int slots = n_frames * g.n_levels;
-	// a level stores at most Kp/MaxFeatures keypoints (orb_select_kernel), and the merge sorts the stored keypoints of all levels of a
+	// a level stores at most Kp/MaxFeatures keypoints (orb_rank_kernel), and the merge sorts the stored keypoints of all levels of a
 	// frame in shared memory: 128 KB for 4 levels at the image-level calls' largest Kp/MaxFeatures; fit_smem checks any other size
 	static_assert(kOrbMaxLevels * kMaxFrameQueries * sizeof(unsigned long long) <= 128 * 1024, "merge keys of the largest frame");
 	const int level_cap = n_features;
@@ -2599,6 +2599,8 @@ static int fast_pyramid(lcd_engine * e, int n_frames, const OrbPrepArgs & prep, 
 	LCD_TRY(fit_smem(e, reinterpret_cast<const void *>(orb_merge_kernel), pad * sizeof(unsigned long long), n_features));
 	LCD_CUDA(e, e->o_cand.reserve(static_cast<size_t>(slots) * kOrbCandCap, 0, false, s));
 	LCD_CUDA(e, e->o_cand_count.reserve(slots, 0, false, s));
+	LCD_CUDA(e, e->o_surv_n.reserve(slots, 0, false, s));
+	LCD_CUDA(e, e->o_rank_ws.reserve(static_cast<size_t>(slots) * kOrbRankWsBytes, 0, false, s));
 	LCD_CUDA(e, e->o_level_n.reserve(slots, 0, false, s));
 	LCD_CUDA(e, e->o_level_kp.reserve(static_cast<size_t>(slots) * level_cap, 0, false, s));
 	uint8_t * const w_gray = prep.gray;
@@ -2606,6 +2608,8 @@ static int fast_pyramid(lcd_engine * e, int n_frames, const OrbPrepArgs & prep, 
 	uint8_t * const w_mask = prep.mask;
 	uint32_t * const w_cand = e->o_cand.p;
 	int * const w_cand_count = e->o_cand_count.p;
+	int * const w_surv_n = e->o_surv_n.p;
+	unsigned char * const w_rank_ws = e->o_rank_ws.p;
 	int * const w_level_n = e->o_level_n.p;
 	OrbKeypoint * const w_level_kp = e->o_level_kp.p;
 	LCD_CUDA(e, zero_fill_async(w_cand_count, slots * sizeof(int), s));
@@ -2662,15 +2666,18 @@ static int fast_pyramid(lcd_engine * e, int n_frames, const OrbPrepArgs & prep, 
 		a.g = g;
 		a.cand = w_cand;
 		a.cand_count = w_cand_count;
+		a.surv_n = w_surv_n;
+		a.rank_ws = w_rank_ws;
 		a.level_kp = w_level_kp;
 		a.level_n = w_level_n;
 		a.level_cap = level_cap;
 		a.overflow = e->o_overflow.p;
 		// The levels are independent: level 0 (the long one) stays on the caller's stream, the coarser ones run FAST + selection on side
-		// streams beside it and join before the merge.  Selection is one CTA per (frame, level), latency-bound: level l holds at most
-		// kOrbCandCap >> l candidates in shared memory (192 KB, 96 KB, 48 KB, ...), so the FAST / blur CTAs of other levels share its SMs.
-		LCD_CUDA(e, cudaFuncSetAttribute(orb_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-		                                 static_cast<int>(static_cast<size_t>(kOrbCandCap) * (4 + 4 + 2 + 2))));
+		// streams beside it and join before the merge.  The order and rank kernels are one CTA per (frame, level), latency-bound: level l
+		// holds at most kOrbCandCap >> l candidates in shared memory (96 KB, 48 KB, 24 KB, ...: two level-0 CTAs per SM), so the FAST / blur
+		// CTAs of other levels share its SMs; Harris and the IC angle run over all survivors / keypoints of the level at once.
+		LCD_CUDA(e, cudaFuncSetAttribute(orb_order_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+		                                 static_cast<int>(static_cast<size_t>(kOrbCandCap) * (4 + 2))));
 		for (int l = g.n_levels - 1; l >= 0; --l)
 		{
 			cudaStream_t ls = s;
@@ -2693,8 +2700,17 @@ static int fast_pyramid(lcd_engine * e, int n_frames, const OrbPrepArgs & prep, 
 			LCD_CHECK_LAUNCH(e);
 			a.level = l;
 			a.cand_cap = std::max(2048, kOrbCandCap >> l);
-			const size_t smem = static_cast<size_t>(a.cand_cap) * (4 + 4 + 2 + 2);
-			orb_select_kernel<<<n_frames, kOrbSelectThreads, smem, ls>>>(a);
+			orb_order_kernel<<<n_frames, kOrbSelectThreads, static_cast<size_t>(a.cand_cap) * (4 + 2), ls>>>(a);
+			LCD_CHECK_LAUNCH(e);
+			// the grids cover the expected survivors (2N) and keypoints (N) of a frame; their blocks stride over the ties beyond
+			const int n_level = std::min(g.n_per_level[l], level_cap);
+			const dim3 hgrd(std::max(1, (std::min(2 * g.n_per_level[l], a.cand_cap) + kOrbHarrisThreads - 1) / kOrbHarrisThreads), n_frames);
+			orb_harris_kernel<<<hgrd, kOrbHarrisThreads, 0, ls>>>(a);
+			LCD_CHECK_LAUNCH(e);
+			orb_rank_kernel<<<n_frames, kOrbSelectThreads, 0, ls>>>(a);
+			LCD_CHECK_LAUNCH(e);
+			const int wpb = kOrbAngleThreads / 32;
+			orb_angle_kernel<<<dim3(std::max(1, (n_level + wpb - 1) / wpb), n_frames), kOrbAngleThreads, 0, ls>>>(a);
 			LCD_CHECK_LAUNCH(e);
 			if (l > 0 && l <= 3) LCD_CUDA(e, cudaEventRecord(e->aux_join[l - 1], ls));
 		}
@@ -3336,6 +3352,7 @@ long long lcd_debug_orb_buffer(lcd_engine * e, int which, void * out, long long 
 	case 3: src = e->o_cand.p; bytes = e->o_cand.cap * sizeof(uint32_t); break;
 	case 4: src = e->o_cand_count.p; bytes = e->o_cand_count.cap * sizeof(int); break;
 	case 5: src = e->o_level_n.p; bytes = e->o_level_n.cap * sizeof(int); break;
+	case 6: src = e->o_surv_n.p; bytes = e->o_surv_n.cap * sizeof(int); break;
 	case 7: src = e->v_clk.p; bytes = e->v_clk.cap * sizeof(long long); break;
 #ifdef LCD_DEBUG_PHASES
 	case 9:

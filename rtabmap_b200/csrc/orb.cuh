@@ -16,7 +16,7 @@
 //   * KeyPointsFilter::retainBest keeps ties and leaves the keypoints in the order libstdc++'s
 //     std::nth_element (introselect, median-of-3, unguarded Hoare partition) and std::partition produce;
 //     that order is the order of the frame's descriptors and therefore of its words, so the two
-//     algorithms are replayed literally (sequentially, one thread per frame and level);
+//     algorithms are replayed literally (block-cooperatively, one CTA per frame and level);
 //   * Harris response and IC angle use float arithmetic in OpenCV's operation order, without FMA;
 //     fastAtan2's polynomial coefficients are float products (c * 57.29578f);
 //   * the 7x7 sigma=2 blur runs on a sub-matrix of the pyramid buffer, which sends OpenCV down the float
@@ -408,7 +408,7 @@ orb_fast_kernel(const uint8_t * __restrict__ gray_all, const uint8_t * __restric
 // [frame][y][x] of the pyramid level; out-of-image pixels arrive as zeros, which is what the manual loop above stores), 64 x 32
 // pixel tiles, and the per-pixel compass test and non-max suppression done four pixels at a time with byte-SIMD instructions
 // (VABSDIFF4 / VSETGTU4): ~5 instead of ~25 instructions per pixel for the two full-tile passes.  Results are the same candidate
-// SET (the selection kernel sorts it), bit for bit.
+// SET (orb_order_kernel sorts it), bit for bit.
 constexpr int kFastTmaTW = 64, kFastTmaTH = 32;
 constexpr int kFastTmaGW = 96, kFastTmaGH = 40;   // staged box: x0-16 .. x0+80, y0-4 .. y0+36: the TMA needs a 16-byte aligned row start
                                                   // (x0 is a multiple of 64) and an inner extent that is a multiple of 16 bytes
@@ -443,7 +443,7 @@ struct alignas(64) OrbTensorMap
 };
 
 __global__ void __launch_bounds__(256)
-orb_fast_tma_kernel(const __grid_constant__ OrbTensorMap tmap, const uint8_t * __restrict__ mask_all, const OrbGeom g, int level,
+orb_fast_tma_kernel(const __grid_constant__ OrbTensorMap tmap, const uint8_t * __restrict__ mask_all, const __grid_constant__ OrbGeom g, int level,
                     uint32_t * __restrict__ cand, int * __restrict__ cand_count)
 {
 	constexpr int GW = kFastTmaGW, GH = kFastTmaGH, SW = kFastTmaSW, SH = kFastTmaSH;
@@ -579,18 +579,28 @@ orb_fast_tma_kernel(const __grid_constant__ OrbTensorMap tmap, const uint8_t * _
 	}
 }
 
-// ---- K3: per (frame, level) selection: raster order, retainBest(2N) on FAST score, Harris, retainBest(N),
-//          IC angle.  One CTA per frame, one launch per level; the two retainBest replays are block-cooperative
-//          (partition_replay below). ----------------------------------------------------------------------
+// ---- K3: per (frame, level) selection: raster order, retainBest(2N) on FAST score, Harris, retainBest(N), IC angle, in four launches
+//          per level.  The two retainBest replays are block-cooperative (partition_replay below) and need one CTA per (frame, level);
+//          Harris and the IC angle are data-parallel and run over every survivor / keypoint of the batch:
+//            orb_order_kernel   CTA per (frame, level): raster order + retainBest(2N), survivors back into the candidate list
+//            orb_harris_kernel  thread per survivor: Harris response
+//            orb_rank_kernel    CTA per (frame, level), over the survivors only: retainBest(N) (+ the limitKeypoints cut), keypoints
+//            orb_angle_kernel   warp per keypoint: IC angle
+// ---------------------------------------------------------------------------------------------------------------------------------------
+constexpr int kOrbRankCap = 4096;     // survivors of the first retainBest a rank CTA holds in shared memory; more replay in global memory
+constexpr int kOrbHarrisThreads = 128;
+constexpr int kOrbAngleThreads = 256;
+constexpr size_t kOrbRankWsBytes = static_cast<size_t>(kOrbCandCap) * (4 + 2 + 2); // per slot: Harris responses, then perm and rpos
+
 // Scratch of the block-cooperative replays below.
 struct SelectScratch
 {
-	uint16_t * rpos; // [kOrbCandCap] positions of the right-hand scan's stops, by rank from the right
+	uint16_t * rpos; // [n] positions of the right-hand scan's stops, by rank from the right
 	int * warp_tot;  // [32]
 	int * cut;       // [1]
 };
 
-// One Hoare-style partition pass over perm[lo..hi), replayed by the whole CTA.
+// One Hoare-style partition pass over e[lo..hi), replayed by the whole CTA; the elements are compared by val(element).
 //
 // Both libstdc++ loops this file replays (std::__unguarded_partition and the bidirectional std::__partition)
 // have the same shape: a left cursor that walks up and STOPS at elements with stop_l(x), a right cursor that walks
@@ -601,17 +611,17 @@ struct SelectScratch
 // all k with L_k < R_k, and the left cursor ends at min(first unswapped L, last swapped R).  Ranks come from one
 // block-wide prefix sum; every thread owns a contiguous segment of <= 32 positions (kOrbCandCap / kOrbSelectThreads).
 // Returns the final left cursor (INT_MAX if neither exists).  All threads must call; result is uniform.
-template <class StopL, class StopR>
-__device__ inline int partition_replay(uint16_t * perm, const float * resp, int lo, int hi, const SelectScratch & sc, StopL stop_l, StopR stop_r)
+template <class T, class Val, class StopL, class StopR>
+__device__ inline int partition_replay(T * e, Val val, int lo, int hi, const SelectScratch & sc, StopL stop_l, StopR stop_r)
 {
 	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
 	const int len = hi - lo;
 	const int seg = (len + static_cast<int>(blockDim.x) - 1) / static_cast<int>(blockDim.x);
-	const int b = lo + tid * seg, e = min(b + seg, hi);
+	const int b = lo + tid * seg, en = min(b + seg, hi);
 	uint32_t ml = 0, mr = 0;
-	for (int i = b; i < e; ++i)
+	for (int i = b; i < en; ++i)
 	{
-		const float x = resp[perm[i]];
+		const float x = val(e[i]);
 		ml |= (stop_l(x) ? 1u : 0u) << (i - b);
 		mr |= (stop_r(x) ? 1u : 0u) << (i - b);
 	}
@@ -654,9 +664,9 @@ __device__ inline int partition_replay(uint16_t * perm, const float * resp, int 
 			const int j = k < tot_r ? static_cast<int>(sc.rpos[k]) : -1;
 			if (i < j)
 			{
-				const uint16_t t = perm[i];
-				perm[i] = perm[j];
-				perm[j] = t;
+				const T t = e[i];
+				e[i] = e[j];
+				e[j] = t;
 				best = min(best, j);
 			}
 			else best = min(best, i);
@@ -669,17 +679,18 @@ __device__ inline int partition_replay(uint16_t * perm, const float * resp, int 
 	return cut;
 }
 
-// libstdc++ std::nth_element(first, nth, last, greater-by-response) on perm[first..last): introselect with the
+// libstdc++ std::nth_element(first, nth, last, greater-by-val) on e[first..last): introselect with the
 // median-of-three pivot moved to `first`, __unguarded_partition on [first+1, last), insertion sort of the last <= 3.
 // Called by all threads of the CTA; thread 0 does the O(1) steps.
-__device__ inline void nth_element_replay(uint16_t * perm, const float * resp, int first, int nth, int last, const SelectScratch & sc)
+template <class T, class Val>
+__device__ inline void nth_element_replay(T * e, Val val, int first, int nth, int last, const SelectScratch & sc)
 {
 	if (first == last || nth == last) return;
-	auto comp = [&](int a, int b) { return resp[perm[a]] > resp[perm[b]]; };
+	auto comp = [&](int a, int b) { return val(e[a]) > val(e[b]); };
 	auto swp = [&](int a, int b) {
-		const uint16_t t = perm[a];
-		perm[a] = perm[b];
-		perm[b] = t;
+		const T t = e[a];
+		e[a] = e[b];
+		e[b] = t;
 	};
 	int depth = 2 * (31 - __clz(last - first));
 	while (last - first > 3)
@@ -715,9 +726,9 @@ __device__ inline void nth_element_replay(uint16_t * perm, const float * resp, i
 			else swp(r, b);
 		}
 		__syncthreads();
-		const float pv = resp[perm[first]];
+		const float pv = val(e[first]);
 		// __unguarded_partition(first+1, last, pivot): left stops at !(x > pv), right at !(pv > x)
-		const int cut = partition_replay(perm, resp, first + 1, last, sc, [pv](float x) { return !(x > pv); }, [pv](float x) { return !(pv > x); });
+		const int cut = partition_replay(e, val, first + 1, last, sc, [pv](float x) { return !(x > pv); }, [pv](float x) { return !(pv > x); });
 		if (cut <= nth) first = cut;
 		else last = cut;
 	}
@@ -726,36 +737,38 @@ __device__ inline void nth_element_replay(uint16_t * perm, const float * resp, i
 		// __insertion_sort(first, last)
 		for (int i = first + 1; i < last; ++i)
 		{
-			const uint16_t val = perm[i];
-			const float rv = resp[val];
-			if (rv > resp[perm[first]])
+			const T v = e[i];
+			const float rv = val(v);
+			if (rv > val(e[first]))
 			{
-				for (int j = i; j > first; --j) perm[j] = perm[j - 1];
-				perm[first] = val;
+				for (int j = i; j > first; --j) e[j] = e[j - 1];
+				e[first] = v;
 			}
 			else
 			{
 				int j = i;
-				while (rv > resp[perm[j - 1]])
+				while (rv > val(e[j - 1]))
 				{
-					perm[j] = perm[j - 1];
+					e[j] = e[j - 1];
 					--j;
 				}
-				perm[j] = val;
+				e[j] = v;
 			}
 		}
 	}
 	__syncthreads();
 }
 
-// KeyPointsFilter::retainBest(keypoints, n_points): returns the new size.  Called by all threads of the CTA.
-__device__ inline int retain_best_replay(uint16_t * perm, const float * resp, int n, int n_points, const SelectScratch & sc)
+// KeyPointsFilter::retainBest(keypoints, n_points) on e[0, n) by response val(element): returns the new size.  Called by all threads of
+// the CTA.
+template <class T, class Val>
+__device__ inline int retain_best_replay(T * e, Val val, int n, int n_points, const SelectScratch & sc)
 {
 	if (n_points < 0 || n <= n_points) return n;
 	if (n_points == 0) return 0;
-	nth_element_replay(perm, resp, 0, n_points - 1, n, sc);
-	const float amb = resp[perm[n_points - 1]];
-	// std::partition(perm + n_points, perm + n, response >= amb) (bidirectional version): left stops at
+	nth_element_replay(e, val, 0, n_points - 1, n, sc);
+	const float amb = val(e[n_points - 1]);
+	// std::partition(e + n_points, e + n, response >= amb) (bidirectional version): left stops at
 	// !(x >= amb), right stops at x >= amb; the result is n_points + #{x >= amb}
 	int keep = 0;
 	{
@@ -764,13 +777,13 @@ __device__ inline int retain_best_replay(uint16_t * perm, const float * resp, in
 		if (threadIdx.x == 0) s_keep = 0;
 		__syncthreads();
 		int c = 0;
-		for (int i = n_points + threadIdx.x; i < n; i += blockDim.x) c += resp[perm[i]] >= amb ? 1 : 0;
+		for (int i = n_points + threadIdx.x; i < n; i += blockDim.x) c += val(e[i]) >= amb ? 1 : 0;
 		if (c) atomicAdd(&s_keep, c);
 		__syncthreads();
 		keep = s_keep;
 		__syncthreads();
 	}
-	partition_replay(perm, resp, n_points, n, sc, [amb](float x) { return !(x >= amb); }, [amb](float x) { return x >= amb; });
+	partition_replay(e, val, n_points, n, sc, [amb](float x) { return !(x >= amb); }, [amb](float x) { return x >= amb; });
 	return n_points + keep;
 }
 
@@ -862,72 +875,64 @@ __device__ __forceinline__ float fast_atan2_deg(float y, float x)
 	return a;
 }
 
+// Arguments of the four selection kernels of one level (one launch of each per level: shared memory is sized per level).
 struct OrbSelectArgs
 {
 	const uint8_t * gray;
 	OrbGeom g;
-	const uint32_t * cand;
+	uint32_t * cand;        // [n_frames][n_levels][kOrbCandCap] FAST keys (pos << 8 | score); orb_order_kernel leaves the survivors of
+	                        // retainBest(2N) there, in the order the replay leaves them
 	const int * cand_count;
+	int * surv_n;           // [n_frames][n_levels] survivors of retainBest(2N)
+	unsigned char * rank_ws;// [n_frames][n_levels][kOrbRankWsBytes]: the survivors' Harris responses, then the rank replay's perm / rpos of
+	                        // a CTA with more than kOrbRankCap survivors
 	OrbKeypoint * level_kp; // [n_frames][n_levels][level_cap]
 	int * level_n;          // [n_frames][n_levels] keypoints the level keeps (level_kp holds at most level_cap of them)
 	int level_cap;          // Kp/MaxFeatures
 	int * overflow;         // set when a candidate list had to be truncated
-	int level;              // pyramid level this launch handles (one launch per level: shared memory is sized per level)
+	int level;              // pyramid level of the launch
 	int cand_cap;           // candidates of this level kept in shared memory (<= kOrbCandCap)
 };
 
+__device__ __forceinline__ float * rank_resp(const OrbSelectArgs & a, int slot)
+{
+	return reinterpret_cast<float *>(a.rank_ws + static_cast<size_t>(slot) * kOrbRankWsBytes);
+}
+
+// Raster order + retainBest(2N) on the FAST score.  The replay permutes the 32-bit keys themselves and compares their low byte as a float
+// (cv::KeyPoint::response of a FAST corner), so the shared memory is the keys + the replay's rpos: cand_cap x 6 bytes.
 __global__ void __launch_bounds__(kOrbSelectThreads)
-orb_select_kernel(const OrbSelectArgs a)
+orb_order_kernel(const OrbSelectArgs a)
 {
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	const int ccap = a.cand_cap;
-	uint32_t * keys = reinterpret_cast<uint32_t *>(smem_raw);   // [ccap]
-	float * resp = reinterpret_cast<float *>(keys + ccap);        // [ccap]
-	uint16_t * perm = reinterpret_cast<uint16_t *>(resp + ccap);  // [ccap]
+	uint32_t * keys = reinterpret_cast<uint32_t *>(smem_raw);    // [ccap]
+	uint16_t * rpos = reinterpret_cast<uint16_t *>(keys + ccap); // [ccap]
 	__shared__ int s_warp_tot[32], s_cut;
-	const SelectScratch sc{perm + ccap, s_warp_tot, &s_cut};
-	__shared__ int s_umax[20];
+	const SelectScratch sc{rpos, s_warp_tot, &s_cut};
 
 	const int tid = threadIdx.x;
 	const int level = a.level, frame = blockIdx.x;
 	const int slot = frame * a.g.n_levels + level;
-	const int w = a.g.w[level], h = a.g.h[level];
-	const uint8_t * img = a.gray + static_cast<size_t>(frame) * a.g.frame_stride + a.g.off[level];
+	uint32_t * cand = a.cand + static_cast<size_t>(slot) * kOrbCandCap;
 	int n = a.cand_count[slot];
 	if (n > ccap)
 	{
 		n = ccap;
 		if (tid == 0) atomicExch(a.overflow, 1);
 	}
-	for (int i = tid; i < n; i += blockDim.x) keys[i] = a.cand[static_cast<size_t>(slot) * kOrbCandCap + i];
-	if (tid == 0)
-	{
-		// umax table of the circular patch (ORB computeKeyPoints)
-		const int half = a.g.patch / 2;
-		const int vmax = static_cast<int>(floorf(half * sqrtf(2.f) / 2 + 1));
-		const int vmin = static_cast<int>(ceilf(half * sqrtf(2.f) / 2));
-		for (int v = 0; v <= vmax; ++v) s_umax[v] = static_cast<int>(rint(sqrt(static_cast<double>(half) * half - static_cast<double>(v) * v)));
-		for (int v = half, v0 = 0; v >= vmin; --v)
-		{
-			while (s_umax[v0] == s_umax[v0 + 1]) ++v0;
-			s_umax[v] = v0;
-			++v0;
-		}
-	}
-	__syncthreads();
 	// raster order (FAST emits keypoints row by row).  Every candidate is a different pixel, so its place in raster order is the number
-	// of candidates at smaller positions: a position bitmap (in the not yet used response array) + one block-wide prefix sum of its
-	// popcounts replaces a 105-stage bitonic sort of 16k keys.
+	// of candidates at smaller positions: a position bitmap (in the not yet used rpos array, in passes of 32 * nw_max positions) + one
+	// block-wide prefix sum of its popcounts replaces a 105-stage bitonic sort of 16k keys.  The keys are read from the candidate list and
+	// land in shared memory in raster order.
 	{
-		// (a static array for the segment prefixes would push the CTA past the 196 KB shared-memory carve-out and halve the L1 left for
-		// the Harris / angle patches: everything lives in the dynamic allocation)
-		const int nw_max = ccap - ccap / 8;
-		uint32_t * bits = reinterpret_cast<uint32_t *>(resp);   // 7/8 of the response array: 32 * nw_max positions per pass
+		const int nw_max = (ccap / 2 * 8 / 9) & ~7;
+		uint32_t * bits = reinterpret_cast<uint32_t *>(rpos);
 		int * s_seg = reinterpret_cast<int *>(bits + nw_max);   // exclusive popcount prefix of every 8-word segment of the bitmap
-		uint32_t * sorted = reinterpret_cast<uint32_t *>(perm); // perm + rpos: ccap words
 		const int lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
 		constexpr int kSegPerThread = kOrbCandCap / 8 / kOrbSelectThreads; // 8-word segments owned by a thread
-		const int n_pos = w * h;
+		static_assert(kSegPerThread * 8 * kOrbSelectThreads >= kOrbCandCap / 2, "the segments cover the largest bitmap pass");
+		const int n_pos = a.g.w[level] * a.g.h[level];
 		int base = 0;
 		for (int p0 = 0; p0 < n_pos; p0 += 32 * nw_max)
 		{
@@ -936,7 +941,7 @@ orb_select_kernel(const OrbSelectArgs a)
 			__syncthreads();
 			for (int i = tid; i < n; i += blockDim.x)
 			{
-				const int rel = static_cast<int>(keys[i] >> 8) - p0;
+				const int rel = static_cast<int>(cand[i] >> 8) - p0;
 				if (rel >= 0 && rel < 32 * nw) atomicOr(&bits[rel >> 5], 1u << (rel & 31));
 			}
 			__syncthreads();
@@ -976,107 +981,183 @@ orb_select_kernel(const OrbSelectArgs a)
 			__syncthreads();
 			for (int i = tid; i < n; i += blockDim.x)
 			{
-				const uint32_t key = keys[i];
+				const uint32_t key = cand[i];
 				const int rel = static_cast<int>(key >> 8) - p0;
 				if (rel >= 0 && rel < 32 * nw)
 				{
 					const int wi = rel >> 5;
 					int r = base + s_seg[wi >> 3] + __popc(bits[wi] & ((1u << (rel & 31)) - 1u));
 					for (int j = wi & ~7; j < wi; ++j) r += __popc(bits[j]);
-					sorted[r] = key;
+					keys[r] = key;
 				}
 			}
 			base += total;
 			__syncthreads();
 		}
-		for (int i = tid; i < n; i += blockDim.x) keys[i] = sorted[i];
-		__syncthreads();
 	}
-	for (int i = tid; i < n; i += blockDim.x)
+	const int m = retain_best_replay(keys, [](uint32_t k) { return static_cast<float>(k & 0xFFu); }, n, 2 * a.g.n_per_level[level], sc);
+	for (int i = tid; i < m; i += blockDim.x) cand[i] = keys[i];
+	if (tid == 0) a.surv_n[slot] = m;
+}
+
+// HarrisResponses (blockSize 7, k 0.04) of the keypoint at (x0, y0) of a w x h level
+__device__ __forceinline__ float harris_response(const uint8_t * img, int w, int h, int x0, int y0)
+{
+	int A = 0, B = 0, Cc = 0;
+	if (x0 >= 4 && x0 < w - 4 && y0 >= 4 && y0 < h - 4)
 	{
-		resp[i] = static_cast<float>(keys[i] & 0xFFu);
-		perm[i] = static_cast<uint16_t>(i);
-	}
-	__syncthreads();
-	const int n_level = a.g.n_per_level[level];
-	int m = retain_best_replay(perm, resp, n, 2 * n_level, sc);
-	// Harris responses of the kept candidates (HarrisResponses, blockSize 7, k 0.04)
-	for (int i = tid; i < m; i += blockDim.x)
-	{
-		const int pos = static_cast<int>(keys[perm[i]] >> 8);
-		const int x0 = pos % w, y0 = pos / w;
-		int A = 0, B = 0, Cc = 0;
-		if (x0 >= 4 && x0 < w - 4 && y0 >= 4 && y0 < h - 4)
-		{
-			// the 9x9 neighbourhood once into registers (81 loads instead of 8 per position of the 7x7 block)
-			int pt[9][9];
+		// the 9x9 neighbourhood once into registers (81 loads instead of 8 per position of the 7x7 block)
+		int pt[9][9];
 #pragma unroll
-			for (int r = 0; r < 9; ++r)
+		for (int r = 0; r < 9; ++r)
 #pragma unroll
-				for (int c = 0; c < 9; ++c) pt[r][c] = img[(y0 - 4 + r) * w + x0 - 4 + c];
+			for (int c = 0; c < 9; ++c) pt[r][c] = img[(y0 - 4 + r) * w + x0 - 4 + c];
 #pragma unroll
-			for (int r = 1; r <= 7; ++r)
+		for (int r = 1; r <= 7; ++r)
 #pragma unroll
-				for (int c = 1; c <= 7; ++c)
-				{
-					const int Ix = (pt[r][c + 1] - pt[r][c - 1]) * 2 + (pt[r - 1][c + 1] - pt[r - 1][c - 1]) + (pt[r + 1][c + 1] - pt[r + 1][c - 1]);
-					const int Iy = (pt[r + 1][c] - pt[r - 1][c]) * 2 + (pt[r + 1][c - 1] - pt[r - 1][c - 1]) + (pt[r + 1][c + 1] - pt[r - 1][c + 1]);
-					A += Ix * Ix;
-					B += Iy * Iy;
-					Cc += Ix * Iy;
-				}
-		}
-		else
-		for (int dy = -3; dy <= 3; ++dy)
-			for (int dx = -3; dx <= 3; ++dx)
+			for (int c = 1; c <= 7; ++c)
 			{
-				const int x = x0 + dx, y = y0 + dy;
-				const int xm = reflect101(x - 1, w), xp = reflect101(x + 1, w), ym = reflect101(y - 1, h), yp = reflect101(y + 1, h);
-				const int xc = reflect101(x, w), yc = reflect101(y, h);
-				const int p00 = img[ym * w + xm], p01 = img[ym * w + xc], p02 = img[ym * w + xp];
-				const int p10 = img[yc * w + xm], p12 = img[yc * w + xp];
-				const int p20 = img[yp * w + xm], p21 = img[yp * w + xc], p22 = img[yp * w + xp];
-				const int Ix = (p12 - p10) * 2 + (p02 - p00) + (p22 - p20);
-				const int Iy = (p21 - p01) * 2 + (p20 - p00) + (p22 - p02);
+				const int Ix = (pt[r][c + 1] - pt[r][c - 1]) * 2 + (pt[r - 1][c + 1] - pt[r - 1][c - 1]) + (pt[r + 1][c + 1] - pt[r + 1][c - 1]);
+				const int Iy = (pt[r + 1][c] - pt[r - 1][c]) * 2 + (pt[r + 1][c - 1] - pt[r - 1][c - 1]) + (pt[r + 1][c + 1] - pt[r - 1][c + 1]);
 				A += Ix * Ix;
 				B += Iy * Iy;
 				Cc += Ix * Iy;
 			}
-		const float scale = __fdiv_rn(1.f, __fmul_rn(static_cast<float>(4 * 7), 255.f));
-		const float s4 = __fmul_rn(__fmul_rn(__fmul_rn(scale, scale), scale), scale);
-		const float fa = static_cast<float>(A), fb = static_cast<float>(B), fc = static_cast<float>(Cc);
-		const float t3 = __fadd_rn(fa, fb);
-		resp[perm[i]] = __fmul_rn(__fsub_rn(__fsub_rn(__fmul_rn(fa, fb), __fmul_rn(fc, fc)), __fmul_rn(__fmul_rn(0.04f, t3), t3)), s4);
+	}
+	else
+	for (int dy = -3; dy <= 3; ++dy)
+		for (int dx = -3; dx <= 3; ++dx)
+		{
+			const int x = x0 + dx, y = y0 + dy;
+			const int xm = reflect101(x - 1, w), xp = reflect101(x + 1, w), ym = reflect101(y - 1, h), yp = reflect101(y + 1, h);
+			const int xc = reflect101(x, w), yc = reflect101(y, h);
+			const int p00 = img[ym * w + xm], p01 = img[ym * w + xc], p02 = img[ym * w + xp];
+			const int p10 = img[yc * w + xm], p12 = img[yc * w + xp];
+			const int p20 = img[yp * w + xm], p21 = img[yp * w + xc], p22 = img[yp * w + xp];
+			const int Ix = (p12 - p10) * 2 + (p02 - p00) + (p22 - p20);
+			const int Iy = (p21 - p01) * 2 + (p20 - p00) + (p22 - p02);
+			A += Ix * Ix;
+			B += Iy * Iy;
+			Cc += Ix * Iy;
+		}
+	const float scale = __fdiv_rn(1.f, __fmul_rn(static_cast<float>(4 * 7), 255.f));
+	const float s4 = __fmul_rn(__fmul_rn(__fmul_rn(scale, scale), scale), scale);
+	const float fa = static_cast<float>(A), fb = static_cast<float>(B), fc = static_cast<float>(Cc);
+	const float t3 = __fadd_rn(fa, fb);
+	return __fmul_rn(__fsub_rn(__fsub_rn(__fmul_rn(fa, fb), __fmul_rn(fc, fc)), __fmul_rn(__fmul_rn(0.04f, t3), t3)), s4);
+}
+
+// Harris response of every survivor of the level, one thread per survivor; grid (x, frame), the x blocks stride over the survivors.
+__global__ void __launch_bounds__(kOrbHarrisThreads)
+orb_harris_kernel(const OrbSelectArgs a)
+{
+	const int level = a.level, frame = blockIdx.y;
+	const int slot = frame * a.g.n_levels + level;
+	const int m = a.surv_n[slot];
+	const int w = a.g.w[level], h = a.g.h[level];
+	const uint8_t * img = a.gray + static_cast<size_t>(frame) * a.g.frame_stride + a.g.off[level];
+	const uint32_t * surv = a.cand + static_cast<size_t>(slot) * kOrbCandCap;
+	float * resp = rank_resp(a, slot);
+	for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x)
+	{
+		const int pos = static_cast<int>(surv[i] >> 8);
+		resp[i] = harris_response(img, w, h, pos % w, pos / w);
+	}
+}
+
+// retainBest(N) on the Harris responses of the survivors and, for a level that keeps more than Kp/MaxFeatures, the limitKeypoints cut;
+// writes the level's keypoints in order, their angle left to orb_angle_kernel.  The replay runs on a permutation of the survivors in
+// shared memory, or in the slot's global workspace when they are more than kOrbRankCap (ties at the FAST-score boundary): same steps.
+__global__ void __launch_bounds__(kOrbSelectThreads)
+orb_rank_kernel(const OrbSelectArgs a)
+{
+	__shared__ float s_resp[kOrbRankCap];
+	__shared__ uint16_t s_perm[kOrbRankCap], s_rpos[kOrbRankCap];
+	__shared__ int s_warp_tot[32], s_cut;
+	const int tid = threadIdx.x;
+	const int level = a.level, frame = blockIdx.x;
+	const int slot = frame * a.g.n_levels + level;
+	const int m = a.surv_n[slot];
+	float * const g_resp = rank_resp(a, slot);
+	uint16_t * const g_perm = reinterpret_cast<uint16_t *>(g_resp + kOrbCandCap);
+	const bool local = m <= kOrbRankCap;
+	float * const resp = local ? s_resp : g_resp;
+	uint16_t * const perm = local ? s_perm : g_perm;
+	const SelectScratch sc{local ? s_rpos : g_perm + kOrbCandCap, s_warp_tot, &s_cut};
+	for (int i = tid; i < m; i += blockDim.x)
+	{
+		if (local) s_resp[i] = g_resp[i];
+		perm[i] = static_cast<uint16_t>(i);
 	}
 	__syncthreads();
-	const int kept = retain_best_replay(perm, resp, m, n_level, sc);
+	const int kept = retain_best_replay(perm, [resp](uint16_t p) { return resp[p]; }, m, a.g.n_per_level[level], sc);
 	// retainBest keeps every keypoint tied with its boundary response.  A level that keeps more than Kp/MaxFeatures makes the frame's
 	// total exceed it, so the merge cuts the frame to its Kp/MaxFeatures strongest, and only the level's own strongest by the same key can
 	// be among them: those are stored, in retainBest's order, and level_n holds the full count so that the merge still cuts.
-	m = kept;
+	int k = kept;
 	if (kept > a.level_cap)
 	{
 		keep_strongest_replay(perm, resp, kept, a.level_cap, sc);
-		m = a.level_cap;
+		k = a.level_cap;
 	}
 	if (tid == 0) a.level_n[slot] = kept;
-	// IC angle + output: one warp per keypoint, lane = column of the circular patch, so that a row of the patch is one coalesced load and
-	// the 31 rows are independent loads in flight (a thread per keypoint walked ~700 dependent byte loads).  The moments are integer sums:
-	// any summation order gives the reference's value.
-	const int half = a.g.patch / 2;
+	const int w = a.g.w[level];
 	const float sf = static_cast<float>(1 << level);
-	const int lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
+	const uint32_t * surv = a.cand + static_cast<size_t>(slot) * kOrbCandCap;
+	for (int i = tid; i < k; i += blockDim.x)
+	{
+		const int p = perm[i];
+		const int pos = static_cast<int>(surv[p] >> 8);
+		OrbKeypoint kp;
+		kp.x = __fmul_rn(static_cast<float>(pos % w), sf);
+		kp.y = __fmul_rn(static_cast<float>(pos / w), sf);
+		kp.size = __fmul_rn(static_cast<float>(a.g.patch), sf);
+		kp.angle = 0.f;
+		kp.response = resp[p];
+		kp.octave = level;
+		a.level_kp[static_cast<size_t>(slot) * a.level_cap + i] = kp;
+	}
+}
+
+// IC angle of every keypoint of the level: one warp per keypoint, lane = column of the circular patch, so that a row of the patch is one
+// coalesced load and the 31 rows are independent loads in flight.  The moments are integer sums: any summation order gives the reference's
+// value.  Grid (x, frame), the x blocks stride over the frame's keypoints.
+__global__ void __launch_bounds__(kOrbAngleThreads)
+orb_angle_kernel(const OrbSelectArgs a)
+{
+	__shared__ int s_umax[20];
+	const int level = a.level, frame = blockIdx.y;
+	const int slot = frame * a.g.n_levels + level;
+	const int k = min(a.level_n[slot], a.level_cap);
+	const int half = a.g.patch / 2;
+	if (threadIdx.x == 0)
+	{
+		// umax table of the circular patch (ORB computeKeyPoints)
+		const int vmax = static_cast<int>(floorf(half * sqrtf(2.f) / 2 + 1));
+		const int vmin = static_cast<int>(ceilf(half * sqrtf(2.f) / 2));
+		for (int v = 0; v <= vmax; ++v) s_umax[v] = static_cast<int>(rint(sqrt(static_cast<double>(half) * half - static_cast<double>(v) * v)));
+		for (int v = half, v0 = 0; v >= vmin; --v)
+		{
+			while (s_umax[v0] == s_umax[v0 + 1]) ++v0;
+			s_umax[v] = v0;
+			++v0;
+		}
+	}
+	__syncthreads();
+	const int w = a.g.w[level], h = a.g.h[level];
+	const uint8_t * img = a.gray + static_cast<size_t>(frame) * a.g.frame_stride + a.g.off[level];
+	const float inv_sf = 1.f / static_cast<float>(1 << level); // exact: the keypoint's level coordinates come back exactly
+	const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
 	// rows of the circular patch that hold column u = lane - half: |v| <= vlim (umax is non-increasing in v); -1 = column outside the patch
 	const int u_lane = lane - half;
 	int vlim = -1;
 	if (u_lane <= half)
 		for (int v = 0; v <= half; ++v)
 			if ((v == 0 ? half : s_umax[v]) >= (u_lane < 0 ? -u_lane : u_lane)) vlim = v;
-	for (int i = warp; i < m; i += nwarps)
+	OrbKeypoint * kps = a.level_kp + static_cast<size_t>(slot) * a.level_cap;
+	for (int i = blockIdx.x * wpb + (threadIdx.x >> 5); i < k; i += gridDim.x * wpb)
 	{
-		const uint32_t key = keys[perm[i]];
-		const int pos = static_cast<int>(key >> 8);
-		const int x0 = pos % w, y0 = pos / w;
+		const int x0 = static_cast<int>(__fmul_rn(kps[i].x, inv_sf)), y0 = static_cast<int>(__fmul_rn(kps[i].y, inv_sf));
 		int m01 = 0, m10 = 0;
 		if (half <= 15 && x0 >= half && x0 < w - half && y0 >= half && y0 < h - half)
 		{
@@ -1112,17 +1193,7 @@ orb_select_kernel(const OrbSelectArgs a)
 		}
 		m10 = __reduce_add_sync(0xFFFFFFFFu, m10);
 		m01 = __reduce_add_sync(0xFFFFFFFFu, m01);
-		if (lane == 0)
-		{
-			OrbKeypoint kp;
-			kp.x = __fmul_rn(static_cast<float>(x0), sf);
-			kp.y = __fmul_rn(static_cast<float>(y0), sf);
-			kp.size = __fmul_rn(static_cast<float>(a.g.patch), sf);
-			kp.angle = fast_atan2_deg(static_cast<float>(m01), static_cast<float>(m10));
-			kp.response = resp[perm[i]];
-			kp.octave = level;
-			a.level_kp[static_cast<size_t>(slot) * a.level_cap + i] = kp;
-		}
+		if (lane == 0) kps[i].angle = fast_atan2_deg(static_cast<float>(m01), static_cast<float>(m10));
 	}
 }
 
@@ -1170,7 +1241,7 @@ orb_merge_kernel(const OrbKeypoint * __restrict__ level_kp, const int * __restri
 	const int frame = blockIdx.x, tid = threadIdx.x;
 	if (tid == 0)
 	{
-		// offsets of the stored keypoints; the cut below is decided on the levels' full counts (orb_select_kernel)
+		// offsets of the stored keypoints; the cut below is decided on the levels' full counts (orb_rank_kernel)
 		s_off[0] = 0;
 		s_kept = 0;
 		for (int l = 0; l < n_levels; ++l)
@@ -1259,7 +1330,7 @@ orb_blur_kernel(const uint8_t * __restrict__ gray_all, uint8_t * __restrict__ bl
 // passes keep a sliding window in registers: a thread produces 8 consecutive outputs of a row (14 bytes in, from 4 aligned words), then 8
 // consecutive outputs of a column (14 floats in) -- ~30 instead of ~200 instructions per pixel, same float operations in the same order.
 __global__ void __launch_bounds__(256)
-orb_blur_tma_kernel(const __grid_constant__ OrbTensorMap tmap, uint8_t * __restrict__ blur_all, const OrbGeom g, int level)
+orb_blur_tma_kernel(const __grid_constant__ OrbTensorMap tmap, uint8_t * __restrict__ blur_all, const __grid_constant__ OrbGeom g, int level)
 {
 	constexpr int GW = kFastTmaGW, GH = kFastTmaGH, TW = kFastTmaTW, TH = kFastTmaTH;
 	constexpr int RH = TH + 6; // rows of the row pass: y0 - 3 .. y0 + TH + 2
@@ -1431,7 +1502,7 @@ orb_describe_kernel(const uint8_t * __restrict__ gray_all, const uint8_t * __res
 constexpr int kOrbPatchR = 19, kOrbPatchPitch = 48;
 
 __global__ void __launch_bounds__(256)
-orb_describe_patch_kernel(const uint8_t * __restrict__ blur_all, const OrbGeom g, const OrbKeypoint * __restrict__ kps, const int * __restrict__ n_kp,
+orb_describe_patch_kernel(const uint8_t * __restrict__ blur_all, const __grid_constant__ OrbGeom g, const OrbKeypoint * __restrict__ kps, const int * __restrict__ n_kp,
                           int cap, uint8_t * __restrict__ desc)
 {
 	__shared__ float4 s_pat[256];
