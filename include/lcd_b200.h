@@ -406,7 +406,8 @@ int lcd_localize_similarity_batch_dev(lcd_engine * e, const void * d_queries, in
 /* ---- geometric verification: Memory::computeTransform ----------------------------------
  * Batched verification of n_pairs (FROM = old signature with 3-D points, TO = new signature with
  * 2-D keypoints) hypotheses.  Buffers are [n_pairs][cap] row-major; n_from/n_to give the valid
- * rows of each pair.  Single camera, identity local transform, rectified (no distortion). */
+ * rows of each pair.  Single camera, identity local transform, rectified (no distortion); the decision calls of localisation clients
+ * take each client's own camera instead (lcd_clients_set_cameras). */
 typedef struct lcd_verify_params {
 	float nndr;            /* Vis/CorNNDR (0.8)                                             */
 	int min_inliers;       /* Vis/MinInliers (20)                                           */
@@ -607,8 +608,30 @@ int lcd_verify_top_dev(lcd_engine * e, const void * d_queries, const float * d_u
  * (Rtabmap.cpp:467, :1094) for n_clients clients at once; calling it again resets every client.  LCD_ERR_CAPACITY when the device
  * cannot hold the state. */
 int lcd_clients_create(lcd_engine * e, int n_clients);
-/* BayesFilter::reset + _highestHypothesis = (0, 0) of the listed clients */
+/* BayesFilter::reset + _highestHypothesis = (0, 0) of the listed clients; their cameras stay */
 int lcd_clients_reset(lcd_engine * e, const int * clients, int n);
+
+/* A client's camera: SensorData::cameraModels()[0] of the frames it sends (rectified, depth registered to the image). */
+typedef struct lcd_camera {
+	double fx, fy, cx, cy;          /* CameraModel::K(); fx, fy > 0; cx, cy read as lcd_orb_params / lcd_verify_params read them */
+	int image_width, image_height;  /* CameraModel::imageSize(): 0 x 0 = not set, otherwise the image size of the calls that decide it */
+	float local_transform[12];      /* CameraModel::localTransform(), 3x4 row-major rtabmap::Transform (base -> optical frame) */
+} lcd_camera;
+/* Sets the cameras of the listed clients (cams NULL: the listed clients go back to the parameters of each call).  For the frames of a
+ * client with a camera, the decision calls (lcd_decide_batch_dev, lcd_decide_gps_batch_dev, lcd_process_decide_batch_dev,
+ * lcd_process_frames_decide_*) take the camera as the call is made, and lcd_decide_proximity_dev and lcd_verify_decided_dev use that
+ * snapshot; a submitted batch keeps the cameras it was submitted with.  Such a frame is lifted with the camera's fx..cy (as floats, as
+ * projectDepthTo3D receives them) and its local transform (util3d::transformPoint, applied when it is not identity, util3d_features.cpp:
+ * 110-114) in lcd_process_frames_decide_*, and every registration of its decision uses the camera's K and image size in place of
+ * lcd_verify_params': transform = (localTransform * pnp)^-1, the covariance with transformCameraFrame = transform * localTransform
+ * (util3d_motion_estimation.cpp:154-258), and RGBD/MaxLoopClosureDistance and the proximity radius read that base-frame transform.
+ * Frames of clients without a camera are computed exactly as before.  LCD_ERR_STATE without clients; LCD_ERR_INVALID, changing nothing,
+ * for a client out of range, a value that is not finite, fx or fy <= 0, a negative image size or only one side set, and a rotation that
+ * is not orthonormal within 1e-5 (transforms are inverted as [R^T | -R^T t]).  lcd_process_frames_decide_* refuse (LCD_ERR_INVALID,
+ * before any state changes) a camera whose image size is set and differs from the images'.  A registration with a client camera of
+ * image size 0 x 0 has no Reg/RepeatOnce pass and takes the covariance from the reprojection RMS when the TO side has no 3-D points.
+ * Not read by lcd_process_frames*, lcd_process_batch*, lcd_verify_batch, the sharded step or mapping mode. */
+int lcd_clients_set_cameras(lcd_engine * e, const int * clients, int n, const lcd_camera * cams);
 /* The working memory the clients localise against: ids[n] ascending, ids[0] the virtual place (a negative id: Memory keeps it in the
  * working memory, Memory.cpp:592), and the neighbour tables, Bayes/PredictionLC and Bayes/VirtualPlacePriorThr exactly as
  * lcd_bayes_compute_posterior takes them (same checks).  The prediction's columns are computed here, once per map, bit-equal to

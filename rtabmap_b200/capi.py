@@ -117,6 +117,35 @@ class DecideParams(C.Structure):
     ]
 
 
+class Camera(C.Structure):
+    """lcd_camera: a localisation client's CameraModel (K, image size, local transform base -> optical, 3x4 row-major)."""
+    _fields_ = [
+        ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
+        ("image_width", C.c_int), ("image_height", C.c_int), ("local_transform", C.c_float * 12),
+    ]
+
+
+# CameraModel::opticalRotation() (CameraModel.h): x right, y down, z forward in a base frame of x forward, y left, z up
+OPTICAL_ROTATION = np.array([[0, 0, 1, 0], [-1, 0, 0, 0], [0, -1, 0, 0]], np.float32)
+
+
+def camera_model(K4, image_size=(0, 0), local_transform=None, optical: bool = False) -> Camera:
+    """The lcd_camera of rtabmap::CameraModel(fx, fy, cx, cy, localTransform, 0, imageSize).  local_transform: 3x4 (or 4x4) base ->
+    camera, identity when None; optical=True appends the optical rotation (localTransform * opticalRotation(), the local transform
+    RTAB-Map's sensors report for a camera whose own frame is x forward, y left, z up), multiplied in float32."""
+    fx, fy, cx, cy = (float(v) for v in K4)
+    L = np.eye(4, dtype=np.float32)
+    if local_transform is not None:
+        L[:3] = np.asarray(local_transform, np.float32).reshape(-1, 4)[:3]
+    if optical:
+        O = np.eye(4, dtype=np.float32)
+        O[:3] = OPTICAL_ROTATION
+        L = (L @ O).astype(np.float32)
+    c = Camera(fx, fy, cx, cy, int(image_size[0]), int(image_size[1]))
+    c.local_transform[:] = [float(v) for v in L[:3].reshape(-1)]
+    return c
+
+
 class EpipolarParams(C.Structure):
     """lcd_epipolar_params (VhEp/MatchCountMin, VhEp/RansacParam1, VhEp/RansacParam2)."""
     _fields_ = [("match_count_min", C.c_int), ("ransac_param1", C.c_double), ("ransac_param2", C.c_double)]
@@ -279,6 +308,7 @@ SIGNATURES = {
     "lcd_verify_top_dev": (_I, [_P, _P, _P, _I, _I, _P, _P, _I, _P, _P]),
     "lcd_clients_create": (_I, [_P, _I]),
     "lcd_clients_reset": (_I, [_P, _P, _I]),
+    "lcd_clients_set_cameras": (_I, [_P, _P, _I, _P]),
     "lcd_clients_set_map": (_I, [_P, _P, _I, _P, _P, _P, _P, _I, _F]),
     "lcd_decide_batch_dev": (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _P]),
     "lcd_decide_fetch": (_I, [_P, _I, _P]),
@@ -1053,6 +1083,17 @@ class Engine:
         """BayesFilter::reset and last highest hypothesis (0, 0) for the listed clients."""
         c = _i32(clients)
         self._check(self._lib.lcd_clients_reset(self._h, _ptr(c), len(c)))
+
+    def clients_set_cameras(self, clients, cams):
+        """Each listed client's own camera (a sequence of Camera, see camera_model), taken by the decision calls for its frames; cams None:
+        the listed clients go back to each call's lcd_orb_params / lcd_verify_params."""
+        c = _i32(clients)
+        arr = None
+        if cams is not None:
+            if len(cams) != len(c):
+                raise LcdError(-1, f"{len(c)} clients but {len(cams)} cameras")
+            arr = (Camera * max(len(c), 1))(*cams)
+        self._check(self._lib.lcd_clients_set_cameras(self._h, _ptr(c), len(c), arr))
 
     def clients_set_map(self, ids, col_ptr, nbr_row, nbr_level, prediction_lc, virtual_place_prior: float = 0.9):
         """The map every client localises against: ids ascending with ids[0] the virtual place, neighbour tables and Bayes/PredictionLC as

@@ -64,4 +64,46 @@ __device__ __forceinline__ void bulk_g2s(void * smem_dst, const void * gmem_src,
 		: "memory");
 }
 
+// A localisation client's camera as one decision call took it (lcd_clients_set_cameras), one record per frame of the call.  A frame
+// whose client has no camera has set = 0 and is computed with the call's parameters.
+struct FrameCam
+{
+	double fx, fy, cx, cy; // CameraModel::K()
+	float L[12];           // CameraModel::localTransform(), 3x4 row-major
+	int w, h;              // CameraModel::imageSize() (0 x 0 = not set)
+	int set;               // 1: the client has a camera
+	int local;             // 1: L is not identity (Transform::isIdentity, Transform.cpp:156-170)
+};
+static_assert(sizeof(FrameCam) == 96, "FrameCam is staged as 12 64-bit words per frame");
+
+// util3d::transformPoint (util3d_transforms.cpp:211-220): float, r0 x + r1 y + r2 z + t, left to right, each operation rounded on its own
+__device__ __forceinline__ void transform_point_f(const float * T, float x, float y, float z, float & ox, float & oy, float & oz)
+{
+	ox = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[0], x), __fmul_rn(T[1], y)), __fmul_rn(T[2], z)), T[3]);
+	oy = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[4], x), __fmul_rn(T[5], y)), __fmul_rn(T[6], z)), T[7]);
+	oz = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[8], x), __fmul_rn(T[9], y)), __fmul_rn(T[10], z)), T[11]);
+}
+
+// rtabmap::Transform A * B of two 3x4 float transforms (Eigen's 4x4 product, the implicit last row 0 0 0 1), left to right
+__device__ __forceinline__ void transform_mul_f(const float * A, const float * B, float * out)
+{
+	for (int i = 0; i < 3; ++i)
+		for (int j = 0; j < 4; ++j)
+		{
+			float v = __fadd_rn(__fadd_rn(__fmul_rn(A[4 * i], B[j]), __fmul_rn(A[4 * i + 1], B[4 + j])), __fmul_rn(A[4 * i + 2], B[8 + j]));
+			if (j == 3) v = __fadd_rn(v, A[4 * i + 3]);
+			out[4 * i + j] = v;
+		}
+}
+
+// the inverse of a rigid 3x4 float transform as [R^T | -R^T t]
+__device__ __forceinline__ void transform_inv_f(const float * A, float * out)
+{
+	for (int i = 0; i < 3; ++i)
+	{
+		for (int j = 0; j < 3; ++j) out[4 * i + j] = A[4 * j + i];
+		out[4 * i + 3] = -__fadd_rn(__fadd_rn(__fmul_rn(A[i], A[3]), __fmul_rn(A[4 + i], A[7])), __fmul_rn(A[8 + i], A[11]));
+	}
+}
+
 } // namespace lcd

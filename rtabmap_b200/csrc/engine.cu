@@ -454,6 +454,9 @@ struct lcd_engine
 	bool dc_hyp_valid = false;            // d_hyp_id / d_hyp_slot hold the last decision's accepted hypotheses
 	float dc_max_dist = 0.f;              // RGBD/MaxLoopClosureDistance of the last decision
 	std::vector<int> dc_h_ids;            // the current map's ids (host copy)
+	std::vector<FrameCam> dc_cams;        // [client] each client's camera (lcd_clients_set_cameras; set = 0: none)
+	const FrameCam * dc_frame_cam = nullptr; // [frame] the last decision's snapshot of its frames' cameras in dc_tab, nullptr when none had one
+	bool dc_cam_sized = false;            // a camera of that snapshot has an image size
 	// proximity detection by space (lcd_clients_set_map_poses / lcd_decide_proximity_dev, proximity.cuh)
 	struct MapPoses
 	{
@@ -2526,9 +2529,9 @@ static int load_gauss7(lcd_engine * e, cudaStream_t s)
 	return LCD_OK;
 }
 
-// 3-D points and plain coordinates of the detected keypoints
+// 3-D points and plain coordinates of the detected keypoints; d_cam[n_frames] (may be null) the frames' client cameras
 static int orb_lift(lcd_engine * e, int n_frames, int width, int height, const void * d_depth, int depth_type, const lcd_orb_params * p, int cap,
-                    const OrbKeypoint * d_kp, const int * d_n, float * d_xyz, float * d_uv, cudaStream_t s)
+                    const OrbKeypoint * d_kp, const int * d_n, float * d_xyz, float * d_uv, cudaStream_t s, const FrameCam * d_cam)
 {
 	if (d_xyz)
 	{
@@ -2543,6 +2546,7 @@ static int orb_lift(lcd_engine * e, int n_frames, int width, int height, const v
 		a.cy = p->cy;
 		a.min_depth = p->min_depth;
 		a.max_depth = p->max_depth;
+		a.cam = d_cam;
 		a.kps = d_kp;
 		a.n_kp = d_n;
 		a.cap = cap;
@@ -2914,7 +2918,8 @@ static int octree_geometry(lcd_engine * e, int width, int height, const lcd_orb_
 // ORB-OCTREE (lcd_detector_set_orb_octree, Kp/DetectorStrategy=10): gray + mask, pyramid, FAST per cell, quadtree per level, angle, blur,
 // descriptors, then the mask and Kp/MaxFeatures of rtabmap::ORBOctree, and the 3-D points
 static int octree_run(lcd_engine * e, int n_frames, const uint8_t * d_images, int width, int height, int channels, const void * d_depth, int depth_type,
-                      const lcd_orb_params * p, int cap, OrbKeypoint * d_kp, uint8_t * d_desc, float * d_xyz, float * d_uv, int * d_n, cudaStream_t s)
+                      const lcd_orb_params * p, int cap, OrbKeypoint * d_kp, uint8_t * d_desc, float * d_xyz, float * d_uv, int * d_n, cudaStream_t s,
+                      const FrameCam * d_cam)
 {
 	OctGeom g{};
 	std::vector<OctCell> cells;
@@ -3034,20 +3039,21 @@ static int octree_run(lcd_engine * e, int n_frames, const uint8_t * d_images, in
 		                                                                               use_mask ? e->o_mask.p : nullptr, p->n_features, d_kp, d_desc, d_n, cap);
 		LCD_CHECK_LAUNCH(e);
 	}
-	LCD_TRY(orb_lift(e, n_frames, width, height, d_depth, depth_type, p, cap, d_kp, d_n, d_xyz, d_uv, s));
+	LCD_TRY(orb_lift(e, n_frames, width, height, d_depth, depth_type, p, cap, d_kp, d_n, d_xyz, d_uv, s, d_cam));
 	prof_mark(e, LCD_PROF_ORB, s);
 	return LCD_OK;
 }
 
 // Detect + describe a batch of frames with the engine's detector (lcd_detector_set): the FAST pyramid or GFTT's corners between the
 // shared preparation and the steered BRIEF descriptors and 3-D points.  A null d_kp / d_n detects into the engine's own buffers.
+// d_cam[n_frames] (may be null): the frames' client cameras the 3-D points are lifted with.
 static int orb_run(lcd_engine * e, int n_frames, const uint8_t * d_images, int width, int height, int channels, const void * d_depth,
                    int depth_type, const lcd_orb_params * p, int cap, OrbKeypoint * d_kp, uint8_t * d_desc, float * d_xyz, float * d_uv,
-                   int * d_n, cudaStream_t s)
+                   int * d_n, cudaStream_t s, const FrameCam * d_cam = nullptr)
 {
 	if (!p) LCD_FAIL(e, LCD_ERR_INVALID, "null ORB parameters");
 	if (e->detector == LCD_DETECTOR_ORB_OCTREE)
-		return octree_run(e, n_frames, d_images, width, height, channels, d_depth, depth_type, p, cap, d_kp, d_desc, d_xyz, d_uv, d_n, s);
+		return octree_run(e, n_frames, d_images, width, height, channels, d_depth, depth_type, p, cap, d_kp, d_desc, d_xyz, d_uv, d_n, s, d_cam);
 	const bool gftt = e->detector == LCD_DETECTOR_GFTT_ORB;
 	lcd_orb_params pl = *p;
 	if (gftt) pl.n_levels = 1; // cv::ORB::compute builds the levels its keypoints use: GFTT corners are all octave 0
@@ -3107,7 +3113,7 @@ static int orb_run(lcd_engine * e, int n_frames, const uint8_t * d_images, int w
 			orb_describe_kernel<<<grd, 256, 0, s>>>(e->o_gray.p, e->o_blur.p, g, d_kp, d_n, cap, d_desc);
 		LCD_CHECK_LAUNCH(e);
 	}
-	LCD_TRY(orb_lift(e, n_frames, width, height, d_depth, depth_type, p, cap, d_kp, d_n, d_xyz, d_uv, s));
+	LCD_TRY(orb_lift(e, n_frames, width, height, d_depth, depth_type, p, cap, d_kp, d_n, d_xyz, d_uv, s, d_cam));
 	prof_mark(e, LCD_PROF_ORB, s);
 	return LCD_OK;
 }
@@ -3538,9 +3544,9 @@ static int launch_match(lcd_engine * e, const PairSource & src, int n_pairs, int
 	return LCD_OK;
 }
 
-// obj_to: words3B of each correspondence (launch_match's v_obj_to) or nullptr
+// obj_to: words3B of each correspondence (launch_match's v_obj_to) or nullptr; src (may be null): the pairs' TO cameras (src->to.cam)
 static int launch_pnp(lcd_engine * e, int n_pairs, int cap, const lcd_verify_params * p, const float * obj_to, cudaStream_t s,
-                      bool gate_min_matches = true, bool want_cov = true)
+                      bool gate_min_matches = true, bool want_cov = true, const PairSource * src = nullptr)
 {
 	const size_t rows = static_cast<size_t>(n_pairs) * cap;
 	if (want_cov && p->var_median_ratio <= 1) LCD_FAIL(e, LCD_ERR_INVALID, "Vis/PnPVarianceMedianRatio must be > 1 (UASSERT in estimateMotion3DTo2D)");
@@ -3571,6 +3577,8 @@ static int launch_pnp(lcd_engine * e, int n_pairs, int cap, const lcd_verify_par
 	a.split_linear = p->split_linear_cov;
 	a.img_w = p->image_width;
 	a.img_h = p->image_height;
+	a.cam_tab = src ? src->to.cam : nullptr;
+	a.cam_row = src ? src->to.row : nullptr;
 	a.cov6 = want_cov ? e->v_cov6.p : nullptr;
 	a.rvec = e->v_rvec.p;
 	a.tvec = e->v_tvec.p;
@@ -3592,9 +3600,11 @@ static int launch_pnp(lcd_engine * e, int n_pairs, int cap, const lcd_verify_par
 
 // Reg/RepeatOnce: the second registration pass of the pairs whose first pass succeeded (guess_match_kernel), then PnP again on all pairs
 // (pairs that keep their first-pass correspondences reproduce their first-pass result).  src and obj_to: those of the first pass.
-static int launch_second_pass(lcd_engine * e, const PairSource & src, int n_pairs, int cap, const lcd_verify_params * p, float * obj_to, cudaStream_t s)
+// cam_sized: a pair's own TO camera (src.to.cam) has an image size; the pass needs one, the call's or the pair's.
+static int launch_second_pass(lcd_engine * e, const PairSource & src, int n_pairs, int cap, const lcd_verify_params * p, float * obj_to, cudaStream_t s,
+                              bool cam_sized)
 {
-	if (!p->repeat_once || p->guess_win_size <= 0 || p->image_width <= 0 || p->image_height <= 0) return LCD_OK;
+	if (!p->repeat_once || p->guess_win_size <= 0 || ((p->image_width <= 0 || p->image_height <= 0) && !cam_sized)) return LCD_OK;
 	GuessMatchArgs a{};
 	a.src = src;
 	a.cap = cap;
@@ -3636,17 +3646,19 @@ static int launch_second_pass(lcd_engine * e, const PairSource & src, int n_pair
 	}
 #undef LCD_GUESS_CASE
 	LCD_CHECK_LAUNCH(e);
-	return launch_pnp(e, n_pairs, cap, p, obj_to, s);
+	return launch_pnp(e, n_pairs, cap, p, obj_to, s, true, true, &src);
 }
 
 // Memory::computeTransform of every pair: global matching, PnP, then the Reg/RepeatOnce pass.  cap: stride of the outputs, at least
-// both row strides of src.  The covariance takes words3B from src.to.xyz when it is set.
-static int register_pairs(lcd_engine * e, const PairSource & src, int n_pairs, int cap, const lcd_verify_params * vp, cudaStream_t s)
+// both row strides of src.  The covariance takes words3B from src.to.xyz when it is set.  A pair whose TO row has a camera in src.to.cam
+// registers with it; cam_sized: one of those cameras has an image size.
+static int register_pairs(lcd_engine * e, const PairSource & src, int n_pairs, int cap, const lcd_verify_params * vp, cudaStream_t s,
+                          bool cam_sized = false)
 {
 	LCD_TRY(launch_match(e, src, n_pairs, cap, vp->nndr, false, s));
 	float * obj_to = src.to.xyz ? e->v_obj_to.p : nullptr;
-	LCD_TRY(launch_pnp(e, n_pairs, cap, vp, obj_to, s));
-	return launch_second_pass(e, src, n_pairs, cap, vp, obj_to, s);
+	LCD_TRY(launch_pnp(e, n_pairs, cap, vp, obj_to, s, true, true, &src));
+	return launch_second_pass(e, src, n_pairs, cap, vp, obj_to, s, cam_sized);
 }
 
 static int check_verify_params(lcd_engine * e, const lcd_verify_params * vp, bool need_store)
@@ -4601,9 +4613,56 @@ int lcd_clients_create(lcd_engine * e, int n_clients)
 	LCD_CUDA(e, cudaMemsetAsync(e->dc_key_ids.p, 0, n * sizeof(long long), s));
 	LCD_CUDA(e, cudaStreamSynchronize(s));
 	e->dc_clients = n_clients;
+	e->dc_cams.assign(n, FrameCam{});
 	e->dc_last_frames = 0;
 	e->dc_hyp_valid = false;
 	return prune_map_versions(e);
+}
+
+int lcd_clients_set_cameras(lcd_engine * e, const int * clients, int n, const lcd_camera * cams)
+{
+	if (!e) return LCD_ERR_INVALID;
+	if (e->dc_clients <= 0) LCD_FAIL(e, LCD_ERR_STATE, "no clients: call lcd_clients_create first");
+	if (n <= 0) return LCD_OK;
+	if (!clients) LCD_FAIL(e, LCD_ERR_INVALID, "null client list");
+	std::vector<FrameCam> rec(n, FrameCam{});
+	for (int i = 0; i < n; ++i)
+	{
+		if (clients[i] < 0 || clients[i] >= e->dc_clients) LCD_FAIL(e, LCD_ERR_INVALID, "client %d is out of range [0, %d)", clients[i], e->dc_clients);
+		if (!cams) continue;
+		const lcd_camera & c = cams[i];
+		bool finite = std::isfinite(c.fx) && std::isfinite(c.fy) && std::isfinite(c.cx) && std::isfinite(c.cy);
+		for (int k = 0; k < 12; ++k) finite = finite && std::isfinite(c.local_transform[k]);
+		if (!finite) LCD_FAIL(e, LCD_ERR_INVALID, "the camera of client %d has a value that is not finite", clients[i]);
+		if (!(c.fx > 0.0) || !(c.fy > 0.0)) LCD_FAIL(e, LCD_ERR_INVALID, "the camera of client %d needs fx, fy > 0", clients[i]);
+		if (c.image_width < 0 || c.image_height < 0 || (c.image_width == 0) != (c.image_height == 0))
+			LCD_FAIL(e, LCD_ERR_INVALID, "the image size of client %d must be 0 x 0 or positive", clients[i]);
+		// the engine inverts transforms as [R^T | -R^T t]: R R^T must be the identity
+		const float * L = c.local_transform;
+		for (int r = 0; r < 3; ++r)
+			for (int q = 0; q < 3; ++q)
+			{
+				const double d = static_cast<double>(L[4 * r]) * L[4 * q] + static_cast<double>(L[4 * r + 1]) * L[4 * q + 1] +
+				                 static_cast<double>(L[4 * r + 2]) * L[4 * q + 2];
+				if (std::fabs(d - (r == q ? 1.0 : 0.0)) > 1e-5)
+					LCD_FAIL(e, LCD_ERR_INVALID, "the local transform of client %d is not a rotation within 1e-5", clients[i]);
+			}
+		FrameCam & f = rec[i];
+		f.fx = c.fx;
+		f.fy = c.fy;
+		f.cx = c.cx;
+		f.cy = c.cy;
+		std::memcpy(f.L, L, sizeof(f.L));
+		f.w = c.image_width;
+		f.h = c.image_height;
+		f.set = 1;
+		// Transform::isIdentity compares the values (-0 is 0)
+		static const float kIdentity[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
+		for (int k = 0; k < 12; ++k) f.local |= L[k] != kIdentity[k] ? 1 : 0;
+	}
+	// checked as a whole: a refused call changes nothing
+	for (int i = 0; i < n; ++i) e->dc_cams[clients[i]] = rec[i];
+	return LCD_OK;
 }
 
 int lcd_clients_reset(lcd_engine * e, const int * clients, int n)
@@ -4760,9 +4819,11 @@ static int check_decide_params(lcd_engine * e, const lcd_decide_params * dp)
 }
 
 // checks of one decision call and the upload of its frame tables (before any kernel of the call is queued); gps[n_frames] (may be null)
-// is uploaded behind them.  stage: pinned staging the caller owns and knows to be free (null: the engine's, once its last upload is done)
+// is uploaded behind them, then the snapshot of the frames' cameras when a frame's client has one.  stage: pinned staging the caller owns
+// and knows to be free (null: the engine's, once its last upload is done).  width x height: the call's image size (0 x 0: no images),
+// which a camera's image size must match when it is set.
 static int decide_prepare(lcd_engine * e, int n_frames, int ns, const int * clients, const int * frame_flags, const lcd_decide_params * dp,
-                          cudaStream_t s, const GpsFrame * gps = nullptr, PinBuf<long long> * stage = nullptr)
+                          cudaStream_t s, const GpsFrame * gps = nullptr, PinBuf<long long> * stage = nullptr, int width = 0, int height = 0)
 {
 	if (e->dc_clients <= 0) LCD_FAIL(e, LCD_ERR_STATE, "no clients: call lcd_clients_create first");
 	if (e->dc_map_ver < 0) LCD_FAIL(e, LCD_ERR_STATE, "no map: call lcd_clients_set_map first");
@@ -4779,10 +4840,21 @@ static int decide_prepare(lcd_engine * e, int n_frames, int ns, const int * clie
 		seen[c] = 1;
 		if (!(frame_flags[f] & (kDcFlagSkip | kDcFlagHold))) e->dc_active.push_back(f);
 	}
+	bool any_cam = false, cam_sized = false;
+	for (int f = 0; f < n_frames; ++f)
+	{
+		const FrameCam & c = e->dc_cams[clients[f]];
+		if (!c.set) continue;
+		any_cam = true;
+		cam_sized = cam_sized || c.w > 0;
+		if (width > 0 && c.w > 0 && (c.w != width || c.h != height))
+			LCD_FAIL(e, LCD_ERR_INVALID, "the camera of client %d is %d x %d, the images of the call %d x %d", clients[f], c.w, c.h, width, height);
+	}
 	const int B = static_cast<int>(e->dc_active.size());
 	static_assert(sizeof(GpsFrame) % sizeof(long long) == 0, "GPS frame table layout");
 	const size_t gps_words = gps ? n_frames * (sizeof(GpsFrame) / sizeof(long long)) : 0;
-	const size_t words = 2 * static_cast<size_t>(n_frames) + 2 * static_cast<size_t>(B) + gps_words;
+	const size_t cam0 = 2 * static_cast<size_t>(n_frames) + 2 * static_cast<size_t>(B) + gps_words;
+	const size_t words = cam0 + (any_cam ? n_frames * (sizeof(FrameCam) / sizeof(long long)) : 0);
 	if (!stage)
 	{
 		if (!e->dc_h_ev) LCD_CUDA(e, cudaEventCreateWithFlags(&e->dc_h_ev, cudaEventDisableTiming));
@@ -4804,9 +4876,14 @@ static int decide_prepare(lcd_engine * e, int n_frames, int ns, const int * clie
 		hb[B + b] = clients[f];
 	}
 	if (gps) std::memcpy(hb + 2 * B, gps, n_frames * sizeof(GpsFrame));
+	FrameCam * hc = reinterpret_cast<FrameCam *>(h + cam0);
+	if (any_cam)
+		for (int f = 0; f < n_frames; ++f) hc[f] = e->dc_cams[clients[f]];
 	LCD_CUDA(e, e->dc_tab.reserve(words, 0, false, s));
 	LCD_CUDA(e, cudaMemcpyAsync(e->dc_tab.p, h, words * sizeof(long long), cudaMemcpyHostToDevice, s));
 	if (stage == &e->dc_h_tab) LCD_CUDA(e, cudaEventRecord(e->dc_h_ev, s));
+	e->dc_frame_cam = any_cam ? reinterpret_cast<const FrameCam *>(e->dc_tab.p + cam0) : nullptr;
+	e->dc_cam_sized = cam_sized;
 	return LCD_OK;
 }
 
@@ -5090,8 +5167,9 @@ static int verify_decided(lcd_engine * e, const uint32_t * d_q, const float * d_
 	LCD_TRY(check_verify_params(e, vp, true));
 	if (e->dc_last_frames == 0 || !e->dc_hyp_valid) LCD_FAIL(e, LCD_ERR_STATE, "no decision to verify: run lcd_decide_batch_dev first");
 	if (n_frames != e->dc_last_frames) LCD_FAIL(e, LCD_ERR_INVALID, "the last decision has %d frames, not %d", e->dc_last_frames, n_frames);
-	const PairSource src{{e->st_desc.p, e->st_xyz.p, e->st_n.p, e->d_hyp_slot.p, e->st_cap}, {d_q, d_uv, d_xyz_to, d_nq_frame, nq, nq, nullptr}};
-	LCD_TRY(register_pairs(e, src, n_frames, std::max(e->st_cap, nq), vp, s));
+	const PairSource src{{e->st_desc.p, e->st_xyz.p, e->st_n.p, e->d_hyp_slot.p, e->st_cap},
+	                     {d_q, d_uv, d_xyz_to, d_nq_frame, nq, nq, nullptr, e->dc_frame_cam}};
+	LCD_TRY(register_pairs(e, src, n_frames, std::max(e->st_cap, nq), vp, s, e->dc_cam_sized));
 	decide_verified_kernel<<<(n_frames + 127) / 128, 128, 0, s>>>(n_frames, e->v_ok.p, e->v_T.p, e->dc_max_dist, e->dc_dec.p, e->d_hyp_id.p,
 	                                                             e->px_valid ? e->px_skip.p : nullptr);
 	LCD_CHECK_LAUNCH(e);
@@ -5272,8 +5350,9 @@ static int proximity_decide(lcd_engine * e, const uint32_t * d_q, const float * 
 	// Memory::computeTransform(place, frame) of every attempted pair in one launch, with a null guess (RGBD/ProximityOdomGuess = false):
 	// FROM = the store row px_slot[i] (-1: none) with its cached dictionary, TO = row px_row[i] of the frames' descriptors, px_nto[i] of
 	// them (0: the pair is not registered)
-	const PairSource src{{e->st_desc.p, e->st_xyz.p, e->st_n.p, e->px_slot.p, e->st_cap}, {d_q, d_uv, d_xyz_to, e->px_nto.p, 0, nq_per_frame, e->px_row.p}};
-	LCD_TRY(register_pairs(e, src, n_pairs, std::max(e->st_cap, nq_per_frame), vp, s));
+	const PairSource src{{e->st_desc.p, e->st_xyz.p, e->st_n.p, e->px_slot.p, e->st_cap},
+	                     {d_q, d_uv, d_xyz_to, e->px_nto.p, 0, nq_per_frame, e->px_row.p, e->dc_frame_cam}};
+	LCD_TRY(register_pairs(e, src, n_pairs, std::max(e->st_cap, nq_per_frame), vp, s, e->dc_cam_sized));
 	LCD_TRY(pack_verify_results(e, n_pairs, e->px_res.p, s));
 	proximity_apply_kernel<<<(n_frames + 127) / 128, 128, 0, s>>>(n_frames, mp, fr, e->v_ok.p, e->v_T.p, e->px_rec.p, e->dc_dec.p, e->d_hyp_id.p,
 	                                                             e->d_hyp_slot.p, e->px_skip.p);
@@ -5369,7 +5448,7 @@ static int frames_decide_dev(lcd_engine * e, int n_frames, const uint8_t * d_ima
 	const int cap = op->n_features;
 	LCD_TRY(frame_front_end(e, n_frames, cap, e->o_kp, e->o_desc, e->o_xyz, &e->o_uv, e->o_n, s));
 	LCD_TRY(orb_run(e, n_frames, d_images, width, height, channels, d_depth, depth_type, op, cap, e->o_kp.p, e->o_desc.p, e->o_xyz.p, e->o_uv.p,
-	                e->o_n.p, s));
+	                e->o_n.p, s, e->dc_frame_cam));
 	const uint32_t * d_q = reinterpret_cast<const uint32_t *>(e->o_desc.p);
 	const int * d_sig_ids = e->dc_versions.at(e->dc_map_ver)->ids.p + 1; // the map's real places, ascending
 	const int * d_qn = e->o_n.p;                                         // quantised words of each frame: Signature::isBadSignature
@@ -5404,7 +5483,7 @@ int lcd_process_frames_decide_dev(lcd_engine * e, int n_frames, const uint8_t * 
 	std::vector<GpsFrame> g;
 	LCD_TRY(frames_decide_check(e, "lcd_process_frames_decide_dev", n_frames, op, n_total, vp, frame_flags, stages, g));
 	cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : e->stream;
-	LCD_TRY(decide_prepare(e, n_frames, ns, clients, frame_flags, dp, s, g.empty() ? nullptr : g.data()));
+	LCD_TRY(decide_prepare(e, n_frames, ns, clients, frame_flags, dp, s, g.empty() ? nullptr : g.data(), nullptr, width, height));
 	int * d_words = d_word_ids_out;
 	if (!d_words)
 	{
@@ -5445,7 +5524,7 @@ int lcd_process_frames_decide_submit(lcd_engine * e, int n_frames, const uint8_t
 		LCD_CUDA(e, cudaEventCreateWithFlags(&f.done, cudaEventDisableTiming));
 	}
 	// the slot's previous batch was waited for, so its staging buffers are free: nothing here waits for the batch in flight
-	LCD_TRY(decide_prepare(e, n_frames, ns, clients, frame_flags, dp, s, g.empty() ? nullptr : g.data(), &f.h_tab));
+	LCD_TRY(decide_prepare(e, n_frames, ns, clients, frame_flags, dp, s, g.empty() ? nullptr : g.data(), &f.h_tab, width, height));
 	const float * poses = nullptr;
 	const int * enabled = nullptr;
 	if (stages && stages->proximity)

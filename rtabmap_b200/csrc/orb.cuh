@@ -1568,12 +1568,13 @@ orb_describe_patch_kernel(const uint8_t * __restrict__ blur_all, const __grid_co
 	}
 }
 
-// ---- K7: generateKeypoints3DDepth (depth the size of the image, one camera, identity local transform) ---
+// ---- K7: generateKeypoints3DDepth (depth the size of the image, one camera per frame) ---
 struct OrbXyzArgs
 {
 	const void * depth;
 	int depth_type, w, h;
 	float fx, fy, cx, cy, min_depth, max_depth;
+	const FrameCam * cam; // [n_frames] each frame's client camera (set = 0: fx..cy above, identity local transform) or nullptr
 	const OrbKeypoint * kps;
 	const int * n_kp;
 	int cap;
@@ -1631,15 +1632,21 @@ __global__ void orb_xyz_kernel(const OrbXyzArgs a)
 	sumWeights = __fadd_rn(sumWeights, 4.0f);
 	depth = __fdiv_rn(__fadd_rn(depth, sumDepths), sumWeights);
 	if (!(depth > 0.0f)) return;
-	const float cx = a.cx > 0.0f ? a.cx : __fsub_rn(static_cast<float>(a.w / 2), 0.5f);
-	const float cy = a.cy > 0.0f ? a.cy : __fsub_rn(static_cast<float>(a.h / 2), 0.5f);
-	const float px = __fdiv_rn(__fmul_rn(__fsub_rn(x, cx), depth), a.fx);
-	const float py = __fdiv_rn(__fmul_rn(__fsub_rn(y, cy), depth), a.fy);
+	const FrameCam * fc = (a.cam && a.cam[frame].set) ? a.cam + frame : nullptr;
+	// projectDepthTo3D takes the camera's K as floats
+	const float fx = fc ? static_cast<float>(fc->fx) : a.fx, fy = fc ? static_cast<float>(fc->fy) : a.fy;
+	const float kcx = fc ? static_cast<float>(fc->cx) : a.cx, kcy = fc ? static_cast<float>(fc->cy) : a.cy;
+	const float cx = kcx > 0.0f ? kcx : __fsub_rn(static_cast<float>(a.w / 2), 0.5f);
+	const float cy = kcy > 0.0f ? kcy : __fsub_rn(static_cast<float>(a.h / 2), 0.5f);
+	const float px = __fdiv_rn(__fmul_rn(__fsub_rn(x, cx), depth), fx);
+	const float py = __fdiv_rn(__fmul_rn(__fsub_rn(y, cy), depth), fy);
 	if ((a.min_depth < 0.0f || depth > a.min_depth) && (a.max_depth <= 0.0f || depth <= a.max_depth))
 	{
 		out[0] = px;
 		out[1] = py;
 		out[2] = depth;
+		// into the frame's base frame (util3d_features.cpp:110-114)
+		if (fc && fc->local) transform_point_f(fc->L, px, py, depth, out[0], out[1], out[2]);
 	}
 }
 

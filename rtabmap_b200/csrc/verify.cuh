@@ -58,9 +58,17 @@ struct PairSource
 		int n_all;
 		int cap;               // row stride of the TO arrays
 		const int * row;       // nullptr: TO row = pair; else the TO row of each pair
+		const FrameCam * cam;  // [n_to_rows] the TO camera of each TO row (set = 0: the call's lcd_verify_params) or nullptr
 	} to;
 
 	__device__ __forceinline__ int from_row(int pair) const { return from.slot ? from.slot[pair] : pair; }
+	// the pair's own TO camera, nullptr when it takes the call's parameters
+	__device__ __forceinline__ const FrameCam * to_cam(int pair) const
+	{
+		if (!to.cam) return nullptr;
+		const FrameCam * c = to.cam + (to.row ? to.row[pair] : pair);
+		return c->set ? c : nullptr;
+	}
 	// TO descriptors of the pair, at most cap (the call's) and the TO row stride
 	__device__ __forceinline__ int to_count(int pair, int cap) const { return min(to.n ? to.n[pair] : to.n_all, min(cap, to.cap)); }
 	__device__ __forceinline__ size_t to_base(int pair) const { return static_cast<size_t>(to.row ? to.row[pair] : pair) * to.cap; }
@@ -728,7 +736,7 @@ struct GuessMatchArgs
 	const int * ok1;        // [n_pairs] first pass accepted
 	const double * rvec;    // [n_pairs][3] first-pass pose
 	const double * tvec;
-	CamK cam;
+	CamK cam;               // the call's TO camera; a pair with its own (src.to_cam) uses that one
 	int img_w, img_h;
 	float win;              // Vis/CorGuessWinSize
 	float nndr;
@@ -797,6 +805,7 @@ guess_match_kernel(const GuessMatchArgs a)
 	uint16_t * rank = L + cap;                                     // [cap]
 	uint8_t * flag = reinterpret_cast<uint8_t *>(rank + cap);      // [cap]
 	__shared__ double s_R[9], s_t[3];
+	__shared__ CamK s_cam;
 	__shared__ int s_n;
 	const int tid = threadIdx.x, pair = blockIdx.x;
 	if (!a.ok1[pair]) return;
@@ -805,6 +814,9 @@ guess_match_kernel(const GuessMatchArgs a)
 	if (rv[0] == 0.0 && rv[1] == 0.0 && rv[2] == 0.0 && tv[0] == 0.0 && tv[1] == 0.0 && tv[2] == 0.0) return; // guess.isIdentity(): global matching again
 	const int frow = a.src.from_row(pair);
 	if (frow < 0) return;
+	const FrameCam * fc = a.src.to_cam(pair);
+	const int img_w = fc ? fc->w : a.img_w, img_h = fc ? fc->h : a.img_h;
+	if (img_w <= 0 || img_h <= 0) return; // no image size: the reference has no guess pass for this camera
 	const int nf = min(a.src.from.n[frow], min(cap, a.src.from.cap));
 	const int nt = a.src.to_count(pair, cap);
 	const size_t base = static_cast<size_t>(pair) * cap;
@@ -815,6 +827,7 @@ guess_match_kernel(const GuessMatchArgs a)
 		s_t[0] = tv[0];
 		s_t[1] = tv[1];
 		s_t[2] = tv[2];
+		s_cam = fc ? CamK{fc->fx, fc->fy, fc->cx, fc->cy} : a.cam;
 	}
 	for (int j = tid; j < nt; j += blockDim.x)
 	{
@@ -824,13 +837,14 @@ guess_match_kernel(const GuessMatchArgs a)
 	}
 	__syncthreads();
 	const float r2 = __fmul_rn(a.win, a.win);
-	const float wmax = static_cast<float>(a.img_w - 1), hmax = static_cast<float>(a.img_h - 1);
+	const float wmax = static_cast<float>(img_w - 1), hmax = static_cast<float>(img_h - 1);
 	for (int i = tid; i < nf; i += blockDim.x)
 	{
 		int m = -1;
 		const float * X = a.src.from.xyz + (fbase + i) * 3;
 		double pu, pv;
-		project_point(s_R, s_t, a.cam, X, pu, pv);
+		// the first pass's PnP pose is (guess * localTransform)^-1 of the reference's projection (RegistrationVis.cpp:1034)
+		project_point(s_R, s_t, s_cam, X, pu, pv);
 		const float px = static_cast<float>(pu), py = static_cast<float>(pv);
 		const float zc = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(static_cast<float>(s_R[6]), X[0]), __fmul_rn(static_cast<float>(s_R[7]), X[1])),
 		                                     __fmul_rn(static_cast<float>(s_R[8]), X[2])), static_cast<float>(s_t[2]));
@@ -916,6 +930,9 @@ struct PnpArgs
 	float max_variance;    // Vis/PnPMaxVariance (0 = off)
 	int split_linear;      // Vis/PnPSplitLinearCovComponents
 	int img_w, img_h;      // CameraModel::imageSize() of the TO camera (0 x 0 = not set)
+	// each pair's own TO camera (K, image size and local transform in place of cam, img_w, img_h and identity) where it has one
+	const FrameCam * cam_tab; // nullptr: every pair takes the fields above
+	const int * cam_row;      // nullptr: cam_tab[pair]; else cam_tab[cam_row[pair]]
 	double * cov6;         // [n_pairs][6] diagonal of the 6x6 covariance (the reference only ever scales the identity)
 	// outputs
 	double * rvec;      // [n_pairs][3]
@@ -924,7 +941,7 @@ struct PnpArgs
 	int * n_inliers;    // [n_pairs]
 	int * iters_run;    // [n_pairs]
 	int * ok;           // [n_pairs] 1 = accepted (inliers >= min_inliers)
-	float * transform;  // [n_pairs][12] (localTransform * pnp)^-1, localTransform = identity
+	float * transform;  // [n_pairs][12] (localTransform * pnp)^-1
 	long long * phase_clk; // [n_pairs][16] clock64() at the phase boundaries (diagnostics; may be null)
 };
 
@@ -1136,12 +1153,15 @@ pnp_ransac_kernel(const PnpArgs a)
 	__shared__ LmState lm;
 	__shared__ int s_best, s_nA, s_nB, s_ctrl, s_sizes[64];
 	__shared__ float s_thr;
+	// the pair's TO camera, loaded once per CTA from the pair table (or the call's parameters)
+	__shared__ CamK s_cam;
+	__shared__ int s_img_w, s_img_h, s_local;
+	__shared__ float s_L[12];
 
 	const int tid = threadIdx.x;
 	const int pair = blockIdx.x;
 	const int n = min(a.n_pts[pair], cap);
 	const size_t base = static_cast<size_t>(pair) * cap;
-	const CamK cam = a.cam;
 	const int iterations = min(max(a.iterations, 1), kMaxRansacIters);
 	const int min_inliers = max(a.min_inliers, 4);
 #define PNP_PHASE(k) do { if (a.phase_clk && tid == 0) a.phase_clk[pair * 16 + (k)] = clock64(); } while (0)
@@ -1163,10 +1183,23 @@ pnp_ransac_kernel(const PnpArgs a)
 	// util3d::estimateMotion3DTo2D runs PnP only with >= Vis/MinInliers correspondences; RANSAC needs >= 6
 	if ((a.gate_min_matches && n < a.min_inliers) || n < 6) return;
 
+	if (tid == 0)
+	{
+		const FrameCam * fc = a.cam_tab ? a.cam_tab + (a.cam_row ? a.cam_row[pair] : pair) : nullptr;
+		if (fc && !fc->set) fc = nullptr;
+		s_cam = fc ? CamK{fc->fx, fc->fy, fc->cx, fc->cy} : a.cam;
+		s_img_w = fc ? fc->w : a.img_w;
+		s_img_h = fc ? fc->h : a.img_h;
+		s_local = fc ? fc->local : 0;
+		if (fc)
+			for (int k = 0; k < 12; ++k) s_L[k] = fc->L[k];
+	}
 	for (int i = tid; i < n * 3; i += blockDim.x) X[i] = a.obj[base * 3 + i];
 	for (int i = tid; i < n * 2; i += blockDim.x) uv[i] = a.img[base * 2 + i];
 	__syncthreads();
 	PNP_PHASE(1);
+	// each thread's copy of the camera, as the kernel always had (a reference to s_cam costs spills): the same registers and stack frame
+	const CamK cam = s_cam;
 
 	// ---- hypotheses in waves, one thread per hypothesis: EPnP on the sample, then the inlier counts; thread 0 then replays the
 	//      sequential bookkeeping of RANSACPointSetRegistrator::run (solvepnp.cpp:358-399) and decides whether the run goes on.
@@ -1444,7 +1477,9 @@ pnp_ransac_kernel(const PnpArgs a)
 		a.tvec[pair * 3 + tid] = lm.param[3 + tid];
 	}
 	for (int k = tid; k < n_fin; k += blockDim.x) a.inliers[base + k] = fin[k];
-	__shared__ float s_T[12], s_P[12]; // transform = (localTransform * pnp)^-1 and pnp itself (= transformCameraFrameInv), 3x4 float
+	// transform = (localTransform * pnp)^-1, transformCameraFrame = transform * localTransform and its inverse, 3x4 float; with an identity
+	// local transform the last two are transform and pnp itself
+	__shared__ float s_T[12], s_C[12], s_P[12];
 	__shared__ int s_acc;
 	__shared__ double s_med[5];
 	if (tid == 0)
@@ -1469,15 +1504,24 @@ pnp_ransac_kernel(const PnpArgs a)
 				s_T[4 * i + 3] = -(Rf[0 + i] * tf[0] + Rf[3 + i] * tf[1] + Rf[6 + i] * tf[2]);
 				s_P[4 * i + 3] = tf[i];
 			}
+			if (s_local)
+			{
+				transform_mul_f(s_L, s_P, s_C); // localTransform * pnp, in s_C until the last two steps
+				transform_inv_f(s_C, s_T);
+				transform_mul_f(s_T, s_L, s_C);
+				transform_inv_f(s_C, s_P);
+			}
+			else
+				for (int k = 0; k < 12; ++k) s_C[k] = s_T[k];
 		}
 	}
 	__syncthreads();
 	int accepted = s_acc;
 	if (accepted && a.cov6)
 	{
-		// ---- covariance (util3d_motion_estimation.cpp:156-258), localTransform = identity --------------------
+		// ---- covariance (util3d_motion_estimation.cpp:156-258) --------------------
 		const bool have3B = a.obj_to != nullptr;
-		if (have3B || a.img_w != 0 || a.img_h != 0)
+		if (have3B || s_img_w != 0 || s_img_h != 0)
 		{
 			// channels: 0 squared 3-D distance, 1 angle (pcl::getAngle3D), 2..4 squared x / y / z error (split components)
 			const int n_ch = a.split_linear ? 5 : 2;
@@ -1508,16 +1552,16 @@ pnp_ransac_kernel(const PnpArgs a)
 						const float zc = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(s_P[8], ox), __fmul_rn(s_P[9], oy)), __fmul_rn(s_P[10], oz)), s_P[11]);
 						const float fx = static_cast<float>(cam.fu), fy = static_cast<float>(cam.fv);
 						float cx = static_cast<float>(cam.uc), cy = static_cast<float>(cam.vc);
-						cx = cx > 0.0f ? cx : static_cast<float>(a.img_w / 2) - 0.5f;
-						cy = cy > 0.0f ? cy : static_cast<float>(a.img_h / 2) - 0.5f;
+						cx = cx > 0.0f ? cx : static_cast<float>(s_img_w / 2) - 0.5f;
+						cy = cy > 0.0f ? cy : static_cast<float>(s_img_h / 2) - 0.5f;
 						const float rx = __fdiv_rn(__fsub_rn(uv[2 * i], cx), fx), ry = __fdiv_rn(__fsub_rn(uv[2 * i + 1], cy), fy);
 						// cv::Point3f * (float * double): the scale is a double product converted back to float per component
 						const double sc = static_cast<double>(zc) * 1.1;
 						const float px = static_cast<float>(static_cast<double>(rx) * sc), py = static_cast<float>(static_cast<double>(ry) * sc),
 						            pz = static_cast<float>(sc);
-						nx = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(s_T[0], px), __fmul_rn(s_T[1], py)), __fmul_rn(s_T[2], pz)), s_T[3]);
-						ny = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(s_T[4], px), __fmul_rn(s_T[5], py)), __fmul_rn(s_T[6], pz)), s_T[7]);
-						nz = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(s_T[8], px), __fmul_rn(s_T[9], py)), __fmul_rn(s_T[10], pz)), s_T[11]);
+						nx = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(s_C[0], px), __fmul_rn(s_C[1], py)), __fmul_rn(s_C[2], pz)), s_C[3]);
+						ny = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(s_C[4], px), __fmul_rn(s_C[5], py)), __fmul_rn(s_C[6], pz)), s_C[7]);
+						nz = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(s_C[8], px), __fmul_rn(s_C[9], py)), __fmul_rn(s_C[10], pz)), s_C[11]);
 					}
 					const float dx = __fsub_rn(ox, nx), dy = __fsub_rn(oy, ny), dz = __fsub_rn(oz, nz);
 					float v;

@@ -30,9 +30,9 @@ Host-side I/O only: SQLite rows in, the arrays the C ABI takes out.  Follows the
   open_localization_map  all of the above into an engine, in one call, refusing a map the engine cannot serve before any change
 
 The FLANN index blob (Admin.dictionary_index, :3622-3660) is not read: the engine searches exhaustively and keeps no tree.  Images,
-depth and calibration (Data) are not read either.  The engine's verification assumes an identity camera local transform: a map recorded
-with a non-identity localTransform stores its 3-D points (Feature.depth_*) in the robot's base frame, and the loader, which does not read
-Data.calibration, passes them on as they are.  Databases older than 0.13.0 (the Map_Node_Word era) are refused.
+depth and calibration (Data) are not read either.  A map's stored 3-D points (Feature.depth_*) are already in each place's base frame,
+whatever its localTransform, and are loaded as they are; the clients' own cameras (K, image size and localTransform of
+SensorData::cameraModels()[0]) are set with Engine.clients_set_cameras.  Databases older than 0.13.0 (the Map_Node_Word era) are refused.
 """
 from __future__ import annotations
 
@@ -478,8 +478,8 @@ def open_localization_map(engine, path: str, node_ids=None, prediction_lc=None, 
     and opt_poses of different lengths, global descriptors the store cannot hold, and a node with more Feature rows than the engine's
     stores accept (with the engine's own LCD_ERR_CAPACITY message).
 
-    The engine's verification assumes an identity camera local transform; 3-D points of a map recorded with another localTransform
-    are in the base frame and are loaded as stored (Data.calibration is not read)."""
+    3-D points are in each place's base frame whatever its localTransform and are loaded as stored (Data.calibration is not read);
+    each localisation client's camera is Engine.clients_set_cameras's."""
     from . import graph
     from .capi import LCD_DESC_U8
 
