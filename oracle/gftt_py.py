@@ -8,7 +8,10 @@ composes those calls with opencv-python 4.13, the dependency itself.
 numpy, in the arithmetic the CUDA kernels (rtabmap_b200/csrc/gftt.cuh) use; tests/test_oracle_gftt.py pins them bit for bit to cv2:
   * Sobel, scale s = 1/(4*3*255) as a float, reflect-101 border:
       dx = fma(U + D, s, C * 2s), U/C/D = I[x+1] - I[x-1] on the rows above, at and below;
-      row pass r = fma(R, s, fma(M, 2s, L * s)), dy = r[y+1] - r[y-1];
+      row pass of column x: r = fma(R, s, fma(M, 2s, L * s)) for x < (w // 32) * 32, ((L * s + M * 2s) + R * s) without fused
+      multiply-add in the last w % 32 columns; dy = r[y+1] - r[y-1].  32 is the width in pixels (one v_uint8 register) of OpenCV's
+      x86 AVX2 row filter: its vector body fuses, its scalar tail does not.  The pinned target is x86 opencv-python 4.13;
+      tests/test_oracle_gftt_edges.py probes the host's cv2 for that boundary (other platforms' vector widths differ);
   * products dx*dx, dx*dy, dy*dy in float; the unnormalised 3x3 box filter sums each row in double, (p[x-1] + p[x]) + p[x+1],
     then keeps a RUNNING column sum in double from the top of the image down (add the row entering, output, subtract the row
     leaving).  The running sum is not exact (the Sobel fma leaves residuals of ~1e-12 whose squares reach below the double's
@@ -45,16 +48,23 @@ def _fma(a, b, c):
     return (a.astype(np.float64) * np.float64(b) + c.astype(np.float64)).astype(np.float32)
 
 
-def corner_min_eig(gray: np.ndarray) -> np.ndarray:
+SIMD_ROW_WIDTH = 32  # pixels per vector of OpenCV's x86 AVX2 row filter (v_uint8): the columns its fused vector body covers
+
+
+def corner_min_eig(gray: np.ndarray, simd_width: int = SIMD_ROW_WIDTH) -> np.ndarray:
+    """cv::cornerMinEigenVal(gray, 3, 3); the row pass of dy is fused in the first (w // simd_width) * simd_width columns (simd_width=1:
+    fused everywhere, the tests' way to see which pixels the unfused tail changes)"""
     f = np.float32
     s = f(1.0 / 3060.0)
     s2 = f(2.0 / 3060.0)
     P = np.pad(gray, 1, mode="reflect").astype(np.float32)
     D = P[:, 2:] - P[:, :-2]
     dx = _fma(D[:-2] + D[2:], s, D[1:-1] * s2)
-    r = _fma(P[:, 2:], s, _fma(P[:, 1:-1], s2, P[:, :-2] * s))
-    dy = r[2:] - r[:-2]
     h, w = gray.shape
+    r = _fma(P[:, 2:], s, _fma(P[:, 1:-1], s2, P[:, :-2] * s))
+    x0 = (w // simd_width) * simd_width
+    r[:, x0:] = (P[:, x0:w] * s + P[:, x0 + 1:w + 1] * s2) + P[:, x0 + 2:w + 2] * s
+    dy = r[2:] - r[:-2]
 
     def box(p):
         q = np.pad(p, 1, mode="reflect").astype(np.float64)

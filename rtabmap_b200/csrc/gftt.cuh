@@ -6,8 +6,10 @@
 // come from orb_prepare*, the descriptors and 3-D points from the ORB kernels (orb.cuh) unchanged.
 //
 // Bit-exactness (the arithmetic of oracle/gftt_py.py, pinned to opencv-python 4.13 by tests/test_oracle_gftt.py):
-//   * Sobel with s = 1/3060: dx = fma(U + D, s, C * 2s) on the row differences above / at / below; row pass
-//     fma(R, s, fma(M, 2s, L * s)), dy = its difference between the rows below and above; reflect-101 border;
+//   * Sobel with s = 1/3060: dx = fma(U + D, s, C * 2s) on the row differences above / at / below; row pass of column c
+//     fma(R, s, fma(M, 2s, L * s)) for c < (w & ~31), ((L * s + M * 2s) + R * s) without fused multiply-add in the last w % 32 columns
+//     (OpenCV's x86 AVX2 row filter fuses in its 32-pixel vector body, not in its scalar tail); dy = the row pass's difference between
+//     the rows below and above; reflect-101 border;
 //   * the 3x3 box filter of the products sums each row in double and keeps a RUNNING column sum in double from the top of the image
 //     down, as OpenCV's column filter does: that sum is not exact, so the corner kernel walks every column from row 0;
 //   * lambda = (a + c) - sqrt((a - c)^2 + b^2) in float, a = 0.5 xx, c = 0.5 yy, no fused multiply-add;
@@ -61,9 +63,11 @@ gftt_eig_kernel(const GfttEigArgs a)
 	const int xc = reflect101(min(x, w), w);
 	const int xm = reflect101(xc - 1, w), xp = reflect101(xc + 1, w);
 	const float s = static_cast<float>(1.0 / 3060.0), s2 = static_cast<float>(2.0 / 3060.0);
+	const bool fused = xc < (w & ~31); // xc, not x: the halo thread at x = w stands for column w - 2
 	auto row_d = [&](int r) { return static_cast<float>(img[r * w + xp]) - static_cast<float>(img[r * w + xm]); };
 	auto row_s = [&](int r) {
-		return __fmaf_rn(static_cast<float>(img[r * w + xp]), s, __fmaf_rn(static_cast<float>(img[r * w + xc]), s2, __fmul_rn(static_cast<float>(img[r * w + xm]), s)));
+		const float L = static_cast<float>(img[r * w + xm]), M = static_cast<float>(img[r * w + xc]), R = static_cast<float>(img[r * w + xp]);
+		return fused ? __fmaf_rn(R, s, __fmaf_rn(M, s2, __fmul_rn(L, s))) : __fadd_rn(__fadd_rn(__fmul_rn(L, s), __fmul_rn(M, s2)), __fmul_rn(R, s));
 	};
 	// row sums (double) of the products of image row r
 	auto row_sums = [&](int r, double & sxx, double & sxy, double & syy) {

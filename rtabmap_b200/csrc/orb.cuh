@@ -1279,6 +1279,17 @@ __constant__ float kOrbGauss7[7];
 
 constexpr int kBlurTW = 32, kBlurTH = 16;
 
+// one output of the row pass, taps in plain order.  OpenCV's x86 AVX2 row filter fuses multiply and add in its vector body, which covers
+// the columns below w & ~31 (32 pixels per vector); its scalar tail, the last w % 32 columns, rounds the product and the sum separately.
+template <bool kFused>
+__device__ __forceinline__ float orb_blur_row(const float * p)
+{
+	float s = __fmul_rn(p[0], kOrbGauss7[0]);
+#pragma unroll
+	for (int k = 1; k < 7; ++k) s = kFused ? __fmaf_rn(p[k], kOrbGauss7[k], s) : __fadd_rn(s, __fmul_rn(p[k], kOrbGauss7[k]));
+	return s;
+}
+
 __global__ void __launch_bounds__(256)
 orb_blur_kernel(const uint8_t * __restrict__ gray_all, uint8_t * __restrict__ blur_all, const OrbGeom g, int level)
 {
@@ -1299,14 +1310,14 @@ orb_blur_kernel(const uint8_t * __restrict__ gray_all, uint8_t * __restrict__ bl
 		s_g[ry][rx] = img[y * w + x];
 	}
 	__syncthreads();
-	// row pass (plain order, fused multiply-add) for the TH+6 rows the column pass needs
+	// row pass (plain order, orb_blur_row) for the TH+6 rows the column pass needs
 	for (int i = tid; i < (kBlurTH + 6) * kBlurTW; i += 256)
 	{
 		const int ry = i / kBlurTW, rx = i % kBlurTW;
-		float s = __fmul_rn(static_cast<float>(s_g[ry][rx]), kOrbGauss7[0]);
+		float p[7];
 #pragma unroll
-		for (int k = 1; k < 7; ++k) s = __fmaf_rn(static_cast<float>(s_g[ry][rx + k]), kOrbGauss7[k], s);
-		rowf[ry][rx] = s;
+		for (int k = 0; k < 7; ++k) p[k] = static_cast<float>(s_g[ry][rx + k]);
+		rowf[ry][rx] = x0 + rx < (w & ~31) ? orb_blur_row<true>(p) : orb_blur_row<false>(p);
 	}
 	__syncthreads();
 	// column pass (symmetric, fused multiply-add), then saturate_cast<uchar> (round half to even)
@@ -1369,9 +1380,8 @@ orb_blur_tma_kernel(const __grid_constant__ OrbTensorMap tmap, uint8_t * __restr
 		}
 		__syncthreads();
 	}
-	const float k0 = kOrbGauss7[0], k1 = kOrbGauss7[1], k2 = kOrbGauss7[2], k3 = kOrbGauss7[3], k4 = kOrbGauss7[4], k5 = kOrbGauss7[5],
-	            k6 = kOrbGauss7[6];
-	// row pass (plain order, fused multiply-add): outputs x0 + 8j .. + 7 of staged row r + 1 read staged columns 8j + 13 .. 8j + 26
+	const float k3 = kOrbGauss7[3], k4 = kOrbGauss7[4], k5 = kOrbGauss7[5], k6 = kOrbGauss7[6];
+	// row pass (plain order, orb_blur_row): outputs x0 + 8j .. + 7 of staged row r + 1 read staged columns 8j + 13 .. 8j + 26
 	for (int it = tid; it < RH * (TW / 8); it += 256)
 	{
 		const int r = it >> 3, j = it & 7;
@@ -1393,17 +1403,15 @@ orb_blur_tma_kernel(const __grid_constant__ OrbTensorMap tmap, uint8_t * __restr
 		p[12] = static_cast<float>((w3 >> 8) & 0xFFu);
 		p[13] = static_cast<float>((w3 >> 16) & 0xFFu);
 		float o[8];
-#pragma unroll
-		for (int q = 0; q < 8; ++q)
+		if (x0 + 8 * j < (w & ~31)) // the 8 outputs lie on one side of w & ~31: both are multiples of 8
 		{
-			float s = __fmul_rn(p[q], k0);
-			s = __fmaf_rn(p[q + 1], k1, s);
-			s = __fmaf_rn(p[q + 2], k2, s);
-			s = __fmaf_rn(p[q + 3], k3, s);
-			s = __fmaf_rn(p[q + 4], k4, s);
-			s = __fmaf_rn(p[q + 5], k5, s);
-			s = __fmaf_rn(p[q + 6], k6, s);
-			o[q] = s;
+#pragma unroll
+			for (int q = 0; q < 8; ++q) o[q] = orb_blur_row<true>(p + q);
+		}
+		else
+		{
+#pragma unroll
+			for (int q = 0; q < 8; ++q) o[q] = orb_blur_row<false>(p + q);
 		}
 		float4 * dst = reinterpret_cast<float4 *>(s_row + r * TW + 8 * j);
 		dst[0] = make_float4(o[0], o[1], o[2], o[3]);
